@@ -1,4 +1,4 @@
-"""dotaclient_b200 -- B200-native implementation of DotaClient's distributed-optimizer hot path.
+"""dotaclient_b200 -- CUDA-native (H100) implementation of DotaClient's distributed-optimizer hot path.
 
 Drop-in module surface of the reference (TimZaman/dotaclient @ 8615b90):
 
@@ -7,7 +7,7 @@ Drop-in module surface of the reference (TimZaman/dotaclient @ 8615b90):
   ``advantage_returns``, ``discount``, ``init_distribution``, ``main``)
 * ``dotaclient_b200.distributed``  <-> reference ``distributed.py``  (``DistributedDataParallelSparseParamCPU``)
 
-The arithmetic runs in hand-written sm_100a CUDA kernels behind the C-ABI declared in
+The arithmetic runs in hand-written sm_90a CUDA kernels behind the C-ABI declared in
 ``include/dotaclient_b200.h`` (``dotaclient_b200/csrc``).  There is no CPU fallback.
 """
 __version__ = "0.1.0"

@@ -71,7 +71,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise NativeLibraryError(
-            "%s not found: build it with `python -m dotaclient_b200.build` (needs nvcc, sm_100a). "
+            "%s not found: build it with `python -m dotaclient_b200.build` (needs nvcc, sm_90a). "
             "dotaclient_b200 has no CPU fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():

@@ -1,4 +1,4 @@
-"""Builds ``libdotaclient_b200.so`` (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Builds ``libdotaclient_b200.so`` (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 ``python -m dotaclient_b200.build`` or ``__graft_entry__.build()``.  The library links the static
 CUDA runtime only -- no torch, no Python -- so the same .so serves ctypes, cgo, JNI or any other FFI.
@@ -11,6 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libdotaclient_b200.so")
+ARCH = "arch=compute_90a,code=sm_90a"       # wgmma and the sm_90a feature set: H100 only
 SOURCES = ["capi.cu", "gae_scan.cu", "ppo_loss.cu", "grad_finish.cu", "rnn_seq.cu", "gemm_tf32x3.cu", "encoder.cu", "actor.cu"]
 
 
@@ -36,7 +37,7 @@ def build(force=False, verbose=False):
     objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
     nvcc = _nvcc()
-    common = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    common = ["-gencode", ARCH, "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
     if verbose:
         common += ["-Xptxas", "-v"]
@@ -56,7 +57,7 @@ def build(force=False, verbose=False):
     if failed:
         raise RuntimeError("nvcc failed")
     if force or procs or _stale(LIB_PATH, objs):
-        subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH] + objs)
+        subprocess.check_call([nvcc, "-shared", "-gencode", ARCH, "-o", LIB_PATH] + objs)
     return LIB_PATH
 
 

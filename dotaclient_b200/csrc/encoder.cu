@@ -32,7 +32,7 @@ __global__ void __launch_bounds__(kThreadsE) unit_basic_fwd_kernel(const float *
                                                                    float *__restrict__ basic, int64_t R) {
     __shared__ float s_u[kWarps][32][kIn];                        // 32 rows of raw features per warp per iteration
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    // weights as channel PAIRS for the packed fp32x2 FMA (FFMA2): w2[p][k] = (W_b[4l+2p][k], W_b[4l+2p+1][k])
+    // weights as channel PAIRS: w2[p][k] = (W_b[4l+2p][k], W_b[4l+2p+1][k])
     float2 w2[2][kIn], b2[2];
 #pragma unroll
     for (int p = 0; p < 2; ++p) {
@@ -53,8 +53,8 @@ __global__ void __launch_bounds__(kThreadsE) unit_basic_fwd_kernel(const float *
             for (int k = 0; k < kIn; ++k) {
                 const float u = s_u[warp][r][k];
                 const float2 uu = make_float2(u, u);
-                a0 = __ffma2_rn(uu, w2[0][k], a0);
-                a1 = __ffma2_rn(uu, w2[1][k], a1);
+                a0 = dc_ffma2(uu, w2[0][k], a0);
+                a1 = dc_ffma2(uu, w2[1][k], a1);
             }
             *reinterpret_cast<float4 *>(basic + (base + r) * kC + lane * 4) =
                 make_float4(fmaxf(a0.x, 0.f), fmaxf(a0.y, 0.f), fmaxf(a1.x, 0.f), fmaxf(a1.y, 0.f));

@@ -2,28 +2,25 @@
 //
 // H = 256 is the reference's own width (policy.py:66 nn.GRU(256, 256)); W_hh is 768 KB (GRU) / 1 MB (LSTM) in fp32 and
 // cannot live in one SM.  At this width the step IS a dense contraction -- [sequences, 256] x [256, G*256] per step --
-// and fp32 FFMA cannot reach even a third of the HBM roofline (512 x 256 x 1024 MACs / step = 3.7 us on all 148 SMs), so
-// the mat-vec runs on tcgen05 with the same 3xTF32 split as the other dense layers (fp32-level accuracy, ~1e-6).
+// so the mat-vec runs on the tensor cores (wgmma) with the same 3xTF32 split as the other dense layers (fp32-level
+// accuracy, ~1e-6).
 //
 //   * a CLUSTER of 8 CTAs owns kNB = 32 sequences for all S steps; CTA r owns hidden units [32r, 32r+32): its 4 x 32
 //     rows of W_hh (forward) / 4 x 32 columns (backward) stay on chip for the whole launch -- the tf32 hi half in
-//     TENSOR MEMORY (256 columns, the A operand of tcgen05.mma [d], [a_tmem], b-desc), the lo half in shared memory
-//     (128 KB of K-major SWIZZLE_128B tiles);
-//   * forward  D^T[(g,u)][b] = W_hh[(g,u)][:] . h[b][:]      M = 128 rows, N = 32 sequences, K = 256: every CTA needs the
+//     REGISTERS as the A fragments of wgmma (64 registers per thread), the lo half in shared memory (128 KB of K-major
+//     SWIZZLE_128B tiles).  Both halves in shared memory would need 256 KB, more than an SM has;
+//   * forward  D[(g,u)][b] = W_hh[(g,u)][:] . h[b][:]      M = 128 rows, N = 32 sequences, K = 256: every CTA needs the
 //     whole h of its 32 sequences -- an all-gather.  h_t is an OUTPUT of the layer anyway (ybuf), so each CTA writes its
 //     32-unit slice to ybuf, the cluster barrier (release/acquire) publishes it, and every CTA reads the [32 x 256] tile
-//     back from L2, splits it hi/lo and stores the B-operand tiles;
-//   * backward D^T[k][b] = sum_{j in own 128 gate columns} W_hh[j][k] dg[b][j]   2 x (M = 128), N = 32, K = 128: the B
-//     operand (this CTA's own gate gradients) is local; the partial sums over the 8 CTAs are exchanged through a small
-//     L2-resident scratch (reduce-scatter, fixed summation order => deterministic);
-//   * gate math: thread = (unit, 4 sequences), 128-byte coalesced global accesses; the per-step global inputs are
-//     prefetched one step ahead into registers while the MMAs run.
-// Per step and CTA: 96 tcgen05.mma (M128 N32 K8), one cluster barrier, one L2 round trip.  ncu (profiles/r2_rnn_cluster_ncu.md):
-// a chain of MMAs into ONE accumulator is latency-bound (~100 cycles per dependent MMA vs ~30 of tensor-pipe work), so every
-// K-panel accumulates into its own TMEM accumulator (8 independent chains of 12) and the epilogue adds them; ONE thread issuing
-// all 96 MMAs is itself a bottleneck (~100 cycles of scalar work per instruction), so eight threads issue one chain each from
-// register-resident descriptors; the cluster barrier is split (arrive.release right after the exchanged slice is stored,
-// wait.acquire after the remaining stores).
+//     back from L2, splits it hi/lo and stores the B-operand tiles.  Warpgroup w takes rows [64 (w%2), +64) and K half
+//     w/2; the two K halves meet in shared memory;
+//   * backward D[k][b] = sum_{j in own 128 gate columns} W_hh[j][k] dg[b][j]   M = 256 (64 rows per warpgroup), N = 32,
+//     K = 128: the B operand (this CTA's own gate gradients) is local; the partial sums over the 8 CTAs are exchanged
+//     through a small L2-resident scratch (reduce-scatter, fixed summation order => deterministic);
+//   * gate math: thread = (unit, 2 sequences), 128-byte coalesced global accesses; the per-step global inputs are
+//     loaded while the wgmma run asynchronously.
+// Per step and CTA: 48 wgmma m64n32k8 per warpgroup, one cluster barrier, one L2 round trip; the cluster barrier is split
+// (arrive.release right after the exchanged slice is stored, wait.acquire after the remaining stores).
 // Algorithmic HBM bytes per token: forward 4*(G+1)*H, backward 8*(G+1)*H (SURVEY.md 8d).
 #pragma once
 #include "dc_common.cuh"
@@ -33,79 +30,43 @@ namespace dc_rnnc {
 constexpr int kH = 256;
 constexpr int kCL = 8;                  // CTAs per cluster
 constexpr int kNB = 32;                 // sequences per cluster = MMA N
-constexpr int kThreads = 512;
+constexpr int kThreads = 512;           // 4 warpgroups
 constexpr int kPanelA = 128 * 128;      // bytes of one A tile: 128 rows x 32 tf32 (one SWIZZLE_128B row each)
 constexpr int kPanelB = kNB * 128;      // bytes of one B tile:  32 rows x 32 tf32
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                     : "=r"(ok)
-                     : "r"(smem_u32(bar)), "r"(parity)
-                     : "memory");
-    } while (!ok);
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor (same encoding as csrc/gemm_tf32x3.cu): 8-row groups 1024 B apart.
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// D = f32, A = B = tf32, both K-major, N = 32 (>>3 at bit 17), M = 128 (>>4 at bit 24)
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kNB >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return dc_smem_u32(p); }
+__device__ __forceinline__ float tf32_rna(float v) { return dc_tf32_rna(v); }
 
-__device__ __forceinline__ float tf32_rna(float v) { return __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xffffe000u); }
-
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr),
-                 "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-                 "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+#define DC_ACC16 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+                 "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+// d (+)= A[smem desc, 64 x 8] B[smem desc, 32 x 8]^T
+__device__ __forceinline__ void wgmma_ss(float (&d)[16], uint64_t desc_a, uint64_t desc_b) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}\n"
+        : DC_ACC16
+        : "l"(desc_a), "l"(desc_b), "r"(1));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+// d (+)= A[registers, 64 x 8] B[smem desc, 32 x 8]^T.  Fragment of thread (warp w of the warpgroup, lane l): a[0] = A[16w + l/4][l%4],
+// a[1] = A[16w + l/4 + 8][l%4], a[2] = A[16w + l/4][l%4 + 4], a[3] = A[16w + l/4 + 8][l%4 + 4].
+__device__ __forceinline__ void wgmma_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}\n"
+        : DC_ACC16
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+}
+#undef DC_ACC16
+// K-major SWIZZLE_128B shared-memory matrix descriptor: 8-row groups 1024 B apart (dc_wgmma_desc)
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) { return dc_wgmma_desc(smem_addr); }
+// accumulator fragment of m64n32: d[i] at row 16*warp + lane/4 + 8*((i/2)%2), column 8*(i/4) + 2*(lane%4) + i%2
+__device__ __forceinline__ int acc_row(int i, int wi, int lane) { return 16 * wi + (lane >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int acc_col(int i, int lane) { return 8 * (i >> 2) + 2 * (lane & 3) + (i & 1); }
+__device__ __forceinline__ void acc_fence(float (&d)[16]) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) dc_reg_fence(d[i]);
 }
 // All threads of all CTAs of the cluster.  release/acquire at cluster scope: global writes made before the barrier by any
 // thread of the cluster are visible to every thread of the cluster after it.
@@ -118,35 +79,16 @@ __device__ __forceinline__ unsigned char *align1024(unsigned char *p) {
 // one 16-byte chunk (4 tf32) of row `row`, 16-byte chunk index `c` (0..7) of a K-major SWIZZLE_128B tile
 __device__ __forceinline__ int swz(int row, int c) { return row * 128 + ((c ^ (row & 7)) << 4); }
 
-__device__ __forceinline__ void tmem_alloc_512(uint32_t *slot, int warp) {
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_free_512(uint32_t tmem_base, int warp) {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-    }
-}
-
 // ---- forward ------------------------------------------------------------------------------------------------------------
-// TMEM: [0,256) W_hh slice, hi half: lane rho = g*32 + u  <->  row g*H + 32*rank + u, column = k;  [256,512) eight
-// accumulators of 32 columns, one per K-panel.
-// shared: W lo half (8 K-panels of [128 rows x 32]), h hi / lo (8 K-panels of [32 sequences x 32]), transposition scratch.
+// W_hh slice row rho = g*32 + u  <->  row g*H + 32*rank + u of W_hh, column = k.  Registers: the hi half of warpgroup w's
+// rows [64 (w%2), +64) and K half w/2.  Shared: W lo half (8 K-panels of [128 rows x 32]), h hi / lo (8 K-panels of
+// [32 sequences x 32]), the two K halves' products [2][4 gates][32 sequences][32 units].
 struct FwdSmem {
     static constexpr size_t wlo = 0;
     static constexpr size_t hhi = wlo + 8 * kPanelA;
     static constexpr size_t hlo = hhi + 8 * kPanelB;
-    static constexpr size_t scratch = hlo + 8 * kPanelB;          // [4 gates][32 sequences][32 units] fp32
-    static constexpr size_t bars = scratch + 4 * kNB * 32 * 4;
-    static constexpr size_t total = bars + 64 + 1024;             // + alignment slack
+    static constexpr size_t scratch = hlo + 8 * kPanelB;          // [2 K halves][4 gates][32 sequences][32 units] fp32
+    static constexpr size_t total = scratch + 2 * 4 * kNB * 32 * 4 + 1024;   // + alignment slack
 };
 constexpr int kNP = 2;                                            // (sequence, unit) pairs per thread in the gate phase
 
@@ -159,32 +101,33 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
     unsigned char *base = align1024(smem_raw);
     unsigned char *wlo = base + FwdSmem::wlo, *hhi = base + FwdSmem::hhi, *hlo = base + FwdSmem::hlo;
     float *scratch = reinterpret_cast<float *>(base + FwdSmem::scratch);
-    uint64_t *mma_done = reinterpret_cast<uint64_t *>(base + FwdSmem::bars);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(mma_done + 1);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int rank = blockIdx.x % kCL, b0 = (blockIdx.x / kCL) * kNB;
 
-    if (tid == 0) {
-        mbar_init(mma_done, 8);                                           // one commit per issuing thread
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    // MMA roles: warpgroup wg takes rows [64 mh, 64 mh + 64) of the slice and K-panels [4 kh, 4 kh + 4)
+    const int wg = warp >> 2, wi = warp & 3, mh = wg & 1, kh = wg >> 1;
+    uint32_t ahi[16][4];                                                   // A fragments of the hi half, one per k-step of 8
+    {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int rho = 64 * mh + 16 * wi + (lane >> 2) + 8 * h, g = rho >> 5;
+            const float *wrow = w_hh + (size_t)(g * H + rank * 32 + (rho & 31)) * H + 128 * kh + (lane & 3);
+#pragma unroll
+            for (int s = 0; s < 16; ++s) {
+                ahi[s][h] = __float_as_uint(g < G ? tf32_rna(__ldg(wrow + 8 * s)) : 0.f);          // GRU has no 4th gate: zero rows
+                ahi[s][h + 2] = __float_as_uint(g < G ? tf32_rna(__ldg(wrow + 8 * s + 4)) : 0.f);
+            }
+        }
     }
-    tmem_alloc_512(tmem_slot, warp);
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_w = tmem_base, tmem_acc = tmem_base + 256;
-    // MMA issue: lane 0 of warp p issues the 12 MMAs of K-panel p into accumulator p.  ncu (v2): ONE thread issuing all 96 MMAs
-    // of a step needs ~100 cycles of scalar work per instruction (descriptor arithmetic, R2UR moves) for ~30 cycles of
-    // tensor-pipe work; eight threads issue concurrently and keep their (step-invariant) descriptors in registers.
-    const bool issuer = lane == 0 && warp < 8;
-    const uint64_t d_alo = make_desc(smem_u32(wlo) + (warp & 7) * kPanelA), d_bhi = make_desc(smem_u32(hhi) + (warp & 7) * kPanelB),
-                   d_blo = make_desc(smem_u32(hlo) + (warp & 7) * kPanelB);
-    const uint32_t t_acc = tmem_acc + 32 * (warp & 7), t_ahi = tmem_w + 32 * (warp & 7);
+    const uint64_t d_alo = make_desc(smem_u32(wlo) + 4 * kh * kPanelA + mh * 64 * 128), d_bhi = make_desc(smem_u32(hhi) + 4 * kh * kPanelB),
+                   d_blo = make_desc(smem_u32(hlo) + 4 * kh * kPanelB);
+    float *my_scratch = scratch + kh * (4 * kNB * 32);
 
-    {   // resident weights, once: warp (q, kq) fills lanes [32q, 32q+32), columns [64*kq, 64*kq+64)
+    {   // resident lo half, once: warp (q, kq) fills rows [32q, 32q+32), columns [64*kq, 64*kq+64)
         const int q = warp & 3, kq = warp >> 2, rho = q * 32 + lane;
         const bool valid = q < G;                                          // q == gate index; GRU has no 4th gate: zero rows
         const float *wrow = w_hh + (size_t)(q * H + rank * 32 + lane) * H;
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
 #pragma unroll 2
         for (int k0 = kq * 64; k0 < kq * 64 + 64; k0 += 8) {
             float w[8], hi[8], lo[8];
@@ -197,18 +140,14 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
             }
 #pragma unroll
             for (int e = 0; e < 8; ++e) { hi[e] = tf32_rna(w[e]); lo[e] = w[e] - hi[e]; }
-            tmem_st8(tmem_w + lane_addr + k0, hi);
             unsigned char *panel = wlo + (size_t)(k0 >> 5) * kPanelA;
             const int c0 = (k0 & 31) >> 2;
             *reinterpret_cast<float4 *>(panel + swz(rho, c0)) = make_float4(lo[0], lo[1], lo[2], lo[3]);
             *reinterpret_cast<float4 *>(panel + swz(rho, c0 + 1)) = make_float4(lo[4], lo[5], lo[6], lo[7]);
         }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 
     // gate phase: thread = (unit ul, sequences sb + 16 i)
     const int ul = lane, unit = rank * 32 + ul, sb = warp;
@@ -253,20 +192,21 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
             }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
-        // ---- B: 96 MMAs, 12 per issuing thread (K-panel = accumulator = warp index)
-        if (issuer) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        // ---- B: 48 wgmma per warpgroup (4 K-panels x 4 k-steps x 3 products), asynchronous until the wait below
+        float d[16];
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-                umma_ss(t_acc, d_alo + 2 * ks, d_bhi + 2 * ks, kIdesc, ks != 0);                 // small terms first
-                umma_ts(t_acc, t_ahi + 8 * ks, d_blo + 2 * ks, kIdesc, 1u);
-                umma_ts(t_acc, t_ahi + 8 * ks, d_bhi + 2 * ks, kIdesc, 1u);
-            }
-            umma_commit(mma_done);
+        for (int i = 0; i < 16; ++i) d[i] = 0.f;
+        acc_fence(d);
+        dc_wgmma_fence();
+#pragma unroll
+        for (int s = 0; s < 16; ++s) {
+            const uint64_t adv = (uint64_t)((s & 3) * 2), pa = (uint64_t)(s >> 2) * (kPanelA >> 4), pb = (uint64_t)(s >> 2) * (kPanelB >> 4);
+            wgmma_ss(d, d_alo + pa + adv, d_bhi + pb + adv);                                     // small terms first
+            wgmma_rs(d, ahi[s], d_blo + pb + adv);
+            wgmma_rs(d, ahi[s], d_bhi + pb + adv);
         }
-        __syncwarp();
+        dc_wgmma_commit();
         // prefetch the next step's i2h pre-activations while the tensor core works
         if (t + 1 < S) {
 #pragma unroll
@@ -275,28 +215,14 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
                 for (int g = 0; g < G; ++g)
                     nxt[i][g] = live[i] ? gates[((size_t)(t + 1) * B + b0 + sb + 16 * i) * GH + g * H + unit] : 0.f;
         }
-        mbar_wait(mma_done, t & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // ---- C: sum of the 8 accumulators -> scratch [gate][sequence][unit] -> gate math
-        {
-            const int q = warp & 3, cgp = warp >> 2;                               // TMEM lane quadrant (= gate), 8-column group
-            const uint32_t taddr = tmem_acc + ((uint32_t)(q * 32) << 16) + 8 * cgp;
-            uint32_t r[8][8];                                                      // all eight loads in flight, one wait
+        dc_wgmma_wait0();
+        acc_fence(d);
+        // ---- C: this K half's product -> scratch [half][gate][sequence][unit]; the gate math adds the halves in a fixed order
 #pragma unroll
-            for (int p = 0; p < 8; ++p) tmem_ld8(taddr + 32 * p, r[p]);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            float sum[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                float a = __uint_as_float(r[0][j]);
-#pragma unroll
-                for (int p = 1; p < 8; ++p) a += __uint_as_float(r[p][j]);         // fixed order: deterministic
-                sum[j] = a;
-            }
-#pragma unroll
-            for (int j = 0; j < 8; ++j) scratch[(q * kNB + 8 * cgp + j) * 32 + lane] = sum[j];
+        for (int i = 0; i < 16; ++i) {
+            const int rho = 64 * mh + acc_row(i, wi, lane);
+            my_scratch[((rho >> 5) * kNB + acc_col(i, lane)) * 32 + (rho & 31)] = d[i];
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
         float act[NP][G + 1];                                                      // activated gates (+ c | hn) of this step
 #pragma unroll
@@ -304,7 +230,7 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
             const int bb = sb + 16 * i;
             float pre[G];
 #pragma unroll
-            for (int g = 0; g < G; ++g) pre[g] = bias[g] + scratch[(g * kNB + bb) * 32 + ul];
+            for (int g = 0; g < G; ++g) pre[g] = bias[g] + (scratch[(g * kNB + bb) * 32 + ul] + scratch[((4 + g) * kNB + bb) * 32 + ul]);
             float hnew;
             if (G == 3) {
                 const float r = dc_sigmoid(cur[i][0] + pre[0]);
@@ -340,19 +266,16 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
         }
         cluster_wait();
     }
-    tmem_free_512(tmem_base, warp);
 }
 
 // ---- backward -----------------------------------------------------------------------------------------------------------
-// TMEM: [0,256) W_hh^T slice, hi half, two M tiles: tile m, lane rho <-> k = 128 m + rho, column kappa = g*32 + u <->
-// j = g*H + 32*rank + u;  [256,512) eight accumulators of 32 columns (M tile m, K-panel g at 256 + 32*(4m + g)).
-// shared: lo half (2 x 4 K-panels), gate-gradient tile hi / lo.
+// W_hh^T slice: row k (two M tiles of 128), column kappa = g*32 + u <-> j = g*H + 32*rank + u.  Registers: the hi half of
+// warpgroup w's rows [64 w, 64 w + 64), all G K-panels.  Shared: lo half (2 x 4 K-panels), gate-gradient tile hi / lo.
 struct BwdSmem {
     static constexpr size_t wlo = 0;
     static constexpr size_t ghi = wlo + 8 * kPanelA;
     static constexpr size_t glo = ghi + 4 * kPanelB;
-    static constexpr size_t bars = glo + 4 * kPanelB;
-    static constexpr size_t total = bars + 64 + 1024;
+    static constexpr size_t total = glo + 4 * kPanelB + 1024;
 };
 
 inline size_t bwd_workspace_bytes(int B) { return (size_t)2 * ((B + kNB - 1) / kNB) * kCL * kNB * kH * sizeof(float); }
@@ -367,30 +290,29 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
     extern __shared__ unsigned char smem_raw[];
     unsigned char *base = align1024(smem_raw);
     unsigned char *wlo = base + BwdSmem::wlo, *ghi = base + BwdSmem::ghi, *glo = base + BwdSmem::glo;
-    uint64_t *mma_done = reinterpret_cast<uint64_t *>(base + BwdSmem::bars);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(mma_done + 1);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int rank = blockIdx.x % kCL, cl = blockIdx.x / kCL, ncl = gridDim.x / kCL, b0 = cl * kNB;
 
-    if (tid == 0) {
-        mbar_init(mma_done, 2 * G);                                       // one commit per issuing thread
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    // MMA roles: warpgroup wg takes rows k in [64 wg, 64 wg + 64) (M tile wg / 2), all of this CTA's G K-panels
+    const int wg = warp >> 2, wi = warp & 3;
+    uint32_t ahi[4 * G][4];                                                // A fragments of the hi half, one per k-step of 8
+#pragma unroll
+    for (int s = 0; s < 4 * G; ++s) {
+        const int g = s >> 2, u = 8 * (s & 3) + (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int k = 64 * wg + 16 * wi + (lane >> 2) + 8 * h;
+            ahi[s][h] = __float_as_uint(tf32_rna(__ldg(w_hh + (size_t)(g * H + rank * 32 + u) * H + k)));
+            ahi[s][h + 2] = __float_as_uint(tf32_rna(__ldg(w_hh + (size_t)(g * H + rank * 32 + u + 4) * H + k)));
+        }
     }
-    tmem_alloc_512(tmem_slot, warp);
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_w = tmem_base, tmem_acc = tmem_base + 256;
-    // MMA issue: lane 0 of warp c < 2G issues the 12 MMAs of chain c = (M tile c / G, K-panel c % G) (see the forward kernel)
-    const bool issuer = lane == 0 && warp < 2 * G;
-    const int im = (warp % (2 * G)) / G, ip = (warp % (2 * G)) % G;
-    const uint64_t d_alo = make_desc(smem_u32(wlo) + (im * 4 + ip) * kPanelA), d_bhi = make_desc(smem_u32(ghi) + ip * kPanelB),
-                   d_blo = make_desc(smem_u32(glo) + ip * kPanelB);
-    const uint32_t t_acc = tmem_acc + 32 * (4 * im + ip), t_ahi = tmem_w + im * 128 + ip * 32;
+    const uint64_t d_alo = make_desc(smem_u32(wlo) + (wg >> 1) * 4 * kPanelA + (wg & 1) * 64 * 128), d_bhi = make_desc(smem_u32(ghi)),
+                   d_blo = make_desc(smem_u32(glo));
 
-    const int q = warp & 3, mt = (warp >> 2) & 1, wh = warp >> 3;          // TMEM lane quadrant, M tile, half (K range / columns)
-    {   // resident W_hh^T slice, once: lane rho of tile mt <-> k; a warp reads 32 consecutive k of one row j (128 B)
+    {   // resident lo half of the W_hh^T slice, once: row rho of tile mt <-> k; a warp reads 32 consecutive k of one row j (128 B)
+        const int q = warp & 3, mt = (warp >> 2) & 1, wh = warp >> 3;      // row quadrant, M tile, half of the columns
         const int rho = q * 32 + lane, k = mt * 128 + rho;
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
 #pragma unroll 2
         for (int kap0 = wh * 64; kap0 < wh * 64 + 64; kap0 += 8) {
             float w[8], hi[8], lo[8];
@@ -400,18 +322,14 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
                 w[e] = g < G ? __ldg(w_hh + (size_t)(g * H + rank * 32 + (kap0 & 31) + e) * H + k) : 0.f;
 #pragma unroll
             for (int e = 0; e < 8; ++e) { hi[e] = tf32_rna(w[e]); lo[e] = w[e] - hi[e]; }
-            tmem_st8(tmem_w + lane_addr + mt * 128 + kap0, hi);
             unsigned char *panel = wlo + (size_t)(mt * 4 + g) * kPanelA;
             const int c0 = (kap0 & 31) >> 2;
             *reinterpret_cast<float4 *>(panel + swz(rho, c0)) = make_float4(lo[0], lo[1], lo[2], lo[3]);
             *reinterpret_cast<float4 *>(panel + swz(rho, c0 + 1)) = make_float4(lo[4], lo[5], lo[6], lo[7]);
         }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 
     // gate phase: thread = (unit ul, sequences sb + 16 i)
     const int ul = lane, unit = rank * 32 + ul, sb = warp;
@@ -509,19 +427,21 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
             }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
-        if (issuer) {                                                              // 2 x G chains of 12, one issuing thread each
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        // 12 G wgmma per warpgroup (G K-panels x 4 k-steps x 3 products), asynchronous until the wait below
+        float d[16];
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-                umma_ss(t_acc, d_alo + 2 * ks, d_bhi + 2 * ks, kIdesc, ks != 0);
-                umma_ts(t_acc, t_ahi + 8 * ks, d_blo + 2 * ks, kIdesc, 1u);
-                umma_ts(t_acc, t_ahi + 8 * ks, d_bhi + 2 * ks, kIdesc, 1u);
-            }
-            umma_commit(mma_done);
+        for (int i = 0; i < 16; ++i) d[i] = 0.f;
+        acc_fence(d);
+        dc_wgmma_fence();
+#pragma unroll
+        for (int s = 0; s < 4 * G; ++s) {
+            const uint64_t adv = (uint64_t)((s & 3) * 2), pa = (uint64_t)(s >> 2) * (kPanelA >> 4), pb = (uint64_t)(s >> 2) * (kPanelB >> 4);
+            wgmma_ss(d, d_alo + pa + adv, d_bhi + pb + adv);
+            wgmma_rs(d, ahi[s], d_blo + pb + adv);
+            wgmma_rs(d, ahi[s], d_bhi + pb + adv);
         }
-        __syncwarp();
+        dc_wgmma_commit();
         // behind the MMAs: this step's global outputs, then the next step's inputs
 #pragma unroll
         for (int i = 0; i < NP; ++i) {
@@ -533,27 +453,13 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
             if (G == 3) cbuf[(tok + B) * H + unit] = daux[i];
         }
         if (t > 0) fetch(t - 1, ng, ndy, na0, na1);
-        mbar_wait(mma_done, it & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        dc_wgmma_wait0();
+        acc_fence(d);
         {   // partial dh_{t-1}[b][k] of this CTA's 128 gate columns -> scratch [buffer][cluster][rank][b][k]
-            const uint32_t taddr = tmem_acc + ((uint32_t)(q * 32) << 16) + 32 * (4 * mt) + 16 * wh;
-            uint32_t r[G][16];                                                     // all G loads in flight, one wait
+            float *dst = part + ((size_t)((it & 1) * ncl + cl) * kCL + rank) * kNB * H + 64 * wg;
 #pragma unroll
-            for (int p = 0; p < G; ++p) tmem_ld16(taddr + 32 * p, r[p]);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            float sum[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                float a = __uint_as_float(r[0][j]);
-#pragma unroll
-                for (int p = 1; p < G; ++p) a += __uint_as_float(r[p][j]);
-                sum[j] = a;
-            }
-            float *dst = part + (((size_t)((it & 1) * ncl + cl) * kCL + rank) * kNB + 16 * wh) * H + mt * 128 + q * 32 + lane;
-#pragma unroll
-            for (int b = 0; b < 16; ++b) __stcg(dst + (size_t)b * H, sum[b]);
+            for (int i = 0; i < 16; ++i) __stcg(dst + (size_t)acc_col(i, lane) * H + acc_row(i, wi, lane), d[i]);
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         cluster_arrive();
 #pragma unroll
         for (int i = 0; i < NP; ++i) {
@@ -575,7 +481,6 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
         if (dh0) dh0[(size_t)(b0 + bb) * H + unit] = dh;
         if (G == 4 && dc0) dc0[(size_t)(b0 + bb) * H + unit] = dc_carry[i];
     }
-    tmem_free_512(tmem_base, warp);
 }
 
 inline bool cluster_supported(int H) { return H == kH; }

@@ -65,11 +65,9 @@ struct Tiling {
     static constexpr int M = NMS * 32;
 };
 
-// Weights are held as (row 2j, row 2j+1) PAIRS so that the inner product runs on the packed fp32x2 FMA of
-// sm_100 (FFMA2, __ffma2_rn): one instruction = two FMAs on 64-bit register pairs.  A plain 3-register FFMA issues
-// at half rate on this SM (register-bank limited); FFMA2 restores the full 128 FMA/clk/SM.  The (h[2j], h[2j+1])
-// operand pairs fall out of the 16-byte shared-memory loads for free; even and odd rows accumulate separately and
-// are added once at the end.
+// Weights are held as (row 2j, row 2j+1) PAIRS: the (h[2j], h[2j+1]) operand pairs fall out of the 16-byte
+// shared-memory loads for free, and even and odd rows accumulate in two independent FMA chains that are added once
+// at the end.
 template <int NT, int NOUT>
 __device__ __forceinline__ void load_weights(const float *__restrict__ A, float2 (&wr)[8][4], float4 *w_s) {
     using T = Tiling<NT, NOUT>;
@@ -111,8 +109,8 @@ __device__ __forceinline__ void matvec_partial(const float2 (&wr)[8][4], const f
             const float2 h0 = make_float2(hv[b].x, hv[b].y), h1 = make_float2(hv[b].z, hv[b].w);
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
-                acc[b][c] = __ffma2_rn(h0, wr[j][c], acc[b][c]);
-                acc[b][c] = __ffma2_rn(h1, wr[j + 1][c], acc[b][c]);
+                acc[b][c] = dc_ffma2(h0, wr[j][c], acc[b][c]);
+                acc[b][c] = dc_ffma2(h1, wr[j + 1][c], acc[b][c]);
             }
         }
     }
@@ -131,10 +129,10 @@ __device__ __forceinline__ void matvec_partial(const float2 (&wr)[8][4], const f
 #pragma unroll
             for (int b = 0; b < BT; ++b) {
                 const float2 h = p == 0 ? make_float2(hv[b].x, hv[b].y) : make_float2(hv[b].z, hv[b].w);
-                acc[b][0] = __ffma2_rn(h, w0, acc[b][0]);
-                acc[b][1] = __ffma2_rn(h, w1, acc[b][1]);
-                acc[b][2] = __ffma2_rn(h, w2, acc[b][2]);
-                acc[b][3] = __ffma2_rn(h, w3, acc[b][3]);
+                acc[b][0] = dc_ffma2(h, w0, acc[b][0]);
+                acc[b][1] = dc_ffma2(h, w1, acc[b][1]);
+                acc[b][2] = dc_ffma2(h, w2, acc[b][2]);
+                acc[b][3] = dc_ffma2(h, w3, acc[b][3]);
             }
         }
     }

@@ -9,9 +9,9 @@
 #include "rnn_stepwise.cuh"
 
 // Kernel selection by width (no environment switches, no library fallback):
-//   H == 128  rnn_resident.cuh  W_hh resident in registers + shared memory of ONE SM, packed-fp32 FFMA2
-//   H == 256  rnn_cluster.cuh   W_hh resident in tensor memory + shared memory of an 8-CTA cluster, tcgen05 3xTF32
-//   H % 128 == 0 (384, 512, ...)  rnn_stepwise.cuh  per step: split-K tcgen05 3xTF32 GEMM over all SMs + gate kernel
+//   H == 128  rnn_resident.cuh  W_hh resident in registers + shared memory of ONE SM, fp32 FFMA
+//   H == 256  rnn_cluster.cuh   W_hh resident in registers + shared memory of an 8-CTA cluster, wgmma 3xTF32
+//   H % 128 == 0 (384, 512, ...)  rnn_stepwise.cuh  per step: split-K wgmma 3xTF32 GEMM over all SMs + gate kernel
 //   other H   rnn_generic.cuh   W_hh streamed from L2 every step, scalar FMA (correct for any H % 4 == 0)
 
 extern "C" size_t dc_rnn_workspace_bytes(int cell, int B, int H) {

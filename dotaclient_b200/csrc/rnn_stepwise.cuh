@@ -3,7 +3,7 @@
 // At H = 512 the fp32 W_hh (4 MB LSTM; 8 MB as tf32 hi + lo) fits neither one SM nor a 16-CTA cluster, so the weights cannot
 // stay on chip across steps the way rnn_resident.cuh / rnn_cluster.cuh keep them.  The step is a genuine dense contraction
 // ([B, H] x [H, G*H], 1.07 GFLOP per step at B = 512), so every step runs as
-//     (1) the split-K tcgen05 3xTF32 GEMM of csrc/gemm_tf32x3.cu over all SMs (W_hh streams from L2, where it stays
+//     (1) the split-K wgmma 3xTF32 GEMM of csrc/gemm_tf32x3.cu over all SMs (W_hh streams from L2, where it stays
 //         resident: 4 MB of 126 MB), writing `ksplit` partial products, and
 //     (2) one elementwise gate kernel that sums the partials in a fixed order (deterministic) and applies the cell.
 // 2 launches per time step; same buffers, same saved tensors and the same in-place reuse of the gate buffer as the other

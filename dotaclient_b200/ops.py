@@ -1,6 +1,6 @@
 """Torch-facing wrappers of the C-ABI kernels (device memory + stream plumbing only).
 
-Every function here requires CUDA tensors and enqueues hand-written sm_100a kernels from
+Every function here requires CUDA tensors and enqueues hand-written sm_90a kernels from
 ``libdotaclient_b200.so`` on torch's current stream.  No CPU path exists: CPU tensors raise.
 """
 import ctypes
@@ -148,14 +148,14 @@ def _rnn_workspace(cell, B, H, device):
 
 
 def _rnn_forward_impl(x, w_ih, w_hh, b_ih, b_hh, h0, c0, cell):
-    """i2h GEMM (tcgen05 3xTF32, ``dc_gemm_tf32x3``) + recurrence kernel.  Returns (x2, w_ih, w_hh, gates, ybuf, cbuf)."""
+    """i2h GEMM (wgmma 3xTF32, ``dc_gemm_tf32x3``) + recurrence kernel.  Returns (x2, w_ih, w_hh, gates, ybuf, cbuf)."""
     _need_cuda(x, w_ih, w_hh, b_ih, b_hh, h0, c0)
     S, B, Hin = x.shape
     H = w_hh.shape[1]
     N = S * B
     x2 = _f32c(x.detach()).view(N, Hin)
     w_ih, w_hh, b_ih, b_hh = _f32c(w_ih.detach()), _f32c(w_hh.detach()), _f32c(b_ih.detach()), _f32c(b_hh.detach())
-    # [N, G*H] = x W_ih^T + b_ih on tcgen05 (3xTF32); shapes outside the kernel's (G*H % 128, Hin % 32) raise DC_EUNSUPPORTED
+    # [N, G*H] = x W_ih^T + b_ih on wgmma (3xTF32); shapes outside the kernel's (G*H % 128, Hin % 32) raise DC_EUNSUPPORTED
     gates = gemm_tf32x3(x2, w_ih, b_ih)
     ybuf = torch.empty((S + 1, B, H), dtype=torch.float32, device=x.device)
     cbuf = torch.empty((S + 1, B, H), dtype=torch.float32, device=x.device)
@@ -180,7 +180,7 @@ def rnn_forward_states(x_tm, w_ih, w_hh, b_ih, b_hh, h0, c0, cell):
 
 
 class RnnSequence(torch.autograd.Function):
-    """Time-major GRU/LSTM layer: i2h GEMM (tcgen05 3xTF32) + hand-written recurrence kernels.
+    """Time-major GRU/LSTM layer: i2h GEMM (wgmma 3xTF32) + hand-written recurrence kernels.
 
     forward(x [S,B,Hin], w_ih [G*H,Hin], w_hh [G*H,H], b_ih, b_hh, h0 [B,H], c0 [B,H]|None, cell)
       -> y [S,B,H], h_n [B,H], c_n [B,H] (zeros-size-0 tensor for GRU)
@@ -318,7 +318,7 @@ def gemm_tf32x3_supported(M, N, K):
 
 
 def gemm_tf32x3(a, b, bias=None, relu=False, out=None):
-    """``out[M,N] = a[M,K] @ b[N,K]^T (+ bias) (ReLU)`` on tcgen05 tensor cores with the 3xTF32 split
+    """``out[M,N] = a[M,K] @ b[N,K]^T (+ bias) (ReLU)`` on Hopper tensor cores (wgmma) with the 3xTF32 split
     (fp32-level accuracy).  ``a``/``b``/``out`` are 2-D fp32 CUDA tensors whose rows are contiguous (row stride
     may exceed the width: column-slice views are fine)."""
     _need_cuda(a, b, bias)
@@ -341,7 +341,7 @@ def gemm_tf32x3(a, b, bias=None, relu=False, out=None):
 
 class LinearTC(torch.autograd.Function):
     """``y = x W^T + b`` (optionally ReLU): forward, data gradient and weight gradient (+ bias gradient from the same pass
-    over ``dy``) all on the tcgen05 3xTF32 GEMMs.  No library GEMM: unsupported shapes raise ``DC_EUNSUPPORTED``."""
+    over ``dy``) all on the wgmma 3xTF32 GEMMs.  No library GEMM: unsupported shapes raise ``DC_EUNSUPPORTED``."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, relu):
@@ -371,7 +371,7 @@ class LinearTC(torch.autograd.Function):
 
 
 def linear(x, weight, bias=None, relu=False):
-    """Dense layer on the tcgen05 3xTF32 GEMM (out features % 128 == 0, in features % 32 == 0; CUDA tensors only)."""
+    """Dense layer on the wgmma 3xTF32 GEMM (out features % 128 == 0, in features % 32 == 0; CUDA tensors only)."""
     _need_cuda(x, weight, bias)
     return LinearTC.apply(x, weight, bias, relu)
 
@@ -384,7 +384,7 @@ def gemm_wgrad_supported(T, No, Ni):
 
 
 def gemm_wgrad_tf32x3(dy, x, want_bias=True, dw_out=None, db_out=None, accumulate=False):
-    """``dW[No,Ni] = dy[T,No]^T @ x[T,Ni]`` and ``db[No] = dy.sum(0)`` on tcgen05 (3xTF32, split-K, deterministic).
+    """``dW[No,Ni] = dy[T,No]^T @ x[T,Ni]`` and ``db[No] = dy.sum(0)`` on wgmma (3xTF32, split-K, deterministic).
 
     ``dy`` / ``x`` are 2-D fp32 CUDA tensors with contiguous rows (column-slice views allowed)."""
     _need_cuda(dy, x)
@@ -449,7 +449,7 @@ def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e
     tensor-core GEMM output (``PACK_COLS``) and the target-unit logits are a separate ``[N,40]`` tensor.
 
     Returns (out[16], n_actions[5], d_packed [N,128], d_logits_tu [N,40]): the gradients go straight back into the two
-    producers, so no slice/cat kernels run and the five tiny K=131072 weight-gradient GEMMs become one tcgen05 wgrad.
+    producers, so no slice/cat kernels run and the five tiny K=131072 weight-gradient GEMMs become one wgmma wgrad.
     """
     _need_cuda(packed, logits_tu)
     p2 = _f32c(packed.detach()).reshape(-1, PACK_WIDTH)

@@ -2,7 +2,7 @@
 
 Keeps the reference's module surface (``DotaOptimizer``, ``Sequence``, ``MessageQueue``,
 ``advantage_returns``, ``discount``, ``init_distribution``, ``main``, the CLI flags) while one
-optimizer step runs as:  unit-encoder kernel chain + tcgen05 3xTF32 GEMMs -> hand-written recurrence kernels ->
+optimizer step runs as:  unit-encoder kernel chain + wgmma 3xTF32 GEMMs -> hand-written recurrence kernels ->
 fused PPO loss+grad kernel -> autograd backward through the same kernels -> ONE NCCL all-reduce of
 a flat gradient buffer -> fused count-divide / grad-norm / clip / Adam kernel -- replayed from a CUDA graph
 when the batch is device-resident.  CUDA only.
@@ -10,6 +10,7 @@ when the batch is device-resident.  CUDA only.
 Line references are to TimZaman/dotaclient ``optimizer.py`` @ 8615b90.
 """
 import argparse
+import gc
 import io
 import logging
 import math
@@ -41,7 +42,7 @@ GAMMA, LAMBDA = 0.98, 0.97                                              # :421
 
 def _device():
     if not torch.cuda.is_available():
-        raise RuntimeError("dotaclient_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise RuntimeError("dotaclient_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     return torch.device('cuda', torch.cuda.current_device())
 
 
@@ -427,7 +428,6 @@ class DotaOptimizer:
         self._graphs.clear()
         self._input_slots.clear()
         self._staging.clear()
-        import gc
         gc.collect()
         if torch.cuda.is_available():
             torch.cuda.synchronize()
@@ -806,6 +806,12 @@ class DotaOptimizer:
                 else:
                     setattr(static, k, c)
         graph = torch.cuda.CUDAGraph()
+        # A garbage collection during the capture would free unreachable objects -- among them the captured graphs of an
+        # optimizer nobody references any more -- and destroying a graph is not permitted while a stream is capturing: it
+        # invalidates this capture.  So collect first and keep the cyclic collector off until the capture has ended.
+        gc.collect()
+        gc_was_enabled = gc.isenabled()
+        gc.disable()
         try:
             torch.cuda.synchronize()
             with torch.cuda.graph(graph, capture_error_mode="thread_local"):
@@ -815,6 +821,9 @@ class DotaOptimizer:
             torch.cuda.synchronize()
             self.flat.rebind()
             return "eager"
+        finally:
+            if gc_was_enabled:
+                gc.enable()
         return static, graph, out
 
     def prefetch(self, experiences):

@@ -2,7 +2,7 @@
 
 Same constructor-created parameters, same ``state_dict`` (34 keys, shapes and order of
 ``policy.py:54-75``), same ``forward`` signature and outputs (``policy.py:92-167``); the recurrent
-layer runs through the hand-written sm_100a recurrence kernels (``dotaclient_b200/csrc``), and the
+layer runs through the hand-written sm_90a recurrence kernels (``dotaclient_b200/csrc``), and the
 unit encoder through the fused encoder kernel when it is available.  Two additions, both
 keyword-only so ``Policy()`` is the reference's network: ``hidden_size`` (reference: 256) and
 ``cell`` ('gru' = the reference's ``nn.GRU``, 'lstm' = the cell BASELINE.json names).
@@ -116,7 +116,7 @@ class Policy(nn.Module):
     # ------------------------------------------------------------------ implementation
     def _encode(self, env, groups):
         """Observation encoders (``policy.py:97-138``) -> (x ``[..., H]``, encoder handle for the target-unit head): the explicit
-        kernel chain of ``csrc/encoder.cu`` + tcgen05 GEMMs (no ``torch.cat``, no materialised ``[..., 40, 128]`` unit embedding)."""
+        kernel chain of ``csrc/encoder.cu`` + wgmma GEMMs (no ``torch.cat``, no materialised ``[..., 40, 128]`` unit embedding)."""
         layers = [getattr(self, "affine_unit_" + s) for s, _, _ in UNIT_GROUPS]
         unit_embedding, x = encoder_ops.unit_encoder(
             env, self.affine_env.weight, self.affine_env.bias,

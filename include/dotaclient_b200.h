@@ -1,4 +1,4 @@
-/* dotaclient_b200 -- C-ABI of the B200-native DotaClient optimizer hot path.
+/* dotaclient_b200 -- C-ABI of the CUDA-native DotaClient optimizer hot path (H100, sm_90a).
  *
  * The reference (TimZaman/dotaclient @ 8615b90) is pure Python on torch CPU; it has no FFI
  * layer.  Each entry point below replaces a stock-torch/scipy op sequence of the reference's
@@ -13,7 +13,7 @@
  *     dc_last_error() returns a thread-local human-readable message for the last failure.
  *   - bool tensors (masks / actions) are bytes holding 0 or 1 (torch.bool layout).
  *   - "time-major" = [S, B, ...]: token (t, b) lives at row t*B + b.
- *   - compiled for sm_100a only; there is no CPU fallback.
+ *   - compiled for sm_90a (H100) only; there is no CPU fallback.
  */
 #ifndef DOTACLIENT_B200_H
 #define DOTACLIENT_B200_H
@@ -73,8 +73,8 @@ int dc_gae_scan(const float *rewards, int n_sub, const float *values, const int6
  *                       GRU : slot t+1 = W_hn h_{t-1} + b_hn (out, saved for backward)
  *   workspace: dc_rnn_workspace_bytes(cell, B, H) bytes of scratch (W_hh^T for H != 256; at H = 256 the partial-sum
  *              exchange of the cluster backward kernel -- the same buffer serves forward and backward).
- * Kernels by width: H = 128 one-SM weight-resident FFMA2 kernels; H = 256 (the reference's width) 8-CTA-cluster
- * tensor-memory-resident tcgen05 3xTF32 kernels; any other H % 4 == 0 a generic kernel that streams W_hh from L2.
+ * Kernels by width: H = 128 one-SM weight-resident FFMA kernels; H = 256 (the reference's width) 8-CTA-cluster
+ * weight-resident wgmma 3xTF32 kernels; any other H % 4 == 0 a generic kernel that streams W_hh from L2.
  * Backward (consumes what forward left behind)
  *   gates  in: activated gates   out: dL/d(gates pre-activation wrt the i2h branch) = dgi
  *   cbuf   LSTM: unchanged.  GRU: slot t+1 out = dL/d(W_hn h + b_hn) (the n-gate part of dgh)
@@ -88,7 +88,7 @@ int dc_rnn_seq_bwd(int cell, float *gates, const float *w_hh, const float *ybuf,
                    const float *dy, const float *dhn, const float *dcn, float *dh0, float *dc0,
                    int B, int S, int H, void *workspace, dc_stream_t stream);
 
-/* ---- fp32-accurate tensor-core GEMM (tcgen05, 3xTF32) ---------------------------------------
+/* ---- fp32-accurate tensor-core GEMM (wgmma, 3xTF32) ---------------------------------------
  * C[M,N] = A[M,K] * B[N,K]^T (+ bias[N]) (ReLU if relu != 0); row-major fp32 with leading dimensions lda/ldb/ldc.
  * Replaces the library SGEMM of the input-to-hidden projection inside nn.GRU / nn.LSTM (policy.py:66,141:
  * gates = x W_ih^T + b_ih) and of the other 128-aligned dense layers (policy.py:101-126,138).  Each product is
@@ -101,7 +101,7 @@ int dc_gemm_tf32x3(const float *A, int lda, const float *B, int ldb, const float
 
 /* Weight gradient of the same layers: dW[No,Ni] (+)= dY[T,No]^T X[T,Ni], db[No] (+)= column sums of dY (NULL = skip).
  * Replaces the dW/db part of AddmmBackward for those layers (loss.backward(), optimizer.py:672).  Contraction over the
- * token dimension with MN-major tcgen05 operands, split-K over the SMs, deterministic two-stage reduction.
+ * token dimension (operands transposed to K-major on the way into shared memory), split-K over the SMs, deterministic two-stage reduction.
  * Requirements: No % 128 == 0, Ni % 128 == 0; workspace of dc_gemm_wgrad_workspace_bytes(No, Ni) bytes. */
 size_t dc_gemm_wgrad_workspace_bytes(int No, int Ni);
 int dc_gemm_wgrad_tf32x3(const float *dY, int ldy, const float *X, int ldx, int64_t T, int No, int Ni,

@@ -1,4 +1,4 @@
-"""GPU test of the tcgen05 3xTF32 GEMM (dc_gemm_tf32x3) against a float64 reference.
+"""GPU test of the wgmma 3xTF32 GEMM (dc_gemm_tf32x3) against a float64 reference.
 
 Tolerance: the 3xTF32 split keeps fp32-level accuracy -- max |err| <= 4e-6 * sqrt(K) * rms(a) * rms(b)-scaled bound below,
 i.e. the same order as an fp32 SIMT GEMM and ~1000x tighter than single-pass TF32."""
@@ -62,7 +62,7 @@ def test_gemm_tf32x3_strided_views_and_unsupported_shapes():
 @pytest.mark.parametrize("T,No,Ni", [(1, 128, 128), (31, 128, 128), (32, 128, 128), (100, 128, 128), (5000, 128, 128),
                                      (100000, 128, 128), (4097, 512, 128), (3000, 128, 896), (777, 256, 256)])
 def test_gemm_wgrad_tf32x3_matches_fp64(T, No, Ni):
-    """dW = dY^T X and db = colsum(dY): MN-major tcgen05 operands, split-K over the SMs, deterministic reduction."""
+    """dW = dY^T X and db = colsum(dY): operands transposed to K-major by the producers, split-K over the SMs, deterministic reduction."""
     from dotaclient_b200 import ops
     g = torch.Generator().manual_seed(T + No + Ni)
     dy = torch.randn(T, No, generator=g)

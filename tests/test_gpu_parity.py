@@ -50,14 +50,14 @@ def ulp_diff(a, b):
 
 
 # ------------------------------------------------------------------------------------------------ library
-def test_native_library_loaded_and_device_is_blackwell():
+def test_native_library_loaded_and_device_is_hopper():
     from dotaclient_b200 import _lib
     lib = _lib.load()
     assert lib.dc_version() >= 100
     import ctypes
     sm, major, minor = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
     _lib.check(lib.dc_device_info(ctypes.byref(sm), ctypes.byref(major), ctypes.byref(minor)), "dc_device_info")
-    assert major.value == 10 and sm.value >= 100
+    assert major.value == 9 and sm.value >= 100
 
 
 # ------------------------------------------------------------------------------------------------ GAE
@@ -127,7 +127,7 @@ def _torch_rnn(cell, H):
 @pytest.mark.parametrize("B,S,H", [(3, 7, 128), (2, 40, 128), (5, 16, 256), (2, 5, 512), (9, 33, 128),
                                    (301, 6, 128), (1, 3, 128), (1, 1, 256), (33, 9, 256), (64, 128, 256), (70, 40, 512), (3, 5, 384)])
 def test_rnn_forward_backward_vs_torch(cell, B, S, H):
-    """Recurrence kernels (+ the tcgen05 i2h GEMM and wgrads) against torch.nn.GRU / nn.LSTM on CPU: outputs, final state,
+    """Recurrence kernels (+ the wgmma i2h GEMM and wgrads) against torch.nn.GRU / nn.LSTM on CPU: outputs, final state,
     all gradients.  H = 128 one-SM kernels, H = 256 cluster kernels (1 / 2 / 3 clusters, partly filled), H = 384 / 512 step-wise."""
     from dotaclient_b200 import ops
     torch.manual_seed(B * 1000 + S * 10 + H)

@@ -293,51 +293,41 @@ def test_bench_config_is_identical_in_both_arms_and_names_the_workload():
     assert bench.algorithmic_rnn_bytes(cfg) == 12.0 * 256 * 512 * 5 * 128            # SURVEY.md 8(d), LSTM: G + 1 = 5
 
 
-def test_kernel_traffic_json_matches_the_committed_ncu_csv(tmp_path):
-    """profiles/kernel_traffic.json (read by bench.py for roofline.traffic) is derived from profiles/r2_ncu_traffic_c2.csv."""
-    import csv
-    import json
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    rec = json.load(open(os.path.join(root, "profiles", "kernel_traffic.json")))["c2_lstm"]
-    total = 0.0
-    for r in csv.reader(open(os.path.join(root, "profiles", "r2_ncu_traffic_c2.csv"))):
-        if len(r) >= 15 and r[0].isdigit() and r[12].startswith("dram__bytes"):
-            total += float(r[14].replace(",", "")) * {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}[r[13]]
-    assert abs(total - rec["step_total"]) <= 1e-6 * total
-    assert 15e9 < rec["step_total"] < 25e9 and rec["gemm_fwd_dgrad"] > rec["rnn"] > 1e9     # 35.2 GB before the fused encoder backward
-    assert rec["unit_dgrad_fused"] < 2e9                                                     # ... whose data-gradient kernel moves ~1 GB
-
-
 def test_dominant_roofline_of_the_committed_bench_line():
     """bench.py's `roofline` names the kernel family with the largest share of the step; checked on the per-kernel table of the
-    committed C2 line (profiles/r2_bench_c2_n1.json): the fused unit-encoder data gradient, bound by the tensor pipe, with
-    its measured DRAM traffic from profiles/kernel_traffic.json; without it the forward/dgrad GEMM family in HBM terms."""
+    committed C2 line (profiles/h100_bench_c2_n1.json, one H100 SXM at 700 W): the family's time and bytes are the sums of its
+    kernels, HBM families report algorithmic bytes over time against the peak, and without the unit-encoder data gradient
+    the roof stays an HBM roof."""
     import json
     import bench
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    line = json.loads(open(os.path.join(root, "profiles", "r2_bench_c2_n1.json")).read().strip().splitlines()[-1])
-    rec = json.load(open(os.path.join(root, "profiles", "kernel_traffic.json")))["c2_lstm"]
+    line = json.loads(open(os.path.join(root, "profiles", "h100_bench_c2_n1.json")).read().strip().splitlines()[-1])
     table = line["roofline"]["kernels"]
-    r = bench.dominant_roofline(table, line["ms_per_step"], 256 * 512, 6576.7, "measured", rec)
-    assert "dc_unit_dgrad_fused" in r["kernel"] and r["bound"] == "tensor" and r["unit"] == "TFLOP/s"
-    assert abs(r["kernel_ms_per_step"] - table["unit_dgrad_fused"]["ms"]) < 1e-9 and 0.2 < r["share_of_step"] < 0.3
-    assert abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-12 and 0.1 < r["frac"] < 0.6
-    assert r["traffic"] == rec["unit_dgrad_fused"] and r["step_traffic"] == rec["step_total"]
+    fam = {label: sum(table[n]["ms"] for n in names if n in table) for label, names in bench.KERNEL_FAMILIES.items()}
+    dominant = max(fam, key=fam.get)
+    r = bench.dominant_roofline(table, line["ms_per_step"], 256 * 512, 3350.0, "data sheet")
+    assert r["kernel"] == dominant == line["roofline"]["kernel"] and abs(r["kernel_ms_per_step"] - fam[dominant]) < 1e-9
+    assert 0.0 < r["share_of_step"] < 1.0 and abs(r["share_of_step"] - fam[dominant] / line["ms_per_step"]) < 1e-12
+    assert abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-12 and r["frac"] > 0
+    names = bench.KERNEL_FAMILIES[dominant]
+    if r["bound"] == "hbm":
+        want = sum(table[n]["bytes"] for n in names if n in table) / (fam[dominant] * 1e-3) / 1e9
+        assert r["unit"] == "GB/s" and abs(r["achieved"] - want) < 1e-6 * want and abs(r["frac"] - want / 3350.0) < 1e-9
+    else:
+        assert names == ["unit_dgrad_fused"] and r["unit"] == "TFLOP/s"
     rest = {k: v for k, v in table.items() if k != "unit_dgrad_fused"}
-    r2 = bench.dominant_roofline(rest, line["ms_per_step"], 256 * 512, 6576.7, "measured", None)
-    assert "dc_gemm_tf32x3" in r2["kernel"] and r2["bound"] == "hbm" and r2["unit"] == "GB/s" and r2["traffic"] is None
-    want = (table["gemm_tf32x3"]["bytes"] + table["gemm_unit_max"]["bytes"]) / ((table["gemm_tf32x3"]["ms"] + table["gemm_unit_max"]["ms"]) * 1e-3) / 1e9
-    assert abs(r2["achieved"] - want) < 1e-6 * want and abs(r2["frac"] - want / 6576.7) < 1e-9
+    r2 = bench.dominant_roofline(rest, line["ms_per_step"], 256 * 512, 3350.0, "data sheet")
+    assert r2["bound"] == "hbm" and r2["unit"] == "GB/s" and "unit_dgrad_fused" not in r2["kernel"].split("(")[1]
 
 
 def test_committed_bench_lines_carry_the_contract_keys():
-    """The bench lines kept as evidence under profiles/ (one GPU, 2 / 4 / 8 GPUs, reference arm) have every key of the bench.py
-    contract, name the BASELINE metric, and their derived fields are consistent with each other."""
+    """The bench lines kept as evidence under profiles/ (one H100, reference arm) have every key of the bench.py contract,
+    name the BASELINE metric, and their derived fields are consistent with each other."""
     import json
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     base = {"metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype",
             "data", "config"}
-    for name, n in (("r2_bench_c2_n1.json", 1), ("r2_bench_c2_n2.json", 2), ("r2_bench_c2_n4.json", 4), ("r2_bench_c4_n8.json", 8)):
+    for name, n in (("h100_bench_c2_n1.json", 1),):
         line = json.loads(open(os.path.join(root, "profiles", name)).read().strip().splitlines()[-1])
         assert base | {"roofline", "gpu_launches", "clocks"} <= set(line), (name, base - set(line))
         assert line["metric"] == "optimizer_steps_per_sec" and line["unit"] == "steps/s" and line["higher_is_better"] is True
@@ -345,14 +335,13 @@ def test_committed_bench_lines_carry_the_contract_keys():
         assert abs(line["value"] - n * 1000.0 / line["ms_per_step"]) <= 1e-6 * line["value"]
         assert "workload" in line["config"] and "model" not in line["config"]
         r = line["roofline"]
-        assert {"bound", "achieved", "peak", "unit", "frac", "traffic"} <= set(r) and abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9
-        if "c2" in name:                              # the C4 evidence run skipped the end-to-end leg (--skip-e2e)
-            assert {"value", "unit", "h2d_bytes_per_step", "d2h_bytes_per_step"} <= set(line["e2e"]) and line["e2e"]["h2d_bytes_per_step"] > 0
+        assert {"bound", "achieved", "peak", "unit", "frac"} <= set(r) and abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9
+        assert {"value", "unit", "h2d_bytes_per_step", "d2h_bytes_per_step"} <= set(line["e2e"]) and line["e2e"]["h2d_bytes_per_step"] > 0
         assert line["gpu_launches"] > 0 and not set(line["clocks"]["reasons"]) & {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"}
         if n == 1:
             cb = line["cpu_baseline"]
             assert {"value", "unit", "cores", "kind", "sample"} <= set(cb) and cb["kind"] == "port" and cb["value"] > 0
             assert set(line["extra_configs"]) == {"c1", "c3", "c4"} and all("ms_per_step" in v for v in line["extra_configs"].values())
-    ref = json.loads(open(os.path.join(root, "profiles", "r2_bench_reference_arm_n1.json")).read().strip().splitlines()[-1])
+    ref = json.loads(open(os.path.join(root, "profiles", "reference_arm_c2.json")).read().strip().splitlines()[-1])
     assert ref["impl"] == "reference" and base <= set(ref) and ref["metric"] == "optimizer_steps_per_sec"
     assert ref["e2e"]["h2d_bytes_per_step"] == 0 and ref["e2e"]["d2h_bytes_per_step"] == 0 and ref["cpu_baseline"]["value"] == ref["value"]

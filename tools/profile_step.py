@@ -1,8 +1,7 @@
 """Per-kernel breakdown of one DotaOptimizer.train() step with torch.profiler (CUDA activities).
 
     python tools/profile_step.py [--config c2] [--steps 3]   ->  gpurun_out/step_profile_<config>.txt
-Not a benchmark (profiler overhead); used to decide what to optimise next.  ncu gives the authoritative
-per-launch times (profiles/).
+Not a benchmark (profiler overhead); used to decide what to optimise next.
 """
 import argparse
 import os
