@@ -23,7 +23,7 @@
 // (arrive.release right after the exchanged slice is stored, wait.acquire after the remaining stores).
 // Algorithmic HBM bytes per token: forward 4*(G+1)*H, backward 8*(G+1)*H (SURVEY.md 8d).
 #pragma once
-#include "dc_common.cuh"
+#include "rnn_cell.cuh"
 
 namespace dc_rnnc {
 
@@ -33,9 +33,6 @@ constexpr int kNB = 32;                 // sequences per cluster = MMA N
 constexpr int kThreads = 512;           // 4 warpgroups
 constexpr int kPanelA = 128 * 128;      // bytes of one A tile: 128 rows x 32 tf32 (one SWIZZLE_128B row each)
 constexpr int kPanelB = kNB * 128;      // bytes of one B tile:  32 rows x 32 tf32
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return dc_smem_u32(p); }
-__device__ __forceinline__ float tf32_rna(float v) { return dc_tf32_rna(v); }
 
 #define DC_ACC16 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
                  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
@@ -59,8 +56,6 @@ __device__ __forceinline__ void wgmma_rs(float (&d)[16], const uint32_t (&a)[4],
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
 }
 #undef DC_ACC16
-// K-major SWIZZLE_128B shared-memory matrix descriptor: 8-row groups 1024 B apart (dc_wgmma_desc)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) { return dc_wgmma_desc(smem_addr); }
 // accumulator fragment of m64n32: d[i] at row 16*warp + lane/4 + 8*((i/2)%2), column 8*(i/4) + 2*(lane%4) + i%2
 __device__ __forceinline__ int acc_row(int i, int wi, int lane) { return 16 * wi + (lane >> 2) + 8 * ((i >> 1) & 1); }
 __device__ __forceinline__ int acc_col(int i, int lane) { return 8 * (i >> 2) + 2 * (lane & 3) + (i & 1); }
@@ -115,13 +110,13 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
             const float *wrow = w_hh + (size_t)(g * H + rank * 32 + (rho & 31)) * H + 128 * kh + (lane & 3);
 #pragma unroll
             for (int s = 0; s < 16; ++s) {
-                ahi[s][h] = __float_as_uint(g < G ? tf32_rna(__ldg(wrow + 8 * s)) : 0.f);          // GRU has no 4th gate: zero rows
-                ahi[s][h + 2] = __float_as_uint(g < G ? tf32_rna(__ldg(wrow + 8 * s + 4)) : 0.f);
+                ahi[s][h] = __float_as_uint(g < G ? dc_tf32_rna(__ldg(wrow + 8 * s)) : 0.f);          // GRU has no 4th gate: zero rows
+                ahi[s][h + 2] = __float_as_uint(g < G ? dc_tf32_rna(__ldg(wrow + 8 * s + 4)) : 0.f);
             }
         }
     }
-    const uint64_t d_alo = make_desc(smem_u32(wlo) + 4 * kh * kPanelA + mh * 64 * 128), d_bhi = make_desc(smem_u32(hhi) + 4 * kh * kPanelB),
-                   d_blo = make_desc(smem_u32(hlo) + 4 * kh * kPanelB);
+    const uint64_t d_alo = dc_wgmma_desc(dc_smem_u32(wlo) + 4 * kh * kPanelA + mh * 64 * 128), d_bhi = dc_wgmma_desc(dc_smem_u32(hhi) + 4 * kh * kPanelB),
+                   d_blo = dc_wgmma_desc(dc_smem_u32(hlo) + 4 * kh * kPanelB);
     float *my_scratch = scratch + kh * (4 * kNB * 32);
 
     {   // resident lo half, once: warp (q, kq) fills rows [32q, 32q+32), columns [64*kq, 64*kq+64)
@@ -139,7 +134,7 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
                 for (int e = 0; e < 8; ++e) w[e] = 0.f;
             }
 #pragma unroll
-            for (int e = 0; e < 8; ++e) { hi[e] = tf32_rna(w[e]); lo[e] = w[e] - hi[e]; }
+            for (int e = 0; e < 8; ++e) { hi[e] = dc_tf32_rna(w[e]); lo[e] = w[e] - hi[e]; }
             unsigned char *panel = wlo + (size_t)(k0 >> 5) * kPanelA;
             const int c0 = (k0 & 31) >> 2;
             *reinterpret_cast<float4 *>(panel + swz(rho, c0)) = make_float4(lo[0], lo[1], lo[2], lo[3]);
@@ -185,7 +180,7 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
             for (int j = 0; j < 4; ++j) {
                 const int p = hp0 + 2 * j;
                 float4 hi, lo;
-                hi.x = tf32_rna(v[j].x); hi.y = tf32_rna(v[j].y); hi.z = tf32_rna(v[j].z); hi.w = tf32_rna(v[j].w);
+                hi.x = dc_tf32_rna(v[j].x); hi.y = dc_tf32_rna(v[j].y); hi.z = dc_tf32_rna(v[j].z); hi.w = dc_tf32_rna(v[j].w);
                 lo.x = v[j].x - hi.x; lo.y = v[j].y - hi.y; lo.z = v[j].z - hi.z; lo.w = v[j].w - hi.w;
                 *reinterpret_cast<float4 *>(hhi + p * kPanelB + off) = hi;
                 *reinterpret_cast<float4 *>(hlo + p * kPanelB + off) = lo;
@@ -224,30 +219,17 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
             my_scratch[((rho >> 5) * kNB + acc_col(i, lane)) * 32 + (rho & 31)] = d[i];
         }
         __syncthreads();
-        float act[NP][G + 1];                                                      // activated gates (+ c | hn) of this step
+        float act[NP][G], aux[NP];                                                 // activated gates, c | hn -> cbuf slot t+1
 #pragma unroll
         for (int i = 0; i < NP; ++i) {
             const int bb = sb + 16 * i;
             float pre[G];
 #pragma unroll
             for (int g = 0; g < G; ++g) pre[g] = bias[g] + (scratch[(g * kNB + bb) * 32 + ul] + scratch[((4 + g) * kNB + bb) * 32 + ul]);
-            float hnew;
-            if (G == 3) {
-                const float r = dc_sigmoid(cur[i][0] + pre[0]);
-                const float z = dc_sigmoid(cur[i][1] + pre[1]);
-                const float n = dc_tanh(cur[i][2] + r * pre[2]);
-                hnew = (1.0f - z) * n + z * h_reg[i];
-                act[i][0] = r; act[i][1] = z; act[i][2] = n; act[i][G] = pre[2];   // W_hn h + b_hn -> cbuf slot t+1
-                h_reg[i] = hnew;
-            } else {
-                const float ig = dc_sigmoid(cur[i][0] + pre[0]);
-                const float fg = dc_sigmoid(cur[i][1] + pre[1]);
-                const float gg = dc_tanh(cur[i][2] + pre[2]);
-                const float og = dc_sigmoid(cur[i][G - 1] + pre[G - 1]);
-                c_reg[i] = fg * c_reg[i] + ig * gg;
-                hnew = og * dc_tanh(c_reg[i]);
-                act[i][0] = ig; act[i][1] = fg; act[i][2] = gg; act[i][G - 1] = og; act[i][G] = c_reg[i];
-            }
+            const float hnew = dc_rnn::cell_fwd<G>([&](int g) { return cur[i][g]; }, [&](int g) { return pre[g]; },
+                                                   G == 3 ? h_reg[i] : c_reg[i], act[i], aux[i]);
+            if (G == 3) h_reg[i] = hnew;
+            else c_reg[i] = aux[i];
             if (live[i]) ybuf[((size_t)(t + 1) * B + b0 + bb) * H + unit] = hnew;  // the slice the other CTAs wait for
         }
         // ---- D: publish this CTA's slice of h_t (release), then write the rest of the step's outputs behind the barrier
@@ -259,7 +241,7 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
                 float *gout = gates + tok * GH + unit;
 #pragma unroll
                 for (int g = 0; g < G; ++g) gout[g * H] = act[i][g];
-                cbuf[(tok + B) * H + unit] = act[i][G];
+                cbuf[(tok + B) * H + unit] = aux[i];
             }
 #pragma unroll
             for (int g = 0; g < G; ++g) cur[i][g] = nxt[i][g];
@@ -303,12 +285,12 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int k = 64 * wg + 16 * wi + (lane >> 2) + 8 * h;
-            ahi[s][h] = __float_as_uint(tf32_rna(__ldg(w_hh + (size_t)(g * H + rank * 32 + u) * H + k)));
-            ahi[s][h + 2] = __float_as_uint(tf32_rna(__ldg(w_hh + (size_t)(g * H + rank * 32 + u + 4) * H + k)));
+            ahi[s][h] = __float_as_uint(dc_tf32_rna(__ldg(w_hh + (size_t)(g * H + rank * 32 + u) * H + k)));
+            ahi[s][h + 2] = __float_as_uint(dc_tf32_rna(__ldg(w_hh + (size_t)(g * H + rank * 32 + u + 4) * H + k)));
         }
     }
-    const uint64_t d_alo = make_desc(smem_u32(wlo) + (wg >> 1) * 4 * kPanelA + (wg & 1) * 64 * 128), d_bhi = make_desc(smem_u32(ghi)),
-                   d_blo = make_desc(smem_u32(glo));
+    const uint64_t d_alo = dc_wgmma_desc(dc_smem_u32(wlo) + (wg >> 1) * 4 * kPanelA + (wg & 1) * 64 * 128), d_bhi = dc_wgmma_desc(dc_smem_u32(ghi)),
+                   d_blo = dc_wgmma_desc(dc_smem_u32(glo));
 
     {   // resident lo half of the W_hh^T slice, once: row rho of tile mt <-> k; a warp reads 32 consecutive k of one row j (128 B)
         const int q = warp & 3, mt = (warp >> 2) & 1, wh = warp >> 3;      // row quadrant, M tile, half of the columns
@@ -321,7 +303,7 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
             for (int e = 0; e < 8; ++e)
                 w[e] = g < G ? __ldg(w_hh + (size_t)(g * H + rank * 32 + (kap0 & 31) + e) * H + k) : 0.f;
 #pragma unroll
-            for (int e = 0; e < 8; ++e) { hi[e] = tf32_rna(w[e]); lo[e] = w[e] - hi[e]; }
+            for (int e = 0; e < 8; ++e) { hi[e] = dc_tf32_rna(w[e]); lo[e] = w[e] - hi[e]; }
             unsigned char *panel = wlo + (size_t)(mt * 4 + g) * kPanelA;
             const int c0 = (kap0 & 31) >> 2;
             *reinterpret_cast<float4 *>(panel + swz(rho, c0)) = make_float4(lo[0], lo[1], lo[2], lo[3]);
@@ -387,41 +369,20 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
 #pragma unroll
                 for (int r = 0; r < kCL; ++r) dh += pv[r];
             }
-            float d[4] = {0.f, 0.f, 0.f, 0.f};                                     // gradients wrt the h2h pre-activations
+            float d[G];                                                            // gradients wrt the h2h pre-activations
 #pragma unroll
-            for (int g = 0; g < G; ++g) dgi[i][g] = 0.f;
-            daux[i] = 0.f;
+            for (int g = 0; g < G; ++g) dgi[i][g] = d[g] = 0.f;
             if (live[i]) {
-                if (G == 3) {
-                    const float r = cg[i][0], z = cg[i][1], n = cg[i][2], hn = ca0[i], hprev = ca1[i];
-                    const float dpn = dh * (1.0f - z) * (1.0f - n * n);
-                    const float dpz = dh * (hprev - n) * z * (1.0f - z);
-                    const float dpr = dpn * hn * r * (1.0f - r);
-                    const float dghn = dpn * r;
-                    dgi[i][0] = dpr; dgi[i][1] = dpz; dgi[i][2] = dpn;             // dgi
-                    daux[i] = dghn;                                                // n-gate part of dgh -> cbuf slot t+1
-                    d[0] = dpr; d[1] = dpz; d[2] = dghn;
-                    dh_carry[i] = dh * z;
-                } else {
-                    const float ig = cg[i][0], fg = cg[i][1], gg = cg[i][2], og = cg[i][G - 1], cprev = ca0[i];
-                    const float tc = dc_tanh(c_cur[i]);
-                    const float dc = dc_carry[i] + dh * og * (1.0f - tc * tc);
-                    const float dpi = dc * gg * ig * (1.0f - ig);
-                    const float dpf = dc * cprev * fg * (1.0f - fg);
-                    const float dpg = dc * ig * (1.0f - gg * gg);
-                    const float dpo = dh * tc * og * (1.0f - og);
-                    dgi[i][0] = dpi; dgi[i][1] = dpf; dgi[i][2] = dpg; dgi[i][G - 1] = dpo;
-                    d[0] = dpi; d[1] = dpf; d[2] = dpg; d[3] = dpo;
-                    dc_carry[i] = dc * fg;
-                    c_cur[i] = cprev;
-                    dh_carry[i] = 0.f;
-                }
+                dh_carry[i] = dc_rnn::cell_bwd<G>([&](int g) { return cg[i][g]; }, G == 3 ? ca0[i] : c_cur[i],   // hn | c_t
+                                                  G == 3 ? ca1[i] : ca0[i], dh, dc_carry[i], dgi[i], d);         // h_{t-1} | c_{t-1}
+                if (G == 4) c_cur[i] = ca0[i];
             }
+            daux[i] = d[2];                                                        // GRU: dghn -> cbuf slot t+1
             // B operand: row = sequence bb, column kappa = g*32 + ul  ->  K-panel g, 16-byte chunk ul/4, word ul%4
             const int off = swz(bb, ul >> 2) + (ul & 3) * 4;
 #pragma unroll
             for (int g = 0; g < G; ++g) {
-                const float hi = tf32_rna(d[g]);
+                const float hi = dc_tf32_rna(d[g]);
                 *reinterpret_cast<float *>(ghi + g * kPanelB + off) = hi;
                 *reinterpret_cast<float *>(glo + g * kPanelB + off) = d[g] - hi;
             }

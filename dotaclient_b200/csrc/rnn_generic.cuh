@@ -1,31 +1,17 @@
 // Shape-generic recurrence kernels (any H that is a multiple of 4, GRU or LSTM).
 //
-// Fallback for widths the register/shared-memory-resident kernels in rnn_seq.cu do not cover.
+// Fallback for the widths that rnn_resident.cuh, rnn_cluster.cuh and rnn_stepwise.cuh do not cover.
 // One CTA owns kBT sequences for all S steps (no inter-CTA communication); h lives in shared
 // memory; W_hh is streamed from L2 every step (it is <= 4 MB and stays L2-resident), read with
 // fully coalesced loads (forward reads the [H, G*H] transpose held in the workspace, backward
 // reads W_hh [G*H, H] as stored).  Correct everywhere, FMA/L2-bound at large H.
 #pragma once
-#include "dc_common.cuh"
+#include "rnn_cell.cuh"
 
 namespace dc_rnn {
 
 constexpr int kBT = 4;         // sequences per CTA
 constexpr int kThreads = 256;
-
-__global__ void transpose_kernel(const float *__restrict__ in, float *__restrict__ out, int rows, int cols) {
-    __shared__ float tile[32][33];
-    const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int r = r0 + i, c = c0 + threadIdx.x;
-        if (r < rows && c < cols) tile[i][threadIdx.x] = in[(size_t)r * cols + c];
-    }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int c = c0 + i, r = r0 + threadIdx.x;
-        if (r < rows && c < cols) out[(size_t)c * rows + r] = tile[threadIdx.x][i];
-    }
-}
 
 // Forward.  gates [S,B,G,H] (in: x W_ih^T + b_ih; out: activated gates), wT [H, G*H].
 template <int G>
@@ -71,25 +57,12 @@ __global__ void __launch_bounds__(kThreads) fwd_generic_kernel(float *__restrict
             const size_t tok = (size_t)t * B + b0 + b;
             float *g = gates + tok * GH;
             const float *pre = pre_s + b * GH;
-            float hnew;
-            if (G == 3) {   // GRU: r, z, n (torch.nn.GRU)
-                const float r = dc_sigmoid(g[u] + pre[u]);
-                const float z = dc_sigmoid(g[H + u] + pre[H + u]);
-                const float hn = pre[2 * H + u];
-                const float n = dc_tanh(g[2 * H + u] + r * hn);
-                hnew = (1.0f - z) * n + z * h_s[b * H + u];
-                g[u] = r; g[H + u] = z; g[2 * H + u] = n;
-                cbuf[((size_t)(t + 1) * B + b0 + b) * H + u] = hn;
-            } else {        // LSTM: i, f, g, o (torch.nn.LSTM)
-                const float ig = dc_sigmoid(g[u] + pre[u]);
-                const float fg = dc_sigmoid(g[H + u] + pre[H + u]);
-                const float gg = dc_tanh(g[2 * H + u] + pre[2 * H + u]);
-                const float og = dc_sigmoid(g[3 * H + u] + pre[3 * H + u]);
-                const float c = fg * cbuf[((size_t)t * B + b0 + b) * H + u] + ig * gg;
-                hnew = og * dc_tanh(c);
-                g[u] = ig; g[H + u] = fg; g[2 * H + u] = gg; g[3 * H + u] = og;
-                cbuf[((size_t)(t + 1) * B + b0 + b) * H + u] = c;
-            }
+            float act[G], aux;
+            const float prev = G == 3 ? h_s[b * H + u] : cbuf[((size_t)t * B + b0 + b) * H + u];
+            const float hnew = cell_fwd<G>([&](int q) { return g[q * H + u]; }, [&](int q) { return pre[q * H + u]; }, prev, act, aux);
+#pragma unroll
+            for (int q = 0; q < G; ++q) g[q * H + u] = act[q];
+            cbuf[((size_t)(t + 1) * B + b0 + b) * H + u] = aux;
             ybuf[((size_t)(t + 1) * B + b0 + b) * H + u] = hnew;
             h_s[b * H + u] = hnew;   // each (b,u) is owned by one thread; matvec readers are behind the barrier
         }
@@ -126,34 +99,13 @@ __global__ void __launch_bounds__(kThreads) bwd_generic_kernel(float *__restrict
             float *g = gates + tok * GH;
             float *dg = dg_s + b * GH;
             const float dh = dy[tok * H + u] + dh_s[b * H + u];
-            if (G == 3) {
-                const float r = g[u], z = g[H + u], n = g[2 * H + u];
-                const size_t ci = ((size_t)(t + 1) * B + b0 + b) * H + u;
-                const float hn = cbuf[ci];
-                const float hprev = ybuf[tok * H + u];       // slot t == h_{t-1}
-                const float dpn = dh * (1.0f - z) * (1.0f - n * n);
-                const float dpz = dh * (hprev - n) * z * (1.0f - z);
-                const float dpr = dpn * hn * r * (1.0f - r);
-                g[u] = dpr; g[H + u] = dpz; g[2 * H + u] = dpn;          // dgi
-                const float dghn = dpn * r;
-                cbuf[ci] = dghn;                                          // n-gate part of dgh
-                dg[u] = dpr; dg[H + u] = dpz; dg[2 * H + u] = dghn;
-                dh_s[b * H + u] = dh * z;                                 // direct path; matvec adds on top
-            } else {
-                const float ig = g[u], fg = g[H + u], gg = g[2 * H + u], og = g[3 * H + u];
-                const float c = cbuf[((size_t)(t + 1) * B + b0 + b) * H + u];
-                const float cprev = cbuf[tok * H + u];
-                const float tc = dc_tanh(c);
-                const float dc = dc_s[b * H + u] + dh * og * (1.0f - tc * tc);
-                const float dpi = dc * gg * ig * (1.0f - ig);
-                const float dpf = dc * cprev * fg * (1.0f - fg);
-                const float dpg = dc * ig * (1.0f - gg * gg);
-                const float dpo = dh * tc * og * (1.0f - og);
-                g[u] = dpi; g[H + u] = dpf; g[2 * H + u] = dpg; g[3 * H + u] = dpo;
-                dg[u] = dpi; dg[H + u] = dpf; dg[2 * H + u] = dpg; dg[3 * H + u] = dpo;
-                dc_s[b * H + u] = dc * fg;
-                dh_s[b * H + u] = 0.f;
-            }
+            const size_t ci = ((size_t)(t + 1) * B + b0 + b) * H + u;
+            float dgi[G], dgh[G];
+            const float prev = G == 3 ? ybuf[tok * H + u] : cbuf[tok * H + u];     // slot t: h_{t-1} | c_{t-1}
+            dh_s[b * H + u] = cell_bwd<G>([&](int q) { return g[q * H + u]; }, cbuf[ci], prev, dh, dc_s[b * H + u], dgi, dgh);   // matvec adds on top
+#pragma unroll
+            for (int q = 0; q < G; ++q) { g[q * H + u] = dgi[q]; dg[q * H + u] = dgh[q]; }
+            if (G == 3) cbuf[ci] = dgh[2];                                            // n-gate part of dgh
         }
         __syncthreads();
         // dh_{t-1}[b][k] += sum_j dgh[b][j] * W[j][k]
@@ -178,6 +130,33 @@ __global__ void __launch_bounds__(kThreads) bwd_generic_kernel(float *__restrict
         if (dh0) dh0[(size_t)(b0 + b) * H + u] = dh_s[b * H + u];
         if (dc0 && G == 4) dc0[(size_t)(b0 + b) * H + u] = dc_s[b * H + u];
     }
+}
+
+template <typename K, typename... Args>
+inline int launch_generic(K kern, int B, size_t smem, cudaStream_t st, Args... args) {
+    DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<(B + kBT - 1) / kBT, kThreads, smem, st>>>(args...);
+    DC_LAUNCH_OK();
+    return DC_OK;
+}
+
+// workspace: W_hh^T [H, G*H] (the forward reads the transpose so that output columns are contiguous)
+inline int launch_fwd_generic(int cell, float *gates, const float *w_hh, const float *b_hh, float *ybuf, float *cbuf, int B, int S,
+                              int H, void *workspace, cudaStream_t st) {
+    const int G = cell == DC_CELL_GRU ? 3 : 4;
+    float *wT = reinterpret_cast<float *>(workspace);
+    int rc = launch_transpose(w_hh, wT, G * H, H, st);
+    if (rc) return rc;
+    const size_t smem = (size_t)kBT * (G + 1) * H * sizeof(float);
+    if (G == 3) return launch_generic(fwd_generic_kernel<3>, B, smem, st, gates, wT, b_hh, ybuf, cbuf, B, S, H);
+    return launch_generic(fwd_generic_kernel<4>, B, smem, st, gates, wT, b_hh, ybuf, cbuf, B, S, H);
+}
+inline int launch_bwd_generic(int cell, float *gates, const float *w_hh, const float *ybuf, float *cbuf, const float *dy,
+                              const float *dhn, const float *dcn, float *dh0, float *dc0, int B, int S, int H, cudaStream_t st) {
+    const int G = cell == DC_CELL_GRU ? 3 : 4;
+    const size_t smem = (size_t)kBT * (G + 2) * H * sizeof(float);
+    if (G == 3) return launch_generic(bwd_generic_kernel<3>, B, smem, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H);
+    return launch_generic(bwd_generic_kernel<4>, B, smem, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H);
 }
 
 }  // namespace dc_rnn

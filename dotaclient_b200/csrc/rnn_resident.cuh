@@ -26,34 +26,21 @@
 // Algorithmic HBM bytes per token: fwd reads G*H*4 (gi) and writes (G+2)*H*4 (gates, h, c|hn);
 // bwd reads (G+3)*H*4 and writes G*H*4 (+H*4 GRU).
 #pragma once
-#include "dc_common.cuh"
+#include "rnn_cell.cuh"
 
 namespace dc_rnn {
 
 constexpr int kH = 128;
 constexpr int kStages = 4;
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(dc_smem_u32(bar)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
+                     dc_smem_u32(dst)),
+                 "l"(src), "r"(bytes), "r"(dc_smem_u32(bar))
                  : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                     : "=r"(ok)
-                     : "r"(smem_u32(bar)), "r"(parity)
-                     : "memory");
-    } while (!ok);
 }
 
 // Thread layout of the stationary mat-vec: tid = ms * NCG + cg; the thread owns rows [ms*32, ms*32+32) and
@@ -176,7 +163,7 @@ __global__ void __launch_bounds__(G *kH, 1) fwd_resident_kernel(float *__restric
     float2 wr[8][4];
     load_weights<NT, GH>(wT, wr, w_s);
     if (tid == 0) {
-        for (int s = 0; s < kStages; ++s) mbar_init(&bars[s], 1);
+        for (int s = 0; s < kStages; ++s) dc_mbar_init(&bars[s], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     // unit threads: (b, u) pairs
@@ -202,7 +189,7 @@ __global__ void __launch_bounds__(G *kH, 1) fwd_resident_kernel(float *__restric
         __syncthreads();
         const int st = t % kStages;
         if (unit) {
-            mbar_wait(&bars[st], (t / kStages) & 1);
+            dc_mbar_wait(&bars[st], (t / kStages) & 1);
             if (live) {
                 const float *gi = stage_s + (size_t)st * BT * GH + ub * GH;
                 float pre[G];
@@ -215,24 +202,13 @@ __global__ void __launch_bounds__(G *kH, 1) fwd_resident_kernel(float *__restric
                 }
                 const size_t tok = (size_t)t * B + b0 + ub;
                 float *gout = gates + tok * GH;
-                float hnew;
-                if (G == 3) {
-                    const float r = dc_sigmoid(gi[uu] + pre[0]);
-                    const float z = dc_sigmoid(gi[H + uu] + pre[1]);
-                    const float n = dc_tanh(gi[2 * H + uu] + r * pre[2]);
-                    hnew = (1.0f - z) * n + z * in_s[ub * H + uu];
-                    gout[uu] = r; gout[H + uu] = z; gout[2 * H + uu] = n;
-                    cbuf[(tok + B) * H + uu] = pre[2];                             // W_hn h + b_hn, slot t+1
-                } else {
-                    const float ig = dc_sigmoid(gi[uu] + pre[0]);
-                    const float fg = dc_sigmoid(gi[H + uu] + pre[1]);
-                    const float gg = dc_tanh(gi[2 * H + uu] + pre[2]);
-                    const float og = dc_sigmoid(gi[3 * H + uu] + pre[G - 1]);
-                    c_reg = fg * c_reg + ig * gg;
-                    hnew = og * dc_tanh(c_reg);
-                    gout[uu] = ig; gout[H + uu] = fg; gout[2 * H + uu] = gg; gout[3 * H + uu] = og;
-                    cbuf[(tok + B) * H + uu] = c_reg;
-                }
+                float act[G], aux;
+                const float hnew = cell_fwd<G, false>([&](int g) { return gi[g * H + uu]; }, [&](int g) { return pre[g]; },
+                                               G == 3 ? in_s[ub * H + uu] : c_reg, act, aux);
+                if (G == 4) c_reg = aux;
+#pragma unroll
+                for (int g = 0; g < G; ++g) gout[g * H + uu] = act[g];
+                cbuf[(tok + B) * H + uu] = aux;                                    // c_t | W_hn h + b_hn, slot t+1
                 ybuf[(tok + B) * H + uu] = hnew;
                 in_s[ub * H + uu] = hnew;
             }
@@ -283,7 +259,7 @@ __global__ void __launch_bounds__(G *kH, 1) bwd_resident_kernel(float *__restric
     float2 wr[8][4];
     load_weights<NT, H>(w, wr, w_s);
     if (tid == 0) {
-        for (int s = 0; s < kStages; ++s) mbar_init(&bars[s], 1);
+        for (int s = 0; s < kStages; ++s) dc_mbar_init(&bars[s], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     const bool unit = tid < BT * H;
@@ -325,7 +301,7 @@ __global__ void __launch_bounds__(G *kH, 1) bwd_resident_kernel(float *__restric
         const int t = S - 1 - it;
         const int st = it % kStages;
         if (unit) {
-            mbar_wait(&bars[st], (it / kStages) & 1);
+            dc_mbar_wait(&bars[st], (it / kStages) & 1);
             if (live) {
                 const float *sg = stage_s + (size_t)st * SM::stage_floats;
                 const float *g = sg + ub * GH;
@@ -335,33 +311,17 @@ __global__ void __launch_bounds__(G *kH, 1) bwd_resident_kernel(float *__restric
                 const size_t tok = (size_t)t * B + b0 + ub;
                 float *gout = gates + tok * GH;
                 float *dg = in_s + ub * GH;
-                if (G == 3) {
-                    const float r = g[uu], z = g[H + uu], n = g[2 * H + uu];
-                    const float hn = sg[BT * (GH + H) + ub * H + uu];
-                    const float hprev = sg[BT * (GH + 2 * H) + ub * H + uu];
-                    const float dpn = dh * (1.0f - z) * (1.0f - n * n);
-                    const float dpz = dh * (hprev - n) * z * (1.0f - z);
-                    const float dpr = dpn * hn * r * (1.0f - r);
-                    const float dghn = dpn * r;
-                    gout[uu] = dpr; gout[H + uu] = dpz; gout[2 * H + uu] = dpn;
-                    cbuf[(tok + B) * H + uu] = dghn;
-                    dg[uu] = dpr; dg[H + uu] = dpz; dg[2 * H + uu] = dghn;
-                    dh_carry = dh * z;
-                } else {
-                    const float ig = g[uu], fg = g[H + uu], gg = g[2 * H + uu], og = g[3 * H + uu];
-                    const float cprev = sg[BT * (GH + H) + ub * H + uu];
-                    const float tc = dc_tanh(c_cur);
-                    const float dc = dc_carry + dh * og * (1.0f - tc * tc);
-                    const float dpi = dc * gg * ig * (1.0f - ig);
-                    const float dpf = dc * cprev * fg * (1.0f - fg);
-                    const float dpg = dc * ig * (1.0f - gg * gg);
-                    const float dpo = dh * tc * og * (1.0f - og);
-                    gout[uu] = dpi; gout[H + uu] = dpf; gout[2 * H + uu] = dpg; gout[3 * H + uu] = dpo;
-                    dg[uu] = dpi; dg[H + uu] = dpf; dg[2 * H + uu] = dpg; dg[3 * H + uu] = dpo;
-                    dc_carry = dc * fg;
-                    c_cur = cprev;
-                    dh_carry = 0.f;
-                }
+                auto act = [&](int q) { return g[q * H + uu]; };
+                const float aux1 = sg[BT * (GH + H) + ub * H + uu];                  // LSTM c_{t-1} | GRU hn
+                float dgi[G], dgh[G];
+                if (G == 3) dh_carry = cell_bwd<G>(act, aux1, sg[BT * (GH + 2 * H) + ub * H + uu], dh, dc_carry, dgi, dgh);
+                else dh_carry = cell_bwd<G>(act, c_cur, aux1, dh, dc_carry, dgi, dgh);
+#pragma unroll
+                for (int q = 0; q < G; ++q) gout[q * H + uu] = dgi[q];
+                if (G == 3) cbuf[(tok + B) * H + uu] = dgh[2];
+#pragma unroll
+                for (int q = 0; q < G; ++q) dg[q * H + uu] = dgh[q];
+                if (G == 4) c_cur = aux1;
             }
         }
         __syncthreads();
@@ -378,7 +338,7 @@ __global__ void __launch_bounds__(G *kH, 1) bwd_resident_kernel(float *__restric
     }
 }
 
-inline bool resident_supported(int cell, int H) { (void)cell; return H == kH; }
+inline bool resident_supported(int H) { return H == kH; }
 
 template <int G, int BT>
 int launch_fwd_t(float *gates, const float *wT, const float *b_hh, float *ybuf, float *cbuf, int B, int S, cudaStream_t st) {
@@ -402,9 +362,12 @@ int launch_bwd_t(float *gates, const float *w, const float *ybuf, float *cbuf, c
 // thread to one (sequence, unit) pair, so kBT * H must not exceed the CTA size G * H: kBT <= 3 (GRU) / 4 (LSTM).
 inline bool small_tile(int B) { return (B + 1) / 2 <= dc_sm_count(); }
 
-inline int launch_fwd_resident(int cell, float *gates, const float *wT, const float *b_hh, float *ybuf, float *cbuf, int B,
-                               int S, int H, cudaStream_t st) {
-    (void)H;
+// workspace: W_hh^T [H, G*H], the [M, NOUT] operand of the forward mat-vec
+inline int launch_fwd_resident(int cell, float *gates, const float *w_hh, const float *b_hh, float *ybuf, float *cbuf, int B,
+                               int S, void *workspace, cudaStream_t st) {
+    float *wT = reinterpret_cast<float *>(workspace);
+    int rc = launch_transpose(w_hh, wT, (cell == DC_CELL_GRU ? 3 : 4) * kH, kH, st);
+    if (rc) return rc;
     if (cell == DC_CELL_GRU)
         return small_tile(B) ? launch_fwd_t<3, 2>(gates, wT, b_hh, ybuf, cbuf, B, S, st)
                              : launch_fwd_t<3, 3>(gates, wT, b_hh, ybuf, cbuf, B, S, st);
@@ -412,8 +375,7 @@ inline int launch_fwd_resident(int cell, float *gates, const float *wT, const fl
                          : launch_fwd_t<4, 4>(gates, wT, b_hh, ybuf, cbuf, B, S, st);
 }
 inline int launch_bwd_resident(int cell, float *gates, const float *w, const float *ybuf, float *cbuf, const float *dy,
-                               const float *dhn, const float *dcn, float *dh0, float *dc0, int B, int S, int H, cudaStream_t st) {
-    (void)H;
+                               const float *dhn, const float *dcn, float *dh0, float *dc0, int B, int S, cudaStream_t st) {
     if (cell == DC_CELL_GRU)
         return small_tile(B) ? launch_bwd_t<3, 2>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, st)
                              : launch_bwd_t<3, 3>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, st);

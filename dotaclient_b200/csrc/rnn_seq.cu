@@ -2,7 +2,6 @@
 //
 // Replaces the time loop inside nn.GRU / nn.LSTM (policy.py:66,141).  Layout, saved tensors and
 // in-place reuse of the gate buffer are described in include/dotaclient_b200.h and DESIGN.md.
-#include "dc_common.cuh"
 #include "rnn_generic.cuh"
 #include "rnn_resident.cuh"
 #include "rnn_cluster.cuh"
@@ -18,7 +17,7 @@ extern "C" size_t dc_rnn_workspace_bytes(int cell, int B, int H) {
     const int G = cell == DC_CELL_GRU ? 3 : 4;
     if (dc_rnnc::cluster_supported(H)) return dc_rnnc::bwd_workspace_bytes(B > 0 ? B : 1);   // partial-sum exchange (backward)
     if (dc_rnns::stepwise_supported(H)) return dc_rnns::workspace_bytes(cell, B > 0 ? B : 1, H);
-    return (size_t)G * H * H * sizeof(float);   // W_hh^T for the forward kernels that read the transpose
+    return (size_t)G * H * H * sizeof(float);   // W_hh^T for the resident and generic forward kernels
 }
 
 static int check_rnn_args(const char *fn, int cell, int B, int S, int H) {
@@ -34,26 +33,10 @@ extern "C" int dc_rnn_seq_fwd(int cell, float *gates, const float *w_hh, const f
     if (rc) return rc;
     DC_REQUIRE(gates && w_hh && b_hh && ybuf && cbuf && workspace, DC_EINVAL, "dc_rnn_seq_fwd: null pointer");
     cudaStream_t st = dc_cu_stream(stream);
-    const int G = cell == DC_CELL_GRU ? 3 : 4;
-    if (dc_rnnc::cluster_supported(H)) return dc_rnnc::launch_fwd(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, st);   // reads W_hh as stored
+    if (dc_rnn::resident_supported(H)) return dc_rnn::launch_fwd_resident(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, workspace, st);
+    if (dc_rnnc::cluster_supported(H)) return dc_rnnc::launch_fwd(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, st);
     if (dc_rnns::stepwise_supported(H)) return dc_rnns::launch_fwd(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, H, workspace, st);
-    // the other forward kernels read W_hh^T [H, G*H] so that output columns are contiguous (coalesced / float4)
-    float *wT = reinterpret_cast<float *>(workspace);
-    dim3 tb(32, 8), tg((H + 31) / 32, (G * H + 31) / 32);
-    dc_rnn::transpose_kernel<<<tg, tb, 0, st>>>(w_hh, wT, G * H, H);
-    DC_LAUNCH_OK();
-    if (dc_rnn::resident_supported(cell, H)) return dc_rnn::launch_fwd_resident(cell, gates, wT, b_hh, ybuf, cbuf, B, S, H, st);
-    const int blocks = (B + dc_rnn::kBT - 1) / dc_rnn::kBT;
-    const size_t smem = (size_t)dc_rnn::kBT * (G + 1) * H * sizeof(float);
-    if (G == 3) {
-        DC_CUDA(cudaFuncSetAttribute(dc_rnn::fwd_generic_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        dc_rnn::fwd_generic_kernel<3><<<blocks, dc_rnn::kThreads, smem, st>>>(gates, wT, b_hh, ybuf, cbuf, B, S, H);
-    } else {
-        DC_CUDA(cudaFuncSetAttribute(dc_rnn::fwd_generic_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        dc_rnn::fwd_generic_kernel<4><<<blocks, dc_rnn::kThreads, smem, st>>>(gates, wT, b_hh, ybuf, cbuf, B, S, H);
-    }
-    DC_LAUNCH_OK();
-    return DC_OK;
+    return dc_rnn::launch_fwd_generic(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, H, workspace, st);
 }
 
 extern "C" int dc_rnn_seq_bwd(int cell, float *gates, const float *w_hh, const float *ybuf, float *cbuf, const float *dy,
@@ -63,7 +46,7 @@ extern "C" int dc_rnn_seq_bwd(int cell, float *gates, const float *w_hh, const f
     if (rc) return rc;
     DC_REQUIRE(gates && w_hh && ybuf && cbuf && dy, DC_EINVAL, "dc_rnn_seq_bwd: null pointer");
     cudaStream_t st = dc_cu_stream(stream);
-    const int G = cell == DC_CELL_GRU ? 3 : 4;
+    if (dc_rnn::resident_supported(H)) return dc_rnn::launch_bwd_resident(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, st);
     if (dc_rnnc::cluster_supported(H)) {
         DC_REQUIRE(workspace, DC_EINVAL, "dc_rnn_seq_bwd: the H = 256 kernels need the workspace (dc_rnn_workspace_bytes)");
         return dc_rnnc::launch_bwd(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, reinterpret_cast<float *>(workspace), B, S, st);
@@ -72,17 +55,5 @@ extern "C" int dc_rnn_seq_bwd(int cell, float *gates, const float *w_hh, const f
         DC_REQUIRE(workspace, DC_EINVAL, "dc_rnn_seq_bwd: the step-wise kernels need the workspace (dc_rnn_workspace_bytes)");
         return dc_rnns::launch_bwd(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, workspace, st);
     }
-    if (dc_rnn::resident_supported(cell, H))
-        return dc_rnn::launch_bwd_resident(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, st);
-    const int blocks = (B + dc_rnn::kBT - 1) / dc_rnn::kBT;
-    const size_t smem = (size_t)dc_rnn::kBT * (G + 2) * H * sizeof(float);
-    if (G == 3) {
-        DC_CUDA(cudaFuncSetAttribute(dc_rnn::bwd_generic_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        dc_rnn::bwd_generic_kernel<3><<<blocks, dc_rnn::kThreads, smem, st>>>(gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H);
-    } else {
-        DC_CUDA(cudaFuncSetAttribute(dc_rnn::bwd_generic_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        dc_rnn::bwd_generic_kernel<4><<<blocks, dc_rnn::kThreads, smem, st>>>(gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H);
-    }
-    DC_LAUNCH_OK();
-    return DC_OK;
+    return dc_rnn::launch_bwd_generic(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, st);
 }

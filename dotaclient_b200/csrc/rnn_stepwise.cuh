@@ -9,8 +9,7 @@
 // 2 launches per time step; same buffers, same saved tensors and the same in-place reuse of the gate buffer as the other
 // recurrence kernels (include/dotaclient_b200.h).  fp32-level accuracy like every other dense layer of the step.
 #pragma once
-#include "dc_common.cuh"
-#include "rnn_generic.cuh"   // transpose_kernel
+#include "rnn_cell.cuh"
 
 namespace dc_rnns {
 
@@ -66,25 +65,11 @@ __global__ void __launch_bounds__(256) fwd_gate_kernel(float *__restrict__ gates
         pre[g] = a;
     }
     float *g = gates_t + (size_t)b * GH + u;
-    float hnew;
-    if (G == 3) {
-        const float r = dc_sigmoid(g[0] + pre[0]);
-        const float z = dc_sigmoid(g[H] + pre[1]);
-        const float n = dc_tanh(g[2 * H] + r * pre[2]);
-        hnew = (1.0f - z) * n + z * h_prev[idx];
-        g[0] = r; g[H] = z; g[2 * H] = n;
-        aux_next[idx] = pre[2];                              // W_hn h + b_hn (cbuf slot t+1)
-    } else {
-        const float ig = dc_sigmoid(g[0] + pre[0]);
-        const float fg = dc_sigmoid(g[H] + pre[1]);
-        const float gg = dc_tanh(g[2 * H] + pre[2]);
-        const float og = dc_sigmoid(g[(G - 1) * H] + pre[G - 1]);
-        const float c = fg * c_prev[idx] + ig * gg;
-        hnew = og * dc_tanh(c);
-        g[0] = ig; g[H] = fg; g[2 * H] = gg; g[(G - 1) * H] = og;
-        aux_next[idx] = c;                                   // c_t (cbuf slot t+1)
-    }
-    h_next[idx] = hnew;
+    float act[G];
+    h_next[idx] = dc_rnn::cell_fwd<G>([&](int q) { return g[q * H]; }, [&](int q) { return pre[q]; },
+                                      G == 3 ? h_prev[idx] : c_prev[idx], act, aux_next[idx]);   // aux: cbuf slot t+1
+#pragma unroll
+    for (int q = 0; q < G; ++q) g[q * H] = act[q];
 }
 
 // ---- backward gate kernel -------------------------------------------------------------------------------------------------
@@ -110,32 +95,14 @@ __global__ void __launch_bounds__(256) bwd_gate_kernel(float *__restrict__ gates
     }
     float *g = gates_t + (size_t)b * GH + u;
     float *dg = dgbuf + (size_t)b * GH + u;
-    if (G == 3) {
-        const float r = g[0], z = g[H], n = g[2 * H];
-        const float hn = aux_cur[idx], hprev = h_prev[idx];
-        const float dpn = dh * (1.0f - z) * (1.0f - n * n);
-        const float dpz = dh * (hprev - n) * z * (1.0f - z);
-        const float dpr = dpn * hn * r * (1.0f - r);
-        const float dghn = dpn * r;
-        g[0] = dpr; g[H] = dpz; g[2 * H] = dpn;
-        aux_cur[idx] = dghn;
-        dg[0] = dpr; dg[H] = dpz; dg[2 * H] = dghn;
-        dh_carry[idx] = dh * z;
-    } else {
-        const float ig = g[0], fg = g[H], gg = g[2 * H], og = g[(G - 1) * H];
-        const float c = aux_cur[idx], cprev = c_prev[idx];
-        const float tc = dc_tanh(c);
-        const float dcin = first ? (dcn ? dcn[idx] : 0.f) : dc_carry[idx];
-        const float dc = dcin + dh * og * (1.0f - tc * tc);
-        const float dpi = dc * gg * ig * (1.0f - ig);
-        const float dpf = dc * cprev * fg * (1.0f - fg);
-        const float dpg = dc * ig * (1.0f - gg * gg);
-        const float dpo = dh * tc * og * (1.0f - og);
-        g[0] = dpi; g[H] = dpf; g[2 * H] = dpg; g[(G - 1) * H] = dpo;
-        dg[0] = dpi; dg[H] = dpf; dg[2 * H] = dpg; dg[(G - 1) * H] = dpo;
-        dc_carry[idx] = dc * fg;
-        dh_carry[idx] = 0.f;
-    }
+    float dgi[G], dgh[G];
+    float dc = G == 3 ? 0.f : first ? (dcn ? dcn[idx] : 0.f) : dc_carry[idx];
+    dh_carry[idx] = dc_rnn::cell_bwd<G>([&](int q) { return g[q * H]; }, aux_cur[idx], G == 3 ? h_prev[idx] : c_prev[idx], dh, dc,
+                                        dgi, dgh);
+#pragma unroll
+    for (int q = 0; q < G; ++q) { g[q * H] = dgi[q]; dg[q * H] = dgh[q]; }
+    if (G == 3) aux_cur[idx] = dgh[2];                       // n-gate part of dgh (cbuf slot t+1)
+    else dc_carry[idx] = dc;
 }
 
 __global__ void __launch_bounds__(256) bwd_final_kernel(const float *__restrict__ part, int ksplit, const float *__restrict__ dh_carry,
@@ -174,8 +141,8 @@ inline int launch_bwd(int cell, float *gates, const float *w_hh, const float *yb
     const Workspace w = carve(workspace, cell, B, H);
     const int blocks = (B * H + 255) / 256;
     const size_t BH = (size_t)B * H;
-    dim3 tb(32, 8), tg((H + 31) / 32, (GH + 31) / 32);
-    dc_rnn::transpose_kernel<<<tg, tb, 0, st>>>(w_hh, w.wT, GH, H);            // W_hh^T [H, G*H]: the GEMM's [N, K] operand
+    int rc = dc_rnn::launch_transpose(w_hh, w.wT, GH, H, st);                  // W_hh^T [H, G*H]: the GEMM's [N, K] operand
+    if (rc) return rc;
     for (int it = 0; it < S; ++it) {
         const int t = S - 1 - it;
         float *gt = gates + (size_t)t * B * GH;
@@ -185,7 +152,7 @@ inline int launch_bwd(int cell, float *gates, const float *w_hh, const float *yb
         else
             bwd_gate_kernel<4><<<blocks, 256, 0, st>>>(gt, dy + t * BH, w.part_b, w.ksb, w.dh_carry, w.dc_carry, dhn, dcn, nullptr,
                                                        cbuf + t * BH, cbuf + (t + 1) * BH, w.dgbuf, it == 0, B, H);
-        int rc = dc_gemm_tf32x3_splitk(w.dgbuf, GH, w.wT, GH, w.part_b, B, H, GH, w.ksb, it == 0, st);
+        rc = dc_gemm_tf32x3_splitk(w.dgbuf, GH, w.wT, GH, w.part_b, B, H, GH, w.ksb, it == 0, st);
         if (rc) return rc;
     }
     bwd_final_kernel<<<blocks, 256, 0, st>>>(w.part_b, w.ksb, w.dh_carry, G == 4 ? w.dc_carry : nullptr, dh0, G == 4 ? dc0 : nullptr, B * H);

@@ -71,10 +71,13 @@ int dc_gae_scan(const float *rewards, int n_sub, const float *values, const int6
  *   ybuf   [S+1, B, H]  slot 0 = h_0 (in), slot t+1 = h_t (out)   -> y = ybuf[1:], h_n = ybuf[S]
  *   cbuf   [S+1, B, H]  LSTM: slot 0 = c_0 (in), slot t+1 = c_t (out)
  *                       GRU : slot t+1 = W_hn h_{t-1} + b_hn (out, saved for backward)
- *   workspace: dc_rnn_workspace_bytes(cell, B, H) bytes of scratch (W_hh^T for H != 256; at H = 256 the partial-sum
- *              exchange of the cluster backward kernel -- the same buffer serves forward and backward).
+ *   workspace: dc_rnn_workspace_bytes(cell, B, H) bytes of scratch; the same buffer serves forward and backward.  It holds
+ *              W_hh^T at H = 128 and for the generic kernels, the partial-sum exchange of the cluster backward kernel at
+ *              H = 256, and W_hh^T plus the split-K partials and carries of the step-wise kernels at the other multiples of 128.
  * Kernels by width: H = 128 one-SM weight-resident FFMA kernels; H = 256 (the reference's width) 8-CTA-cluster
- * weight-resident wgmma 3xTF32 kernels; any other H % 4 == 0 a generic kernel that streams W_hh from L2.
+ * weight-resident wgmma 3xTF32 kernels; other multiples of 128 (384, 512, ...) step-wise kernels: per step a split-K
+ * wgmma 3xTF32 GEMM over all SMs that streams W_hh from L2, then a gate kernel; any other H % 4 == 0 a generic kernel
+ * that streams W_hh from L2.
  * Backward (consumes what forward left behind)
  *   gates  in: activated gates   out: dL/d(gates pre-activation wrt the i2h branch) = dgi
  *   cbuf   LSTM: unchanged.  GRU: slot t+1 out = dL/d(W_hn h + b_hn) (the n-gate part of dgh)

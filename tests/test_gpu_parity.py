@@ -170,6 +170,74 @@ def test_rnn_forward_backward_vs_torch(cell, B, S, H):
         torch.testing.assert_close(p[k].grad.cpu(), v.grad, rtol=5e-4, atol=5e-6 * scale * B)
 
 
+@pytest.mark.parametrize("cell", ["gru", "lstm"])
+@pytest.mark.parametrize("H", [64, 96])
+def test_rnn_generic_kernels_vs_torch(cell, H):
+    """The shape-generic recurrence kernels (H % 4 == 0 but not a multiple of 128), called through the C-ABI directly:
+    ops.rnn_sequence needs H % 128 == 0 for its i2h GEMM.  B = 5 leaves the last CTA's 4-sequence tile partly filled.
+    The i2h pre-activations and the weight gradients are computed on the CPU from what the kernels leave behind."""
+    from dotaclient_b200 import _lib, ops
+    B, S = 5, 6
+    torch.manual_seed(B * 1000 + S * 10 + H)
+    ref = _torch_rnn(cell, H)
+    x = torch.randn(S, B, H)
+    h0 = torch.randn(1, B, H) * 0.5
+    c0 = torch.randn(1, B, H) * 0.5
+    wy, wh, wc = torch.randn(S, B, H), torch.randn(B, H), torch.randn(B, H)
+    xr = x.clone().requires_grad_(True)
+    h0r, c0r = h0.clone().requires_grad_(True), c0.clone().requires_grad_(True)
+    if cell == "lstm":
+        yr, (hn, cn) = ref(xr, (h0r, c0r))
+        loss = (yr * wy).sum() + (hn[0] * wh).sum() + (cn[0] * wc).sum()
+    else:
+        yr, hn = ref(xr, h0r)
+        loss = (yr * wy).sum() + (hn[0] * wh).sum()
+    loss.backward()
+
+    d = dev()
+    lib = _lib.load()
+    w_ih, w_hh, b_ih, b_hh = (getattr(ref, k).detach() for k in ("weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0"))
+    x2 = x.view(S * B, H)
+    gates = (x2 @ w_ih.t() + b_ih).to(d).contiguous()
+    ybuf = torch.zeros(S + 1, B, H, device=d)
+    cbuf = torch.zeros(S + 1, B, H, device=d)
+    ybuf[0] = h0[0].to(d)
+    if cell == "lstm":
+        cbuf[0] = c0[0].to(d)
+    ws = torch.empty(max(int(lib.dc_rnn_workspace_bytes(ops.CELL_ID[cell], B, H)), 16), dtype=torch.uint8, device=d)
+    w_hh_d, b_hh_d = w_hh.to(d).contiguous(), b_hh.to(d).contiguous()
+    _lib.check(lib.dc_rnn_seq_fwd(ops.CELL_ID[cell], gates.data_ptr(), w_hh_d.data_ptr(), b_hh_d.data_ptr(), ybuf.data_ptr(),
+                                  cbuf.data_ptr(), B, S, H, ws.data_ptr(), _lib.stream_ptr()), "dc_rnn_seq_fwd")
+    torch.testing.assert_close(ybuf[1:].cpu(), yr.detach(), rtol=1e-4, atol=2e-5)
+    torch.testing.assert_close(ybuf[S].cpu(), hn[0].detach(), rtol=1e-4, atol=2e-5)
+    if cell == "lstm":
+        torch.testing.assert_close(cbuf[S].cpu(), cn[0].detach(), rtol=1e-4, atol=2e-5)
+
+    dy, dhn = wy.to(d).contiguous(), wh.to(d).contiguous()
+    dcn = wc.to(d).contiguous() if cell == "lstm" else None
+    dh0 = torch.empty(B, H, device=d)
+    dc0 = torch.empty(B, H, device=d) if cell == "lstm" else None
+    _lib.check(lib.dc_rnn_seq_bwd(ops.CELL_ID[cell], gates.data_ptr(), w_hh_d.data_ptr(), ybuf.data_ptr(), cbuf.data_ptr(),
+                                  dy.data_ptr(), dhn.data_ptr(), _lib.ptr(dcn), dh0.data_ptr(), _lib.ptr(dc0), B, S, H,
+                                  ws.data_ptr(), _lib.stream_ptr()), "dc_rnn_seq_bwd")
+    torch.cuda.synchronize()
+    dgi = gates.cpu().double()                                    # [S*B, G*H], written in place of the saved gates
+    hprev = ybuf[:S].cpu().double().view(S * B, H)                # h_{t-1} of every token
+    if cell == "lstm":
+        dgh = dgi                                                 # LSTM: the h2h gate gradients equal dgi
+    else:
+        dgh = torch.cat([dgi[:, :2 * H], cbuf[1:].cpu().double().view(S * B, H)], dim=1)   # GRU: n gate from cbuf
+    scale = max(1.0, float(S))
+    torch.testing.assert_close(dh0.cpu(), h0r.grad[0], rtol=2e-4, atol=2e-6 * scale)
+    if cell == "lstm":
+        torch.testing.assert_close(dc0.cpu(), c0r.grad[0], rtol=2e-4, atol=2e-6 * scale)
+    torch.testing.assert_close((dgi @ w_ih.double()).float().view(S, B, H), xr.grad, rtol=2e-4, atol=2e-6 * scale)
+    grads = {"weight_ih_l0": dgi.t() @ x2.double(), "bias_ih_l0": dgi.sum(0),
+             "weight_hh_l0": dgh.t() @ hprev, "bias_hh_l0": dgh.sum(0)}
+    for k, v in ref.named_parameters():
+        torch.testing.assert_close(grads[k].float(), v.grad, rtol=5e-4, atol=5e-6 * scale * B)
+
+
 @pytest.mark.parametrize("cell,H,B", [("lstm", 128, 256), ("gru", 128, 256), ("lstm", 256, 512), ("gru", 256, 512)])
 def test_rnn_full_size_sampled_sequences(cell, H, B):
     """C2 shape (B=256, S=512, H=128) and C3's per-GPU shape (B=512, S=512, H=256): sequences are independent, so sampled
