@@ -13,6 +13,10 @@ namespace dc_rnn {
 constexpr int kBT = 4;         // sequences per CTA
 constexpr int kThreads = 256;
 
+// The backward's dh mat-vec splits its contraction over kThreads / H slices when H < kThreads (H = 32, 64, 96 here); the
+// slices' partial sums go through shared memory and are added in slice order, so that the result is deterministic.
+__host__ __device__ constexpr int bwd_slices(int H) { return kThreads >= H ? kThreads / H : 1; }
+
 // Forward.  gates [S,B,G,H] (in: x W_ih^T + b_ih; out: activated gates), wT [H, G*H].
 template <int G>
 __global__ void __launch_bounds__(kThreads) fwd_generic_kernel(float *__restrict__ gates, const float *__restrict__ wT,
@@ -81,6 +85,7 @@ __global__ void __launch_bounds__(kThreads) bwd_generic_kernel(float *__restrict
     float *dh_s = smem;                    // [kBT][H] recurrent gradient wrt h
     float *dc_s = smem + kBT * H;          // [kBT][H] (LSTM) recurrent gradient wrt c
     float *dg_s = smem + 2 * kBT * H;      // [kBT][G*H] gradient wrt the hidden-to-hidden pre-activations
+    float *part_s = dg_s + kBT * G * H;    // [nslice][kBT][H] partial mat-vec sums (nslice > 1 only)
     const int GH = G * H;
     const int b0 = blockIdx.x * kBT;
     const int nb = min(kBT, B - b0);
@@ -91,7 +96,7 @@ __global__ void __launch_bounds__(kThreads) bwd_generic_kernel(float *__restrict
     }
     for (int i = threadIdx.x; i < kBT * GH; i += kThreads) dg_s[i] = 0.f;
     __syncthreads();
-    const int nslice = (kThreads >= H) ? kThreads / H : 1;   // split the contraction when H < kThreads
+    const int nslice = bwd_slices(H);
     for (int t = S - 1; t >= 0; --t) {
         for (int i = threadIdx.x; i < nb * H; i += kThreads) {
             const int b = i / H, u = i % H;
@@ -120,10 +125,23 @@ __global__ void __launch_bounds__(kThreads) bwd_generic_kernel(float *__restrict
 #pragma unroll
                 for (int b = 0; b < kBT; ++b) acc[b] = fmaf(dg_s[b * GH + j], wv, acc[b]);
             }
+            if (nslice == 1) {                 // the only contribution to dh_s[b][k]
 #pragma unroll
-            for (int b = 0; b < kBT; ++b) atomicAdd(&dh_s[b * H + k], acc[b]);
+                for (int b = 0; b < kBT; ++b) dh_s[b * H + k] += acc[b];
+            } else {
+#pragma unroll
+                for (int b = 0; b < kBT; ++b) part_s[(sl * kBT + b) * H + k] = acc[b];
+            }
         }
         __syncthreads();
+        if (nslice > 1) {                      // fixed order: cell value, then slice 0, 1, ...
+            for (int i = threadIdx.x; i < kBT * H; i += kThreads) {
+                float v = dh_s[i];
+                for (int sl = 0; sl < nslice; ++sl) v += part_s[sl * kBT * H + i];
+                dh_s[i] = v;
+            }
+            __syncthreads();
+        }
     }
     for (int i = threadIdx.x; i < nb * H; i += kThreads) {
         const int b = i / H, u = i % H;
@@ -154,7 +172,8 @@ inline int launch_fwd_generic(int cell, float *gates, const float *w_hh, const f
 inline int launch_bwd_generic(int cell, float *gates, const float *w_hh, const float *ybuf, float *cbuf, const float *dy,
                               const float *dhn, const float *dcn, float *dh0, float *dc0, int B, int S, int H, cudaStream_t st) {
     const int G = cell == DC_CELL_GRU ? 3 : 4;
-    const size_t smem = (size_t)kBT * (G + 2) * H * sizeof(float);
+    const int nslice = bwd_slices(H);
+    const size_t smem = ((size_t)kBT * (G + 2) * H + (nslice > 1 ? (size_t)nslice * kBT * H : 0)) * sizeof(float);
     if (G == 3) return launch_generic(bwd_generic_kernel<3>, B, smem, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H);
     return launch_generic(bwd_generic_kernel<4>, B, smem, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H);
 }

@@ -155,7 +155,7 @@ def _rnn_forward_impl(x, w_ih, w_hh, b_ih, b_hh, h0, c0, cell):
     N = S * B
     x2 = _f32c(x.detach()).view(N, Hin)
     w_ih, w_hh, b_ih, b_hh = _f32c(w_ih.detach()), _f32c(w_hh.detach()), _f32c(b_ih.detach()), _f32c(b_hh.detach())
-    # [N, G*H] = x W_ih^T + b_ih on wgmma (3xTF32); shapes outside the kernel's (G*H % 128, Hin % 32) raise DC_EUNSUPPORTED
+    # [N, G*H] = x W_ih^T + b_ih on wgmma (3xTF32); shapes outside the kernel's (G*H % 32, Hin % 32) raise DC_EUNSUPPORTED
     gates = gemm_tf32x3(x2, w_ih, b_ih)
     ybuf = torch.empty((S + 1, B, H), dtype=torch.float32, device=x.device)
     cbuf = torch.empty((S + 1, B, H), dtype=torch.float32, device=x.device)
@@ -371,7 +371,7 @@ class LinearTC(torch.autograd.Function):
 
 
 def linear(x, weight, bias=None, relu=False):
-    """Dense layer on the wgmma 3xTF32 GEMM (out features % 128 == 0, in features % 32 == 0; CUDA tensors only)."""
+    """Dense layer on the wgmma 3xTF32 GEMM (out features % 32 == 0, in features % 32 == 0; CUDA tensors only)."""
     _need_cuda(x, weight, bias)
     return LinearTC.apply(x, weight, bias, relu)
 
@@ -380,7 +380,7 @@ _wgrad_ws = {}
 
 
 def gemm_wgrad_supported(T, No, Ni):
-    return T > 0 and No % 128 == 0 and Ni % 128 == 0
+    return T > 0 and No % 32 == 0 and Ni % 32 == 0
 
 
 def gemm_wgrad_tf32x3(dy, x, want_bias=True, dw_out=None, db_out=None, accumulate=False):

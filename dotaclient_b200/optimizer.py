@@ -1058,7 +1058,7 @@ def build_arg_parser():
     p.add_argument("-l", "--log", dest="log_level", help="Set the logging level",
                    choices=['DEBUG', 'INFO', 'WARNING', 'ERROR', 'CRITICAL'], default='INFO')
     p.add_argument("--run-local", type=bool, help="set to true to run locally (not using GCP)", default=False)
-    p.add_argument("--hidden-size", type=int, help="recurrent width (reference: 256)", default=256)
+    p.add_argument("--hidden-size", type=int, help="recurrent width, a multiple of 32 (reference: 256)", default=256)
     p.add_argument("--cell", type=str, choices=['gru', 'lstm'], help="recurrent cell (reference: gru)", default='gru')
     return p
 

@@ -7,6 +7,11 @@ unit encoder through the fused encoder kernel when it is available.  Two additio
 keyword-only so ``Policy()`` is the reference's network: ``hidden_size`` (reference: 256) and
 ``cell`` ('gru' = the reference's ``nn.GRU``, 'lstm' = the cell BASELINE.json names).
 
+Every ``hidden_size`` that is a multiple of 32 runs on the GPU: 128, 256 and the other multiples of 128 on their
+dedicated recurrence kernels, the rest (64, 96, 160, 192, ...) on the generic ones.  Any width constructs, so that a
+``state_dict`` of any width can be held or converted on the CPU; the first CUDA forward of another width raises the
+GEMM's ``DC_EUNSUPPORTED`` error.
+
 CUDA only: calling ``forward`` with CPU tensors raises (there is no CPU fallback).
 """
 import logging

@@ -77,7 +77,7 @@ int dc_gae_scan(const float *rewards, int n_sub, const float *values, const int6
  * Kernels by width: H = 128 one-SM weight-resident FFMA kernels; H = 256 (the reference's width) 8-CTA-cluster
  * weight-resident wgmma 3xTF32 kernels; other multiples of 128 (384, 512, ...) step-wise kernels: per step a split-K
  * wgmma 3xTF32 GEMM over all SMs that streams W_hh from L2, then a gate kernel; any other H % 4 == 0 a generic kernel
- * that streams W_hh from L2.
+ * that streams W_hh from L2 (through the Python layers: every other H % 32 == 0, e.g. 64, 96, 160, 192).
  * Backward (consumes what forward left behind)
  *   gates  in: activated gates   out: dL/d(gates pre-activation wrt the i2h branch) = dgi
  *   cbuf   LSTM: unchanged.  GRU: slot t+1 out = dL/d(W_hn h + b_hn) (the n-gate part of dgh)
@@ -94,9 +94,11 @@ int dc_rnn_seq_bwd(int cell, float *gates, const float *w_hh, const float *ybuf,
 /* ---- fp32-accurate tensor-core GEMM (wgmma, 3xTF32) ---------------------------------------
  * C[M,N] = A[M,K] * B[N,K]^T (+ bias[N]) (ReLU if relu != 0); row-major fp32 with leading dimensions lda/ldb/ldc.
  * Replaces the library SGEMM of the input-to-hidden projection inside nn.GRU / nn.LSTM (policy.py:66,141:
- * gates = x W_ih^T + b_ih) and of the other 128-aligned dense layers (policy.py:101-126,138).  Each product is
+ * gates = x W_ih^T + b_ih) and of the other dense layers (policy.py:101-126,138).  Each product is
  * evaluated as a_lo*b_hi + a_hi*b_lo + a_hi*b_hi with tf32 hi/lo splits (fp32-level accuracy, ~1e-6 relative).
- * Requirements: N % 128 == 0, K % 32 == 0, 16-byte aligned pointers, ld* % 4 == 0 (dc_gemm_tf32x3_supported).
+ * Requirements: N % 32 == 0, K % 32 == 0, 16-byte aligned pointers, ld* % 4 == 0 (dc_gemm_tf32x3_supported).  With N % 128 != 0
+ * the last 128-column tile is partly filled; nothing is stored past column N.  So every layer of a Policy whose width H is a
+ * multiple of 32 has a GEMM here (N or K = H, 3H, 4H, 128, 896).
  */
 int dc_gemm_tf32x3_supported(int64_t M, int N, int K);
 int dc_gemm_tf32x3(const float *A, int lda, const float *B, int ldb, const float *bias, float *C, int ldc,
@@ -105,7 +107,8 @@ int dc_gemm_tf32x3(const float *A, int lda, const float *B, int ldb, const float
 /* Weight gradient of the same layers: dW[No,Ni] (+)= dY[T,No]^T X[T,Ni], db[No] (+)= column sums of dY (NULL = skip).
  * Replaces the dW/db part of AddmmBackward for those layers (loss.backward(), optimizer.py:672).  Contraction over the
  * token dimension (operands transposed to K-major on the way into shared memory), split-K over the SMs, deterministic two-stage reduction.
- * Requirements: No % 128 == 0, Ni % 128 == 0; workspace of dc_gemm_wgrad_workspace_bytes(No, Ni) bytes. */
+ * Requirements: No % 32 == 0, Ni % 32 == 0; workspace of dc_gemm_wgrad_workspace_bytes(No, Ni) bytes (one full 128 x 128
+ * partial per output tile and split, tiles = ceil(No/128) * ceil(Ni/128)). */
 size_t dc_gemm_wgrad_workspace_bytes(int No, int Ni);
 int dc_gemm_wgrad_tf32x3(const float *dY, int ldy, const float *X, int ldx, int64_t T, int No, int Ni,
                          float *dW, int ldw, float *db, int accumulate, void *workspace, dc_stream_t stream);
