@@ -9,7 +9,6 @@
 //   unit_basic reduce   fixed-order sum of the dW_b / db_b partials of the fused data-gradient kernel (gemm_tf32x3.cu)
 //   target_unit_q_fwd   logits[n,u] = <att[n] W_g, basic[n,u]> + <att[n], b_g>: the head WITHOUT the [N,40,128] embedding
 //   target_unit_q_bwd   s_g[n] = sum_u dlogits[n,u] basic_g[n,u] (-> d_att and the head's share of dW_g as token-level GEMMs)
-//   target_unit_fwd/bwd the dense form on a materialised embedding (policy.py:152-153), for callers that keep one
 // The max-pool over a group's units lives in the embedding GEMM's epilogue (dc_gemm_unit_max) and its backward routing is
 // generated inside the weight- / data-gradient kernels (dc_unit_wgrad_routed, dc_unit_dgrad_fused), all in gemm_tf32x3.cu.
 //
@@ -187,63 +186,6 @@ __global__ void __launch_bounds__(256) env_bwd_reduce_kernel(const float *__rest
     }
 }
 
-// ---- target-unit attention head ---------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreadsE) target_unit_fwd_kernel(const float *__restrict__ att,
-                                                                    const float *__restrict__ ue,
-                                                                    float *__restrict__ logits, int64_t N) {
-    const int lane = threadIdx.x & 31;
-    const int64_t n = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
-    if (n >= N) return;
-    const float4 a = __ldg(reinterpret_cast<const float4 *>(att + n * kC) + lane);
-    const float4 *row = reinterpret_cast<const float4 *>(ue + n * kMaxUnits * kC) + lane;
-    float mine = 0.f;                                             // lane u keeps logit u (u < 32), lanes 0..7 also u+32
-    float mine_hi = 0.f;
-#pragma unroll 8
-    for (int u = 0; u < kMaxUnits; ++u) {
-        const float4 v = __ldg(row + u * (kC / 4));
-        float d = v.x * a.x + v.y * a.y + v.z * a.z + v.w * a.w;
-        d = dc_warp_sum(d);
-        if (u < 32) { if (lane == u) mine = d; } else { if (lane == u - 32) mine_hi = d; }
-    }
-    logits[n * kMaxUnits + lane] = mine;
-    if (lane < kMaxUnits - 32) logits[n * kMaxUnits + 32 + lane] = mine_hi;
-}
-
-__global__ void __launch_bounds__(kThreadsE) target_unit_bwd_kernel(const float *__restrict__ dlogits,
-                                                                    const float *__restrict__ att,
-                                                                    const float *__restrict__ ue,
-                                                                    float *__restrict__ d_att, float *__restrict__ d_ue,
-                                                                    int64_t N) {
-    const int lane = threadIdx.x & 31;
-    const int64_t n = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
-    if (n >= N) return;
-    const float g_lo = dlogits[n * kMaxUnits + lane];
-    const float g_hi = lane < kMaxUnits - 32 ? dlogits[n * kMaxUnits + 32 + lane] : 0.f;
-    const bool any = __any_sync(0xffffffffu, g_lo != 0.f || g_hi != 0.f);
-    float4 *drow = d_ue ? reinterpret_cast<float4 *>(d_ue + n * kMaxUnits * kC) + lane : nullptr;   // NULL: d_att only
-    float4 da = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (!any) {                                                   // head unused on this token: exact zeros, no reads
-        if (drow) {
-#pragma unroll 8
-            for (int u = 0; u < kMaxUnits; ++u) drow[u * (kC / 4)] = da;
-        }
-    } else {
-        const float4 a = __ldg(reinterpret_cast<const float4 *>(att + n * kC) + lane);
-        const float4 *row = reinterpret_cast<const float4 *>(ue + n * kMaxUnits * kC) + lane;
-#pragma unroll 8
-        for (int u = 0; u < kMaxUnits; ++u) {
-            const float g = __shfl_sync(0xffffffffu, u < 32 ? g_lo : g_hi, u & 31);
-            const float4 v = __ldg(row + u * (kC / 4));
-            da.x = fmaf(g, v.x, da.x); da.y = fmaf(g, v.y, da.y); da.z = fmaf(g, v.z, da.z); da.w = fmaf(g, v.w, da.w);
-            if (drow) drow[u * (kC / 4)] = make_float4(g * a.x, g * a.y, g * a.z, g * a.w);
-        }
-    }
-    *(reinterpret_cast<float4 *>(d_att + n * kC) + lane) = da;
-}
-
-int grid_rows(int64_t rows_per_block_iter_unused) { (void)rows_per_block_iter_unused; return 4 * dc_sm_count(); }
-
-
 // ---- target-unit head without the unit embedding ------------------------------------------------------------------------
 // logits[n,u] = <att[n], W_g basic[n,u] + b_g> = <att[n] W_g, basic[n,u]> + <att[n], b_g> (policy.py:144-153; algebra pinned in
 // tests/test_oracle.py): with q[n, g*128 + j] = (att W_g)[n, j] and q[n, 768 + g] = <att[n], b_g> from ONE small GEMM over tokens,
@@ -323,7 +265,7 @@ extern "C" int dc_unit_basic_fwd(const float *units, const float *w_b, const flo
                                  dc_stream_t stream) {
     DC_REQUIRE(units && w_b && b_b && basic && R > 0, DC_EINVAL, "dc_unit_basic_fwd: bad arguments");
     DC_REQUIRE(((uintptr_t)basic & 15) == 0, DC_EINVAL, "dc_unit_basic_fwd: output must be 16-byte aligned");
-    unit_basic_fwd_kernel<<<grid_rows(0), kThreadsE, 0, dc_cu_stream(stream)>>>(units, w_b, b_b, basic, R);
+    unit_basic_fwd_kernel<<<4 * dc_sm_count(), kThreadsE, 0, dc_cu_stream(stream)>>>(units, w_b, b_b, basic, R);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -340,7 +282,7 @@ extern "C" int dc_env_fwd(const float *env, const float *w_e, const float *b_e, 
                           dc_stream_t stream) {
     DC_REQUIRE(env && w_e && b_e && out && N > 0 && ld_out >= kC && ld_out % 4 == 0 && ((uintptr_t)out & 15) == 0, DC_EINVAL,
                "dc_env_fwd: bad arguments");
-    env_fwd_kernel<<<grid_rows(0), kThreadsE, 0, dc_cu_stream(stream)>>>(env, w_e, b_e, out, ld_out, N);
+    env_fwd_kernel<<<4 * dc_sm_count(), kThreadsE, 0, dc_cu_stream(stream)>>>(env, w_e, b_e, out, ld_out, N);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -358,14 +300,6 @@ extern "C" int dc_env_bwd(const float *d_out, const float *out, int ld, const fl
     env_bwd_kernel<<<blocks, kThreadsE, 0, st>>>(d_out, out, ld, env, N, partial);
     DC_LAUNCH_OK();
     env_bwd_reduce_kernel<<<(kC * (kEnvIn + 1) + 31) / 32, 256, 0, st>>>(partial, blocks, dw_e, db_e);
-    DC_LAUNCH_OK();
-    return DC_OK;
-}
-
-extern "C" int dc_target_unit_fwd(const float *att, const float *ue, float *logits, int64_t N, dc_stream_t stream) {
-    DC_REQUIRE(att && ue && logits && N > 0, DC_EINVAL, "dc_target_unit_fwd: bad arguments");
-    DC_REQUIRE((((uintptr_t)att | (uintptr_t)ue) & 15) == 0, DC_EINVAL, "dc_target_unit_fwd: alignment");
-    target_unit_fwd_kernel<<<(unsigned)((N + kWarps - 1) / kWarps), kThreadsE, 0, dc_cu_stream(stream)>>>(att, ue, logits, N);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -394,17 +328,6 @@ extern "C" int dc_target_unit_q_bwd(const float *dlogits, const float *const bas
     }
     DC_REQUIRE(((uintptr_t)s & 15) == 0, DC_EINVAL, "dc_target_unit_q_bwd: alignment");
     target_unit_q_bwd_kernel<<<(unsigned)((N + kWarps - 1) / kWarps), kThreadsE, 0, dc_cu_stream(stream)>>>(dlogits, bp, s, ld_s, N);
-    DC_LAUNCH_OK();
-    return DC_OK;
-}
-
-extern "C" int dc_target_unit_bwd(const float *dlogits, const float *att, const float *ue, float *d_att, float *d_ue,
-                                  int64_t N, dc_stream_t stream) {
-    DC_REQUIRE(dlogits && att && ue && d_att && N > 0, DC_EINVAL, "dc_target_unit_bwd: bad arguments");
-    DC_REQUIRE((((uintptr_t)att | (uintptr_t)ue | (uintptr_t)d_att | (uintptr_t)d_ue) & 15) == 0, DC_EINVAL,
-               "dc_target_unit_bwd: alignment");
-    target_unit_bwd_kernel<<<(unsigned)((N + kWarps - 1) / kWarps), kThreadsE, 0, dc_cu_stream(stream)>>>(dlogits, att, ue,
-                                                                                                         d_att, d_ue, N);
     DC_LAUNCH_OK();
     return DC_OK;
 }

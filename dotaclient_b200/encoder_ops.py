@@ -122,8 +122,8 @@ class UnitEncoder(torch.autograd.Function):
                                "dc_gemm_unit_max")
             elif g < 5:                               # one unit: the embedding IS the maximum -> straight into its slot
                 with PROFILE.span("gemm_tf32x3", 1, 4 * (2 * R * C + C * C)):
-                    _lib.check(lib.dc_gemm_tf32x3_blocked(basic.data_ptr(), C, 0, 0, weights[g].data_ptr(), C, biases[g].data_ptr(),
-                                                          _ptr(xcat, (g + 1) * C), XCAT, 0, 0, R, C, C, 0, st), "dc_gemm_tf32x3_blocked")
+                    _lib.check(lib.dc_gemm_tf32x3(basic.data_ptr(), C, weights[g].data_ptr(), C, biases[g].data_ptr(),
+                                                  _ptr(xcat, (g + 1) * C), XCAT, R, C, C, 0, st), "dc_gemm_tf32x3")
             basics.append(basic)
         link["basics"], link["weights"], link["biases"] = basics, weights, biases
         ctx.N = N

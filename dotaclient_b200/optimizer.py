@@ -505,68 +505,14 @@ class DotaOptimizer:
         return self._rollout_q.get()
 
     def experiences_from_rollout(self, data):
-        """Rollout -> list of ``Sequence`` (:328-430), in ONE padded pass instead of a per-chunk loop.
+        """Rollout -> list of ``Sequence`` (:328-430): ``experiences_from_rollouts`` on a batch of one.
 
         Running the recurrence over the whole zero-padded rollout from the zero state is exactly the
         reference's chunk-by-chunk forward with carried hidden (:340,384-385); the hidden state entering
         chunk i is read back from the recurrence's state buffer.  Old log-probs come from the fused
         selected-log-prob kernel, advantages/returns from the GAE scan kernel (padding inside the scan).
         """
-        S, dev = self.seq_len, self.device
-        L = data['rewards'].shape[0]
-        n_chunks = (L + S - 1) // S
-        Lp = n_chunks * S
-
-        def padded(t):
-            t = torch.as_tensor(t).to(dev)
-            if Lp == L:
-                return t
-            out = torch.zeros((Lp,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)      # :367-382
-            out[:L] = t
-            return out
-
-        obs = {k: padded(v) for k, v in data['observations'].items()}
-        masks = {k: padded(v).bool() for k, v in data['masks'].items()}
-        actions = {k: padded(v).bool() for k, v in data['actions'].items()}
-        rewards_np = np.asarray(data['rewards'], dtype=np.float32)
-        if Lp != L:
-            rewards_np = np.pad(rewards_np, ((0, Lp - L), (0, 0)), mode='constant')
-        rewards = torch.from_numpy(rewards_np).to(dev)
-        with torch.no_grad():
-            pol = self.policy_base
-            x, unit_embedding = pol._encode(obs['env'].unsqueeze(1),
-                                            [obs[k].unsqueeze(1) for k in Policy.INPUT_KEYS[1:]])
-            hidden = pol.init_hidden()
-            hidden = tuple(h.to(dev) for h in hidden) if isinstance(hidden, tuple) else hidden.to(dev)
-            r = pol.rnn
-            h0 = hidden[0][0] if pol.cell == "lstm" else hidden[0]
-            c0 = hidden[1][0] if pol.cell == "lstm" else None
-            ybuf, cbuf = ops.rnn_forward_states(x.contiguous(), r.weight_ih_l0, r.weight_hh_l0, r.bias_ih_l0,
-                                                r.bias_hh_l0, h0, c0, pol.cell)
-            logits, values = pol._heads(ybuf[1:], unit_embedding)
-            keys = ops.HEAD_KEYS
-            old_logp = ops.selected_logp([logits[k] for k in keys], [masks[k] for k in keys],
-                                         [actions[k] for k in keys])                         # :387-390
-            seg = torch.tensor([0, Lp], dtype=torch.int64, device=dev)
-            adv, ret = ops.gae_scan(rewards, values.reshape(-1), seg, gamma=GAMMA, lam=LAMBDA)   # :417-421
-        sequences = []
-        for i in range(n_chunks):
-            sl = slice(i * S, (i + 1) * S)
-            if pol.cell == "lstm":
-                hid = (ybuf[i * S].unsqueeze(0), cbuf[i * S].unsqueeze(0))
-            else:
-                hid = ybuf[i * S].unsqueeze(0)
-            seq = Sequence(game_id=data.get('game_id'), weight_version=data.get('weight_version'),
-                           team_id=data.get('team_id'),
-                           observations={k: v[sl] for k, v in obs.items()},
-                           actions={k: v[sl] for k, v in actions.items()},
-                           masks={k: v[sl] for k, v in masks.items()},
-                           values=values[sl].reshape(1, S, 1), rewards=rewards_np[sl], hidden=hid,
-                           old_logp=old_logp[sl])
-            seq.advantages = adv[sl]
-            seq.returns = ret[sl]
-            sequences.append(seq)
-        return sequences
+        return self.experiences_from_rollouts([data])[0]
 
     def _prepare_rollouts(self, datas):
         """The batched no-grad half of an iteration (SURVEY.md 8(f)2): all rollouts become the batch dimension of ONE
@@ -632,8 +578,8 @@ class DotaOptimizer:
                     adv_c=adv_c, ret_c=ret_c, ybuf=ybuf, cbuf=cbuf, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same)
 
     def experiences_from_rollouts(self, datas):
-        """``experiences_from_rollout`` (:328-430) for all rollouts of an iteration at once: per rollout the result equals the
-        per-rollout path -- own padding to a multiple of ``seq_len``, own terminal bootstrap, chunks beyond its padded
+        """``experiences_from_rollout`` (:328-430) for all rollouts of an iteration at once: per rollout the result equals a
+        batch of one -- own padding to a multiple of ``seq_len``, own terminal bootstrap, chunks beyond its padded
         length are not emitted -- but the work is one batched pass instead of ``R`` batch-1 passes."""
         S, pol = self.seq_len, self.policy_base
         p = self._prepare_rollouts(datas)

@@ -113,23 +113,10 @@ size_t dc_gemm_wgrad_workspace_bytes(int No, int Ni);
 int dc_gemm_wgrad_tf32x3(const float *dY, int ldy, const float *X, int ldx, int64_t T, int No, int Ni,
                          float *dW, int ldw, float *db, int accumulate, void *workspace, dc_stream_t stream);
 
-/* Two-level row addressing variants: row r of A / C / dY lives at (r / rows_per_block) * block_stride +
- * (r % rows_per_block) * ld (floats); rows_per_block = 0 selects the plain form.  They let the per-group GEMMs read
- * and write one unit group of the [N, 40, 128] unit-embedding tensor in place, so the torch.cat of policy.py:130-131
- * (and its backward split) never materialises. */
-int dc_gemm_tf32x3_blocked(const float *A, int lda, int64_t a_rows_per_block, int64_t a_block_stride,
-                           const float *B, int ldb, const float *bias, float *C, int ldc,
-                           int64_t c_rows_per_block, int64_t c_block_stride, int64_t M, int N, int K,
-                           int relu, dc_stream_t stream);
-int dc_gemm_wgrad_tf32x3_blocked(const float *dY, int ldy, int64_t y_rows_per_block, int64_t y_block_stride,
-                                 const float *X, int ldx, int64_t T, int No, int Ni, float *dW, int ldw,
-                                 float *db, int accumulate, void *workspace, dc_stream_t stream);
-
 /* ---- unit encoder / target-unit head: the bandwidth-bound pieces ------------------------------
- * (policy.py:99-136,144-153; the 128x128 embedding GEMMs themselves are dc_gemm_tf32x3*)
+ * (policy.py:99-136,144-153; the 128x128 embedding GEMMs themselves are dc_gemm_tf32x3 for the 1-unit groups and
+ * dc_gemm_unit_max for the others)
  *   dc_unit_basic_fwd   basic[R,128] = relu(units[R,12] W_b^T + b_b)            policy.py:100,105,...
- *   dc_target_unit_fwd  logits[n,u] = <att[n,:], ue[n,u,:]>, ue = [N,40,128]    policy.py:152-153
- *   dc_target_unit_bwd  d_att[n,:] = sum_u dlogits[n,u] ue[n,u,:];  d_ue[n,u,:] = dlogits[n,u] att[n,:]
  */
 int dc_unit_basic_fwd(const float *units, const float *w_b, const float *b_b, float *basic, int64_t R,
                       dc_stream_t stream);
@@ -172,9 +159,6 @@ int dc_unit_dgrad_fused(const float *d_xmax, const float *d_xmax2, int ld_dx, co
                         int ld_dl, const float *att, const float *w_t, const float *units, const float *w_b,
                         const float *b_b, int64_t n_tokens, int n_units, float *dw_b, float *db_b, int accumulate,
                         void *workspace, dc_stream_t stream);
-int dc_target_unit_fwd(const float *att, const float *ue, float *logits, int64_t N, dc_stream_t stream);
-int dc_target_unit_bwd(const float *dlogits, const float *att, const float *ue, float *d_att, float *d_ue,
-                       int64_t N, dc_stream_t stream);
 
 /* ---- fused PPO loss + gradient ----------------------------------------------------------
  * Replaces optimizer.py:587-589 (advantage normalisation) and :621-665 (masked log-softmax x5,

@@ -122,26 +122,6 @@ def test_unit_encoder_with_target_unit_head(lead, use_head):
         torch.testing.assert_close(att_d.grad.cpu(), att.grad, rtol=1e-4, atol=1e-4)
 
 
-def test_dense_target_unit_kernels_through_the_c_abi():
-    """dc_target_unit_fwd / _bwd (the dense form for callers that keep a materialised embedding): logits = att . ue^T."""
-    from dotaclient_b200 import _lib
-    lib = _lib.load()
-    g = torch.Generator().manual_seed(3)
-    N = 77
-    att, ue = torch.randn(N, 128, generator=g), torch.randn(N, 40, 128, generator=g)
-    go = torch.randn(N, 40, generator=g)
-    go[::3] = 0
-    d = torch.device("cuda", 0)
-    a, u, gd = att.to(d), ue.to(d), go.to(d)
-    logits = torch.empty(N, 40, device=d)
-    _lib.check(lib.dc_target_unit_fwd(a.data_ptr(), u.data_ptr(), logits.data_ptr(), N, _lib.stream_ptr()), "fwd")
-    torch.testing.assert_close(logits.cpu(), torch.einsum("nc,nuc->nu", att, ue), rtol=1e-5, atol=1e-5)
-    d_att, d_ue = torch.empty_like(a), torch.empty_like(u)
-    _lib.check(lib.dc_target_unit_bwd(gd.data_ptr(), a.data_ptr(), u.data_ptr(), d_att.data_ptr(), d_ue.data_ptr(), N, _lib.stream_ptr()), "bwd")
-    torch.testing.assert_close(d_att.cpu(), torch.einsum("nu,nuc->nc", go, ue), rtol=1e-5, atol=1e-5)
-    torch.testing.assert_close(d_ue.cpu(), go.unsqueeze(-1) * att.unsqueeze(1), rtol=1e-6, atol=1e-6)
-
-
 def _encoder_check():
     import importlib.util
     import os

@@ -112,34 +112,6 @@ def main():
             print("dgrad fused %2d units %-12s       rows=%8d | %.3f ms (%.1f TF/s 3xTF32, %s)"
                   % (n_u, "with head" if head else "without head", R, t, flops / t / 1e9, _floor(flops, bytes_, t)))
 
-    # the unit-embedding GEMMs as the encoder issues them: one unit group (16 of 40 rows per token) of [N, 40, 128] in place
-    N_tok, n_u, C = 131072, 16, 128
-    R = N_tok * n_u
-    ue = torch.empty(N_tok, 40, C, device=d)
-    basic = torch.randn(R, C, device=d)
-    w = torch.randn(C, C, device=d) * 0.1
-    bias = torch.randn(C, device=d)
-    off = 6 * C * 4
-    t_c = timeit(lambda: _lib.check(lib.dc_gemm_tf32x3_blocked(basic.data_ptr(), C, 0, 0, w.data_ptr(), C, bias.data_ptr(),
-                                                              ue.data_ptr() + off, C, n_u, 40 * C, R, C, C, 0, st), "gemm"))
-    t_a = timeit(lambda: _lib.check(lib.dc_gemm_tf32x3_blocked(ue.data_ptr() + off, C, n_u, 40 * C, w.data_ptr(), C, None,
-                                                              basic.data_ptr(), C, 0, 0, R, C, C, 0, st), "gemm"))
-    ref = torch.addmm(bias, basic, w.t()).view(N_tok, n_u, C)
-    _lib.check(lib.dc_gemm_tf32x3_blocked(basic.data_ptr(), C, 0, 0, w.data_ptr(), C, bias.data_ptr(), ue.data_ptr() + off, C, n_u,
-                                          40 * C, R, C, C, 0, st), "gemm")
-    err = (ue[:, 6:22] - ref).abs().max().item()
-    print("unit group 16/40: C blocked (fwd) %.3f ms | A blocked (dgrad) %.3f ms | %.0f / %.0f GB/s | max|diff| %.2e"
-          % (t_c, t_a, 8.0 * R * C / t_c / 1e6, 8.0 * R * C / t_a / 1e6, err))
-
-    # weight gradient of the same group: dW = d_ue_g^T basic (dY two-level rows, X plain), db = column sums
-    ws = torch.empty(int(lib.dc_gemm_wgrad_workspace_bytes(C, C)), dtype=torch.uint8, device=d)
-    dw, db = torch.empty(C, C, device=d), torch.empty(C, device=d)
-    t_w = timeit(lambda: _lib.check(lib.dc_gemm_wgrad_tf32x3_blocked(ue.data_ptr() + off, C, n_u, 40 * C, basic.data_ptr(), C, R, C, C,
-                                                                    dw.data_ptr(), C, db.data_ptr(), 0, ws.data_ptr(), st), "wgrad"))
-    ref_w = (ue[:, 6:22].reshape(R, C).double().t() @ basic.double()).float()
-    print("unit group 16/40 weight gradient: %.3f ms | %.0f GB/s | max|diff|/max|ref| %.2e"
-          % (t_w, 8.0 * R * C / t_w / 1e6, ((dw - ref_w).abs().max() / ref_w.abs().max()).item()))
-
 
 if __name__ == "__main__":
     main()
