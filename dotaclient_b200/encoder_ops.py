@@ -60,7 +60,7 @@ def _wgrad_workspace(No, Ni, device):
 # max-pool routing R (d_xmax[n,:] to the arg-max unit of every channel; arrives with the pre-rnn gradient, after the recurrence).
 # TargetUnit parks (dlogits, att, s) in the `link` cell the two Functions of one graph share; UnitEncoder.backward then needs no
 # dense [N, 40, 128] tensor at all:
-#   dW_g  = R^T basic_g  (dc_unit_wgrad_routed: R generated in the A producer)  +  att^T s_g   (one token-level GEMM for all groups,
+#   dW_g  = R^T basic_g  (dc_unit_wgrad_routed: R generated in the dY^T producer)  +  att^T s_g   (one token-level GEMM for all groups,
 #           s_g = sum_u dlogits_u basic_u from dc_target_unit_q_bwd; its bias block gives the head's share of db_g)
 #   dW_b += (relu'(.) (R + dlogits x att) W_g)^T units   (dc_unit_dgrad_fused: d_emb generated in the producers, the ReLU mask
 #           recomputed and dW_b reduced in the epilogue) -- d_basic never exists either.
