@@ -50,6 +50,7 @@ SIGNATURES = {
 PPO_WORKSPACE_BYTES = 512
 FINISH_WORKSPACE_BYTES = 1024
 LOSS_SLOTS = 16
+MAX_PARAM_TENSORS = 96      # kMaxSeg of csrc/grad_finish.cu: parameter tensors dc_grad_flags / dc_grad_finish can handle
 
 _lib = None
 

@@ -179,6 +179,24 @@ def rnn_forward_states(x_tm, w_ih, w_hh, b_ih, b_hh, h0, c0, cell):
     return ybuf, cbuf
 
 
+def rnn_stack_forward_states(x_tm, layers, h0, c0, cell):
+    """``rnn_forward_states`` through a stack of layers: ``layers`` = [(w_ih, w_hh, b_ih, b_hh)] per layer, h0 / c0
+    ``[L, B, H]`` (c0 None for the GRU).  Layer k reads layer k-1's ``ybuf[1:]`` view.  Returns the per-layer lists of
+    ybuf and cbuf ``[S+1, B, H]``: the hidden state entering step t of layer k is ``ybufs[k][t]``."""
+    ybufs, cbufs, x = [], [], x_tm
+    for k, (w_ih, w_hh, b_ih, b_hh) in enumerate(layers):
+        ybuf, cbuf = rnn_forward_states(x, w_ih, w_hh, b_ih, b_hh, h0[k], None if c0 is None else c0[k], cell)
+        ybufs.append(ybuf)
+        cbufs.append(cbuf)
+        x = ybuf[1:]
+    return ybufs, cbufs
+
+
+def stack_layers(states):
+    """Per-layer ``[B, H]`` states -> torch's ``[L, B, H]`` (a view, no copy, for a single layer)."""
+    return states[0].unsqueeze(0) if len(states) == 1 else torch.stack(states)
+
+
 class RnnSequence(torch.autograd.Function):
     """Time-major GRU/LSTM layer: i2h GEMM (wgmma 3xTF32) + hand-written recurrence kernels.
 

@@ -338,11 +338,18 @@ class DotaOptimizer:
     SPEED_KEY = 'steps per s'
     ADAM_BETAS = (0.9, 0.999)       # torch.optim.Adam defaults (:275)
     ADAM_EPS = 1e-8
+    # Policy has 30 parameter tensors outside the recurrent core and 4 per recurrent layer; the fused gradient-finish
+    # kernel (csrc/grad_finish.cu) keeps per-tensor slots for at most _lib.MAX_PARAM_TENSORS = 96 of them -> 16 layers.
+    MAX_LAYERS = (_lib.MAX_PARAM_TENSORS - 30) // 4
 
     def __init__(self, rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len,
                  learning_rate, checkpoint, pretrained_model, mq_prefetch_count, log_dir,
-                 entropy_coef, vf_coef, run_local, *, hidden_size=256, cell="gru", mq=None, iterations=100000,
-                 rollout_prefetch=0):
+                 entropy_coef, vf_coef, run_local, *, hidden_size=256, cell="gru", num_layers=1, mq=None,
+                 iterations=100000, rollout_prefetch=0):
+        if not 1 <= num_layers <= self.MAX_LAYERS:
+            raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
+                             "handles at most %d parameter tensors, 30 + 4 per layer)"
+                             % (num_layers, self.MAX_LAYERS, _lib.MAX_PARAM_TENSORS))
         self.rmq_host, self.rmq_port = rmq_host, rmq_port
         self.epochs = epochs
         self.min_seq_per_epoch = min_seq_per_epoch
@@ -363,7 +370,7 @@ class DotaOptimizer:
 
         with torch.random.fork_rng(devices=[]):     # :34 seeds torch with 7 at import and Policy() init depends on it;
             torch.manual_seed(7)                    # forked so that constructing an optimizer leaves the caller's RNG alone
-            self.policy_base = Policy(hidden_size=hidden_size, cell=cell)
+            self.policy_base = Policy(hidden_size=hidden_size, cell=cell, num_layers=num_layers)
 
         if self.checkpoint:
             logger.info('Checkpointing to: {}'.format(self.log_dir))
@@ -379,7 +386,10 @@ class DotaOptimizer:
             if pretrained_model is not None:
                 self.iteration_start = self.iteration_from_model_filename(filename=pretrained_model) + 1   # :253
         if pretrained_model is not None:
-            self.policy_base.load_state_dict(torch.load(pretrained_model, map_location='cpu'), strict=False)  # :263-266
+            # strict=False as the reference (:263-266): a checkpoint with fewer recurrent layers (e.g. a 1-layer model
+            # loaded into num_layers=2) sets the layers it has and leaves rnn.*_l1 ... at their seeded initial values; its
+            # Adam moments (keyed by parameter index) do not fit the new layout and are not restored (below)
+            self.policy_base.load_state_dict(torch.load(pretrained_model, map_location='cpu'), strict=False)
 
         self.policy_base.to(self.device)
         self.flat = FlatParameterSpace(self.policy_base, self.device)
@@ -397,7 +407,10 @@ class DotaOptimizer:
             adam_file = os.path.join(os.path.dirname(pretrained_model), self.ADAM_FILENAME_FMT % (self.iteration_start - 1))
             if os.path.isfile(adam_file):
                 logger.info('Restoring Adam state from {}'.format(adam_file))
-                self.optimizer.load_state_dict(torch.load(adam_file, map_location='cpu'))
+                try:
+                    self.optimizer.load_state_dict(torch.load(adam_file, map_location='cpu'))
+                except ValueError as e:     # e.g. a 1-layer run's moments next to the weights loaded into num_layers=2
+                    logger.warning('Not restoring Adam state from %s (%s): the moments start from zero', adam_file, e)
         self._sync_resume_state()
         self._n_actions = torch.zeros(8, dtype=torch.int32, device=self.device)
         self._n_actions[VALUE_SLOT] = 1 if vf_coef > 0 else 0
@@ -555,12 +568,13 @@ class DotaOptimizer:
             rewards_np[i, :Ls[i]] = np.asarray(d['rewards'], dtype=np.float32)
         with torch.no_grad():
             x, unit_embedding = pol._encode(obs['env'], [obs[k] for k in Policy.INPUT_KEYS[1:]])
-            r = pol.rnn
-            h0 = torch.zeros((R, pol.hidden_size), dtype=torch.float32, device=dev)
+            n_layers = pol.num_layers
+            h0 = torch.zeros((n_layers, R, pol.hidden_size), dtype=torch.float32, device=dev)
             c0 = torch.zeros_like(h0) if pol.cell == "lstm" else None
-            ybuf, cbuf = ops.rnn_forward_states(x.contiguous(), r.weight_ih_l0, r.weight_hh_l0, r.bias_ih_l0, r.bias_hh_l0,
-                                                h0, c0, pol.cell)
-            logits, values = pol._heads(ybuf[1:], unit_embedding)
+            # every layer's state buffers are kept: the state entering chunk j of rollout i is ybufs[k][j*S, i] per layer k
+            ybufs, cbufs = ops.rnn_stack_forward_states(x.contiguous(), [pol.rnn.layer(k) for k in range(n_layers)],
+                                                        h0, c0, pol.cell)
+            logits, values = pol._heads(ybufs[-1][1:], unit_embedding)
             keys = ops.HEAD_KEYS
             old_logp = ops.selected_logp([logits[k] for k in keys], [masks[k] for k in keys],
                                          [actions[k] for k in keys]).view(Lmax, R, 5)        # :387-390
@@ -575,7 +589,7 @@ class DotaOptimizer:
             seg = torch.tensor(np.concatenate([[0], np.cumsum(Lps)]), dtype=torch.int64, device=dev)
             adv_c, ret_c = ops.gae_scan(rew_c, vals_c, seg, gamma=GAMMA, lam=LAMBDA)          # :417-421
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
-                    adv_c=adv_c, ret_c=ret_c, ybuf=ybuf, cbuf=cbuf, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same)
+                    adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same)
 
     def experiences_from_rollouts(self, datas):
         """``experiences_from_rollout`` (:328-430) for all rollouts of an iteration at once: per rollout the result equals a
@@ -583,17 +597,18 @@ class DotaOptimizer:
         length are not emitted -- but the work is one batched pass instead of ``R`` batch-1 passes."""
         S, pol = self.seq_len, self.policy_base
         p = self._prepare_rollouts(datas)
-        obs, masks, actions, ybuf, cbuf, Lps = p['obs'], p['masks'], p['actions'], p['ybuf'], p['cbuf'], p['Lps']
+        obs, masks, actions, ybufs, cbufs, Lps = p['obs'], p['masks'], p['actions'], p['ybufs'], p['cbufs'], p['Lps']
         out = []
         for i, d in enumerate(datas):
             base = int(sum(Lps[:i]))
             sequences = []
             for j in range(Lps[i] // S):
                 sl = slice(j * S, (j + 1) * S)
+                h = ops.stack_layers([yb[j * S, i] for yb in ybufs]).unsqueeze(1)             # [L, 1, H]
                 if pol.cell == "lstm":
-                    hid = (ybuf[j * S, i].reshape(1, 1, -1), cbuf[j * S, i].reshape(1, 1, -1))
+                    hid = (h, ops.stack_layers([cb[j * S, i] for cb in cbufs]).unsqueeze(1))
                 else:
-                    hid = ybuf[j * S, i].reshape(1, 1, -1)
+                    hid = h
                 seq = Sequence(game_id=d.get('game_id'), weight_version=d.get('weight_version'), team_id=d.get('team_id'),
                                observations={k: v[sl, i] for k, v in obs.items()},
                                actions={k: v[sl, i] for k, v in actions.items()},
@@ -628,11 +643,12 @@ class DotaOptimizer:
         B = sum(n_chunks)
         adv = p['adv_c'].view(B, S).t().contiguous()                  # the GAE outputs are rollout-major back-to-back segments
         ret = p['ret_c'].view(B, S).t().contiguous()
-        # hidden state entering chunk j of rollout i = state buffer slot j*S (:340,384-385: carried, not re-zeroed)
+        # hidden state entering chunk j of rollout i = state buffer slot j*S of every layer (:340,384-385: carried, not
+        # re-zeroed), stacked [L, B, H]
         t_idx = torch.tensor([j * S for i in range(R) for j in range(n_chunks[i])], dtype=torch.int64, device=self.device)
         r_idx = torch.tensor([i for i in range(R) for _ in range(n_chunks[i])], dtype=torch.int64, device=self.device)
-        h0 = p['ybuf'][t_idx, r_idx].unsqueeze(0)
-        c0 = p['cbuf'][t_idx, r_idx].unsqueeze(0) if pol.cell == "lstm" else None
+        h0 = ops.stack_layers([yb[t_idx, r_idx] for yb in p['ybufs']])
+        c0 = ops.stack_layers([cb[t_idx, r_idx] for cb in p['cbufs']]) if pol.cell == "lstm" else None
         return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0)
 
     @staticmethod
@@ -937,10 +953,26 @@ class _FusedAdamHandle:
         return {'state': state, 'param_groups': [group]}
 
     def load_state_dict(self, sd):
+        """Restores the moments and step counters.  A state saved for another parameter layout (another number of tensors,
+        or another shape at the same index -- e.g. a model with another ``num_layers``) raises ``ValueError`` before anything
+        is changed: the state is keyed by parameter index, so it cannot be applied to a different layout."""
         o = self._owner
         if 'state' not in sd:                      # round-1 flat layout
+            if (sd['exp_avg'].numel(), sd['exp_avg_sq'].numel(), sd['step'].numel()) != \
+                    (o.exp_avg.numel(), o.exp_avg_sq.numel(), o.adam_steps.numel()):
+                raise ValueError("Adam state was saved for another parameter layout (flat buffer of %d elements, %d tensors; "
+                                 "this model: %d, %d)" % (sd['exp_avg'].numel(), sd['step'].numel(), o.exp_avg.numel(),
+                                                          o.adam_steps.numel()))
             o.exp_avg.copy_(sd['exp_avg']); o.exp_avg_sq.copy_(sd['exp_avg_sq']); o.adam_steps.copy_(sd['step'])
             return
+        n_saved = sum(len(g['params']) for g in sd['param_groups'])
+        if n_saved != o.flat.n_seg:
+            raise ValueError("Adam state was saved for %d parameter tensors; this model has %d" % (n_saved, o.flat.n_seg))
+        for i, st in sd['state'].items():
+            p = o.flat.params[int(i)]
+            if st['exp_avg'].shape != p.shape or st['exp_avg_sq'].shape != p.shape:
+                raise ValueError("Adam state of parameter %d (%s) has shape %s; the parameter is %s"
+                                 % (int(i), o.flat.names[int(i)], tuple(st['exp_avg'].shape), tuple(p.shape)))
         o.exp_avg.zero_(); o.exp_avg_sq.zero_(); o.adam_steps.zero_()
         steps = torch.zeros(o.flat.n_seg, dtype=torch.int32)
         for i, st in sd['state'].items():
@@ -968,14 +1000,14 @@ def init_distribution(backend='nccl'):
 
 def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          pretrained_model, mq_prefetch_count, log_dir, entropy_coef, vf_coef, run_local,
-         hidden_size=256, cell="gru"):
+         hidden_size=256, cell="gru", num_layers=1):
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
     dota_optimizer = DotaOptimizer(
         rmq_host=rmq_host, rmq_port=rmq_port, epochs=epochs, min_seq_per_epoch=min_seq_per_epoch, seq_len=seq_len,
         learning_rate=learning_rate, checkpoint=is_master(), pretrained_model=pretrained_model,
         mq_prefetch_count=mq_prefetch_count, log_dir=log_dir, entropy_coef=entropy_coef, vf_coef=vf_coef,
-        run_local=run_local, hidden_size=hidden_size, cell=cell)
+        run_local=run_local, hidden_size=hidden_size, cell=cell, num_layers=num_layers)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -988,7 +1020,7 @@ def default_log_dir():
 
 
 def build_arg_parser():
-    """The reference's flags and defaults (:777-794) plus ``--hidden-size`` and ``--cell``."""
+    """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell`` and ``--num-layers``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -1006,6 +1038,7 @@ def build_arg_parser():
     p.add_argument("--run-local", type=bool, help="set to true to run locally (not using GCP)", default=False)
     p.add_argument("--hidden-size", type=int, help="recurrent width, a multiple of 32 (reference: 256)", default=256)
     p.add_argument("--cell", type=str, choices=['gru', 'lstm'], help="recurrent cell (reference: gru)", default='gru')
+    p.add_argument("--num-layers", type=int, help="recurrent layers (reference: 1)", default=1)
     return p
 
 
@@ -1016,6 +1049,7 @@ if __name__ == '__main__':
         main(rmq_host=args.ip, rmq_port=args.port, epochs=args.epochs, min_seq_per_epoch=args.min_seq_per_epoch,
              seq_len=args.seq_len, learning_rate=args.learning_rate, pretrained_model=args.pretrained_model,
              mq_prefetch_count=args.mq_prefetch_count, log_dir=args.log_dir, entropy_coef=args.entropy_coef,
-             vf_coef=args.vf_coef, run_local=args.run_local, hidden_size=args.hidden_size, cell=args.cell)
+             vf_coef=args.vf_coef, run_local=args.run_local, hidden_size=args.hidden_size, cell=args.cell,
+             num_layers=args.num_layers)
     except KeyboardInterrupt:
         pass

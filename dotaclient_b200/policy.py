@@ -3,9 +3,12 @@
 Same constructor-created parameters, same ``state_dict`` (34 keys, shapes and order of
 ``policy.py:54-75``), same ``forward`` signature and outputs (``policy.py:92-167``); the recurrent
 layer runs through the hand-written sm_90a recurrence kernels (``dotaclient_b200/csrc``), and the
-unit encoder through the fused encoder kernel when it is available.  Two additions, both
-keyword-only so ``Policy()`` is the reference's network: ``hidden_size`` (reference: 256) and
-``cell`` ('gru' = the reference's ``nn.GRU``, 'lstm' = the cell BASELINE.json names).
+unit encoder through the fused encoder kernel when it is available.  Three additions, all
+keyword-only so ``Policy()`` is the reference's network: ``hidden_size`` (reference: 256),
+``cell`` ('gru' = the reference's ``nn.GRU``, 'lstm' = the cell BASELINE.json names) and
+``num_layers`` (reference: 1), the depth of the recurrent core with the semantics of
+``nn.GRU(num_layers=L)``: layer k consumes layer k-1's output sequence, every hidden state is
+``[L, B, H]`` and the ``state_dict`` carries ``rnn.*_l{k}`` for every layer (34 + 4(L-1) keys).
 
 Every ``hidden_size`` that is a multiple of 32 runs on the GPU: 128, 256 and the other multiples of 128 on their
 dedicated recurrence kernels, the rest (64, 96, 160, 192, ...) on the generic ones.  Any width constructs, so that a
@@ -46,12 +49,19 @@ class MaskedCategorical:
 
 
 class _RnnParams(nn.Module):
-    """Parameter holder with ``nn.GRU``/``nn.LSTM`` names so ``rnn.weight_ih_l0`` ... load unchanged."""
+    """Parameter holder with ``nn.GRU``/``nn.LSTM`` names and order (``weight_ih_l{k}, weight_hh_l{k}, bias_ih_l{k},
+    bias_hh_l{k}`` for every layer k) so ``rnn.weight_ih_l0`` ... load unchanged."""
 
     def __init__(self, template):
         super().__init__()
-        for name in ("weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0"):
-            self.register_parameter(name, nn.Parameter(getattr(template, name).detach().clone()))
+        self.num_layers = template.num_layers
+        for k in range(self.num_layers):
+            for name in ("weight_ih_l%d" % k, "weight_hh_l%d" % k, "bias_ih_l%d" % k, "bias_hh_l%d" % k):
+                self.register_parameter(name, nn.Parameter(getattr(template, name).detach().clone()))
+
+    def layer(self, k):
+        """(w_ih, w_hh, b_ih, b_hh) of layer ``k``."""
+        return tuple(getattr(self, "%s_l%d" % (n, k)) for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
 
 
 class Policy(nn.Module):
@@ -68,19 +78,23 @@ class Policy(nn.Module):
     INPUT_KEYS = ['env', 'allied_heroes', 'enemy_heroes', 'allied_nonheroes', 'enemy_nonheroes',
                   'allied_towers', 'enemy_towers']
 
-    def __init__(self, *, hidden_size=256, cell="gru"):
+    def __init__(self, *, hidden_size=256, cell="gru", num_layers=1):
         super().__init__()
         if cell not in ("gru", "lstm"):
             raise ValueError("cell must be 'gru' or 'lstm'")
+        if int(num_layers) != num_layers or num_layers < 1:
+            raise ValueError("num_layers must be an integer >= 1, got %r" % (num_layers,))
         self.hidden_size = H = int(hidden_size)
         self.cell = cell
+        self.num_layers = int(num_layers)
         # Creation order == reference (policy.py:54-75) so torch.manual_seed(7); Policy() reproduces its init.
         self.affine_env = nn.Linear(3, 128)
         self.affine_unit_basic_stats = nn.Linear(12, 128)
         for suffix, _, _ in UNIT_GROUPS:
             setattr(self, "affine_unit_" + suffix, nn.Linear(128, 128))
         self.affine_pre_rnn = nn.Linear(896, H)
-        template = (nn.GRU if cell == "gru" else nn.LSTM)(input_size=H, hidden_size=H, num_layers=1, batch_first=True)
+        template = (nn.GRU if cell == "gru" else nn.LSTM)(input_size=H, hidden_size=H, num_layers=self.num_layers,
+                                                          batch_first=True)
         self.rnn = _RnnParams(template)
         self.affine_head_enum = nn.Linear(H, 4)
         self.affine_move_x = nn.Linear(H, self.N_MOVE_ENUMS)
@@ -91,8 +105,8 @@ class Policy(nn.Module):
 
     # ------------------------------------------------------------------ reference API
     def init_hidden(self):
-        """Zero state ``[1, 1, H]`` (``policy.py:77-78``); an ``(h, c)`` tuple for the LSTM."""
-        h = torch.zeros([1, 1, self.hidden_size], dtype=torch.float32)
+        """Zero state ``[L, 1, H]`` (``policy.py:77-78``, L = ``num_layers``); an ``(h, c)`` tuple for the LSTM."""
+        h = torch.zeros([self.num_layers, 1, self.hidden_size], dtype=torch.float32)
         return (h, torch.zeros_like(h)) if self.cell == "lstm" else h
 
     def single(self, hidden, **kwargs):
@@ -109,7 +123,8 @@ class Policy(nn.Module):
 
     def forward(self, env, allied_heroes, enemy_heroes, allied_nonheroes, enemy_nonheroes,
                 allied_towers, enemy_towers, hidden):
-        """Batch-first ``(b, s, ...)`` inputs -> (logits dict ``(b, s, n)``, value ``(b, s, 1)``, hidden)."""
+        """Batch-first ``(b, s, ...)`` inputs -> (logits dict ``(b, s, n)``, value ``(b, s, 1)``, hidden).  ``hidden`` is
+        ``[L, b, H]`` (an ``(h, c)`` pair for the LSTM) in and out: as in torch, not batch-first."""
         return self._run((env, allied_heroes, enemy_heroes, allied_nonheroes, enemy_nonheroes,
                           allied_towers, enemy_towers), hidden, time_major=False)
 
@@ -130,15 +145,21 @@ class Policy(nn.Module):
         return ops.linear(x, self.affine_pre_rnn.weight, self.affine_pre_rnn.bias, relu=True), unit_embedding
 
     def _recur(self, x_tm, hidden):
-        """x_tm ``[S, B, H]`` time-major -> y_tm ``[S, B, H]``, new hidden in the reference's ``[1, B, H]`` form."""
+        """x_tm ``[S, B, H]`` time-major -> y_tm ``[S, B, H]``, new hidden in torch's ``[L, B, H]`` form.
+
+        One ``ops.rnn_sequence`` (i2h GEMM + width-selected recurrence kernel) per layer, as ``nn.GRU(num_layers=L)``
+        stacks them: layer k reads layer k-1's output sequence, a view of that layer's state buffer (no copy), so
+        autograd chains the backward through layer k's ``dx``."""
         r = self.rnn
-        if self.cell == "lstm":
-            h0, c0 = hidden[0][0], hidden[1][0]
-        else:
-            h0, c0 = hidden[0], None
-        y, hn, cn = ops.rnn_sequence(x_tm, r.weight_ih_l0, r.weight_hh_l0, r.bias_ih_l0, r.bias_hh_l0, h0, c0, self.cell)
-        new_hidden = (hn.unsqueeze(0), cn.unsqueeze(0)) if self.cell == "lstm" else hn.unsqueeze(0)
-        return y, new_hidden
+        lstm = self.cell == "lstm"
+        h0, c0 = hidden if lstm else (hidden, None)
+        y, hs, cs = x_tm, [], []
+        for k in range(self.num_layers):
+            y, hn, cn = ops.rnn_sequence(y, *r.layer(k), h0[k], c0[k] if lstm else None, self.cell)
+            hs.append(hn)
+            cs.append(cn)
+        h_n = ops.stack_layers(hs)
+        return y, ((h_n, ops.stack_layers(cs)) if lstm else h_n)
 
     def _heads(self, y, unit_embedding):
         """Action heads + value (``policy.py:144-155``): the attention projection and ONE packed ``[*, 128]`` tensor-core GEMM
@@ -221,7 +242,7 @@ class Policy(nn.Module):
         recurrence and heads on the same kernels as the optimizer -- followed by the hierarchical masked sampling kernel
         (``select_actions_batched``, one launch for the pool).
 
-        ``hidden``: ``[1, A, H]`` (``(h, c)`` for the LSTM); ``observations``: ``{key: [A, ...]}`` (what ``single`` takes, with
+        ``hidden``: ``[L, A, H]`` (``(h, c)`` for the LSTM; L = ``num_layers``); ``observations``: ``{key: [A, ...]}`` (what ``single`` takes, with
         a leading agent dimension); ``masks``: ``{head: [A, n]}`` legal-action masks (``action_masks``); ``u``: optional
         ``[A, 5]`` uniforms.  Returns ``(chosen {head: int32 [A], -1 = not sampled}, logp [A, 5], logits {head: [A, n]},
         value [A], new hidden)``.  Index selection is bit-exact against ``oracle.ref_policy.sample_index``."""
