@@ -40,16 +40,26 @@ SIGNATURES = {
                                    _vp, _vp, _vp]),
     "dc_ppo_loss_fwd_bwd_strided": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _i64, _f32, _f32, _f32,
                                            _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "dc_ppo_loss_fwd_bwd_dev": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp,
+                                       _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "dc_selected_logp": (_i32, [_ptr5, _ptr5, _ptr5, _i64, _vp, _vp]),
     "dc_select_actions": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _vp, _i64, _vp, _vp, _vp]),
     "dc_grad_flags": (_i32, [_vp, _i64, _vp, _i32, _vp, _vp]),
     "dc_grad_finish": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _f64, _f64, _f64, _f64, _f64, _vp, _vp,
                               _vp, _vp]),
+    "dc_grad_finish_dev": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _vp, _f64, _f64, _f64, _vp, _vp, _vp,
+                                  _vp]),
 }
 
 PPO_WORKSPACE_BYTES = 512
 FINISH_WORKSPACE_BYTES = 1024
 LOSS_SLOTS = 16
+# the device hyper-parameter block of the `_dev` entry points (fp64, DC_HP_* in include/dotaclient_b200.h)
+HPARAM_SLOTS = 8
+HP_LR, HP_E_CLIP, HP_ENTROPY_COEF, HP_VF_COEF, HP_MAX_GRAD_NORM, HP_VALUE_CLIP = range(6)
+# the PPO diagnostics written by dc_ppo_loss_fwd_bwd_dev (DC_STAT_* in include/dotaclient_b200.h)
+PPO_STATS_SLOTS = 16
+STAT_APPROX_KL, STAT_CLIP_FRACTION, STAT_EXPLAINED_VAR = 0, 6, 12
 MAX_PARAM_TENSORS = 96      # kMaxSeg of csrc/grad_finish.cu: parameter tensors dc_grad_flags / dc_grad_finish can handle
 
 _lib = None

@@ -10,6 +10,7 @@
 //
 // Three small launches over <= 11 MB: (A) divide + per-parameter sum of squares (float64 atomics),
 // (B) clip coefficient + Adam in one elementwise sweep, (C) step counters + metrics.
+// dc_grad_finish_dev reads lr and the clip norm from the device hyper-parameter block (DC_HPARAM_SLOTS) in (B).
 // HBM-bound elementwise work: 4 B read + 4 B written per element in A, 16 B read + 12 B written in B.
 #include "dc_common.cuh"
 
@@ -87,10 +88,14 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(float *__restrict__ para
                                                         const int64_t *__restrict__ seg_lo,
                                                         const int64_t *__restrict__ seg_hi, int n_seg, int64_t total,
                                                         double lr, double beta1_d, double beta2_d, double eps_d,
-                                                        float max_norm, const float *__restrict__ loss_out,
-                                                        FinishWs *ws) {
+                                                        float max_norm, const double *__restrict__ hparams,
+                                                        const float *__restrict__ loss_out, FinishWs *ws) {
     __shared__ float s_coef;
     __shared__ int s_nan;
+    if (hparams) {                                       // the device block overrides the scalar arguments
+        lr = hparams[DC_HP_LR];
+        max_norm = (float)hparams[DC_HP_MAX_GRAD_NORM];
+    }
     if (threadIdx.x == 0) {
         float coef, mn, tn;
         int nf;
@@ -144,6 +149,28 @@ __global__ void finish_tail_kernel(int32_t *steps, const float *g_tail, int n_se
     }
 }
 
+int launch_finish(float *flat_param, float *flat_grad, float *exp_avg, float *exp_avg_sq, int32_t *steps,
+                  const int64_t *seg_lo, const int64_t *seg_hi, int n_seg, int64_t total, double lr, double beta1, double beta2,
+                  double adam_eps, double max_norm, const double *hparams, const float *loss_out, float *metrics,
+                  void *workspace, dc_stream_t stream) {
+    DC_REQUIRE(flat_param && flat_grad && exp_avg && exp_avg_sq && steps && seg_lo && seg_hi && metrics && workspace,
+               DC_EINVAL, "dc_grad_finish: null pointer");
+    DC_REQUIRE(n_seg > 0 && n_seg <= kMaxSeg && total > 0, DC_EINVAL, "dc_grad_finish: n_seg=%d total=%lld", n_seg,
+               (long long)total);
+    cudaStream_t st = dc_cu_stream(stream);
+    FinishWs *ws = reinterpret_cast<FinishWs *>(workspace);
+    DC_CUDA(cudaMemsetAsync(ws, 0, sizeof(FinishWs), st));
+    const int blocks = 2 * dc_sm_count();
+    grad_sumsq_kernel<<<blocks, kThreads, 0, st>>>(flat_grad, seg_lo, seg_hi, n_seg, total, ws);
+    DC_LAUNCH_OK();
+    adam_kernel<<<blocks, kThreads, 0, st>>>(flat_param, flat_grad, exp_avg, exp_avg_sq, steps, seg_lo, seg_hi, n_seg, total,
+                                             lr, beta1, beta2, adam_eps, (float)max_norm, hparams, loss_out, ws);
+    DC_LAUNCH_OK();
+    finish_tail_kernel<<<1, kMaxSeg, 0, st>>>(steps, flat_grad + total, n_seg, ws, metrics);
+    DC_LAUNCH_OK();
+    return DC_OK;
+}
+
 }  // namespace
 
 extern "C" int dc_grad_flags(float *flat_grad, int64_t total, const int32_t *seg_head, int n_seg,
@@ -161,20 +188,16 @@ extern "C" int dc_grad_finish(float *flat_param, float *flat_grad, float *exp_av
                               double beta1, double beta2, double adam_eps, double max_norm, const float *loss_out,
                               float *metrics, void *workspace, dc_stream_t stream) {
     (void)seg_head;
-    DC_REQUIRE(flat_param && flat_grad && exp_avg && exp_avg_sq && steps && seg_lo && seg_hi && metrics && workspace,
-               DC_EINVAL, "dc_grad_finish: null pointer");
-    DC_REQUIRE(n_seg > 0 && n_seg <= kMaxSeg && total > 0, DC_EINVAL, "dc_grad_finish: n_seg=%d total=%lld", n_seg,
-               (long long)total);
-    cudaStream_t st = dc_cu_stream(stream);
-    FinishWs *ws = reinterpret_cast<FinishWs *>(workspace);
-    DC_CUDA(cudaMemsetAsync(ws, 0, sizeof(FinishWs), st));
-    const int blocks = 2 * dc_sm_count();
-    grad_sumsq_kernel<<<blocks, kThreads, 0, st>>>(flat_grad, seg_lo, seg_hi, n_seg, total, ws);
-    DC_LAUNCH_OK();
-    adam_kernel<<<blocks, kThreads, 0, st>>>(flat_param, flat_grad, exp_avg, exp_avg_sq, steps, seg_lo, seg_hi, n_seg, total,
-                                             lr, beta1, beta2, adam_eps, (float)max_norm, loss_out, ws);
-    DC_LAUNCH_OK();
-    finish_tail_kernel<<<1, kMaxSeg, 0, st>>>(steps, flat_grad + total, n_seg, ws, metrics);
-    DC_LAUNCH_OK();
-    return DC_OK;
+    return launch_finish(flat_param, flat_grad, exp_avg, exp_avg_sq, steps, seg_lo, seg_hi, n_seg, total, lr, beta1, beta2,
+                         adam_eps, max_norm, nullptr, loss_out, metrics, workspace, stream);
+}
+
+extern "C" int dc_grad_finish_dev(float *flat_param, float *flat_grad, float *exp_avg, float *exp_avg_sq, int32_t *steps,
+                                  const int64_t *seg_lo, const int64_t *seg_hi, const int32_t *seg_head, int n_seg,
+                                  int64_t total, const double *hparams, double beta1, double beta2, double adam_eps,
+                                  const float *loss_out, float *metrics, void *workspace, dc_stream_t stream) {
+    (void)seg_head;
+    DC_REQUIRE(hparams, DC_EINVAL, "dc_grad_finish_dev: null hyper-parameter block");
+    return launch_finish(flat_param, flat_grad, exp_avg, exp_avg_sq, steps, seg_lo, seg_hi, n_seg, total, 0.0, beta1, beta2,
+                         adam_eps, 0.0, hparams, loss_out, metrics, workspace, stream);
 }

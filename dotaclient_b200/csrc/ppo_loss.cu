@@ -15,8 +15,14 @@
 // so per-thread row reads from global would waste most of every sector), the tile is overwritten
 // in place with d loss / d logits and written back with coalesced 16-byte stores.
 //
+// The second launch also accumulates the PPO diagnostics (approximate KL and clip fraction per head, explained variance)
+// from the values it already holds in registers, and optionally clips the value loss PPO2-style against old values.
+// The `_dev` entry point reads its hyper-parameters from a device block (DC_HPARAM_SLOTS), so a captured CUDA graph of
+// the step picks up new values on every replay; the scalar-argument entry points run the same kernel body.
+//
 // Algorithmic HBM bytes per token: logits 260 + masks 65 + actions 65 + old 20 + adv/ret/value 12
-// read, dlogits 260 + dvalue 4 written = 686 (+ 69 for the statistics pass).
+// read, dlogits 260 + dvalue 4 written = 686 (+ 69 for the statistics pass, + 4 for the old value when the value loss
+// is clipped).
 #include "dc_common.cuh"
 
 namespace {
@@ -51,12 +57,19 @@ struct HeadPtrs {
     long long ld_v, ld_dv;      // pitches of value / dvalue
 };
 
+// PPO diagnostics accumulated per token: k3 KL and clipped rows per head, then sums of (ret - v), (ret - v)^2, ret, ret^2
+constexpr int kStats = 2 * kHeads + 4;
+constexpr int kStKl = 0, kStClip = kHeads, kStD = 2 * kHeads, kStD2 = kStD + 1, kStR = kStD + 2, kStR2 = kStD + 3;
+constexpr int kTokD = 2 * kHeads, kTokR = kTokD + 1, kTokRows = kTokR + 1;   // rows of the per-token staging
+static_assert(2 * kHeads + 3 < DC_PPO_STATS_SLOTS, "stats output too small");
+
 // Workspace layout (DC_PPO_WORKSPACE_BYTES, zeroed per call)
 struct Workspace {
     double pol[kHeads];   // sum over action rows of min(surr1, surr2)
     double ent[kHeads];   // sum over masked entries of -p*logp
-    double vl;            // sum (ret - v)^2
+    double vl;            // sum (ret - v)^2, or of the clipped value loss term
     double adv_sum, adv_sq;
+    double st[kStats];    // diagnostics (kSt* above)
     int cnt[kHeads];
     unsigned ticket_stats, ticket_loss;
     float adv_mean, adv_std;
@@ -192,7 +205,7 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
 template <int H, bool kGrad>
 __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, const uint8_t *arow, float old_lp,
                                            float adv_n, int n_h, float e_clip, float entropy_coef, float &pol_acc,
-                                           float &ent_acc, float *logp_out) {
+                                           float &ent_acc, float *kl_out, float *clip_out, float *logp_out) {
     constexpr int N = head_n(H);
     float l[N], e[N];
     int mask_any = 0, a_idx = -1;
@@ -242,7 +255,12 @@ __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, con
         float lpa = lp[0];
 #pragma unroll
         for (int j = 1; j < N; ++j) lpa = (j == a_idx) ? lp[j] : lpa;
-        const float ratio = __expf(lpa - old_lp);                     // optimizer.py:638
+        const float log_r = lpa - old_lp;
+        const float ratio = __expf(log_r);                             // optimizer.py:638
+        // k3 estimator of KL(old || new); expm1f keeps it accurate for small |log r|, where r - 1 from __expf
+        // would carry an error as large as the value itself
+        *kl_out = expm1f(log_r) - log_r;
+        *clip_out = fabsf(ratio - 1.0f) > e_clip ? 1.f : 0.f;
         const float lo = 1.0f - e_clip, hi = 1.0f + e_clip;
         const float s1 = ratio * adv_n;                                // :639
         const float s2 = fminf(fmaxf(ratio, lo), hi) * adv_n;          // :640
@@ -271,15 +289,32 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
                                                           const float *__restrict__ ret,
                                                           const float *__restrict__ value, int64_t N, float e_clip,
                                                           float entropy_coef, float vf_coef,
+                                                          const float *__restrict__ old_value,
+                                                          const double *__restrict__ hparams,
                                                           float *__restrict__ dvalue, float *__restrict__ out,
-                                                          Workspace *ws, float *__restrict__ logp_out) {
+                                                          float *__restrict__ stats, Workspace *ws,
+                                                          float *__restrict__ logp_out) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *s_logits = reinterpret_cast<float *>(smem_raw);
     float *s_old = s_logits + kLogitFloats;
     uint8_t *s_mask = reinterpret_cast<uint8_t *>(s_old + kOldFloats);
     uint8_t *s_act = s_mask + kByteTile;
     __shared__ float s_red[kTile / 32];
+    // per-token diagnostics (rows kStKl.., kStClip.., then ret - v and ret), staged here rather than held in registers
+    // across the head loop, and their block sums
+    __shared__ float s_tok[kTokRows][kTile];
+    __shared__ double s_st[kStats];
     __shared__ bool s_last;
+
+    // hyper-parameters from the device block when given, rounded to the types of the scalar arguments
+    float value_clip = 0.f;
+    if (!kSelectOnly && hparams) {
+        e_clip = (float)hparams[DC_HP_E_CLIP];
+        entropy_coef = (float)hparams[DC_HP_ENTROPY_COEF];
+        vf_coef = (float)hparams[DC_HP_VF_COEF];
+        value_clip = (float)hparams[DC_HP_VALUE_CLIP];
+    }
+    const bool clip_value = old_value != nullptr && value_clip > 0.f;
 
     const int64_t t0 = (int64_t)blockIdx.x * kTile;
     const int count = (int)min((int64_t)kTile, N - t0);
@@ -300,6 +335,10 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
     const bool live = t < count;
     float pol[kHeads] = {0, 0, 0, 0, 0}, ent[kHeads] = {0, 0, 0, 0, 0};
     float vl = 0.f;
+    if (!kSelectOnly) {
+#pragma unroll
+        for (int i = 0; i < kTokRows; ++i) s_tok[i][t] = 0.f;     // rows without an action (and dead threads) count 0
+    }
     int cnt[kHeads] = {0, 0, 0, 0, 0};
     float adv_n = 0.f;
     if (!kSelectOnly) {
@@ -315,7 +354,8 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
 #define DC_HEAD(H)                                                                                              \
         head_token<H, true>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H),  \
                             s_act + byte_off(H) + t * head_n(H), kSelectOnly ? 0.f : s_old[t * 5 + H], adv_n,   \
-                            cnt[H], e_clip, entropy_coef, pol[H], ent[H], kSelectOnly ? &lp_sel[H] : nullptr);
+                            cnt[H], e_clip, entropy_coef, pol[H], ent[H], &s_tok[kStKl + H][t],                 \
+                            &s_tok[kStClip + H][t], kSelectOnly ? &lp_sel[H] : nullptr);
         DC_HEAD(0) DC_HEAD(1) DC_HEAD(2) DC_HEAD(3) DC_HEAD(4)
 #undef DC_HEAD
         if (kSelectOnly) {
@@ -324,8 +364,25 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         } else {
             const float v = value[(t0 + t) * hp.ld_v], r = ret[t0 + t];
             const float d = r - v;
-            vl = d * d;                                                     // optimizer.py:660
-            dvalue[(t0 + t) * hp.ld_dv] = vf_coef > 0.f ? vf_coef * (v - r) / (float)N : 0.f;
+            float g = v - r;                                                // d value_loss / d v, up to vf_coef / N
+            if (clip_value) {
+                // PPO2: max((v - R)^2, (v_old + clip(v - v_old, -eps, eps) - R)^2); autograd of torch.maximum (ties split
+                // the gradient in half) and of clamp (passes it inside [-eps, eps])
+                const float vo = old_value[t0 + t];
+                const float dv = v - vo;
+                const float dc = (vo + fminf(fmaxf(dv, -value_clip), value_clip)) - r;
+                const float l1 = d * d, l2 = dc * dc;
+                vl = fmaxf(l1, l2);
+                const float w1 = l1 > l2 ? 1.f : (l1 == l2 ? 0.5f : 0.f);
+                const float w2 = l2 > l1 ? 1.f : (l1 == l2 ? 0.5f : 0.f);
+                const float in_range = (dv >= -value_clip && dv <= value_clip) ? 1.f : 0.f;
+                g = w1 * g + w2 * in_range * dc;
+            } else {
+                vl = d * d;                                                 // optimizer.py:660
+            }
+            dvalue[(t0 + t) * hp.ld_dv] = vf_coef > 0.f ? vf_coef * g / (float)N : 0.f;
+            s_tok[kTokD][t] = d;
+            s_tok[kTokR][t] = r;
         }
     }
     if (kSelectOnly) return;
@@ -343,6 +400,21 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         sums[kHeads + h] = block_sum(ent[h], s_red);
     }
     sums[2 * kHeads] = block_sum(vl, s_red);
+    if (stats) {    // the diagnostics (s_tok is complete: block_sum synchronised the block): one warp per sum, in float64
+        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+        for (int i = warp; i < kStats; i += kTile / 32) {
+            const int row = i < kStD ? i : (i < kStR ? kTokD : kTokR);
+            const bool square = i == kStD2 || i == kStR2;
+            double s = 0.0;
+            for (int j = lane; j < kTile; j += 32) {
+                const double v = (double)s_tok[row][j];
+                s += square ? v * v : v;
+            }
+            s = dc_warp_sum(s);
+            if (lane == 0) s_st[i] = s;
+        }
+        __syncthreads();
+    }
     if (threadIdx.x == 0) {
 #pragma unroll
         for (int h = 0; h < kHeads; ++h) {
@@ -350,6 +422,10 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             if (sums[kHeads + h] != 0.f) atomicAdd(&ws->ent[h], (double)sums[kHeads + h]);
         }
         atomicAdd(&ws->vl, (double)sums[2 * kHeads]);
+        if (stats) {
+            for (int i = 0; i < kStats; ++i)
+                if (s_st[i] != 0.0) atomicAdd(&ws->st[i], s_st[i]);
+        }
         __threadfence();
         s_last = atomicAdd(&ws->ticket_loss, 1u) == gridDim.x - 1;
     }
@@ -376,6 +452,28 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         out[3] = v_loss;
         out[14] = w->adv_mean;
         out[15] = w->adv_std;
+        if (stats) {
+            float kl_sum = 0.f, clip_sum = 0.f;
+            int used = 0;
+            for (int h = 0; h < kHeads; ++h) {      // a head without action rows reports 0 and is left out of the mean
+                const int n = w->cnt[h];
+                const float kl_h = n ? (float)(w->st[kStKl + h] / (double)n) : 0.f;
+                const float clip_h = n ? (float)(w->st[kStClip + h] / (double)n) : 0.f;
+                stats[DC_STAT_APPROX_KL + 1 + h] = kl_h;
+                stats[DC_STAT_CLIP_FRACTION + 1 + h] = clip_h;
+                kl_sum += kl_h;
+                clip_sum += clip_h;
+                used += n > 0;
+            }
+            stats[DC_STAT_APPROX_KL] = used ? kl_sum / (float)used : 0.f;
+            stats[DC_STAT_CLIP_FRACTION] = used ? clip_sum / (float)used : 0.f;
+            // 1 - Var(ret - v) / Var(ret) over all N tokens (population variances); NaN when the returns are constant
+            const double n = (double)N;
+            const double md = w->st[kStD] / n, mr = w->st[kStR] / n;
+            const double var_d = w->st[kStD2] / n - md * md, var_r = w->st[kStR2] / n - mr * mr;
+            stats[DC_STAT_EXPLAINED_VAR] = var_r > 0.0 ? (float)(1.0 - var_d / var_r) : __int_as_float(0x7fc00000);
+            for (int i = DC_STAT_EXPLAINED_VAR + 1; i < DC_PPO_STATS_SLOTS; ++i) stats[i] = 0.f;
+        }
     }
 }
 
@@ -385,16 +483,15 @@ int check_heads(const float *const logits[], const uint8_t *const masks[], const
     return 1;
 }
 
-}  // namespace
-
-extern "C" int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
-                                           const uint8_t *const masks[DC_NUM_HEADS],
-                                           const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
-                                           const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
-                                           int64_t N, float e_clip, float entropy_coef, float vf_coef,
-                                           float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
-                                           float *dvalue, int64_t ld_dvalue, float *out, int32_t *n_actions, void *workspace,
-                                           dc_stream_t stream) {
+// Both launches of one loss evaluation.  hparams == nullptr: e_clip / entropy_coef / vf_coef are the scalar arguments and
+// the value loss is not clipped; otherwise they come from the device block.  stats == nullptr skips the diagnostics.
+int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                    const uint8_t *const masks[DC_NUM_HEADS], const uint8_t *const actions[DC_NUM_HEADS],
+                    const float *old_logp, const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                    const float *old_value, int64_t N, float e_clip, float entropy_coef, float vf_coef,
+                    const double *hparams, float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                    float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions, void *workspace,
+                    dc_stream_t stream) {
     DC_REQUIRE(N > 0, DC_EINVAL, "dc_ppo_loss_fwd_bwd: N=%lld", (long long)N);
     DC_REQUIRE(check_heads(logits, masks, actions) && old_logp && adv_raw && ret && value && dvalue && out &&
                    n_actions && workspace && ld_logits && ld_dlogits, DC_EINVAL, "dc_ppo_loss_fwd_bwd: null pointer");
@@ -417,9 +514,38 @@ extern "C" int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEAD
     DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     ppo_loss_kernel<false><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
-                                                              entropy_coef, vf_coef, dvalue, out, ws, nullptr);
+                                                              entropy_coef, vf_coef, old_value, hparams, dvalue, out,
+                                                              stats, ws, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
+}
+
+}  // namespace
+
+extern "C" int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                                           const uint8_t *const masks[DC_NUM_HEADS],
+                                           const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
+                                           const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                                           int64_t N, float e_clip, float entropy_coef, float vf_coef,
+                                           float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                                           float *dvalue, int64_t ld_dvalue, float *out, int32_t *n_actions, void *workspace,
+                                           dc_stream_t stream) {
+    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, nullptr, N, e_clip,
+                           entropy_coef, vf_coef, nullptr, dlogits, ld_dlogits, dvalue, ld_dvalue, out, nullptr, n_actions,
+                           workspace, stream);
+}
+
+extern "C" int dc_ppo_loss_fwd_bwd_dev(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                                       const uint8_t *const masks[DC_NUM_HEADS], const uint8_t *const actions[DC_NUM_HEADS],
+                                       const float *old_logp, const float *adv_raw, const float *ret, const float *value,
+                                       int64_t ld_value, const float *old_value, int64_t N, const double *hparams,
+                                       float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                                       float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
+                                       void *workspace, dc_stream_t stream) {
+    DC_REQUIRE(hparams, DC_EINVAL, "dc_ppo_loss_fwd_bwd_dev: null hyper-parameter block");
+    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, old_value, N, 0.f,
+                           0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions, workspace,
+                           stream);
 }
 
 extern "C" int dc_ppo_loss_fwd_bwd(const float *const logits[DC_NUM_HEADS], const uint8_t *const masks[DC_NUM_HEADS],
@@ -448,7 +574,8 @@ extern "C" int dc_selected_logp(const float *const logits[DC_NUM_HEADS], const u
     DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
     ppo_loss_kernel<true><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
-        hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, logp_out);
+        hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+        logp_out);
     DC_LAUNCH_OK();
     return DC_OK;
 }

@@ -262,12 +262,41 @@ def rnn_sequence(x_tm, w_ih, w_hh, b_ih, b_hh, h0, c0, cell):
 
 
 # --------------------------------------------------------------------------------------------- PPO loss
-def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_clip, entropy_coef, vf_coef):
+def hparam_block(device, lr=0.0, e_clip=0.0, entropy_coef=0.0, vf_coef=0.0, max_grad_norm=0.0, value_clip=None):
+    """A device hyper-parameter block (``_lib.HPARAM_SLOTS`` fp64) holding the given values, for the ``hparams=``
+    argument of ``ppo_loss_fwd_bwd`` / ``ppo_loss_packed`` / ``grad_finish``."""
+    vals = [0.0] * _lib.HPARAM_SLOTS
+    vals[_lib.HP_LR], vals[_lib.HP_E_CLIP], vals[_lib.HP_ENTROPY_COEF] = float(lr), float(e_clip), float(entropy_coef)
+    vals[_lib.HP_VF_COEF], vals[_lib.HP_MAX_GRAD_NORM] = float(vf_coef), float(max_grad_norm)
+    vals[_lib.HP_VALUE_CLIP] = float(value_clip or 0.0)
+    return torch.tensor(vals, dtype=torch.float64, device=device)
+
+
+def _ppo_dev_args(hparams, old_value, stats, N, dev):
+    """Checks the extra operands of ``dc_ppo_loss_fwd_bwd_dev``; allocates ``stats`` when not given."""
+    _need_cuda(hparams, old_value)
+    assert hparams.dtype == torch.float64 and hparams.numel() == _lib.HPARAM_SLOTS and hparams.is_contiguous()
+    if old_value is not None:
+        old_value = _f32c(old_value)
+        assert old_value.numel() == N
+    if stats is None:
+        stats = torch.empty(_lib.PPO_STATS_SLOTS, dtype=torch.float32, device=dev)
+    assert stats.dtype == torch.float32 and stats.numel() == _lib.PPO_STATS_SLOTS and stats.is_contiguous()
+    return old_value, stats
+
+
+def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_clip, entropy_coef, vf_coef, hparams=None,
+                     old_value=None, stats=None):
     """Fused PPO loss + gradients (``optimizer.py:587-589,621-665`` and their backward).
 
     logits/masks/actions: sequences of 5 tensors [..., n_h] in HEAD_KEYS order (any leading dims,
     same token order everywhere); old_logp [..., 5]; adv_raw/ret/value [...].
     Returns (out[16] fp32, n_actions[5] int32, dlogits list, dvalue) -- all on device, no sync.
+
+    ``hparams`` (a device block from ``hparam_block``): the hyper-parameters are read from it on the device
+    (``dc_ppo_loss_fwd_bwd_dev``; ``e_clip`` / ``entropy_coef`` / ``vf_coef`` are then ignored), the value loss is clipped
+    against ``old_value`` [...] when the block's value clip is > 0, and the PPO diagnostics go to ``stats``
+    [``_lib.PPO_STATS_SLOTS``]; the return value gains that tensor as a fifth element.
     """
     logits = [_f32c(l.detach()) for l in logits]
     _need_cuda(*logits)
@@ -286,6 +315,17 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     n_actions = torch.empty(5, dtype=torch.int32, device=dev)
     ws = torch.empty(_lib.PPO_WORKSPACE_BYTES, dtype=torch.uint8, device=dev)
     lib = _lib.load()
+    if hparams is not None:
+        old_value, stats = _ppo_dev_args(hparams, old_value, stats, N, dev)
+        ld = (ctypes.c_int64 * 5)(*HEAD_SIZES)
+        with PROFILE.span("ppo_loss", 2):
+            _lib.check(lib.dc_ppo_loss_fwd_bwd_dev(_lib.ptr5(logits), ld, _lib.ptr5(masks), _lib.ptr5(actions),
+                                                   old_logp.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(), value.data_ptr(),
+                                                   1, _lib.ptr(old_value), N, hparams.data_ptr(), _lib.ptr5(dlogits), ld,
+                                                   dvalue.data_ptr(), 1, out.data_ptr(), stats.data_ptr(),
+                                                   n_actions.data_ptr(), ws.data_ptr(), _lib.stream_ptr()),
+                       "dc_ppo_loss_fwd_bwd_dev")
+        return out, n_actions, dlogits, dvalue, stats
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd(_lib.ptr5(logits), _lib.ptr5(masks), _lib.ptr5(actions),
                                            old_logp.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(), value.data_ptr(),
@@ -319,8 +359,21 @@ def grad_flags(flat_grad, total, seg_head, n_actions):
 
 
 def grad_finish(flat_param, flat_grad, exp_avg, exp_avg_sq, steps, seg_lo, seg_hi, seg_head, total, lr, betas, eps,
-                max_norm, loss_out, metrics, workspace):
+                max_norm, loss_out, metrics, workspace, hparams=None):
+    """Count-divide, grad norms, clip and Adam on the flat buffers.  With ``hparams`` (a device block, ``hparam_block``)
+    ``lr`` and ``max_norm`` are read from it on the device (``dc_grad_finish_dev``) and the arguments are ignored."""
     lib = _lib.load()
+    if hparams is not None:
+        _need_cuda(hparams)
+        assert hparams.dtype == torch.float64 and hparams.numel() == _lib.HPARAM_SLOTS and hparams.is_contiguous()
+        with PROFILE.span("grad_finish", 3):
+            _lib.check(lib.dc_grad_finish_dev(flat_param.data_ptr(), flat_grad.data_ptr(), exp_avg.data_ptr(),
+                                              exp_avg_sq.data_ptr(), steps.data_ptr(), seg_lo.data_ptr(), seg_hi.data_ptr(),
+                                              seg_head.data_ptr(), seg_head.numel(), total, hparams.data_ptr(),
+                                              float(betas[0]), float(betas[1]), float(eps), _lib.ptr(loss_out),
+                                              metrics.data_ptr(), workspace.data_ptr(), _lib.stream_ptr()),
+                       "dc_grad_finish_dev")
+        return
     with PROFILE.span("grad_finish", 3):
         _lib.check(lib.dc_grad_finish(flat_param.data_ptr(), flat_grad.data_ptr(), exp_avg.data_ptr(),
                                       exp_avg_sq.data_ptr(), steps.data_ptr(), seg_lo.data_ptr(), seg_hi.data_ptr(),
@@ -462,12 +515,14 @@ PACK_COLS = {"enum": (0, 4), "x": (4, 13), "y": (13, 22), "ability": (22, 25), "
 PACK_WIDTH = 128
 
 
-def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e_clip, entropy_coef, vf_coef):
+def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e_clip, entropy_coef, vf_coef, hparams=None,
+                    old_value=None, stats=None):
     """Fused PPO loss where the four small heads and the value head are column ranges of ONE packed ``[N,128]``
     tensor-core GEMM output (``PACK_COLS``) and the target-unit logits are a separate ``[N,40]`` tensor.
 
     Returns (out[16], n_actions[5], d_packed [N,128], d_logits_tu [N,40]): the gradients go straight back into the two
     producers, so no slice/cat kernels run and the five tiny K=131072 weight-gradient GEMMs become one wgmma wgrad.
+    ``hparams`` / ``old_value`` / ``stats``: as ``ppo_loss_fwd_bwd`` (the fifth element of the result is then ``stats``).
     """
     _need_cuda(packed, logits_tu)
     p2 = _f32c(packed.detach()).reshape(-1, PACK_WIDTH)
@@ -490,6 +545,16 @@ def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e
     dptr = _lib._ptr5(col(d_packed, "enum"), col(d_packed, "x"), col(d_packed, "y"), d_tu.data_ptr(), col(d_packed, "ability"))
     ld = (c.c_int64 * 5)(PACK_WIDTH, PACK_WIDTH, PACK_WIDTH, 40, PACK_WIDTH)
     lib = _lib.load()
+    if hparams is not None:
+        old_value, stats = _ppo_dev_args(hparams, old_value, stats, N, dev)
+        with PROFILE.span("ppo_loss", 2):
+            _lib.check(lib.dc_ppo_loss_fwd_bwd_dev(lptr, ld, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(),
+                                                   adv_raw.data_ptr(), ret.data_ptr(), col(p2, "value"), PACK_WIDTH,
+                                                   _lib.ptr(old_value), N, hparams.data_ptr(), dptr, ld,
+                                                   col(d_packed, "value"), PACK_WIDTH, out.data_ptr(), stats.data_ptr(),
+                                                   n_actions.data_ptr(), ws.data_ptr(), _lib.stream_ptr()),
+                       "dc_ppo_loss_fwd_bwd_dev")
+        return out, n_actions, d_packed.view_as(packed), d_tu.view_as(logits_tu), stats
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd_strided(lptr, ld, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(),
                                                    adv_raw.data_ptr(), ret.data_ptr(), col(p2, "value"), PACK_WIDTH, N,

@@ -10,10 +10,12 @@ when the batch is device-resident.  CUDA only.
 Line references are to TimZaman/dotaclient ``optimizer.py`` @ 8615b90.
 """
 import argparse
+import collections.abc
 import gc
 import io
 import logging
 import math
+import numbers
 import os
 import pickle
 import queue
@@ -207,12 +209,15 @@ class ExperienceBatch:
 
     ``DotaOptimizer.train`` accepts either a list of ``Sequence`` (reference API) or one of these.
     Tensors may live in pinned host memory; ``to(device)`` issues the asynchronous H2D copies.
+    ``old_values [S, B]`` (optional) are the critic's values at experience prep, which the clipped value loss
+    (``DotaOptimizer(value_clip=...)``) needs; a batch without them has no such entry in ``tensors()``.
     """
-    FIELDS = ("advantages", "returns", "old_logp", "h0", "c0")
+    FIELDS = ("advantages", "returns", "old_logp", "h0", "c0", "old_values")
 
-    def __init__(self, observations, masks, actions, old_logp, advantages, returns, h0, c0=None):
+    def __init__(self, observations, masks, actions, old_logp, advantages, returns, h0, c0=None, old_values=None):
         self.observations, self.masks, self.actions = observations, masks, actions
         self.old_logp, self.advantages, self.returns, self.h0, self.c0 = old_logp, advantages, returns, h0, c0
+        self.old_values = old_values
 
     def __del__(self):
         # a batch that was uploaded (prefetched) but never trained on must not leave its ready-events behind: a later tensor
@@ -308,7 +313,11 @@ class ExperienceBatch:
             c0 = torch.cat([e.hidden[1].to(device) for e in experiences], dim=1)
         else:
             h0, c0 = torch.cat([e.hidden.to(device) for e in experiences], dim=1), None      # :591
-        return ExperienceBatch(obs, masks, actions, old, adv, ret, h0.detach(), None if c0 is None else c0.detach())
+        old_values = None
+        if all(e.values is not None for e in experiences):
+            old_values = stack([torch.as_tensor(e.values).detach().reshape(-1).float() for e in experiences])
+        return ExperienceBatch(obs, masks, actions, old, adv, ret, h0.detach(), None if c0 is None else c0.detach(),
+                               old_values=old_values)
 
 
 _copy_streams = {}
@@ -328,6 +337,25 @@ def all_gather(t):                                                        # :193
 
 
 # ------------------------------------------------------------------------------------------ optimizer
+def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None):
+    """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
+    max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too).  NaN fails every check."""
+    def number(name, v):
+        if isinstance(v, bool) or not isinstance(v, numbers.Real):
+            raise ValueError("%s=%r is not a number" % (name, v))
+        return float(v)
+    if not 0.0 < number('gamma', gamma) <= 1.0:
+        raise ValueError("gamma=%r: the discount factor must be in (0, 1]" % (gamma,))
+    if not 0.0 <= number('gae_lambda', gae_lambda) <= 1.0:
+        raise ValueError("gae_lambda=%r: the GAE lambda must be in [0, 1]" % (gae_lambda,))
+    if not number('clip_range', clip_range) > 0.0:
+        raise ValueError("clip_range=%r: the PPO clip range must be > 0" % (clip_range,))
+    if not number('max_grad_norm', max_grad_norm) > 0.0:
+        raise ValueError("max_grad_norm=%r: the gradient-norm limit must be > 0" % (max_grad_norm,))
+    if value_clip is not None and not number('value_clip', value_clip) >= 0.0:
+        raise ValueError("value_clip=%r: the value clip range must be >= 0 (or None: no value clipping)" % (value_clip,))
+
+
 class DotaOptimizer:
     MODEL_FILENAME_FMT = "model_%09d.pt"
     ADAM_FILENAME_FMT = "adam_%09d.state"         # extension: Adam moments of the same iteration (torch.optim.Adam layout)
@@ -345,11 +373,16 @@ class DotaOptimizer:
     def __init__(self, rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len,
                  learning_rate, checkpoint, pretrained_model, mq_prefetch_count, log_dir,
                  entropy_coef, vf_coef, run_local, *, hidden_size=256, cell="gru", num_layers=1, mq=None,
-                 iterations=100000, rollout_prefetch=0):
+                 iterations=100000, rollout_prefetch=0, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1,
+                 max_grad_norm=0.5, value_clip=None):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
                              % (num_layers, self.MAX_LAYERS, _lib.MAX_PARAM_TENSORS))
+        check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip)
+        self.gamma, self.gae_lambda = float(gamma), float(gae_lambda)     # GAE of experience prep (:421)
+        self.MAX_GRAD_NORM = float(max_grad_norm)     # shadows the class constant; read before every step, like lr below
+        self.value_clip = None if value_clip is None else float(value_clip)
         self.rmq_host, self.rmq_port = rmq_host, rmq_port
         self.epochs = epochs
         self.min_seq_per_epoch = min_seq_per_epoch
@@ -364,7 +397,7 @@ class DotaOptimizer:
         self.run_local = run_local
         self.iterations = iterations        # :226
         self.model_upload_freq = 10         # :227
-        self.e_clip = 0.1                   # :229
+        self.e_clip = float(clip_range)     # :229
         self.device = _device()
         _lib.load()                         # fail loudly, up front, if the CUDA library is missing
 
@@ -412,11 +445,19 @@ class DotaOptimizer:
                 except ValueError as e:     # e.g. a 1-layer run's moments next to the weights loaded into num_layers=2
                     logger.warning('Not restoring Adam state from %s (%s): the moments start from zero', adam_file, e)
         self._sync_resume_state()
-        self._n_actions = torch.zeros(8, dtype=torch.int32, device=self.device)
-        self._n_actions[VALUE_SLOT] = 1 if vf_coef > 0 else 0
-        self._metrics = torch.zeros(4, dtype=torch.float32, device=self.device)
+        self._n_actions = torch.zeros(8, dtype=torch.int32, device=self.device)   # + value-head flag (_upload_hparams)
+        # grad-norm metrics and PPO diagnostics side by side: the step reads both back with one copy
+        self._result_dev = torch.zeros(4 + _lib.PPO_STATS_SLOTS, dtype=torch.float32, device=self.device)
+        self._metrics, self._ppo_stats = self._result_dev[:4], self._result_dev[4:]
         self._finish_ws = torch.zeros(_lib.FINISH_WORKSPACE_BYTES, dtype=torch.uint8, device=self.device)
-        self._host_result = torch.zeros(_lib.LOSS_SLOTS + 4, dtype=torch.float32).pin_memory()
+        # learning_rate, e_clip, entropy_coef, vf_coef, MAX_GRAD_NORM and value_clip are read by the step's kernels from this
+        # device block, rewritten from the pinned host copy before every step: a captured graph of the step holds the
+        # block's address, not the values, so assignments between steps reach replayed steps too
+        self._hparams_host = torch.zeros(_lib.HPARAM_SLOTS, dtype=torch.float64).pin_memory()
+        self._hparams_dev = torch.zeros(_lib.HPARAM_SLOTS, dtype=torch.float64, device=self.device)
+        self._hparams_uploaded = None       # the values the device block holds
+        self.last_ppo_stats = None          # approx_kl, clip_fraction (and per head), explained_variance of the last step
+        self._host_result = torch.zeros(_lib.LOSS_SLOTS + 4 + _lib.PPO_STATS_SLOTS, dtype=torch.float32).pin_memory()
         self.last_step_launch_estimate = 0
         self._staging, self._staging_event = {}, None    # pinned host staging of the batched experience prep
         # rollout_prefetch > 0: a background thread pulls and unpickles up to that many rollouts ahead (same order, same
@@ -587,7 +628,7 @@ class DotaOptimizer:
                 vals_c = torch.cat([values_lr[:Lps[i], i] for i in range(R)])
                 rew_c = torch.from_numpy(np.concatenate([rewards_np[i, :Lps[i]] for i in range(R)])).to(dev)
             seg = torch.tensor(np.concatenate([[0], np.cumsum(Lps)]), dtype=torch.int64, device=dev)
-            adv_c, ret_c = ops.gae_scan(rew_c, vals_c, seg, gamma=GAMMA, lam=LAMBDA)          # :417-421
+            adv_c, ret_c = ops.gae_scan(rew_c, vals_c, seg, gamma=self.gamma, lam=self.gae_lambda)   # :417-421
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
                     adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same)
 
@@ -649,7 +690,8 @@ class DotaOptimizer:
         r_idx = torch.tensor([i for i in range(R) for _ in range(n_chunks[i])], dtype=torch.int64, device=self.device)
         h0 = ops.stack_layers([yb[t_idx, r_idx] for yb in p['ybufs']])
         c0 = ops.stack_layers([cb[t_idx, r_idx] for cb in p['cbufs']]) if pol.cell == "lstm" else None
-        return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0)
+        old_values = chunked(p['values_lr']).contiguous()               # the critic at prep time (value clipping)
+        return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values)
 
     @staticmethod
     def list_of_dicts_to_dict_of_lists(x):
@@ -659,16 +701,22 @@ class DotaOptimizer:
     def train(self, experiences):
         """One PPO/Adam step on a list of ``Sequence`` (or an ``ExperienceBatch``).
 
-        Returns the reference's three dicts: losses, per-head entropies, grad norms (CPU scalars).
+        Returns the reference's three dicts: losses, per-head entropies, grad norms (CPU scalars).  The PPO diagnostics of
+        the step (approximate KL, clip fraction, explained variance) are left in ``last_ppo_stats``.
         A device-resident batch of a shape seen before is replayed from a CUDA graph of the whole step (forward, loss,
         backward, all-reduce, finish: ~80 kernel launches -> one graph launch); batches still in flight from the host
-        (``prefetch``) run the same kernels launch by launch so that the upload overlaps them.
+        (``prefetch``) run the same kernels launch by launch so that the upload overlaps them.  Either way the step uses
+        the current ``learning_rate``, ``e_clip``, ``entropy_coef``, ``vf_coef``, ``MAX_GRAD_NORM`` and ``value_clip``.
         """
         if isinstance(experiences, ExperienceBatch):
             batch = experiences if experiences.advantages.is_cuda else experiences.to(self.device)
         else:
             batch = ExperienceBatch.from_sequences(experiences, self.device)
+        if self.value_clip and batch.old_values is None:
+            raise ValueError("value_clip=%r needs the critic values of experience prep, and this batch has no old_values"
+                             % self.value_clip)
         t_enter = time.perf_counter()
+        self._upload_hparams()
         slot = getattr(batch, "_slot", None)
         if slot is not None:                       # uploaded by prefetch() straight into a graph's static input buffers
             torch.cuda.current_stream().wait_event(slot["ready"])
@@ -681,11 +729,12 @@ class DotaOptimizer:
             out, metrics = self._enqueue_step(batch)
         host = self._host_result
         host[:_lib.LOSS_SLOTS].copy_(out, non_blocking=True)
-        host[_lib.LOSS_SLOTS:].copy_(metrics, non_blocking=True)
+        host[_lib.LOSS_SLOTS:].copy_(self._result_dev, non_blocking=True)        # metrics, then the PPO diagnostics
         self.host_enqueue_s = time.perf_counter() - t_enter   # host time to launch the step (the GPU runs behind it)
         torch.cuda.current_stream().synchronize()      # the step's single host sync (result read-back)
         res = host.clone()
         keys = ops.HEAD_KEYS
+        self.last_ppo_stats = self._ppo_stats_dict(res[_lib.LOSS_SLOTS + 4:].tolist())
         if res[_lib.LOSS_SLOTS + 3] != 0:               # :667-669, :678-679 (parameters were left untouched)
             if math.isnan(float(res[0])):
                 raise ValueError('loss={}, policy_loss={}, entropy_loss={}, value_loss={}'.format(
@@ -694,6 +743,34 @@ class DotaOptimizer:
         losses = {'loss': res[0], 'policy_loss': res[1], 'entropy_loss': res[2], 'value_loss': res[3]}
         entropies = {k: res[4 + h] for h, k in enumerate(keys)}
         return losses, entropies, {'unclipped': res[_lib.LOSS_SLOTS], 'clipped': res[_lib.LOSS_SLOTS + 1]}
+
+    @staticmethod
+    def _ppo_stats_dict(st):
+        out = {'approx_kl': st[_lib.STAT_APPROX_KL], 'clip_fraction': st[_lib.STAT_CLIP_FRACTION]}
+        for h, k in enumerate(ops.HEAD_KEYS):
+            out['approx_kl/' + k] = st[_lib.STAT_APPROX_KL + 1 + h]
+            out['clip_fraction/' + k] = st[_lib.STAT_CLIP_FRACTION + 1 + h]
+        out['explained_variance'] = st[_lib.STAT_EXPLAINED_VAR]
+        return out
+
+    def _upload_hparams(self):
+        """Writes the current hyper-parameters into the device block the step's kernels read: one asynchronous copy on the
+        current stream, before the step is launched or replayed (never inside a captured graph), and only when a value
+        changed (with the value head's has-gradient flag, which follows vf_coef).  The pinned source is free to rewrite: the
+        previous step's copy completed before that step's result was read back."""
+        vals = (float(self.learning_rate), float(self.e_clip), float(self.entropy_coef), float(self.vf_coef),
+                float(self.MAX_GRAD_NORM), float(self.value_clip or 0.0))
+        if vals == self._hparams_uploaded:
+            return
+        h = self._hparams_host.numpy()
+        for slot, v in zip((_lib.HP_LR, _lib.HP_E_CLIP, _lib.HP_ENTROPY_COEF, _lib.HP_VF_COEF, _lib.HP_MAX_GRAD_NORM,
+                            _lib.HP_VALUE_CLIP), vals):
+            h[slot] = v
+        self._hparams_dev.copy_(self._hparams_host, non_blocking=True)
+        # the value head has a gradient only while the value loss is on (optimizer.py:660-662): with vf_coef = 0 the
+        # gradient finish skips its tensors (no Adam step, no share of the mean grad norm), like the reference's .grad = None
+        self._n_actions[VALUE_SLOT:VALUE_SLOT + 1].fill_(1 if self.vf_coef > 0 else 0)
+        self._hparams_uploaded = vals
 
     def _enqueue_step(self, batch):
         """Launches one optimizer step (:581-689) on the current stream; returns the device result vectors (loss slots, metrics)."""
@@ -705,12 +782,14 @@ class DotaOptimizer:
             ddp.auto_reduce = False        # the count-divide is fused into the finish kernel below
         ops.wait_h2d(batch.observations['env'], batch.h0, batch.c0)
         logits, values, _ = self.policy.forward_time_major(batch.observations, hidden)   # :619
-        ops.wait_h2d(batch.old_logp, batch.advantages, batch.returns, *batch.masks.values(), *batch.actions.values(),
-                     *batch.observations.values())
+        ops.wait_h2d(batch.old_logp, batch.advantages, batch.returns, batch.old_values, *batch.masks.values(),
+                     *batch.actions.values(), *batch.observations.values())
         packed = self.policy_base._packed_heads     # small heads + value are column ranges of one packed GEMM output
-        out, n_actions, d_packed, d_tu = ops.ppo_loss_packed(
+        # e_clip / entropy_coef / vf_coef / value_clip are read from the device block (_upload_hparams)
+        out, n_actions, d_packed, d_tu, _ = ops.ppo_loss_packed(
             packed, logits['target_unit'], [batch.masks[k] for k in keys], [batch.actions[k] for k in keys],
-            batch.old_logp, batch.advantages, batch.returns, self.e_clip, self.entropy_coef, self.vf_coef)
+            batch.old_logp, batch.advantages, batch.returns, self.e_clip, self.entropy_coef, self.vf_coef,
+            hparams=self._hparams_dev, old_value=batch.old_values, stats=self._ppo_stats)
         self._n_actions[:5].copy_(n_actions)
         torch.autograd.backward([packed, logits['target_unit']], [d_packed, d_tu])                     # :672
         # drop every reference into this step's autograd graph: a graph kept alive until the next forward keeps its saved
@@ -726,7 +805,8 @@ class DotaOptimizer:
             ddp.auto_reduce = True
         ops.grad_finish(self.flat.param, self.flat.grad_full, self.exp_avg, self.exp_avg_sq, self.adam_steps,
                         self.flat.seg_lo, self.flat.seg_hi, self.flat.seg_head, self.flat.total, self.learning_rate, self.ADAM_BETAS,
-                        self.ADAM_EPS, self.MAX_GRAD_NORM, out, self._metrics, self._finish_ws)     # :674-681
+                        self.ADAM_EPS, self.MAX_GRAD_NORM, out, self._metrics, self._finish_ws,
+                        hparams=self._hparams_dev)                                                  # :674-681
         return out, self._metrics
 
     # -- CUDA graph of the step ----------------------------------------------------------------------
@@ -736,7 +816,9 @@ class DotaOptimizer:
         buffers (device to device) -- or, for a batch that ``prefetch`` uploaded into an input slot (``static`` = the batch
         itself), are already there; parameters, gradients, Adam state and step counters are the same device buffers the
         eager path uses, so eager and graphed steps can be mixed freely."""
-        key = (batch.seq_len, batch.batch_size) if static is None else (batch.seq_len, batch.batch_size, id(static._slot))
+        key = (batch.seq_len, batch.batch_size, batch.old_values is not None)      # old_values: one more static input
+        if static is not None:
+            key += (id(static._slot),)
         entry = self._graphs.get(key)
         if entry is None:
             self._graphs[key] = "seen"
@@ -808,7 +890,7 @@ class DotaOptimizer:
         the pinned host batch into the set that is not being trained on (copy stream, behind the replay that last read that
         set) and ``train`` replays the graph captured over that set -- so the upload of step k+1 overlaps the graph of step k.
         Returns None (caller falls back to per-tensor uploads) when both sets are still waiting to be trained on."""
-        key = (host.seq_len, host.batch_size)
+        key = (host.seq_len, host.batch_size, host.old_values is not None)
         slots = self._input_slots.setdefault(key, [])
         slot = next((sl for sl in slots if not sl["busy"]), None)
         if slot is None:
@@ -874,7 +956,7 @@ class DotaOptimizer:
         graph_setting, self.use_cuda_graph = self.use_cuda_graph, self.use_cuda_graph and shape == self._last_iteration_shape
         self._last_iteration_shape = shape
 
-        losses, entropies, grad_norms = [], [], []
+        losses, entropies, grad_norms, ppo_stats = [], [], [], []
         start_optimizing = time.time()
         try:
             for ep in range(self.epochs):                                  # :469
@@ -883,6 +965,7 @@ class DotaOptimizer:
                 losses.append(loss_d)
                 entropies.append(entropy_d)
                 grad_norms.append(grad_norm_d)
+                ppo_stats.append(self.last_ppo_stats)
         finally:
             self.use_cuda_graph = graph_setting
         time_optimizing = time.time() - start_optimizing
@@ -914,6 +997,8 @@ class DotaOptimizer:
             metrics['grad_norm/{}'.format(k)] = v.mean()
         for k, v in reward_dict.items():
             metrics['reward_per_sec/{}'.format(k)] = v
+        for k in ppo_stats[0]:                                             # means over the epochs
+            metrics['ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
         logger.info('steps_per_s={:.2f}, avg_weight_age={:.1f}, loss={:.4f}, entropy={:.3f}'.format(
             metrics[self.SPEED_KEY], float(metrics['avg_weight_age']), float(metrics['loss/sum']), float(metrics['entropy'])))
         if self.checkpoint:
@@ -922,16 +1007,51 @@ class DotaOptimizer:
         return metrics
 
 
+class _ParamGroup(collections.abc.MutableMapping):
+    """The one torch-style parameter group of ``_FusedAdamHandle``.  Its ``'lr'`` is the owner's ``learning_rate``, read
+    and written through, so the usual ``optimizer.param_groups[0]['lr'] = x`` sets the learning rate of the next step."""
+
+    def __init__(self, owner, entries):
+        self._owner = owner
+        self._entries = {k: v for k, v in entries.items() if k != 'lr'}
+
+    def __getitem__(self, key):
+        return self._owner.learning_rate if key == 'lr' else self._entries[key]
+
+    def __setitem__(self, key, value):
+        if key == 'lr':
+            self._owner.learning_rate = value
+        else:
+            self._entries[key] = value
+
+    def __delitem__(self, key):
+        if key == 'lr':
+            raise KeyError("'lr' is the optimizer's learning_rate and cannot be removed")
+        del self._entries[key]
+
+    def __iter__(self):
+        yield 'lr'
+        yield from self._entries
+
+    def __len__(self):
+        return 1 + len(self._entries)
+
+    def __repr__(self):
+        return repr(dict(self))
+
+
 class _FusedAdamHandle:
     """Minimal ``optimizer``-attribute stand-in: the Adam update itself is fused into ``dc_grad_finish``."""
 
     def __init__(self, owner):
         self._owner = owner
         self.defaults = {'lr': owner.learning_rate, 'betas': owner.ADAM_BETAS, 'eps': owner.ADAM_EPS, 'weight_decay': 0}
+        self._param_groups = [_ParamGroup(owner, dict(self.defaults, params=list(owner.flat.params)))]
 
     @property
     def param_groups(self):
-        return [dict(self.defaults, lr=self._owner.learning_rate, params=list(self._owner.flat.params))]
+        """Persistent groups: writes to ``param_groups[0]['lr']`` reach the owner's ``learning_rate``."""
+        return self._param_groups
 
     def zero_grad(self, set_to_none=False):
         self._owner.flat.zero_grad()
@@ -1000,14 +1120,17 @@ def init_distribution(backend='nccl'):
 
 def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          pretrained_model, mq_prefetch_count, log_dir, entropy_coef, vf_coef, run_local,
-         hidden_size=256, cell="gru", num_layers=1):
+         hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
+         value_clip=None):
+    check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip)     # before any process-group setup
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
     dota_optimizer = DotaOptimizer(
         rmq_host=rmq_host, rmq_port=rmq_port, epochs=epochs, min_seq_per_epoch=min_seq_per_epoch, seq_len=seq_len,
         learning_rate=learning_rate, checkpoint=is_master(), pretrained_model=pretrained_model,
         mq_prefetch_count=mq_prefetch_count, log_dir=log_dir, entropy_coef=entropy_coef, vf_coef=vf_coef,
-        run_local=run_local, hidden_size=hidden_size, cell=cell, num_layers=num_layers)
+        run_local=run_local, hidden_size=hidden_size, cell=cell, num_layers=num_layers, gamma=gamma,
+        gae_lambda=gae_lambda, clip_range=clip_range, max_grad_norm=max_grad_norm, value_clip=value_clip)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -1020,7 +1143,8 @@ def default_log_dir():
 
 
 def build_arg_parser():
-    """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell`` and ``--num-layers``."""
+    """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell``, ``--num-layers`` and the PPO
+    settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm`` and ``--value-clip``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -1039,6 +1163,12 @@ def build_arg_parser():
     p.add_argument("--hidden-size", type=int, help="recurrent width, a multiple of 32 (reference: 256)", default=256)
     p.add_argument("--cell", type=str, choices=['gru', 'lstm'], help="recurrent cell (reference: gru)", default='gru')
     p.add_argument("--num-layers", type=int, help="recurrent layers (reference: 1)", default=1)
+    p.add_argument("--gamma", type=float, help="discount factor, in (0, 1] (reference: 0.98)", default=GAMMA)
+    p.add_argument("--gae-lambda", type=float, help="GAE lambda, in [0, 1] (reference: 0.97)", default=LAMBDA)
+    p.add_argument("--clip-range", type=float, help="PPO ratio clip range (reference: 0.1)", default=0.1)
+    p.add_argument("--max-grad-norm", type=float, help="global gradient-norm clip (reference: 0.5)", default=0.5)
+    p.add_argument("--value-clip", type=float, default=None,
+                   help="PPO2 value-loss clip range around the prep-time values (default: no value clipping)")
     return p
 
 
@@ -1050,6 +1180,7 @@ if __name__ == '__main__':
              seq_len=args.seq_len, learning_rate=args.learning_rate, pretrained_model=args.pretrained_model,
              mq_prefetch_count=args.mq_prefetch_count, log_dir=args.log_dir, entropy_coef=args.entropy_coef,
              vf_coef=args.vf_coef, run_local=args.run_local, hidden_size=args.hidden_size, cell=args.cell,
-             num_layers=args.num_layers)
+             num_layers=args.num_layers, gamma=args.gamma, gae_lambda=args.gae_lambda, clip_range=args.clip_range,
+             max_grad_norm=args.max_grad_norm, value_clip=args.value_clip)
     except KeyboardInterrupt:
         pass

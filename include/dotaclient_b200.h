@@ -194,6 +194,45 @@ int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEADS], const i
                                 float *dvalue, int64_t ld_dvalue, float *out, int32_t *n_actions,
                                 void *workspace, dc_stream_t stream);
 
+/* ---- device-resident hyper-parameters --------------------------------------------------
+ * The `_dev` entry points read their scalar hyper-parameters from a small DEVICE block of DC_HPARAM_SLOTS fp64 values
+ * instead of from kernel arguments, so a CUDA graph that captured them sees new values on every replay (the caller
+ * rewrites the block with an asynchronous copy before launching).  Each value is rounded to the type the scalar-argument
+ * entry point uses: e_clip, entropy_coef, vf_coef, value_clip to float, lr to double, max_grad_norm to float, so at the
+ * same values the results are bit-identical to dc_ppo_loss_fwd_bwd_strided / dc_grad_finish.
+ */
+#define DC_HPARAM_SLOTS 8
+#define DC_HP_LR 0             /* Adam learning rate                                               */
+#define DC_HP_E_CLIP 1         /* PPO ratio clip range epsilon                                     */
+#define DC_HP_ENTROPY_COEF 2
+#define DC_HP_VF_COEF 3
+#define DC_HP_MAX_GRAD_NORM 4  /* global gradient-norm clip                                        */
+#define DC_HP_VALUE_CLIP 5     /* PPO2 value clip range; <= 0: unclipped value loss. Slots 6, 7: 0 */
+
+/* Loss + gradient as dc_ppo_loss_fwd_bwd_strided, hyper-parameters from `hparams` [DC_HPARAM_SLOTS] (device), plus:
+ *   old_value [N] fp32 or NULL: critic values at experience prep.  When hparams[DC_HP_VALUE_CLIP] = eps > 0 and
+ *       old_value is not NULL, the value loss is 0.5*vf_coef*mean(max((v-R)^2, (v_old + clip(v-v_old, -eps, eps) - R)^2))
+ *       and its gradient goes through the larger branch; otherwise it is exactly the unclipped loss.
+ *   stats [DC_PPO_STATS_SLOTS] fp32 out, or NULL to skip: accumulated in the same pass over the tokens, in float64:
+ *       0 approximate KL (k3 estimator (r-1) - log r, r = exp(logp - old_logp)), the mean over the heads with action rows;
+ *       1..5 per head, averaged over the head's action rows (0 for a head without any);
+ *       6 clip fraction (share of action rows with |r-1| > e_clip), the same mean; 7..11 per head;
+ *       12 explained variance 1 - Var(ret - v) / Var(ret) over all N tokens, padding included (NaN if Var(ret) = 0);
+ *       13..15 zero.
+ */
+#define DC_PPO_STATS_SLOTS 16
+#define DC_STAT_APPROX_KL 0
+#define DC_STAT_CLIP_FRACTION 6
+#define DC_STAT_EXPLAINED_VAR 12
+int dc_ppo_loss_fwd_bwd_dev(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                            const uint8_t *const masks[DC_NUM_HEADS],
+                            const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
+                            const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                            const float *old_value, int64_t N, const double *hparams,
+                            float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                            float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
+                            void *workspace, dc_stream_t stream);
+
 /* Log-prob of the taken action per head, [N,5] dense (0 where the head took no action):
  * the no-grad half of experiences_from_rollout (optimizer.py:387-390). */
 int dc_selected_logp(const float *const logits[DC_NUM_HEADS],
@@ -223,6 +262,11 @@ int dc_grad_finish(float *flat_param, float *flat_grad, float *exp_avg, float *e
                    int64_t total, double lr, double beta1, double beta2, double adam_eps,
                    double max_norm, const float *loss_out, float *metrics, void *workspace,
                    dc_stream_t stream);
+/* Same, with lr and max_norm read from hparams[DC_HP_LR] / hparams[DC_HP_MAX_GRAD_NORM] (device, see above). */
+int dc_grad_finish_dev(float *flat_param, float *flat_grad, float *exp_avg, float *exp_avg_sq,
+                       int32_t *steps, const int64_t *seg_lo, const int64_t *seg_hi, const int32_t *seg_head, int n_seg,
+                       int64_t total, const double *hparams, double beta1, double beta2, double adam_eps,
+                       const float *loss_out, float *metrics, void *workspace, dc_stream_t stream);
 #define DC_FINISH_WORKSPACE_BYTES 1024
 
 /* ---- actor side: hierarchical action selection for a batch of A agents in one launch ----------------
