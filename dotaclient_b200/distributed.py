@@ -40,8 +40,8 @@ class DistributedDataParallelSparseParamCPU(Module):
         self.module = module
         self.flat = flat_space if flat_space is not None else FlatParameterSpace.of(module)
         self.needs_reduction = False
-        # When an owner (DotaOptimizer.train) fuses the count-divide into its finish kernel it takes over
-        # the reduction and sets this to False for the duration of its backward.
+        # A caller that runs a backward through the wrapper's forward but reduces by itself (allreduce_gradients) sets
+        # this to False.  DotaOptimizer.train does not need it: it runs the module directly, so needs_reduction stays False.
         self.auto_reduce = True
         self.sync_parameters()
 

@@ -9,7 +9,7 @@ data-gradient kernels and takes the head's rank-1 share through token-level prod
 import torch
 
 from . import _lib
-from .ops import PROFILE, _f32c, _need_cuda, gemm_tf32x3, gemm_wgrad_supported, wait_h2d
+from .ops import PROFILE, _f32c, _need_cuda, gemm_tf32x3, gemm_wgrad_supported
 
 UNITS = (1, 5, 16, 16, 1, 1)              # allied/enemy heroes, allied/enemy non-heroes, allied/enemy towers
 OFFSETS = (0, 1, 6, 22, 38, 39)
@@ -80,10 +80,11 @@ class UnitEncoder(torch.autograd.Function):
 
     maxima slot 5 (enemy towers) is a copy of slot 3 (enemy non-heroes): the reference's ``policy.py:127``.
     ``link`` (a dict) receives the per-group ``basic`` activations and the embedding weights for the target-unit head.
+    ``wait``: see ``unit_encoder``.
     """
 
     @staticmethod
-    def forward(ctx, link, env, w_e, b_e, w_b, b_b, *rest):
+    def forward(ctx, link, wait, env, w_e, b_e, w_b, b_b, *rest):
         units, weights, biases = rest[:6], rest[6:12], rest[12:18]
         ctx.link = link
         _need_cuda(env, w_b, *units)
@@ -103,14 +104,16 @@ class UnitEncoder(torch.autograd.Function):
         argmax = torch.zeros((5, N, C), dtype=torch.uint8, device=dev)         # 1-unit groups: the maximum is unit 0
         env2 = _f32c(env.detach()).reshape(N, 3)
         w_e, b_e = _f32c(w_e.detach()), _f32c(b_e.detach())
-        wait_h2d(env2)
+        if wait is not None:
+            wait(env2)
         with PROFILE.span("env_fwd", 1, 4 * N * (3 + C)):
             _lib.check(lib.dc_env_fwd(env2.data_ptr(), w_e.data_ptr(), b_e.data_ptr(), xcat.data_ptr(), XCAT, N, st), "dc_env_fwd")
         basics = []
         for g, n_u in enumerate(UNITS):
             R = N * n_u
             basic = torch.empty((R, C), dtype=torch.float32, device=dev)
-            wait_h2d(units[g])                       # this group's observations may still be in flight over PCIe
+            if wait is not None:                      # this group's observations may still be in flight over PCIe
+                wait(units[g])
             with PROFILE.span("unit_basic_fwd", 1, 4 * R * (12 + C)):
                 _lib.check(lib.dc_unit_basic_fwd(units[g].data_ptr(), w_b.data_ptr(), b_b.data_ptr(), basic.data_ptr(), R, st),
                            "dc_unit_basic_fwd")
@@ -186,7 +189,7 @@ class UnitEncoder(torch.autograd.Function):
             dw_all += dw_head[:, :6 * C].reshape(C, 6, C).permute(1, 0, 2)
             db_all += dw_head[:, 6 * C:6 * C + 6].t()
         dws, dbs = list(dw_all.unbind(0)), list(db_all.unbind(0))
-        return (None, None, dw_e, db_e, dw_b, db_b) + (None,) * 6 + tuple(dws) + tuple(dbs)
+        return (None, None, None, dw_e, db_e, dw_b, db_b) + (None,) * 6 + tuple(dws) + tuple(dbs)
 
 
 QW = 7 * C     # width of the head's token-level operands: six groups x 128 channels + one block carrying the six bias dots
@@ -235,10 +238,12 @@ class TargetUnit(torch.autograd.Function):
         return d_att.view(ctx.att_shape), None
 
 
-def unit_encoder(env, w_e, b_e, w_b, b_b, units, weights, biases):
-    """-> (``link``: the handle ``target_unit`` needs, pre-rnn input ``[..., 896]``)."""
+def unit_encoder(env, w_e, b_e, w_b, b_b, units, weights, biases, wait=None):
+    """-> (``link``: the handle ``target_unit`` needs, pre-rnn input ``[..., 896]``).  ``wait(tensor)``, when given, makes
+    the current stream wait for an input still being uploaded: it is called for ``env`` and for each unit group right
+    before their first kernel, so the upload of group g+1 overlaps the kernels of group g."""
     link = {}
-    xcat = UnitEncoder.apply(link, env, w_e, b_e, w_b, b_b, *units, *weights, *biases)
+    xcat = UnitEncoder.apply(link, wait, env, w_e, b_e, w_b, b_b, *units, *weights, *biases)
     return link, xcat
 
 

@@ -73,22 +73,6 @@ class _Profile:
 PROFILE = _Profile()
 
 
-# Events of in-flight host->device copies issued on a side stream (ExperienceBatch.to), keyed by the destination's
-# data pointer; the consumer makes the compute stream wait right before the tensor's first use.
-H2D_EVENTS = {}
-
-
-def wait_h2d(*tensors):
-    if not H2D_EVENTS:
-        return
-    for t in tensors:
-        if t is None:
-            continue
-        ev = H2D_EVENTS.pop(t.data_ptr(), None)
-        if ev is not None:
-            torch.cuda.current_stream().wait_event(ev)
-
-
 def _need_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:

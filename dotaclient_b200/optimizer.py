@@ -23,6 +23,7 @@ import re
 import socket
 import threading
 import time
+import typing
 from datetime import datetime
 
 import numpy as np
@@ -218,15 +219,27 @@ class ExperienceBatch:
         self.observations, self.masks, self.actions = observations, masks, actions
         self.old_logp, self.advantages, self.returns, self.h0, self.c0 = old_logp, advantages, returns, h0, c0
         self.old_values = old_values
+        self._ready = {}        # data_ptr -> event of an upload still to be waited for (``to`` from pinned memory)
+        self._slot = None       # the DotaOptimizer input slot whose static buffers these tensors are (``prefetch``)
 
-    def __del__(self):
-        # a batch that was uploaded (prefetched) but never trained on must not leave its ready-events behind: a later tensor
-        # allocated at the same address would otherwise match a stale event
-        try:
-            for ptr in getattr(self, "_h2d_ptrs", ()):
-                ops.H2D_EVENTS.pop(ptr, None)
-        except Exception:                       # interpreter shutdown: module globals may already be gone
-            pass
+    def map(self, fn):
+        """A batch of the same structure with ``fn(tensor)`` in every slot; absent optional fields stay None."""
+        def opt(v):
+            return None if v is None else fn(v)
+        return ExperienceBatch({k: fn(v) for k, v in self.observations.items()}, {k: fn(v) for k, v in self.masks.items()},
+                               {k: fn(v) for k, v in self.actions.items()}, **{f: opt(getattr(self, f)) for f in self.FIELDS})
+
+    def graph_key(self):
+        """The shape a captured step graph is specialised to (old_values: one more static input)."""
+        return self.seq_len, self.batch_size, self.old_values is not None
+
+    def wait(self, *tensors):
+        """Makes the current stream wait for the uploads of ``tensors`` (None allowed) that are still outstanding; each
+        upload is waited for once."""
+        for t in tensors:
+            ev = None if t is None else self._ready.pop(t.data_ptr(), None)
+            if ev is not None:
+                torch.cuda.current_stream().wait_event(ev)
 
     @property
     def seq_len(self):
@@ -250,10 +263,9 @@ class ExperienceBatch:
 
     def to(self, device, non_blocking=True, prefetch=False):
         """Host -> device.  From pinned memory the copies are issued on a side stream in the order the step consumes
-        them (env, states, unit groups, then the loss inputs) and every tensor gets an event: ``train`` makes the
-        compute stream wait per tensor right before first use, so the PCIe transfer of unit group g+1 overlaps the
-        encoder kernels of group g and the loss inputs arrive during forward/backward."""
-        out = ExperienceBatch({}, {}, {}, None, None, None, None, None)
+        them (env, states, unit groups, then the loss inputs) and every tensor gets an event, kept by the returned batch:
+        ``train`` makes the compute stream wait per tensor (``wait``) right before first use, so the PCIe transfer of unit
+        group g+1 overlaps the encoder kernels of group g and the loss inputs arrive during forward/backward."""
         overlap = non_blocking and self.advantages.is_pinned()
         compute = torch.cuda.current_stream(device)
         side = _copy_stream(device) if overlap else None
@@ -266,36 +278,24 @@ class ExperienceBatch:
             if not isinstance(holder, dict) and k in ('h0', 'c0'):
                 return 1
             return 100
-        items = sorted(self.tensors(), key=priority)
-        out._h2d_ptrs = []
-        for holder, k, v in items:
+        moved, ready = {}, {}
+        for _, _, v in sorted(self.tensors(), key=priority):
             if overlap:
                 with torch.cuda.stream(side):
-                    moved = v.to(device, non_blocking=True)
+                    d = v.to(device, non_blocking=True)
                     ev = torch.cuda.Event()
                     ev.record(side)
-                moved.record_stream(compute)
-                ops.H2D_EVENTS[moved.data_ptr()] = ev
-                out._h2d_ptrs.append(moved.data_ptr())
+                d.record_stream(compute)
+                ready[d.data_ptr()] = ev
             else:
-                moved = v.to(device, non_blocking=non_blocking)
-            if isinstance(holder, dict):
-                target = out.observations if holder is self.observations else out.masks if holder is self.masks else out.actions
-                target[k] = moved
-            else:
-                setattr(out, k, moved)
+                d = v.to(device, non_blocking=non_blocking)
+            moved[id(v)] = d
+        out = self.map(lambda v: moved[id(v)])
+        out._ready = ready
         return out
 
     def pin_memory(self):
-        out = ExperienceBatch({}, {}, {}, None, None, None, None, None)
-        for holder, k, v in self.tensors():
-            moved = v.cpu().pin_memory()
-            if isinstance(holder, dict):
-                target = out.observations if holder is self.observations else out.masks if holder is self.masks else out.actions
-                target[k] = moved
-            else:
-                setattr(out, k, moved)
-        return out
+        return self.map(lambda v: v.cpu().pin_memory())
 
     @staticmethod
     def from_sequences(experiences, device):
@@ -318,6 +318,13 @@ class ExperienceBatch:
             old_values = stack([torch.as_tensor(e.values).detach().reshape(-1).float() for e in experiences])
         return ExperienceBatch(obs, masks, actions, old, adv, ret, h0.detach(), None if c0 is None else c0.detach(),
                                old_values=old_values)
+
+
+class _CapturedStep(typing.NamedTuple):
+    """A CUDA graph of the whole step, its static input batch and its device result vector (loss slots)."""
+    static: ExperienceBatch
+    graph: torch.cuda.CUDAGraph
+    out: torch.Tensor
 
 
 _copy_streams = {}
@@ -465,7 +472,7 @@ class DotaOptimizer:
         self.rollout_prefetch = int(rollout_prefetch)
         self._rollout_q, self._prefetch_thread = None, None
         self.use_cuda_graph = True          # replay device-resident batches of a known shape from a captured graph of the step
-        self._graphs = {}
+        self._graphs = {}                   # graph key -> "seen" (ran once), "eager" (capture failed) or a _CapturedStep
         self._input_slots = {}              # batch shape -> up to two sets of static device input buffers (prefetch + graph)
         self._last_iteration_shape = None
         self.time_last_it = time.time()
@@ -717,16 +724,18 @@ class DotaOptimizer:
                              % self.value_clip)
         t_enter = time.perf_counter()
         self._upload_hparams()
-        slot = getattr(batch, "_slot", None)
+        slot = batch._slot
         if slot is not None:                       # uploaded by prefetch() straight into a graph's static input buffers
             torch.cuda.current_stream().wait_event(slot["ready"])
-            out, metrics = self._replay_step(batch, static=batch) if not ops.PROFILE.enabled else self._enqueue_step(batch)
-            slot["done"].record()
-            slot["busy"] = False
-        elif self.use_cuda_graph and not ops.H2D_EVENTS and not ops.PROFILE.enabled:
+        # a batch whose uploads are still in flight runs launch by launch, so that each kernel waits only for its own inputs
+        replay = slot is not None or (self.use_cuda_graph and not batch._ready)
+        if replay and not ops.PROFILE.enabled:
             out, metrics = self._replay_step(batch)
         else:
             out, metrics = self._enqueue_step(batch)
+        if slot is not None:
+            slot["done"].record()
+            slot["busy"] = False
         host = self._host_result
         host[:_lib.LOSS_SLOTS].copy_(out, non_blocking=True)
         host[_lib.LOSS_SLOTS:].copy_(self._result_dev, non_blocking=True)        # metrics, then the PPO diagnostics
@@ -777,32 +786,25 @@ class DotaOptimizer:
         keys = ops.HEAD_KEYS
         self.flat.zero_grad_detached()                                    # :671 (grads gathered into the flat buffer below)
         hidden = (batch.h0, batch.c0) if self.policy_base.cell == "lstm" else batch.h0
-        ddp = self.policy if isinstance(self.policy, DistributedDataParallelSparseParamCPU) else None
-        if ddp is not None:
-            ddp.auto_reduce = False        # the count-divide is fused into the finish kernel below
-        ops.wait_h2d(batch.observations['env'], batch.h0, batch.c0)
-        logits, values, _ = self.policy.forward_time_major(batch.observations, hidden)   # :619
-        ops.wait_h2d(batch.old_logp, batch.advantages, batch.returns, batch.old_values, *batch.masks.values(),
-                     *batch.actions.values(), *batch.observations.values())
-        packed = self.policy_base._packed_heads     # small heads + value are column ranges of one packed GEMM output
+        batch.wait(batch.observations['env'], batch.h0, batch.c0)
+        # :619 on the module itself: the data-parallel wrapper's hook-driven reduction stays idle, the step reduces below
+        packed, target_unit = self.policy_base._train_forward(batch.observations, hidden, wait=batch.wait)
+        batch.wait(batch.old_logp, batch.advantages, batch.returns, batch.old_values, *batch.masks.values(),
+                   *batch.actions.values(), *batch.observations.values())
         # e_clip / entropy_coef / vf_coef / value_clip are read from the device block (_upload_hparams)
         out, n_actions, d_packed, d_tu, _ = ops.ppo_loss_packed(
-            packed, logits['target_unit'], [batch.masks[k] for k in keys], [batch.actions[k] for k in keys],
+            packed, target_unit, [batch.masks[k] for k in keys], [batch.actions[k] for k in keys],
             batch.old_logp, batch.advantages, batch.returns, self.e_clip, self.entropy_coef, self.vf_coef,
             hparams=self._hparams_dev, old_value=batch.old_values, stats=self._ppo_stats)
         self._n_actions[:5].copy_(n_actions)
-        torch.autograd.backward([packed, logits['target_unit']], [d_packed, d_tu])                     # :672
-        # drop every reference into this step's autograd graph: a graph kept alive until the next forward keeps its saved
-        # activations (GBs) AND the parameters' AccumulateGrad nodes, whose stream then mismatches a later graph capture
-        self.policy_base._packed_heads = None
-        del logits, values, packed, d_packed, d_tu
+        torch.autograd.backward([packed, target_unit], [d_packed, d_tu])                                # :672
+        # drop every reference into this step's autograd graph before the gradient finish: it holds the saved activations
+        del packed, target_unit, d_packed, d_tu
         self.flat.gather_grads()
         # distributed.py:29-57 -> flags + ONE all-reduce; divide fused into the finish kernel
         ops.grad_flags(self.flat.grad_full, self.flat.total, self.flat.seg_head, self._n_actions)
-        if ddp is not None:
-            ddp.allreduce_gradients(divide=False, flags_ready=True)
-            ddp.needs_reduction = False
-            ddp.auto_reduce = True
+        if self.policy is not self.policy_base:
+            self.policy.allreduce_gradients(divide=False, flags_ready=True)
         ops.grad_finish(self.flat.param, self.flat.grad_full, self.exp_avg, self.exp_avg_sq, self.adam_steps,
                         self.flat.seg_lo, self.flat.seg_hi, self.flat.seg_head, self.flat.total, self.learning_rate, self.ADAM_BETAS,
                         self.ADAM_EPS, self.MAX_GRAD_NORM, out, self._metrics, self._finish_ws,
@@ -810,45 +812,28 @@ class DotaOptimizer:
         return out, self._metrics
 
     # -- CUDA graph of the step ----------------------------------------------------------------------
-    def _replay_step(self, batch, static=None):
+    def _replay_step(self, batch):
         """Replays the captured step for this batch shape (captures it the second time the shape is seen: the first call of
         a shape runs launch by launch, which also warms every kernel up).  Inputs are copied into the graph's static
-        buffers (device to device) -- or, for a batch that ``prefetch`` uploaded into an input slot (``static`` = the batch
-        itself), are already there; parameters, gradients, Adam state and step counters are the same device buffers the
-        eager path uses, so eager and graphed steps can be mixed freely."""
-        key = (batch.seq_len, batch.batch_size, batch.old_values is not None)      # old_values: one more static input
-        if static is not None:
-            key += (id(static._slot),)
+        buffers (device to device) -- or, for a batch that ``prefetch`` uploaded into an input slot (the graph's static
+        inputs are then the batch itself), are already there; parameters, gradients, Adam state and step counters are the
+        same device buffers the eager path uses, so eager and graphed steps can be mixed freely."""
+        key = batch.graph_key() if batch._slot is None else batch.graph_key() + (id(batch._slot),)
         entry = self._graphs.get(key)
-        if entry is None:
-            self._graphs[key] = "seen"
-            return self._enqueue_step(batch)
         if entry == "seen":
-            for k in [k for k, v in self._graphs.items() if isinstance(v, tuple)][:-1]:
+            for k in [k for k, v in self._graphs.items() if isinstance(v, _CapturedStep)][:-1]:
                 del self._graphs[k]            # at most two captured shapes alive: a graph pins its step's activations
-            entry = self._capture_step(batch, static)
-            self._graphs[key] = entry
-            if entry == "eager":
-                return self._enqueue_step(batch)
-        elif entry == "eager":
+            entry = self._graphs[key] = self._capture_step(batch)
+        if not isinstance(entry, _CapturedStep):   # first sight of this shape, or its capture failed
+            self._graphs.setdefault(key, "seen")
             return self._enqueue_step(batch)
-        graph_static, graph, out = entry
-        if static is None:
-            srcs = [v for _, _, v in batch.tensors()]
-            dsts = [v for _, _, v in graph_static.tensors()]
-            torch._foreach_copy_(dsts, srcs)
-        graph.replay()
-        return out, self._metrics
+        if entry.static is not batch:
+            torch._foreach_copy_([v for _, _, v in entry.static.tensors()], [v for _, _, v in batch.tensors()])
+        entry.graph.replay()
+        return entry.out, self._metrics
 
-    def _capture_step(self, batch, static=None):
-        if static is None:
-            static = ExperienceBatch({}, {}, {}, None, None, None, None, None)
-            for holder, k, v in batch.tensors():
-                c = v.detach().clone()
-                if isinstance(holder, dict):
-                    (static.observations if holder is batch.observations else static.masks if holder is batch.masks else static.actions)[k] = c
-                else:
-                    setattr(static, k, c)
+    def _capture_step(self, batch):
+        static = batch if batch._slot is not None else batch.map(lambda v: v.detach().clone())
         graph = torch.cuda.CUDAGraph()
         # A garbage collection during the capture would free unreachable objects -- among them the captured graphs of an
         # optimizer nobody references any more -- and destroying a graph is not permitted while a stream is capturing: it
@@ -868,7 +853,7 @@ class DotaOptimizer:
         finally:
             if gc_was_enabled:
                 gc.enable()
-        return static, graph, out
+        return _CapturedStep(static, graph, out)
 
     def prefetch(self, experiences):
         """Starts the asynchronous upload of a pinned-host ``ExperienceBatch`` on the copy stream and returns the device batch
@@ -890,19 +875,12 @@ class DotaOptimizer:
         the pinned host batch into the set that is not being trained on (copy stream, behind the replay that last read that
         set) and ``train`` replays the graph captured over that set -- so the upload of step k+1 overlaps the graph of step k.
         Returns None (caller falls back to per-tensor uploads) when both sets are still waiting to be trained on."""
-        key = (host.seq_len, host.batch_size, host.old_values is not None)
-        slots = self._input_slots.setdefault(key, [])
+        slots = self._input_slots.setdefault(host.graph_key(), [])
         slot = next((sl for sl in slots if not sl["busy"]), None)
         if slot is None:
             if len(slots) >= 2:
                 return None
-            dev_batch = ExperienceBatch({}, {}, {}, None, None, None, None, None)
-            for holder, k, v in host.tensors():
-                c = torch.empty(v.shape, dtype=v.dtype, device=self.device)
-                if isinstance(holder, dict):
-                    (dev_batch.observations if holder is host.observations else dev_batch.masks if holder is host.masks else dev_batch.actions)[k] = c
-                else:
-                    setattr(dev_batch, k, c)
+            dev_batch = host.map(lambda v: torch.empty(v.shape, dtype=v.dtype, device=self.device))
             slot = {"batch": dev_batch, "busy": False, "ready": torch.cuda.Event(), "done": torch.cuda.Event()}
             slot["done"].record()
             dev_batch._slot = slot

@@ -133,15 +133,23 @@ class Policy(nn.Module):
         so ``DotaOptimizer.train`` pays no transposes.  ``observations`` is a dict keyed by INPUT_KEYS."""
         return self._run(tuple(observations[k] for k in self.INPUT_KEYS), hidden, time_major=True)
 
+    def _train_forward(self, observations, hidden, wait=None):
+        """The training step's forward on time-major inputs -> (the packed ``[S, B, ops.PACK_WIDTH]`` output of the four
+        small heads and the value head, target-unit logits ``[S, B, 40]``): the tensors the fused PPO loss reads and
+        backward starts from.  ``wait`` (see ``encoder_ops.unit_encoder``) lets the observations arrive while it runs."""
+        x, unit_embedding = self._encode(observations['env'], [observations[k] for k in self.INPUT_KEYS[1:]], wait=wait)
+        y, _ = self._recur(x.contiguous(), hidden)
+        return self._head_outputs(y, unit_embedding)
+
     # ------------------------------------------------------------------ implementation
-    def _encode(self, env, groups):
+    def _encode(self, env, groups, wait=None):
         """Observation encoders (``policy.py:97-138``) -> (x ``[..., H]``, encoder handle for the target-unit head): the explicit
         kernel chain of ``csrc/encoder.cu`` + wgmma GEMMs (no ``torch.cat``, no materialised ``[..., 40, 128]`` unit embedding)."""
         layers = [getattr(self, "affine_unit_" + s) for s, _, _ in UNIT_GROUPS]
         unit_embedding, x = encoder_ops.unit_encoder(
             env, self.affine_env.weight, self.affine_env.bias,
             self.affine_unit_basic_stats.weight, self.affine_unit_basic_stats.bias, list(groups),
-            [l.weight for l in layers], [l.bias for l in layers])
+            [l.weight for l in layers], [l.bias for l in layers], wait=wait)
         return ops.linear(x, self.affine_pre_rnn.weight, self.affine_pre_rnn.bias, relu=True), unit_embedding
 
     def _recur(self, x_tm, hidden):
@@ -161,10 +169,10 @@ class Policy(nn.Module):
         h_n = ops.stack_layers(hs)
         return y, ((h_n, ops.stack_layers(cs)) if lstm else h_n)
 
-    def _heads(self, y, unit_embedding):
-        """Action heads + value (``policy.py:144-155``): the attention projection and ONE packed ``[*, 128]`` tensor-core GEMM
-        for the four small heads + the value head (26 real rows, zero padding; their logits are column ranges of its
-        output, ``ops.PACK_COLS``), then the target-unit dot products."""
+    def _head_outputs(self, y, unit_embedding):
+        """The attention projection and ONE packed ``[*, 128]`` tensor-core GEMM for the four small heads + the value head
+        (26 real rows, zero padding; their logits are column ranges of its output, ``ops.PACK_COLS``), then the target-unit
+        dot products -> (packed output, target-unit logits)."""
         attention = ops.linear(y, self.affine_unit_attention.weight, self.affine_unit_attention.bias)
         H = self.hidden_size
         pad = y.new_zeros(ops.PACK_WIDTH - 26, H)
@@ -173,11 +181,14 @@ class Policy(nn.Module):
         b_pack = torch.cat([self.affine_head_enum.bias, self.affine_move_x.bias, self.affine_move_y.bias,
                             self.affine_head_ability.bias, self.affine_value.bias, pad[:, 0]], dim=0)
         packed = ops.linear(y, w_pack, b_pack)
-        self._packed_heads = packed                      # DotaOptimizer.train feeds gradients to it directly
+        return packed, encoder_ops.target_unit(attention, unit_embedding)
+
+    def _heads(self, y, unit_embedding):
+        """Action heads + value (``policy.py:144-155``): column ranges of the packed output, and the target-unit logits."""
+        packed, target_unit = self._head_outputs(y, unit_embedding)
         cols = ops.PACK_COLS
         head_enum, move_x, move_y, ability, value = (packed[..., cols[k][0]:cols[k][1]]
                                                      for k in ("enum", "x", "y", "ability", "value"))
-        target_unit = encoder_ops.target_unit(attention, unit_embedding)
         return {'enum': head_enum, 'x': move_x, 'y': move_y, 'target_unit': target_unit, 'ability': ability}, value
 
     def _run(self, obs, hidden, time_major):

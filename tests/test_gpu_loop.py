@@ -122,6 +122,26 @@ def test_prefetch_double_buffers_the_upload(tmp_path):
     torch.testing.assert_close(opt.flat.param, twin.flat.param, rtol=0, atol=1e-7)
 
 
+def test_pending_upload_leaves_other_batches_on_the_graph_path(tmp_path):
+    """A batch uploaded from pinned memory and not trained on yet keeps its ready-events to itself: a different
+    device-resident batch trained meanwhile is captured and replayed from a CUDA graph, and the uploaded batch, trained
+    afterwards, gives the same step as the same batch trained from device memory."""
+    from dotaclient_b200.optimizer import ExperienceBatch
+    opt = _optimizer(tmp_path, uuid.uuid4().int % 100000, checkpoint=False)
+    twin = _optimizer(tmp_path, uuid.uuid4().int % 100000, checkpoint=False)
+    a, p_dev = [ExperienceBatch.from_sequences(opt.experiences_from_rollout(make_rollout(32, s)), opt.device) for s in (5, 6)]
+    p = p_dev.pin_memory().to(opt.device)                                # copies in flight on the side stream, not prefetch()
+    for _ in range(3):
+        opt.train(a)
+        twin.train(a)
+    assert isinstance(opt._graphs.get((8, 4, True)), tuple), "the step was never captured"
+    l1, _, g1 = opt.train(p)
+    l2, _, g2 = twin.train(p_dev)
+    np.testing.assert_allclose(float(l1["loss"]), float(l2["loss"]), rtol=1e-6)
+    np.testing.assert_allclose(float(g1["unclipped"]), float(g2["unclipped"]), rtol=1e-6)
+    torch.testing.assert_close(opt.flat.param, twin.flat.param, rtol=0, atol=1e-7)
+
+
 @pytest.mark.parametrize("cell", ["gru", "lstm"])
 def test_batched_experience_prep_equals_per_rollout_prep(tmp_path, cell):
     """experiences_from_rollouts (one batched pass over ragged rollouts) == experiences_from_rollout per rollout

@@ -169,6 +169,21 @@ def test_experience_batch_old_values_is_optional():
     assert positional.old_values is None and positional.c0 is None
 
 
+@pytest.mark.parametrize("old_values", [False, True])
+def test_experience_batch_map_keeps_structure(old_values):
+    batch = _tiny_batch(old_values)
+    doubled = batch.map(lambda v: torch.cat([v, v], dim=-1))
+    assert doubled.c0 is None and (doubled.old_values is None) == (not old_values)
+    assert [(type(h), k) for h, k, _ in doubled.tensors()] == [(type(h), k) for h, k, _ in batch.tensors()]
+    for (_, _, a), (_, _, b) in zip(batch.tensors(), doubled.tensors()):
+        assert b.dtype == a.dtype and b.shape == a.shape[:-1] + (2 * a.shape[-1],) and torch.equal(b[..., :a.shape[-1]], a)
+    same = batch.map(lambda v: v)
+    assert all(a is b for (_, _, a), (_, _, b) in zip(batch.tensors(), same.tensors()))
+    assert same.graph_key() == batch.graph_key() == (4, 3, old_values)
+    if torch.cuda.is_available():                       # pinning needs the CUDA driver
+        assert batch.pin_memory().graph_key() == batch.graph_key()
+
+
 def test_from_sequences_fills_old_values_from_sequence_values():
     from dotaclient_b200.optimizer import ExperienceBatch, Sequence
     from dotaclient_b200.synthetic import make_rollout
