@@ -19,6 +19,7 @@ SIGNATURES = {
     "dc_last_error": (_c.c_char_p, []),
     "dc_device_info": (_i32, [_c.POINTER(_i32)] * 3),
     "dc_gae_scan": (_i32, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _vp, _vp, _vp]),
+    "dc_vtrace_scan": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _f64, _f64, _vp, _vp, _vp, _vp]),
     "dc_rnn_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "dc_rnn_seq_fwd": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "dc_rnn_seq_bwd": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
@@ -60,6 +61,7 @@ HP_LR, HP_E_CLIP, HP_ENTROPY_COEF, HP_VF_COEF, HP_MAX_GRAD_NORM, HP_VALUE_CLIP =
 # the PPO diagnostics written by dc_ppo_loss_fwd_bwd_dev (DC_STAT_* in include/dotaclient_b200.h)
 PPO_STATS_SLOTS = 16
 STAT_APPROX_KL, STAT_CLIP_FRACTION, STAT_EXPLAINED_VAR = 0, 6, 12
+VTRACE_STATS_SLOTS = 8      # per-segment fp64 sums written by dc_vtrace_scan (DC_VTRACE_STATS_SLOTS)
 MAX_PARAM_TENSORS = 96      # kMaxSeg of csrc/grad_finish.cu: parameter tensors dc_grad_flags / dc_grad_finish can handle
 
 _lib = None

@@ -12,31 +12,11 @@
 //
 // HBM traffic: (4*n_sub + 4) read + 8 written bytes per row -- 16 B/row with pre-summed rewards.
 #include "dc_common.cuh"
+#include "np_sum.cuh"
 
 namespace {
 
-// numpy's pairwise float32 add-reduce over a contiguous axis for n < 128 (8 accumulators,
-// combined as ((0+1)+(2+3))+((4+5)+(6+7)), remainder added sequentially).
-__device__ __forceinline__ float np_sum_row(const float *__restrict__ p, int n) {
-    if (n == 1) return p[0];
-    if (n < 8) {
-        float s = p[0];
-        for (int i = 1; i < n; ++i) s = __fadd_rn(s, p[i]);
-        return s;
-    }
-    float r[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) r[j] = p[j];
-    int i = 8;
-    for (; i < n - (n % 8); i += 8) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) r[j] = __fadd_rn(r[j], p[i + j]);
-    }
-    float s = __fadd_rn(__fadd_rn(__fadd_rn(r[0], r[1]), __fadd_rn(r[2], r[3])),
-                        __fadd_rn(__fadd_rn(r[4], r[5]), __fadd_rn(r[6], r[7])));
-    for (; i < n; ++i) s = __fadd_rn(s, p[i]);
-    return s;
-}
+using dc::np_sum_row;
 
 __global__ void __launch_bounds__(128) gae_scan_kernel(const float *__restrict__ rewards, int n_sub,
                                                         const float *__restrict__ values,

@@ -117,6 +117,44 @@ def gae_scan(rewards, values, seg_off, gamma=0.98, lam=0.97, boot_value=None, bo
     return adv, ret
 
 
+def vtrace_scan(rewards, values, logp_target, logp_behaviour, seg_off, gamma, lam, rho_clip, c_clip, boot_value=None,
+                valid_len=None, stats=False):
+    """V-trace value targets and policy-gradient advantages for many rollouts (``dc_vtrace_scan``).
+
+    rewards [n_rows] or [n_rows, n_sub] fp32; values [n_rows]; logp_target / logp_behaviour [n_rows, 5] (0 where a head
+    took no action); seg_off int64 [n_seg+1]; boot_value [n_seg] fp32 or None (0); valid_len int64 [n_seg] or None: the
+    real steps of each segment, the only rows the statistics cover.  Returns ``(pg_adv, vs)``, and with ``stats`` also the
+    per-segment sums ``[n_seg, _lib.VTRACE_STATS_SLOTS]`` fp64 (token count, sum log rho, sum clipped rho, rows with
+    rho > rho_clip, rows with rho > c_clip).
+    """
+    _need_cuda(rewards, values, logp_target, logp_behaviour, seg_off, boot_value, valid_len)
+    rewards, values = _f32c(rewards), _f32c(values)
+    logp_target, logp_behaviour = _f32c(logp_target), _f32c(logp_behaviour)
+    n_sub = 1 if rewards.dim() == 1 else rewards.shape[1]
+    n_rows = values.numel()
+    assert rewards.numel() == n_rows * n_sub
+    assert logp_target.numel() == n_rows * 5 and logp_behaviour.numel() == n_rows * 5
+    seg_off = seg_off.to(torch.int64).contiguous()
+    n_seg = seg_off.numel() - 1
+    if boot_value is not None:
+        boot_value = _f32c(boot_value)
+        assert boot_value.numel() == n_seg
+    if valid_len is not None:
+        valid_len = valid_len.to(torch.int64).contiguous()
+        assert valid_len.numel() == n_seg
+    pg_adv = torch.empty(n_rows, dtype=torch.float32, device=values.device)
+    vs = torch.empty_like(pg_adv)
+    seg_stats = torch.empty((n_seg, _lib.VTRACE_STATS_SLOTS), dtype=torch.float64, device=values.device) if stats else None
+    lib = _lib.load()
+    with PROFILE.span("vtrace_scan", 1):
+        _lib.check(lib.dc_vtrace_scan(rewards.data_ptr(), n_sub, values.data_ptr(), logp_target.data_ptr(),
+                                      logp_behaviour.data_ptr(), seg_off.data_ptr(), n_seg, _lib.ptr(valid_len),
+                                      _lib.ptr(boot_value), float(gamma), float(lam), float(rho_clip), float(c_clip),
+                                      pg_adv.data_ptr(), vs.data_ptr(), _lib.ptr(seg_stats), _lib.stream_ptr()),
+                   "dc_vtrace_scan")
+    return (pg_adv, vs, seg_stats) if stats else (pg_adv, vs)
+
+
 # --------------------------------------------------------------------------------------------- RNN
 _workspaces = {}
 

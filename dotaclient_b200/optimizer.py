@@ -344,9 +344,14 @@ def all_gather(t):                                                        # :193
 
 
 # ------------------------------------------------------------------------------------------ optimizer
-def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None):
+ADVANTAGE_ESTIMATORS = ('gae', 'vtrace')
+
+
+def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
+                       vtrace_rho_clip=1.0, vtrace_c_clip=1.0):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
-    max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too).  NaN fails every check."""
+    max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
+    vtrace_rho_clip > 0 and vtrace_c_clip > 0.  NaN fails every check."""
     def number(name, v):
         if isinstance(v, bool) or not isinstance(v, numbers.Real):
             raise ValueError("%s=%r is not a number" % (name, v))
@@ -361,6 +366,34 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
         raise ValueError("max_grad_norm=%r: the gradient-norm limit must be > 0" % (max_grad_norm,))
     if value_clip is not None and not number('value_clip', value_clip) >= 0.0:
         raise ValueError("value_clip=%r: the value clip range must be >= 0 (or None: no value clipping)" % (value_clip,))
+    if advantage_estimator not in ADVANTAGE_ESTIMATORS:
+        raise ValueError("advantage_estimator=%r: must be one of %s" % (advantage_estimator, ", ".join(ADVANTAGE_ESTIMATORS)))
+    if not number('vtrace_rho_clip', vtrace_rho_clip) > 0.0:
+        raise ValueError("vtrace_rho_clip=%r: the V-trace rho truncation must be > 0" % (vtrace_rho_clip,))
+    if not number('vtrace_c_clip', vtrace_c_clip) > 0.0:
+        raise ValueError("vtrace_c_clip=%r: the V-trace c truncation must be > 0" % (vtrace_c_clip,))
+
+
+def check_behaviour_logp(datas):
+    """Raises ``ValueError``, naming the rollout's ``game_id`` / ``player_id``, when a rollout lacks ``'behaviour_logp'``,
+    when it is not ``[L, 5]``, or when it is not finite on a head that took an action (the host ``actions`` say which).
+    Runs on the host before anything is uploaded; values on heads that did not act are ignored."""
+    for d in datas:
+        who = "rollout game_id=%r player_id=%r" % (d.get('game_id'), d.get('player_id'))
+        if 'behaviour_logp' not in d:
+            raise ValueError("%s has no 'behaviour_logp': advantage_estimator='vtrace' needs the actor's log-probabilities "
+                             "of its actions ([L, 5], the logp of Policy.act_batched)" % who)
+        L = int(d['rewards'].shape[0])
+        blp = torch.as_tensor(d['behaviour_logp'])
+        if tuple(blp.shape) != (L, len(ops.HEAD_KEYS)) or not blp.is_floating_point():
+            raise ValueError("%s: 'behaviour_logp' must be a float [%d, %d] array, got %s %s"
+                             % (who, L, len(ops.HEAD_KEYS), blp.dtype, tuple(blp.shape)))
+        acted = torch.stack([torch.as_tensor(d['actions'][k]).reshape(L, -1).any(dim=1) for k in ops.HEAD_KEYS], dim=1)
+        bad = acted & ~torch.isfinite(blp)
+        if bool(bad.any()):
+            t, h = (int(i) for i in bad.nonzero()[0])
+            raise ValueError("%s: 'behaviour_logp' is %r at step %d on head %r, which took an action there"
+                             % (who, float(blp[t, h]), t, ops.HEAD_KEYS[h]))
 
 
 class DotaOptimizer:
@@ -381,13 +414,19 @@ class DotaOptimizer:
                  learning_rate, checkpoint, pretrained_model, mq_prefetch_count, log_dir,
                  entropy_coef, vf_coef, run_local, *, hidden_size=256, cell="gru", num_layers=1, mq=None,
                  iterations=100000, rollout_prefetch=0, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1,
-                 max_grad_norm=0.5, value_clip=None):
+                 max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
                              % (num_layers, self.MAX_LAYERS, _lib.MAX_PARAM_TENSORS))
-        check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip)
+        check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
+                           vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip)
         self.gamma, self.gae_lambda = float(gamma), float(gae_lambda)     # GAE of experience prep (:421)
+        # 'vtrace': experience prep corrects advantages and value targets for the actors' stale weights, from the
+        # behaviour log-probabilities each rollout carries ('behaviour_logp')
+        self.advantage_estimator = advantage_estimator
+        self.vtrace_rho_clip, self.vtrace_c_clip = float(vtrace_rho_clip), float(vtrace_c_clip)
+        self._vtrace_seg_stats = None       # per-rollout sums of the last V-trace prep (device), see last_vtrace_stats
         self.MAX_GRAD_NORM = float(max_grad_norm)     # shadows the class constant; read before every step, like lr below
         self.value_clip = None if value_clip is None else float(value_clip)
         self.rmq_host, self.rmq_port = rmq_host, rmq_port
@@ -578,10 +617,14 @@ class DotaOptimizer:
     def _prepare_rollouts(self, datas):
         """The batched no-grad half of an iteration (SURVEY.md 8(f)2): all rollouts become the batch dimension of ONE
         time-major ``[L_max, R, ...]`` pass -- encoder chain, recurrence from the zero state, heads, selected log-probs
-        (:384-390) -- followed by ONE segmented GAE scan over every rollout's own padded length (:417-421).  Returns the raw
-        device tensors; ``experiences_from_rollouts`` / ``batch_from_rollouts`` slice them."""
+        (:384-390) -- followed by ONE segmented GAE scan over every rollout's own padded length (:417-421), or with
+        ``advantage_estimator='vtrace'`` ONE segmented V-trace scan of the same segments.  Returns the raw device tensors;
+        ``experiences_from_rollouts`` / ``batch_from_rollouts`` slice them."""
         S, dev, pol = self.seq_len, self.device, self.policy_base
         R = len(datas)
+        vtrace = self.advantage_estimator == 'vtrace'
+        if vtrace:
+            check_behaviour_logp(datas)                # refused before anything is uploaded
         Ls = [int(d['rewards'].shape[0]) for d in datas]
         Lps = [(L + S - 1) // S * S for L in Ls]
         Lmax = max(Lps)
@@ -593,8 +636,9 @@ class DotaOptimizer:
         def batched(group, key, dtype):
             """Rollouts -> one time-major ``[Lmax, R, ...]`` device tensor.  The host side only does contiguous per-rollout
             copies into a cached PINNED ``[R, Lmax, ...]`` staging buffer (memcpy speed; stacking time-major on the host is a
-            768-byte-granular scatter, 3x slower) and uploads asynchronously; the transposition to time-major runs on the GPU."""
-            srcs = [torch.as_tensor(d[group][key]) for d in datas]
+            768-byte-granular scatter, 3x slower) and uploads asynchronously; the transposition to time-major runs on the GPU.
+            ``group`` None: a top-level key of the rollout."""
+            srcs = [torch.as_tensor(d[group][key] if group else d[key]) for d in datas]
             shape = (R, Lmax) + tuple(srcs[0].shape[1:])
             buf = self._staging.get((group, key))
             if buf is None or buf.shape != shape or buf.dtype != dtype:
@@ -609,6 +653,7 @@ class DotaOptimizer:
         obs = {k: batched('observations', k, torch.float32) for k in Policy.INPUT_KEYS}
         masks = {k: batched('masks', k, torch.bool) for k in Policy.OUTPUT_KEYS}
         actions = {k: batched('actions', k, torch.bool) for k in Policy.OUTPUT_KEYS}
+        behaviour_logp = batched(None, 'behaviour_logp', torch.float32) if vtrace else None      # [Lmax, R, 5]
         self._staging_event = torch.cuda.Event()
         self._staging_event.record()
         rewards_np = np.zeros((R, Lmax, len(REWARD_KEYS)), dtype=np.float32)
@@ -628,14 +673,28 @@ class DotaOptimizer:
                                          [actions[k] for k in keys]).view(Lmax, R, 5)        # :387-390
             # GAE per rollout over ITS padded length: back-to-back segments, rollout-major
             values_lr = values.reshape(Lmax, R)
+
+            def rollout_major(t):                    # [Lmax, R, ...] -> the rows of every rollout's padded length in turn
+                if same:
+                    return t.transpose(0, 1).reshape((R * Lmax,) + tuple(t.shape[2:]))
+                return torch.cat([t[:Lps[i], i] for i in range(R)])
+            vals_c = rollout_major(values_lr)
             if same:
-                vals_c = values_lr.t().reshape(-1)
                 rew_c = torch.from_numpy(rewards_np.reshape(R * Lmax, -1)).to(dev, non_blocking=True)
             else:
-                vals_c = torch.cat([values_lr[:Lps[i], i] for i in range(R)])
                 rew_c = torch.from_numpy(np.concatenate([rewards_np[i, :Lps[i]] for i in range(R)])).to(dev)
             seg = torch.tensor(np.concatenate([[0], np.cumsum(Lps)]), dtype=torch.int64, device=dev)
-            adv_c, ret_c = ops.gae_scan(rew_c, vals_c, seg, gamma=self.gamma, lam=self.gae_lambda)   # :417-421
+            if vtrace:
+                # heads that took no action carry no behaviour log-prob (old_logp is 0 there too); padding rows are 0 already
+                acted = torch.stack([actions[k].any(dim=-1) for k in keys], dim=-1)
+                behaviour_logp = torch.where(acted, behaviour_logp, 0.0)
+                valid_len = torch.tensor(Ls, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
+                adv_c, ret_c, self._vtrace_seg_stats = ops.vtrace_scan(
+                    rew_c, vals_c, rollout_major(old_logp), rollout_major(behaviour_logp), seg, gamma=self.gamma,
+                    lam=self.gae_lambda, rho_clip=self.vtrace_rho_clip, c_clip=self.vtrace_c_clip, valid_len=valid_len,
+                    stats=True)
+            else:
+                adv_c, ret_c = ops.gae_scan(rew_c, vals_c, seg, gamma=self.gamma, lam=self.gae_lambda)   # :417-421
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
                     adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same)
 
@@ -752,6 +811,19 @@ class DotaOptimizer:
         losses = {'loss': res[0], 'policy_loss': res[1], 'entropy_loss': res[2], 'value_loss': res[3]}
         entropies = {k: res[4 + h] for h, k in enumerate(keys)}
         return losses, entropies, {'unclipped': res[_lib.LOSS_SLOTS], 'clipped': res[_lib.LOSS_SLOTS + 1]}
+
+    @property
+    def last_vtrace_stats(self):
+        """Diagnostics of the last experience prep with ``advantage_estimator='vtrace'`` (None before one), over the rollouts'
+        real steps (padding excluded): ``mean_log_rho`` (the mean log importance weight, log pi/mu), ``mean_clipped_rho``
+        (the mean truncated weight), ``rho_clip_fraction`` and ``c_clip_fraction`` (the share of steps whose weight exceeds
+        ``vtrace_rho_clip`` / ``vtrace_c_clip``).  Read back from the device, which waits for the prep, when accessed."""
+        if self._vtrace_seg_stats is None:
+            return None
+        s = self._vtrace_seg_stats.sum(dim=0).tolist()
+        n = max(s[0], 1.0)
+        return {'mean_log_rho': s[1] / n, 'mean_clipped_rho': s[2] / n, 'rho_clip_fraction': s[3] / n,
+                'c_clip_fraction': s[4] / n}
 
     @staticmethod
     def _ppo_stats_dict(st):
@@ -977,6 +1049,9 @@ class DotaOptimizer:
             metrics['reward_per_sec/{}'.format(k)] = v
         for k in ppo_stats[0]:                                             # means over the epochs
             metrics['ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
+        if self.advantage_estimator == 'vtrace':                           # read now: the steps have synced the device
+            for k, v in self.last_vtrace_stats.items():
+                metrics['vtrace/{}'.format(k)] = v
         logger.info('steps_per_s={:.2f}, avg_weight_age={:.1f}, loss={:.4f}, entropy={:.3f}'.format(
             metrics[self.SPEED_KEY], float(metrics['avg_weight_age']), float(metrics['loss/sum']), float(metrics['entropy'])))
         if self.checkpoint:
@@ -1099,8 +1174,9 @@ def init_distribution(backend='nccl'):
 def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          pretrained_model, mq_prefetch_count, log_dir, entropy_coef, vf_coef, run_local,
          hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
-         value_clip=None):
-    check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip)     # before any process-group setup
+         value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0):
+    check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
+                       vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip)     # before any process-group setup
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
     dota_optimizer = DotaOptimizer(
@@ -1108,7 +1184,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         learning_rate=learning_rate, checkpoint=is_master(), pretrained_model=pretrained_model,
         mq_prefetch_count=mq_prefetch_count, log_dir=log_dir, entropy_coef=entropy_coef, vf_coef=vf_coef,
         run_local=run_local, hidden_size=hidden_size, cell=cell, num_layers=num_layers, gamma=gamma,
-        gae_lambda=gae_lambda, clip_range=clip_range, max_grad_norm=max_grad_norm, value_clip=value_clip)
+        gae_lambda=gae_lambda, clip_range=clip_range, max_grad_norm=max_grad_norm, value_clip=value_clip,
+        advantage_estimator=advantage_estimator, vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -1122,7 +1199,8 @@ def default_log_dir():
 
 def build_arg_parser():
     """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell``, ``--num-layers`` and the PPO
-    settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm`` and ``--value-clip``."""
+    settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm``, ``--value-clip``,
+    ``--advantage-estimator``, ``--vtrace-rho-clip`` and ``--vtrace-c-clip``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -1147,6 +1225,10 @@ def build_arg_parser():
     p.add_argument("--max-grad-norm", type=float, help="global gradient-norm clip (reference: 0.5)", default=0.5)
     p.add_argument("--value-clip", type=float, default=None,
                    help="PPO2 value-loss clip range around the prep-time values (default: no value clipping)")
+    p.add_argument("--advantage-estimator", type=str, choices=ADVANTAGE_ESTIMATORS, default='gae',
+                   help="'vtrace' corrects for actors that played with older weights (rollouts must carry behaviour_logp)")
+    p.add_argument("--vtrace-rho-clip", type=float, help="V-trace truncation rho-bar of the importance weights", default=1.0)
+    p.add_argument("--vtrace-c-clip", type=float, help="V-trace truncation c-bar of the trace coefficients", default=1.0)
     return p
 
 
@@ -1159,6 +1241,7 @@ if __name__ == '__main__':
              mq_prefetch_count=args.mq_prefetch_count, log_dir=args.log_dir, entropy_coef=args.entropy_coef,
              vf_coef=args.vf_coef, run_local=args.run_local, hidden_size=args.hidden_size, cell=args.cell,
              num_layers=args.num_layers, gamma=args.gamma, gae_lambda=args.gae_lambda, clip_range=args.clip_range,
-             max_grad_norm=args.max_grad_norm, value_clip=args.value_clip)
+             max_grad_norm=args.max_grad_norm, value_clip=args.value_clip, advantage_estimator=args.advantage_estimator,
+             vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip)
     except KeyboardInterrupt:
         pass

@@ -256,7 +256,11 @@ class Policy(nn.Module):
         ``hidden``: ``[L, A, H]`` (``(h, c)`` for the LSTM; L = ``num_layers``); ``observations``: ``{key: [A, ...]}`` (what ``single`` takes, with
         a leading agent dimension); ``masks``: ``{head: [A, n]}`` legal-action masks (``action_masks``); ``u``: optional
         ``[A, 5]`` uniforms.  Returns ``(chosen {head: int32 [A], -1 = not sampled}, logp [A, 5], logits {head: [A, n]},
-        value [A], new hidden)``.  Index selection is bit-exact against ``oracle.ref_policy.sample_index``."""
+        value [A], new hidden)``.  Index selection is bit-exact against ``oracle.ref_policy.sample_index``.
+
+        Row ``a`` of ``logp`` (log-probability of each sampled head in ``ops.HEAD_KEYS`` order, 0 for heads not sampled) is
+        the ``behaviour_logp`` row of this step in agent ``a``'s rollout: what ``DotaOptimizer(advantage_estimator='vtrace')``
+        needs to correct for the weights the agent played with."""
         with torch.no_grad():
             obs = {k: v.unsqueeze(0) for k, v in observations.items()}              # [1 (time), A, ...]
             logits, value, new_hidden = self.forward_time_major(obs, hidden)

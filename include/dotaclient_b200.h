@@ -60,6 +60,30 @@ int dc_gae_scan(const float *rewards, int n_sub, const float *values, const int6
                 int n_seg, const float *boot_value, const float *boot_reward, double gamma,
                 double lam, float *adv, float *ret, dc_stream_t stream);
 
+/* ---- V-trace -----------------------------------------------------------------------------
+ * Off-policy counterpart of dc_gae_scan (Espeholt et al. 2018, IMPALA) for rollouts an actor sampled with older
+ * weights: truncated importance weights correct the value targets and the policy-gradient advantages.
+ *   rewards, n_sub, values, seg_off, boot_value: as dc_gae_scan (boot_value NULL = 0; there is no boot_reward)
+ *   logp_target    [n_rows, 5]  log-prob of the taken action per head under the policy being trained (the dense
+ *                               old_logp of dc_selected_logp); 0 where the head took no action
+ *   logp_behaviour [n_rows, 5]  the same under the policy the actor sampled with; 0 where the head took no action
+ *   valid_len [n_seg] int64 or NULL  the first valid_len[r] rows of segment r are real steps (NULL: all rows)
+ *   rho_clip, c_clip > 0        the truncation levels rho-bar and c-bar
+ *   pg_adv, vs [n_rows]         outputs: A_t and vs_t below
+ *   seg_stats [n_seg][DC_VTRACE_STATS_SLOTS] fp64 or NULL  per-segment sums over the real steps:
+ *       0 token count, 1 sum log rho, 2 sum rho-bar_t, 3 #(rho > rho_clip), 4 #(rho > c_clip), 5..7 zero
+ * Per row: log rho_t = sum_h (logp_target - logp_behaviour) (fp64, heads in order), rho-bar_t = min(rho_clip, rho_t),
+ * c_t = lam min(c_clip, rho_t), r_t = the sub-rewards summed as dc_gae_scan does, and
+ *   vs_t = V_t + rho-bar_t (r_t + gamma V_{t+1} - V_t) + gamma c_t (vs_{t+1} - V_{t+1}),   vs_{end} = V_{end} = boot
+ *   A_t  = rho-bar_t (r_t + gamma vs_{t+1} - V_t)
+ * Float64 throughout after the reward reduction, each output rounded once to fp32.  One warp per segment.
+ */
+#define DC_VTRACE_STATS_SLOTS 8
+int dc_vtrace_scan(const float *rewards, int n_sub, const float *values, const float *logp_target,
+                   const float *logp_behaviour, const int64_t *seg_off, int n_seg, const int64_t *valid_len,
+                   const float *boot_value, double gamma, double lam, double rho_clip, double c_clip, float *pg_adv,
+                   float *vs, double *seg_stats, dc_stream_t stream);
+
 /* ---- recurrent core --------------------------------------------------------------------
  * Replaces the time recurrence inside nn.GRU / nn.LSTM (policy.py:66,141) -- forward and
  * backward -- given the input-to-hidden pre-activations of all steps.
