@@ -13,6 +13,11 @@ _c = ctypes
 _vp, _i32, _i64, _f32, _f64, _sz = _c.c_void_p, _c.c_int, _c.c_int64, _c.c_float, _c.c_double, _c.c_size_t
 _ptr5 = _c.c_void_p * 5
 
+
+class GatherDesc(_c.Structure):
+    """``dc_gather_desc``: one tensor of a ``dc_gather_columns`` call."""
+    _fields_ = [("src", _vp), ("dst", _vp), ("outer", _i64), ("src_cols", _i64), ("row_bytes", _i64)]
+
 # name -> (restype, argtypes); must list every symbol include/dotaclient_b200.h declares.
 SIGNATURES = {
     "dc_version": (_i32, []),
@@ -20,6 +25,7 @@ SIGNATURES = {
     "dc_device_info": (_i32, [_c.POINTER(_i32)] * 3),
     "dc_gae_scan": (_i32, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _vp, _vp, _vp]),
     "dc_vtrace_scan": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _f64, _f64, _vp, _vp, _vp, _vp]),
+    "dc_gather_columns": (_i32, [_c.POINTER(GatherDesc), _i32, _vp, _i64, _vp]),
     "dc_rnn_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "dc_rnn_seq_fwd": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "dc_rnn_seq_bwd": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
@@ -62,6 +68,7 @@ HP_LR, HP_E_CLIP, HP_ENTROPY_COEF, HP_VF_COEF, HP_MAX_GRAD_NORM, HP_VALUE_CLIP =
 PPO_STATS_SLOTS = 16
 STAT_APPROX_KL, STAT_CLIP_FRACTION, STAT_EXPLAINED_VAR = 0, 6, 12
 VTRACE_STATS_SLOTS = 8      # per-segment fp64 sums written by dc_vtrace_scan (DC_VTRACE_STATS_SLOTS)
+GATHER_MAX_TENSORS = 32     # descriptors per dc_gather_columns call (DC_GATHER_MAX_TENSORS)
 MAX_PARAM_TENSORS = 96      # kMaxSeg of csrc/grad_finish.cu: parameter tensors dc_grad_flags / dc_grad_finish can handle
 
 _lib = None

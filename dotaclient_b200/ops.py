@@ -4,7 +4,9 @@ Every function here requires CUDA tensors and enqueues hand-written sm_90a kerne
 ``libdotaclient_b200.so`` on torch's current stream.  No CPU path exists: CPU tensors raise.
 """
 import ctypes
+import math
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -153,6 +155,70 @@ def vtrace_scan(rewards, values, logp_target, logp_behaviour, seg_off, gamma, la
                                       pg_adv.data_ptr(), vs.data_ptr(), _lib.ptr(seg_stats), _lib.stream_ptr()),
                    "dc_vtrace_scan")
     return (pg_adv, vs, seg_stats) if stats else (pg_adv, vs)
+
+
+# --------------------------------------------------------------------------------------------- minibatch gather
+_index_staging = {}     # device -> (pinned int64 buffer, event recorded after the last upload from it)
+
+
+def _upload_index(idx, device):
+    """Asynchronous upload of a host index through a cached pinned buffer: a copy from pageable memory may wait for the
+    stream, which would stall the host behind the GPU at every minibatch."""
+    buf, ev = _index_staging.get(device, (None, None))
+    if ev is not None:
+        ev.synchronize()                     # the previous upload has left the buffer
+    if buf is None or buf.numel() < idx.size:
+        buf = torch.empty(max(idx.size, 4096), dtype=torch.int64).pin_memory()
+    buf.numpy()[:idx.size] = idx
+    out = buf[:idx.size].to(device, non_blocking=True)
+    ev = torch.cuda.Event()
+    ev.record()
+    _index_staging[device] = (buf, ev)
+    return out
+
+
+def gather_columns(pairs, index):
+    """``dst.copy_(src.index_select(1, index))`` for every ``(src, dst)`` pair, in one ``dc_gather_columns`` launch per
+    ``_lib.GATHER_MAX_TENSORS`` pairs.
+
+    Every ``src`` is a contiguous CUDA tensor of at least 2 dims; its ``dst`` is contiguous, on the same device, of the same
+    dtype, and of shape ``(src.shape[0], len(index)) + src.shape[2:]``.  ``index`` is a 1-D integer array or tensor on the
+    HOST (a CUDA tensor is read back first): it is checked there -- every value in ``[0, src.shape[1])`` -- and uploaded,
+    because the kernel cannot check a device index.  Raises ``ValueError`` before any launch.
+    """
+    if isinstance(index, torch.Tensor):
+        index = index.cpu().numpy()
+    idx = np.asarray(index)
+    if idx.ndim != 1 or idx.dtype.kind not in "iu":
+        raise ValueError("gather_columns: index must be a 1-D integer array, got %s %s" % (idx.dtype, idx.shape))
+    lo, hi = (int(idx.min()), int(idx.max())) if idx.size else (0, -1)
+    descs, device = [], None
+    for src, dst in pairs:
+        if src.dim() < 2 or not src.is_contiguous() or not dst.is_contiguous():
+            raise ValueError("gather_columns: tensors must be contiguous with at least 2 dims, got %s" % (tuple(src.shape),))
+        shape = src.shape
+        if lo < 0 or hi >= shape[1]:
+            raise ValueError("gather_columns: index values %d..%d outside [0, %d)" % (lo, hi, shape[1]))
+        _need_cuda(src, dst)
+        if dst.shape != (shape[0], idx.size) + shape[2:] or dst.dtype != src.dtype or dst.device != src.device:
+            raise ValueError("gather_columns: dst %s %s does not match src %s %s gathered at %d columns"
+                             % (dst.dtype, tuple(dst.shape), src.dtype, tuple(shape), idx.size))
+        if device is not None and src.device != device:
+            raise ValueError("gather_columns: all tensors must be on one device")
+        device = src.device
+        row_bytes = math.prod(shape[2:]) * src.element_size()
+        if row_bytes and shape[0]:               # an empty tensor has nothing to copy
+            descs.append(_lib.GatherDesc(src.data_ptr(), dst.data_ptr(), shape[0], shape[1], row_bytes))
+    if not descs or idx.size == 0:
+        return
+    index_dev = _upload_index(idx, device)
+    lib = _lib.load()
+    n_max = _lib.GATHER_MAX_TENSORS
+    for k in range(0, len(descs), n_max):
+        chunk = descs[k:k + n_max]
+        with PROFILE.span("gather_columns", 1):
+            _lib.check(lib.dc_gather_columns((_lib.GatherDesc * len(chunk))(*chunk), len(chunk), index_dev.data_ptr(),
+                                             idx.size, _lib.stream_ptr()), "dc_gather_columns")
 
 
 # --------------------------------------------------------------------------------------------- RNN

@@ -297,6 +297,19 @@ class ExperienceBatch:
     def pin_memory(self):
         return self.map(lambda v: v.cpu().pin_memory())
 
+    def gather(self, index):
+        """A new device batch of the sequence columns ``index`` (host integers, in that order; repeats allowed) of every
+        tensor, ``h0`` / ``c0`` included: ``index_select(1, index)`` of each, done by ONE ``dc_gather_columns`` launch.
+        Each sequence carries its own initial recurrent state, so the result is an exact batch of those sequences."""
+        n = len(index)
+        out = self.map(lambda v: torch.empty((v.shape[0], n) + tuple(v.shape[2:]), dtype=v.dtype, device=v.device))
+        srcs = [v for _, _, v in self.tensors()]
+        if self._slot is not None:               # uploaded by prefetch() into graph input buffers: wait for that upload
+            torch.cuda.current_stream().wait_event(self._slot["ready"])
+        self.wait(*srcs)
+        ops.gather_columns(list(zip(srcs, [v for _, _, v in out.tensors()])), index)
+        return out
+
     @staticmethod
     def from_sequences(experiences, device):
         """Stacks ``Sequence`` records along dim 1 (the reference stacks along dim 0, :587-615)."""
@@ -348,10 +361,12 @@ ADVANTAGE_ESTIMATORS = ('gae', 'vtrace')
 
 
 def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
-                       vtrace_rho_clip=1.0, vtrace_c_clip=1.0):
+                       vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
-    vtrace_rho_clip > 0 and vtrace_c_clip > 0.  NaN fails every check."""
+    vtrace_rho_clip > 0, vtrace_c_clip > 0 and num_minibatches an int >= 1 (not a bool).  NaN fails every check."""
+    if isinstance(num_minibatches, bool) or not isinstance(num_minibatches, numbers.Integral) or num_minibatches < 1:
+        raise ValueError("num_minibatches=%r: the number of minibatches per epoch must be an int >= 1" % (num_minibatches,))
     def number(name, v):
         if isinstance(v, bool) or not isinstance(v, numbers.Real):
             raise ValueError("%s=%r is not a number" % (name, v))
@@ -372,6 +387,24 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
         raise ValueError("vtrace_rho_clip=%r: the V-trace rho truncation must be > 0" % (vtrace_rho_clip,))
     if not number('vtrace_c_clip', vtrace_c_clip) > 0.0:
         raise ValueError("vtrace_c_clip=%r: the V-trace c truncation must be > 0" % (vtrace_c_clip,))
+
+
+def check_minibatch_count(num_minibatches, min_seq_per_epoch):
+    """Raises ``ValueError`` when an iteration could hold fewer sequences than minibatches.  An iteration holds at least
+    ``min_seq_per_epoch`` sequences on every rank, so with ``num_minibatches <= min_seq_per_epoch`` every rank forms all its
+    minibatches and the ranks' all-reduces stay in lockstep, whatever their batch sizes."""
+    if num_minibatches > min_seq_per_epoch:
+        raise ValueError("num_minibatches=%r exceeds min_seq_per_epoch=%r: every minibatch needs at least one sequence"
+                         % (num_minibatches, min_seq_per_epoch))
+
+
+def minibatch_indices(B, num_minibatches, rng):
+    """The sequence columns of each minibatch of one epoch over a batch of ``B`` sequences: with one minibatch the whole
+    batch in order (``rng`` is not drawn from), otherwise ``np.array_split`` of a permutation drawn from ``rng`` (a numpy
+    ``Generator``), so the sizes differ by at most one and every sequence is used exactly once per epoch."""
+    if num_minibatches == 1:
+        return [np.arange(B)]
+    return np.array_split(rng.permutation(B), num_minibatches)
 
 
 def check_behaviour_logp(datas):
@@ -414,13 +447,18 @@ class DotaOptimizer:
                  learning_rate, checkpoint, pretrained_model, mq_prefetch_count, log_dir,
                  entropy_coef, vf_coef, run_local, *, hidden_size=256, cell="gru", num_layers=1, mq=None,
                  iterations=100000, rollout_prefetch=0, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1,
-                 max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0):
+                 max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0,
+                 num_minibatches=1):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
                              % (num_layers, self.MAX_LAYERS, _lib.MAX_PARAM_TENSORS))
         check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
-                           vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip)
+                           vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches)
+        check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # every epoch is split into num_minibatches shuffled minibatches of sequences, one optimizer step each (train_epochs)
+        self.num_minibatches = int(num_minibatches)
+        self.minibatch_rng = np.random.default_rng(7 + (dist.get_rank() if is_distributed() else 0))   # seed 7 as :34-36
         self.gamma, self.gae_lambda = float(gamma), float(gae_lambda)     # GAE of experience prep (:421)
         # 'vtrace': experience prep corrects advantages and value targets for the actors' stale weights, from the
         # behaviour log-probabilities each rollout carries ('behaviour_logp')
@@ -975,6 +1013,29 @@ class DotaOptimizer:
                              zip(self.flat.starts, self.flat.ends)])
         return norms[has].mean()
 
+    def train_epochs(self, batch):
+        """The PPO epochs of one iteration on ``batch`` (an ``ExperienceBatch``): ``epochs`` passes, each split into
+        ``num_minibatches`` minibatches of whole sequences (``minibatch_indices`` with ``minibatch_rng``), one ``train`` step
+        per minibatch -- forward, loss (advantages normalised over the minibatch), backward, all-reduce, clip, Adam.  With
+        one minibatch every epoch trains on ``batch`` itself, as the reference does (:469).  Returns the per-step lists
+        ``(losses, entropies, grad_norms, ppo_stats)``.  Raises ``ValueError`` when the batch has fewer sequences than
+        minibatches."""
+        M = self.num_minibatches
+        if batch.batch_size < M:
+            raise ValueError("the batch has %d sequences, fewer than num_minibatches=%d" % (batch.batch_size, M))
+        if M > 1 and not batch.advantages.is_cuda:
+            batch = batch.to(self.device)                  # uploaded once; the minibatches are gathered on the device
+        losses, entropies, grad_norms, ppo_stats = [], [], [], []
+        for ep in range(self.epochs):                                      # :469
+            self.mq.process_data_events()
+            for idx in minibatch_indices(batch.batch_size, M, self.minibatch_rng):
+                loss_d, entropy_d, grad_norm_d = self.train(experiences=batch if M == 1 else batch.gather(idx))
+                losses.append(loss_d)
+                entropies.append(entropy_d)
+                grad_norms.append(grad_norm_d)
+                ppo_stats.append(self.last_ppo_stats)
+        return losses, entropies, grad_norms, ppo_stats
+
     # -- iteration driver (:436-579) ----------------------------------------------------------------
     def run(self):
         for it in range(self.iteration_start, self.iterations):
@@ -1001,21 +1062,16 @@ class DotaOptimizer:
         batch = self.batch_from_rollouts(rollouts)                        # prepared + stacked once, reused by every epoch
         time_xp = time.time() - start_xp
         # a stream of rollouts gives every iteration its own batch size: capturing a graph per shape would cost more than the
-        # `epochs` replays return, so the graph path is used only while consecutive iterations keep the same shape
+        # `epochs` replays return, so the graph path is used only while consecutive iterations keep the same shape.  The
+        # minibatch shapes follow from (S, B, num_minibatches): at most two, ceil and floor, and _replay_step keeps two
+        # captured graphs alive, so the same rule serves minibatches
         shape = (batch.seq_len, batch.batch_size)
         graph_setting, self.use_cuda_graph = self.use_cuda_graph, self.use_cuda_graph and shape == self._last_iteration_shape
         self._last_iteration_shape = shape
 
-        losses, entropies, grad_norms, ppo_stats = [], [], [], []
         start_optimizing = time.time()
         try:
-            for ep in range(self.epochs):                                  # :469
-                self.mq.process_data_events()
-                loss_d, entropy_d, grad_norm_d = self.train(experiences=batch)
-                losses.append(loss_d)
-                entropies.append(entropy_d)
-                grad_norms.append(grad_norm_d)
-                ppo_stats.append(self.last_ppo_stats)
+            losses, entropies, grad_norms, ppo_stats = self.train_epochs(batch)
         finally:
             self.use_cuda_graph = graph_setting
         time_optimizing = time.time() - start_optimizing
@@ -1047,7 +1103,7 @@ class DotaOptimizer:
             metrics['grad_norm/{}'.format(k)] = v.mean()
         for k, v in reward_dict.items():
             metrics['reward_per_sec/{}'.format(k)] = v
-        for k in ppo_stats[0]:                                             # means over the epochs
+        for k in ppo_stats[0]:                                             # means over the steps
             metrics['ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
         if self.advantage_estimator == 'vtrace':                           # read now: the steps have synced the device
             for k, v in self.last_vtrace_stats.items():
@@ -1174,9 +1230,11 @@ def init_distribution(backend='nccl'):
 def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          pretrained_model, mq_prefetch_count, log_dir, entropy_coef, vf_coef, run_local,
          hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
-         value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0):
+         value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
-                       vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip)     # before any process-group setup
+                       vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip,
+                       num_minibatches=num_minibatches)                                  # before any process-group setup
+    check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
     dota_optimizer = DotaOptimizer(
@@ -1185,7 +1243,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         mq_prefetch_count=mq_prefetch_count, log_dir=log_dir, entropy_coef=entropy_coef, vf_coef=vf_coef,
         run_local=run_local, hidden_size=hidden_size, cell=cell, num_layers=num_layers, gamma=gamma,
         gae_lambda=gae_lambda, clip_range=clip_range, max_grad_norm=max_grad_norm, value_clip=value_clip,
-        advantage_estimator=advantage_estimator, vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip)
+        advantage_estimator=advantage_estimator, vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip,
+        num_minibatches=num_minibatches)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -1200,7 +1259,7 @@ def default_log_dir():
 def build_arg_parser():
     """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell``, ``--num-layers`` and the PPO
     settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm``, ``--value-clip``,
-    ``--advantage-estimator``, ``--vtrace-rho-clip`` and ``--vtrace-c-clip``."""
+    ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip`` and ``--num-minibatches``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -1229,6 +1288,8 @@ def build_arg_parser():
                    help="'vtrace' corrects for actors that played with older weights (rollouts must carry behaviour_logp)")
     p.add_argument("--vtrace-rho-clip", type=float, help="V-trace truncation rho-bar of the importance weights", default=1.0)
     p.add_argument("--vtrace-c-clip", type=float, help="V-trace truncation c-bar of the trace coefficients", default=1.0)
+    p.add_argument("--num-minibatches", type=int, default=1,
+                   help="shuffled minibatches of sequences per epoch, one optimizer step each (reference: 1)")
     return p
 
 
@@ -1242,6 +1303,6 @@ if __name__ == '__main__':
              vf_coef=args.vf_coef, run_local=args.run_local, hidden_size=args.hidden_size, cell=args.cell,
              num_layers=args.num_layers, gamma=args.gamma, gae_lambda=args.gae_lambda, clip_range=args.clip_range,
              max_grad_norm=args.max_grad_norm, value_clip=args.value_clip, advantage_estimator=args.advantage_estimator,
-             vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip)
+             vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip, num_minibatches=args.num_minibatches)
     except KeyboardInterrupt:
         pass

@@ -84,6 +84,33 @@ int dc_vtrace_scan(const float *rewards, int n_sub, const float *values, const f
                    const float *boot_value, double gamma, double lam, double rho_clip, double c_clip, float *pg_adv,
                    float *vs, double *seg_stats, dc_stream_t stream);
 
+/* ---- minibatch assembly: column gather ----------------------------------------------------
+ * Picks the sequence columns `index` out of many time-major tensors in ONE launch (the minibatches of PPO epochs,
+ * DotaOptimizer.train_epochs; the reference trains on the whole batch and has no counterpart).  Descriptor d describes a
+ * contiguous [outer, src_cols, row_bytes] source and a contiguous [outer, n_index, row_bytes] destination; for every
+ * o < outer and j < n_index:
+ *   dst[(o*n_index + j)*row_bytes + b] = src[(o*src_cols + index[j])*row_bytes + b]         (b < row_bytes)
+ * which is torch.index_select(t, 1, index) for each tensor.
+ *   descs    host array of n_desc descriptors (0 <= n_desc <= DC_GATHER_MAX_TENSORS), passed by value to the kernel
+ *   index    [n_index] int64, DEVICE; repeats allowed
+ * Preconditions the library cannot check (the index is on the device): 0 <= index[j] < src_cols for every j.  The
+ * caller validates the index where it is made, on the host, before uploading it.
+ * Checked: n_desc range, n_index >= 0, outer >= 0, src_cols >= 0, row_bytes > 0, non-null pointers where there is work
+ * (src_cols > 0 there too), dst not overlapping src -> DC_EINVAL before any CUDA call.  n_desc == 0 or n_index == 0:
+ * nothing to do, returns 0.  Copies in 16-byte units when row_bytes and both base pointers are multiples of 16, else in
+ * 4-byte units under the same test, else bytes.
+ */
+typedef struct {
+    const void *src;
+    void *dst;
+    int64_t outer;
+    int64_t src_cols;
+    int64_t row_bytes;
+} dc_gather_desc;
+#define DC_GATHER_MAX_TENSORS 32
+int dc_gather_columns(const dc_gather_desc *descs, int n_desc, const int64_t *index, int64_t n_index,
+                      dc_stream_t stream);
+
 /* ---- recurrent core --------------------------------------------------------------------
  * Replaces the time recurrence inside nn.GRU / nn.LSTM (policy.py:66,141) -- forward and
  * backward -- given the input-to-hidden pre-activations of all steps.
