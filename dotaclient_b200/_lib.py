@@ -49,6 +49,8 @@ SIGNATURES = {
                                            _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp]),
     "dc_ppo_loss_fwd_bwd_dev": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp,
                                        _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "dc_ppo_loss_fwd_bwd_masked": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
+                                          _vp, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "dc_selected_logp": (_i32, [_ptr5, _ptr5, _ptr5, _i64, _vp, _vp]),
     "dc_select_actions": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _vp, _i64, _vp, _vp, _vp]),
     "dc_grad_flags": (_i32, [_vp, _i64, _vp, _i32, _vp, _vp]),

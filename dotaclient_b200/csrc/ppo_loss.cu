@@ -20,9 +20,14 @@
 // The `_dev` entry point reads its hyper-parameters from a device block (DC_HPARAM_SLOTS), so a captured CUDA graph of
 // the step picks up new values on every replay; the scalar-argument entry points run the same kernel body.
 //
+// The `_masked` entry point takes a per-token `valid` byte: a token with valid = 0 (the zero padding of a rollout's last
+// chunk) is left out of every count, sum and divisor -- advantage mean / std, action counts, policy / entropy means, the
+// value loss and its 1/N, the diagnostics -- and receives exactly zero gradient.  The statistics pass counts the valid
+// tokens into the workspace (n_valid); with valid == NULL every token counts and the arithmetic is the unmasked one.
+//
 // Algorithmic HBM bytes per token: logits 260 + masks 65 + actions 65 + old 20 + adv/ret/value 12
 // read, dlogits 260 + dvalue 4 written = 686 (+ 69 for the statistics pass, + 4 for the old value when the value loss
-// is clipped).
+// is clipped, + 1 in each pass for `valid` when given).
 #include "dc_common.cuh"
 
 namespace {
@@ -71,6 +76,7 @@ struct Workspace {
     double adv_sum, adv_sq;
     double st[kStats];    // diagnostics (kSt* above)
     int cnt[kHeads];
+    unsigned long long n_valid;   // tokens that count (all N when no valid mask is given)
     unsigned ticket_stats, ticket_loss;
     float adv_mean, adv_std;
 };
@@ -150,7 +156,8 @@ __device__ __forceinline__ T block_sum(T v, T *scratch) {
 }
 
 // ---- pass 1: counts + advantage statistics ------------------------------------------------
-__global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const float *__restrict__ adv, int64_t N,
+__global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const float *__restrict__ adv,
+                                                           const uint8_t *__restrict__ valid, int64_t N,
                                                            Workspace *ws, int32_t *n_actions_out) {
     __shared__ __align__(16) uint8_t s_act[kByteTile];
     __shared__ double s_red[kTile / 32];
@@ -160,7 +167,8 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
 #pragma unroll
     for (int h = 0; h < kHeads; ++h) stage_bytes(s_act + byte_off(h), hp.actions[h] + t0 * head_n(h), count * head_n(h));
     __syncthreads();
-    const bool live = threadIdx.x < count;
+    // a token that does not count (valid = 0) adds nothing to the sums and the action counts
+    const bool live = threadIdx.x < count && (valid == nullptr || valid[t0 + threadIdx.x] != 0);
     double a = 0.0;
     if (live) a = (double)adv[t0 + threadIdx.x];
     int has[kHeads];
@@ -178,9 +186,11 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
     int tot[kHeads];
 #pragma unroll
     for (int h = 0; h < kHeads; ++h) tot[h] = __syncthreads_count(has[h]);
+    const int n_live = __syncthreads_count(live);
     if (threadIdx.x == 0) {
         atomicAdd(&ws->adv_sum, sa);
         atomicAdd(&ws->adv_sq, sq);
+        atomicAdd(&ws->n_valid, (unsigned long long)n_live);
 #pragma unroll
         for (int h = 0; h < kHeads; ++h)
             if (tot[h]) atomicAdd(&ws->cnt[h], tot[h]);
@@ -190,10 +200,11 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
     __syncthreads();
     if (s_last && threadIdx.x == 0) {
         __threadfence();
-        const double n = (double)N;
+        // over the tokens that count: N without a valid mask (the same double), N_v with one
+        const double n = (double)*((volatile unsigned long long *)&ws->n_valid);
         const double sum = *((volatile double *)&ws->adv_sum), sq2 = *((volatile double *)&ws->adv_sq);
         const double mean = sum / n;
-        // torch.std: unbiased (N-1); NaN for N == 1 like torch.
+        // torch.std: unbiased (N-1); NaN for N == 1 (and for N_v = 0 or 1) like torch.
         const double var = (sq2 - n * mean * mean) / (n - 1.0);
         ws->adv_mean = (float)mean;
         ws->adv_std = (float)sqrt(var > 0.0 ? var : (var == var ? 0.0 : var));
@@ -290,6 +301,7 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
                                                           const float *__restrict__ value, int64_t N, float e_clip,
                                                           float entropy_coef, float vf_coef,
                                                           const float *__restrict__ old_value,
+                                                          const uint8_t *__restrict__ valid,
                                                           const double *__restrict__ hparams,
                                                           float *__restrict__ dvalue, float *__restrict__ out,
                                                           float *__restrict__ stats, Workspace *ws,
@@ -341,10 +353,12 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
     }
     int cnt[kHeads] = {0, 0, 0, 0, 0};
     float adv_n = 0.f;
+    // a token that does not count (valid = 0): every contribution below is skipped and its gradients are zero
+    const bool use = live && (valid == nullptr || valid[t0 + t] != 0);
     if (!kSelectOnly) {
 #pragma unroll
         for (int h = 0; h < kHeads; ++h) cnt[h] = ws->cnt[h];
-        if (live) {
+        if (use) {
             // (advantage - mean) / (std + eps), fp32 like optimizer.py:588
             adv_n = __fdiv_rn(__fsub_rn(adv_raw[t0 + t], ws->adv_mean), __fadd_rn(ws->adv_std, 1.1920928955078125e-07f));
         }
@@ -354,13 +368,15 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
 #define DC_HEAD(H)                                                                                              \
         head_token<H, true>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H),  \
                             s_act + byte_off(H) + t * head_n(H), kSelectOnly ? 0.f : s_old[t * 5 + H], adv_n,   \
-                            cnt[H], e_clip, entropy_coef, pol[H], ent[H], &s_tok[kStKl + H][t],                 \
+                            use ? cnt[H] : 0, e_clip, entropy_coef, pol[H], ent[H], &s_tok[kStKl + H][t],       \
                             &s_tok[kStClip + H][t], kSelectOnly ? &lp_sel[H] : nullptr);
         DC_HEAD(0) DC_HEAD(1) DC_HEAD(2) DC_HEAD(3) DC_HEAD(4)
 #undef DC_HEAD
         if (kSelectOnly) {
 #pragma unroll
             for (int h = 0; h < kHeads; ++h) logp_out[(t0 + t) * 5 + h] = lp_sel[h];
+        } else if (!use) {              // masked out: zero gradient rows (head_token with a count of 0), zero dvalue
+            dvalue[(t0 + t) * hp.ld_dv] = 0.f;
         } else {
             const float v = value[(t0 + t) * hp.ld_v], r = ret[t0 + t];
             const float d = r - v;
@@ -380,7 +396,7 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             } else {
                 vl = d * d;                                                 // optimizer.py:660
             }
-            dvalue[(t0 + t) * hp.ld_dv] = vf_coef > 0.f ? vf_coef * g / (float)N : 0.f;
+            dvalue[(t0 + t) * hp.ld_dv] = vf_coef > 0.f ? vf_coef * g / (float)ws->n_valid : 0.f;   // N_v, or N unmasked
             s_tok[kTokD][t] = d;
             s_tok[kTokR][t] = r;
         }
@@ -445,7 +461,8 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         }
         policy /= (float)kHeads;                                            // optimizer.py:650
         const float e_loss = entropy_coef > 0.f ? -entropy_coef * entropy : 0.f;
-        const float v_loss = vf_coef > 0.f ? vf_coef * (0.5f * (float)(w->vl / (double)N)) : 0.f;
+        const double n_tok_d = (double)w->n_valid;                          // N, or N_v under a valid mask
+        const float v_loss = vf_coef > 0.f ? vf_coef * (0.5f * (float)(w->vl / n_tok_d)) : 0.f;
         out[0] = policy + e_loss + v_loss;                                  // optimizer.py:665
         out[1] = policy;
         out[2] = e_loss;
@@ -467,8 +484,9 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             }
             stats[DC_STAT_APPROX_KL] = used ? kl_sum / (float)used : 0.f;
             stats[DC_STAT_CLIP_FRACTION] = used ? clip_sum / (float)used : 0.f;
-            // 1 - Var(ret - v) / Var(ret) over all N tokens (population variances); NaN when the returns are constant
-            const double n = (double)N;
+            // 1 - Var(ret - v) / Var(ret) over the tokens that count (population variances); NaN when the returns are
+            // constant
+            const double n = n_tok_d;
             const double md = w->st[kStD] / n, mr = w->st[kStR] / n;
             const double var_d = w->st[kStD2] / n - md * md, var_r = w->st[kStR2] / n - mr * mr;
             stats[DC_STAT_EXPLAINED_VAR] = var_r > 0.0 ? (float)(1.0 - var_d / var_r) : __int_as_float(0x7fc00000);
@@ -488,7 +506,7 @@ int check_heads(const float *const logits[], const uint8_t *const masks[], const
 int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
                     const uint8_t *const masks[DC_NUM_HEADS], const uint8_t *const actions[DC_NUM_HEADS],
                     const float *old_logp, const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
-                    const float *old_value, int64_t N, float e_clip, float entropy_coef, float vf_coef,
+                    const float *old_value, const uint8_t *valid, int64_t N, float e_clip, float entropy_coef, float vf_coef,
                     const double *hparams, float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
                     float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions, void *workspace,
                     dc_stream_t stream) {
@@ -508,13 +526,13 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
     Workspace *ws = reinterpret_cast<Workspace *>(workspace);
     DC_CUDA(cudaMemsetAsync(ws, 0, sizeof(Workspace), st));
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
-    ppo_stats_kernel<<<blocks, kTile, 0, st>>>(hp, adv_raw, N, ws, n_actions);
+    ppo_stats_kernel<<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
     DC_LAUNCH_OK();
     // per-device attribute: set on every call (a process-wide "done" flag breaks the second GPU of a process)
     DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     ppo_loss_kernel<false><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
-                                                              entropy_coef, vf_coef, old_value, hparams, dvalue, out,
+                                                              entropy_coef, vf_coef, old_value, valid, hparams, dvalue, out,
                                                               stats, ws, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
@@ -530,8 +548,8 @@ extern "C" int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEAD
                                            float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
                                            float *dvalue, int64_t ld_dvalue, float *out, int32_t *n_actions, void *workspace,
                                            dc_stream_t stream) {
-    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, nullptr, N, e_clip,
-                           entropy_coef, vf_coef, nullptr, dlogits, ld_dlogits, dvalue, ld_dvalue, out, nullptr, n_actions,
+    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, nullptr, nullptr, N,
+                           e_clip, entropy_coef, vf_coef, nullptr, dlogits, ld_dlogits, dvalue, ld_dvalue, out, nullptr, n_actions,
                            workspace, stream);
 }
 
@@ -543,9 +561,23 @@ extern "C" int dc_ppo_loss_fwd_bwd_dev(const float *const logits[DC_NUM_HEADS], 
                                        float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
                                        void *workspace, dc_stream_t stream) {
     DC_REQUIRE(hparams, DC_EINVAL, "dc_ppo_loss_fwd_bwd_dev: null hyper-parameter block");
-    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, old_value, N, 0.f,
-                           0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions, workspace,
-                           stream);
+    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, old_value, nullptr,
+                           N, 0.f, 0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions,
+                           workspace, stream);
+}
+
+extern "C" int dc_ppo_loss_fwd_bwd_masked(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                                          const uint8_t *const masks[DC_NUM_HEADS],
+                                          const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
+                                          const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                                          const float *old_value, const uint8_t *valid, int64_t N, const double *hparams,
+                                          float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                                          float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
+                                          void *workspace, dc_stream_t stream) {
+    DC_REQUIRE(hparams, DC_EINVAL, "dc_ppo_loss_fwd_bwd_masked: null hyper-parameter block");
+    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, old_value, valid,
+                           N, 0.f, 0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions,
+                           workspace, stream);
 }
 
 extern "C" int dc_ppo_loss_fwd_bwd(const float *const logits[DC_NUM_HEADS], const uint8_t *const masks[DC_NUM_HEADS],
@@ -575,7 +607,7 @@ extern "C" int dc_selected_logp(const float *const logits[DC_NUM_HEADS], const u
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
     ppo_loss_kernel<true><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
         hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-        logp_out);
+        nullptr, logp_out);
     DC_LAUNCH_OK();
     return DC_OK;
 }

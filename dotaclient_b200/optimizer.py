@@ -170,7 +170,7 @@ class Sequence:
     """
 
     def __init__(self, game_id, weight_version, team_id, observations, actions, masks, values, rewards, hidden,
-                 log_probs_sel=None, old_logp=None):
+                 log_probs_sel=None, old_logp=None, valid=None):
         self.game_id = game_id
         self.weight_version = weight_version
         self.team_id = team_id
@@ -182,6 +182,7 @@ class Sequence:
         self.hidden = hidden
         self._log_probs_sel = log_probs_sel
         self.old_logp = old_logp
+        self.valid = valid          # [S] bool, real steps vs zero padding (set by prep under DotaOptimizer(mask_padding=True))
         self.advantages = None
         self.returns = None
 
@@ -212,13 +213,17 @@ class ExperienceBatch:
     Tensors may live in pinned host memory; ``to(device)`` issues the asynchronous H2D copies.
     ``old_values [S, B]`` (optional) are the critic's values at experience prep, which the clipped value loss
     (``DotaOptimizer(value_clip=...)``) needs; a batch without them has no such entry in ``tensors()``.
+    ``valid [S, B]`` (optional, bool) marks the real steps against the zero padding of each rollout's last chunk, which
+    ``DotaOptimizer(mask_padding=True)`` leaves out of the loss; like ``old_values`` it is absent from ``tensors()`` when None.
     """
-    FIELDS = ("advantages", "returns", "old_logp", "h0", "c0", "old_values")
+    FIELDS = ("advantages", "returns", "old_logp", "h0", "c0", "old_values", "valid")
 
-    def __init__(self, observations, masks, actions, old_logp, advantages, returns, h0, c0=None, old_values=None):
+    def __init__(self, observations, masks, actions, old_logp, advantages, returns, h0, c0=None, old_values=None,
+                 valid=None):
         self.observations, self.masks, self.actions = observations, masks, actions
         self.old_logp, self.advantages, self.returns, self.h0, self.c0 = old_logp, advantages, returns, h0, c0
         self.old_values = old_values
+        self.valid = valid
         self._ready = {}        # data_ptr -> event of an upload still to be waited for (``to`` from pinned memory)
         self._slot = None       # the DotaOptimizer input slot whose static buffers these tensors are (``prefetch``)
 
@@ -230,8 +235,9 @@ class ExperienceBatch:
                                {k: fn(v) for k, v in self.actions.items()}, **{f: opt(getattr(self, f)) for f in self.FIELDS})
 
     def graph_key(self):
-        """The shape a captured step graph is specialised to (old_values: one more static input)."""
-        return self.seq_len, self.batch_size, self.old_values is not None
+        """The shape a captured step graph is specialised to (old_values, valid: one more static input each)."""
+        key = (self.seq_len, self.batch_size, self.old_values is not None)
+        return key if self.valid is None else key + ('valid',)
 
     def wait(self, *tensors):
         """Makes the current stream wait for the uploads of ``tensors`` (None allowed) that are still outstanding; each
@@ -329,8 +335,11 @@ class ExperienceBatch:
         old_values = None
         if all(e.values is not None for e in experiences):
             old_values = stack([torch.as_tensor(e.values).detach().reshape(-1).float() for e in experiences])
+        valid = None
+        if all(getattr(e, 'valid', None) is not None for e in experiences):
+            valid = stack([torch.as_tensor(e.valid).reshape(-1).bool() for e in experiences])
         return ExperienceBatch(obs, masks, actions, old, adv, ret, h0.detach(), None if c0 is None else c0.detach(),
-                               old_values=old_values)
+                               old_values=old_values, valid=valid)
 
 
 class _CapturedStep(typing.NamedTuple):
@@ -361,10 +370,13 @@ ADVANTAGE_ESTIMATORS = ('gae', 'vtrace')
 
 
 def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
-                       vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1):
+                       vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
-    vtrace_rho_clip > 0, vtrace_c_clip > 0 and num_minibatches an int >= 1 (not a bool).  NaN fails every check."""
+    vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool) and mask_padding a bool.  NaN fails
+    every check."""
+    if not isinstance(mask_padding, bool):
+        raise ValueError("mask_padding=%r: must be True or False" % (mask_padding,))
     if isinstance(num_minibatches, bool) or not isinstance(num_minibatches, numbers.Integral) or num_minibatches < 1:
         raise ValueError("num_minibatches=%r: the number of minibatches per epoch must be an int >= 1" % (num_minibatches,))
     def number(name, v):
@@ -405,6 +417,27 @@ def minibatch_indices(B, num_minibatches, rng):
     if num_minibatches == 1:
         return [np.arange(B)]
     return np.array_split(rng.permutation(B), num_minibatches)
+
+
+def padded_segment_offsets(lengths, seq_len):
+    """Row offsets of the scan segments of experience prep under ``mask_padding``: rollout i occupies its padded length
+    ``Lp_i`` (``lengths[i]`` rounded up to a multiple of ``seq_len``) of the rollout-major rows and is split into a real
+    segment of ``lengths[i]`` rows and a padding segment of ``Lp_i - lengths[i]`` rows (possibly empty), so that the real
+    segment ends on the terminal bootstrap of 0.  Returns int64 ``[2R + 1]``: ``0, L_0, Lp_0, Lp_0 + L_1, Lp_0 + Lp_1, ...``."""
+    out = np.zeros(2 * len(lengths) + 1, dtype=np.int64)
+    base = 0
+    for i, L in enumerate(lengths):
+        L = int(L)
+        out[2 * i + 1] = base + L
+        base += (L + seq_len - 1) // seq_len * seq_len
+        out[2 * i + 2] = base
+    return out
+
+
+def chunk_valid_lengths(lengths, seq_len):
+    """The real steps of every ``seq_len`` chunk, rollout by rollout and chunk by chunk (the batch's sequence order): chunk
+    j of a rollout of length L has ``min(seq_len, L - j * seq_len)``."""
+    return [min(seq_len, int(L) - j * seq_len) for L in lengths for j in range((int(L) + seq_len - 1) // seq_len)]
 
 
 def check_behaviour_logp(datas):
@@ -448,14 +481,18 @@ class DotaOptimizer:
                  entropy_coef, vf_coef, run_local, *, hidden_size=256, cell="gru", num_layers=1, mq=None,
                  iterations=100000, rollout_prefetch=0, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1,
                  max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0,
-                 num_minibatches=1):
+                 num_minibatches=1, mask_padding=False):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
                              % (num_layers, self.MAX_LAYERS, _lib.MAX_PARAM_TENSORS))
         check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
-                           vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches)
+                           vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
+                           mask_padding=mask_padding)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # True: the zero padding of each rollout's last chunk counts for nothing -- prep bootstraps at the real end and
+        # marks the real steps (ExperienceBatch.valid), the loss leaves padded tokens out of every mean
+        self.mask_padding = mask_padding
         # every epoch is split into num_minibatches shuffled minibatches of sequences, one optimizer step each (train_epochs)
         self.num_minibatches = int(num_minibatches)
         self.minibatch_rng = np.random.default_rng(7 + (dist.get_rank() if is_distributed() else 0))   # seed 7 as :34-36
@@ -656,8 +693,11 @@ class DotaOptimizer:
         """The batched no-grad half of an iteration (SURVEY.md 8(f)2): all rollouts become the batch dimension of ONE
         time-major ``[L_max, R, ...]`` pass -- encoder chain, recurrence from the zero state, heads, selected log-probs
         (:384-390) -- followed by ONE segmented GAE scan over every rollout's own padded length (:417-421), or with
-        ``advantage_estimator='vtrace'`` ONE segmented V-trace scan of the same segments.  Returns the raw device tensors;
-        ``experiences_from_rollouts`` / ``batch_from_rollouts`` slice them."""
+        ``advantage_estimator='vtrace'`` ONE segmented V-trace scan of the same segments.  With ``mask_padding`` each
+        rollout is two segments, its real steps and its padding (``padded_segment_offsets``), so the terminal bootstrap
+        follows the last real step; advantages and returns of padded rows are then zeroed and ``valid [S, B]`` marks the
+        real steps of every chunk.  Returns the raw device tensors; ``experiences_from_rollouts`` / ``batch_from_rollouts``
+        slice them."""
         S, dev, pol = self.seq_len, self.device, self.policy_base
         R = len(datas)
         vtrace = self.advantage_estimator == 'vtrace'
@@ -721,20 +761,31 @@ class DotaOptimizer:
                 rew_c = torch.from_numpy(rewards_np.reshape(R * Lmax, -1)).to(dev, non_blocking=True)
             else:
                 rew_c = torch.from_numpy(np.concatenate([rewards_np[i, :Lps[i]] for i in range(R)])).to(dev)
-            seg = torch.tensor(np.concatenate([[0], np.cumsum(Lps)]), dtype=torch.int64, device=dev)
+            if self.mask_padding:                    # [real | padding] per rollout: the bootstrap of 0 follows step L_i
+                seg = torch.tensor(padded_segment_offsets(Ls, S), dtype=torch.int64, device=dev)
+            else:
+                seg = torch.tensor(np.concatenate([[0], np.cumsum(Lps)]), dtype=torch.int64, device=dev)
             if vtrace:
                 # heads that took no action carry no behaviour log-prob (old_logp is 0 there too); padding rows are 0 already
                 acted = torch.stack([actions[k].any(dim=-1) for k in keys], dim=-1)
                 behaviour_logp = torch.where(acted, behaviour_logp, 0.0)
-                valid_len = torch.tensor(Ls, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
+                lens = [n for L in Ls for n in (L, 0)] if self.mask_padding else Ls     # padding segments: no real steps
+                valid_len = torch.tensor(lens, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
                 adv_c, ret_c, self._vtrace_seg_stats = ops.vtrace_scan(
                     rew_c, vals_c, rollout_major(old_logp), rollout_major(behaviour_logp), seg, gamma=self.gamma,
                     lam=self.gae_lambda, rho_clip=self.vtrace_rho_clip, c_clip=self.vtrace_c_clip, valid_len=valid_len,
                     stats=True)
             else:
                 adv_c, ret_c = ops.gae_scan(rew_c, vals_c, seg, gamma=self.gamma, lam=self.gae_lambda)   # :417-421
+            valid = None
+            if self.mask_padding:
+                lens = torch.tensor(chunk_valid_lengths(Ls, S), dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
+                valid = torch.arange(S, device=dev).unsqueeze(1) < lens.unsqueeze(0)             # [S, B]
+                real = valid.t().reshape(-1)                                                      # rollout-major rows
+                adv_c.masked_fill_(~real, 0.0)
+                ret_c.masked_fill_(~real, 0.0)
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
-                    adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same)
+                    adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same, valid=valid)
 
     def experiences_from_rollouts(self, datas):
         """``experiences_from_rollout`` (:328-430) for all rollouts of an iteration at once: per rollout the result equals a
@@ -746,6 +797,7 @@ class DotaOptimizer:
         out = []
         for i, d in enumerate(datas):
             base = int(sum(Lps[:i]))
+            col = base // S                          # the batch column of the rollout's first chunk
             sequences = []
             for j in range(Lps[i] // S):
                 sl = slice(j * S, (j + 1) * S)
@@ -759,7 +811,8 @@ class DotaOptimizer:
                                actions={k: v[sl, i] for k, v in actions.items()},
                                masks={k: v[sl, i] for k, v in masks.items()},
                                values=p['values_lr'][sl, i].reshape(1, S, 1), rewards=p['rewards_np'][i, sl], hidden=hid,
-                               old_logp=p['old_logp'][sl, i])
+                               old_logp=p['old_logp'][sl, i],
+                               valid=None if p['valid'] is None else p['valid'][:, col + j])
                 seq.advantages = p['adv_c'][base + j * S: base + (j + 1) * S]
                 seq.returns = p['ret_c'][base + j * S: base + (j + 1) * S]
                 sequences.append(seq)
@@ -795,7 +848,7 @@ class DotaOptimizer:
         h0 = ops.stack_layers([yb[t_idx, r_idx] for yb in p['ybufs']])
         c0 = ops.stack_layers([cb[t_idx, r_idx] for cb in p['cbufs']]) if pol.cell == "lstm" else None
         old_values = chunked(p['values_lr']).contiguous()               # the critic at prep time (value clipping)
-        return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values)
+        return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values, valid=p['valid'])
 
     @staticmethod
     def list_of_dicts_to_dict_of_lists(x):
@@ -819,6 +872,8 @@ class DotaOptimizer:
         if self.value_clip and batch.old_values is None:
             raise ValueError("value_clip=%r needs the critic values of experience prep, and this batch has no old_values"
                              % self.value_clip)
+        if self.mask_padding and batch.valid is None:
+            raise ValueError("mask_padding=True needs the valid mask of experience prep, and this batch has no valid")
         t_enter = time.perf_counter()
         self._upload_hparams()
         slot = batch._slot
@@ -899,13 +954,15 @@ class DotaOptimizer:
         batch.wait(batch.observations['env'], batch.h0, batch.c0)
         # :619 on the module itself: the data-parallel wrapper's hook-driven reduction stays idle, the step reduces below
         packed, target_unit = self.policy_base._train_forward(batch.observations, hidden, wait=batch.wait)
-        batch.wait(batch.old_logp, batch.advantages, batch.returns, batch.old_values, *batch.masks.values(),
+        valid = batch.valid if self.mask_padding else None
+        batch.wait(batch.old_logp, batch.advantages, batch.returns, batch.old_values, valid, *batch.masks.values(),
                    *batch.actions.values(), *batch.observations.values())
-        # e_clip / entropy_coef / vf_coef / value_clip are read from the device block (_upload_hparams)
+        # e_clip / entropy_coef / vf_coef / value_clip are read from the device block (_upload_hparams); padded tokens
+        # (valid = False) count for nothing under mask_padding
         out, n_actions, d_packed, d_tu, _ = ops.ppo_loss_packed(
             packed, target_unit, [batch.masks[k] for k in keys], [batch.actions[k] for k in keys],
             batch.old_logp, batch.advantages, batch.returns, self.e_clip, self.entropy_coef, self.vf_coef,
-            hparams=self._hparams_dev, old_value=batch.old_values, stats=self._ppo_stats)
+            hparams=self._hparams_dev, old_value=batch.old_values, stats=self._ppo_stats, valid=valid)
         self._n_actions[:5].copy_(n_actions)
         torch.autograd.backward([packed, target_unit], [d_packed, d_tu])                                # :672
         # drop every reference into this step's autograd graph before the gradient finish: it holds the saved activations
@@ -1105,6 +1162,8 @@ class DotaOptimizer:
             metrics['reward_per_sec/{}'.format(k)] = v
         for k in ppo_stats[0]:                                             # means over the steps
             metrics['ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
+        if self.mask_padding:                                              # share of the trained tokens that were padding
+            metrics['padding_fraction'] = (n_steps - sum(rollout_lens)) / n_steps
         if self.advantage_estimator == 'vtrace':                           # read now: the steps have synced the device
             for k, v in self.last_vtrace_stats.items():
                 metrics['vtrace/{}'.format(k)] = v
@@ -1230,10 +1289,11 @@ def init_distribution(backend='nccl'):
 def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          pretrained_model, mq_prefetch_count, log_dir, entropy_coef, vf_coef, run_local,
          hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
-         value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1):
+         value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
+         mask_padding=False):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
-                       vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip,
-                       num_minibatches=num_minibatches)                                  # before any process-group setup
+                       vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
+                       mask_padding=mask_padding)                                        # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -1244,7 +1304,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         run_local=run_local, hidden_size=hidden_size, cell=cell, num_layers=num_layers, gamma=gamma,
         gae_lambda=gae_lambda, clip_range=clip_range, max_grad_norm=max_grad_norm, value_clip=value_clip,
         advantage_estimator=advantage_estimator, vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip,
-        num_minibatches=num_minibatches)
+        num_minibatches=num_minibatches, mask_padding=mask_padding)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -1259,7 +1319,7 @@ def default_log_dir():
 def build_arg_parser():
     """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell``, ``--num-layers`` and the PPO
     settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm``, ``--value-clip``,
-    ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip`` and ``--num-minibatches``."""
+    ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches`` and ``--mask-padding``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -1290,6 +1350,9 @@ def build_arg_parser():
     p.add_argument("--vtrace-c-clip", type=float, help="V-trace truncation c-bar of the trace coefficients", default=1.0)
     p.add_argument("--num-minibatches", type=int, default=1,
                    help="shuffled minibatches of sequences per epoch, one optimizer step each (reference: 1)")
+    p.add_argument("--mask-padding", action="store_true",
+                   help="leave the zero padding of each rollout's last chunk out of GAE / V-trace and the loss "
+                        "(reference: padding is trained on)")
     return p
 
 
@@ -1303,6 +1366,7 @@ if __name__ == '__main__':
              vf_coef=args.vf_coef, run_local=args.run_local, hidden_size=args.hidden_size, cell=args.cell,
              num_layers=args.num_layers, gamma=args.gamma, gae_lambda=args.gae_lambda, clip_range=args.clip_range,
              max_grad_norm=args.max_grad_norm, value_clip=args.value_clip, advantage_estimator=args.advantage_estimator,
-             vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip, num_minibatches=args.num_minibatches)
+             vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip, num_minibatches=args.num_minibatches,
+             mask_padding=args.mask_padding)
     except KeyboardInterrupt:
         pass

@@ -268,7 +268,8 @@ int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEADS], const i
  *       0 approximate KL (k3 estimator (r-1) - log r, r = exp(logp - old_logp)), the mean over the heads with action rows;
  *       1..5 per head, averaged over the head's action rows (0 for a head without any);
  *       6 clip fraction (share of action rows with |r-1| > e_clip), the same mean; 7..11 per head;
- *       12 explained variance 1 - Var(ret - v) / Var(ret) over all N tokens, padding included (NaN if Var(ret) = 0);
+ *       12 explained variance 1 - Var(ret - v) / Var(ret) over all N tokens, padding included (NaN if Var(ret) = 0;
+ *          over the valid tokens only under dc_ppo_loss_fwd_bwd_masked);
  *       13..15 zero.
  */
 #define DC_PPO_STATS_SLOTS 16
@@ -283,6 +284,27 @@ int dc_ppo_loss_fwd_bwd_dev(const float *const logits[DC_NUM_HEADS], const int64
                             float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
                             float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
                             void *workspace, dc_stream_t stream);
+
+/* Same as dc_ppo_loss_fwd_bwd_dev, plus a per-token mask (no counterpart in the reference, which trains on its zero
+ * padding: optimizer.py:587-589,660 average over all tokens and :417-421 bootstrap after the padded length):
+ *   valid [N] bytes (0/1) or NULL.  A token with valid = 0 contributes to nothing and gets exactly zero dlogits rows
+ *       and dvalue.  With N_v the number of valid tokens: n_actions counts valid rows only (and so drives the
+ *       has-gradient flags); out[14] / out[15] are the mean and unbiased std over the valid tokens; policy and entropy
+ *       are per-head means over valid action rows; the value loss is 0.5*vf_coef*sum_valid(...)/N_v (clipped or not) and
+ *       dvalue = vf_coef*g/N_v; the KL / clip-fraction statistics use valid action rows and the explained variance the
+ *       valid tokens.  So the result over N tokens is the unmasked result over the valid tokens alone.
+ *   valid NULL or all 1: bit-identical to dc_ppo_loss_fwd_bwd_dev (N_v = N, same summation order).
+ *   N_v = 0 or 1: the advantage std is NaN, as torch.std gives, and so is the loss when a head has an action row.
+ * Algorithmic bytes: 1 more per token read by each of the two passes.
+ */
+int dc_ppo_loss_fwd_bwd_masked(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                               const uint8_t *const masks[DC_NUM_HEADS],
+                               const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
+                               const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                               const float *old_value, const uint8_t *valid, int64_t N, const double *hparams,
+                               float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                               float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
+                               void *workspace, dc_stream_t stream);
 
 /* Log-prob of the taken action per head, [N,5] dense (0 where the head took no action):
  * the no-grad half of experiences_from_rollout (optimizer.py:387-390). */
