@@ -132,10 +132,12 @@ def _encoder_check():
     return mod
 
 
-@pytest.mark.parametrize("N,n_u,dx2", [(1, 16, False), (7, 5, False), (130, 16, True), (1000, 5, False), (1001, 16, True)])
+@pytest.mark.parametrize("N,n_u,dx2", [(1, 16, False), (7, 5, False), (130, 16, True), (1000, 5, False), (1001, 16, True),
+                                       (40000, 5, True), (40000, 5, False), (20011, 16, True), (20011, 16, False)])
 def test_routed_wgrad_through_the_c_abi(N, n_u, dx2):
     """dc_unit_wgrad_routed: dW = R^T basic, db = colsum R with the max-pool routing R generated inside the kernel
-    (30-row K-chunks of whole tokens for the 5-unit group, ragged last chunk) against the dense fp64 product."""
+    (30-row K-chunks of whole tokens for the 5-unit group, ragged last chunk) against the dense fp64 product; at N = 40000 /
+    20011 every CTA runs several K-chunks.  The reduction has a fixed order: a repeated call is bitwise equal."""
     from dotaclient_b200 import _lib
     ec = _encoder_check()
     lib, st, dev = _lib.load(), _lib.stream_ptr(), torch.device("cuda", 0)
@@ -148,15 +150,25 @@ def test_routed_wgrad_through_the_c_abi(N, n_u, dx2):
                                         dW.data_ptr(), db.data_ptr(), ws.data_ptr(), st), "dc_unit_wgrad_routed")
     torch.testing.assert_close(dW.cpu().double(), dW_r, rtol=1e-4, atol=2e-5 * max(1.0, float(dW_r.abs().max())))
     torch.testing.assert_close(db.cpu().double(), db_r, rtol=1e-4, atol=2e-5 * max(1.0, float(db_r.abs().max())))
+    dW1, db1 = dW.clone(), db.clone()
+    _lib.check(lib.dc_unit_wgrad_routed(dx + 4 * 256, dx + 4 * 640 if dx2 else None, 896, t["am"].data_ptr(), t["basic"].data_ptr(), N, n_u,
+                                        dW.data_ptr(), db.data_ptr(), ws.data_ptr(), st), "dc_unit_wgrad_routed")
+    assert torch.equal(dW, dW1) and torch.equal(db, db1)
 
 
 @pytest.mark.parametrize("N,n_u,dx2,head,routed", [(1, 1, False, True, True), (7, 5, False, True, True), (130, 16, True, True, True),
                                                    (1000, 5, False, False, True), (1001, 16, False, True, True),
-                                                   (300, 1, False, True, False), (26, 5, False, True, True)])
+                                                   (300, 1, False, True, False), (26, 5, False, True, True),
+                                                   (40000, 1, False, True, True), (40000, 1, False, False, True),
+                                                   (40000, 5, True, True, True), (40000, 5, False, False, True),
+                                                   (20011, 16, True, True, True), (20011, 16, False, False, True),
+                                                   (20011, 16, False, True, False)])
 def test_fused_dgrad_through_the_c_abi(N, n_u, dx2, head, routed):
     """dc_unit_dgrad_fused: dW_b, db_b of the shared basic layer from (d_xmax, argmax, dlogits, att) without d(embedding) or
     d_basic in memory -- routing and the rank-1 head term generated in the producers, ReLU mask recomputed in the epilogue --
-    against the dense fp64 chain; 125-row tiles for the 5-unit group, tiles split over the two epilogue halves."""
+    against the dense fp64 chain; 125-row tiles for the 5-unit group, tiles split over the two epilogue halves.  From N = 20011
+    on there are more tiles than SMs, so each CTA carries its ring phase, its dW_b registers and the re-staged units across
+    several tiles.  The reduction has a fixed order: a repeated call is bitwise equal."""
     from dotaclient_b200 import _lib
     ec = _encoder_check()
     lib, st, dev = _lib.load(), _lib.stream_ptr(), torch.device("cuda", 0)
@@ -173,7 +185,93 @@ def test_fused_dgrad_through_the_c_abi(N, n_u, dx2, head, routed):
     tol = dict(rtol=1e-4, atol=2e-5 * max(1.0, float(dwb_r.abs().max())))
     torch.testing.assert_close(dwb.cpu().double(), dwb_r, **tol)
     torch.testing.assert_close(dbb.cpu().double(), dbb_r, **tol)
+    dwb1, dbb1 = dwb.clone(), dbb.clone()
     _lib.check(lib.dc_unit_dgrad_fused(*args, 1, ws.data_ptr(), st), "dc_unit_dgrad_fused")       # accumulate: twice the gradient
     torch.testing.assert_close(dwb.cpu().double(), 2 * dwb_r, **tol)
+    _lib.check(lib.dc_unit_dgrad_fused(*args, 0, ws.data_ptr(), st), "dc_unit_dgrad_fused")
+    assert torch.equal(dwb, dwb1) and torch.equal(dbb, dbb1)
     # bad arguments are reported, not launched
     assert lib.dc_unit_dgrad_fused(*args[:12], 3, *args[13:], 0, ws.data_ptr(), st) != 0
+
+
+def _grid(g, shape, k, scale):
+    """Integers in [-k, k] / scale: few significant bits, so sums of products of such values are exact in fp32 (and in each
+    TF32 half) in any order, and ReLU masks and max-pool arg-maxes cannot differ from a float64 reference by rounding."""
+    return torch.randint(-k, k + 1, shape, generator=g).float() / scale
+
+
+def test_env_encoder_past_one_pass_vs_fp64():
+    """dc_env_fwd / dc_env_bwd at N = 140001 rows of the 896-wide pre-rnn row: both grid-stride loops wrap (135168 rows per
+    forward pass, 67584 per backward pass on 132 SMs).  Forward exact against float64 (grid inputs) and columns >= 128
+    untouched; dW_e, db_e within 4e-6 of the sum of |terms| of float64; a repeated backward is bitwise equal."""
+    from dotaclient_b200 import _lib
+    lib, st, d = _lib.load(), _lib.stream_ptr(), torch.device("cuda", 0)
+    N, ld = 140001, 896
+    g = torch.Generator().manual_seed(140001)
+    env, w_e, b_e = _grid(g, (N, 3), 48, 16), _grid(g, (128, 3), 32, 64), _grid(g, (128,), 8, 64)
+    out_r = F.relu(env.double() @ w_e.double().t() + b_e.double())
+    d_out = torch.randn(N, 128, generator=g)
+    gm = d_out.double() * (out_r > 0)
+    dw_r, db_r = gm.t() @ env.double(), gm.sum(0)
+    dw_abs, db_abs = gm.abs().t() @ env.double().abs(), gm.abs().sum(0)
+
+    out = torch.full((N, ld), 7.0, device=d)
+    env_d, w_d, b_d = env.to(d), w_e.to(d), b_e.to(d)
+    _lib.check(lib.dc_env_fwd(env_d.data_ptr(), w_d.data_ptr(), b_d.data_ptr(), out.data_ptr(), ld, N, st), "dc_env_fwd")
+    assert torch.equal(out[:, :128].cpu().double(), out_r)
+    assert bool((out[:, 128:] == 7.0).all())
+    d_full = torch.zeros(N, ld, device=d)
+    d_full[:, :128] = d_out.to(d)
+    ws = torch.empty(int(lib.dc_env_bwd_workspace_bytes()), dtype=torch.uint8, device=d)
+    results = []
+    for _ in range(2):
+        dw, db = torch.full((128, 3), 7.0, device=d), torch.full((128,), 7.0, device=d)
+        _lib.check(lib.dc_env_bwd(d_full.data_ptr(), out.data_ptr(), ld, env_d.data_ptr(), dw.data_ptr(), db.data_ptr(), N,
+                                  ws.data_ptr(), st), "dc_env_bwd")
+        results.append((dw.cpu(), db.cpu()))
+    (dw, db), (dw2, db2) = results
+    assert ((dw.double() - dw_r).abs() <= 4e-6 * dw_abs).all(), float(((dw.double() - dw_r).abs() / dw_abs).max())
+    assert ((db.double() - db_r).abs() <= 4e-6 * db_abs).all(), float(((db.double() - db_r).abs() / db_abs).max())
+    assert torch.equal(dw, dw2) and torch.equal(db, db2)
+
+
+def test_unit_encoder_with_target_unit_head_many_tiles_vs_fp64():
+    """unit_encoder + target_unit forward and backward at lead (48, 128) = 6144 tokens, 245760 unit rows: the basic-layer
+    loop wraps and each CTA of the 16-unit groups' fused data gradient runs about 6 tiles.  Inputs and weights on coarse
+    grids make the forward exact, so the pre-rnn row must equal float64 exactly (arg-max ties included: the first unit
+    wins on both sides); the target-unit logits and every gradient against float64 autograd."""
+    from dotaclient_b200 import encoder_ops
+    lead = (48, 128)
+    g = torch.Generator().manual_seed(6144)
+    env = _grid(g, (*lead, 3), 48, 16)
+    w_e, b_e = _grid(g, (128, 3), 32, 64), _grid(g, (128,), 8, 64)
+    w_b, b_b = _grid(g, (128, 12), 4, 8), _grid(g, (128,), 16, 32)
+    units = [_grid(g, (*lead, n, 12), 4, 4) for n in UNITS]
+    weights = [_grid(g, (128, 128), 8, 64) for _ in UNITS]
+    biases = [_grid(g, (128,), 8, 64) for _ in UNITS]
+    att = torch.randn(*lead, 128, generator=g)
+    g_x = torch.randn(*lead, 7 * 128, generator=g)
+    g_tu = torch.randn(*lead, 40, generator=g)
+    g_tu[..., ::2, :] = 0                                  # tokens where the head was not used
+
+    refs = [t.double().requires_grad_(True) for t in [w_b, b_b] + weights + biases + [w_e, b_e]]
+    att_r = att.double().requires_grad_(True)
+    ue_r, x_r = _reference(env.double(), refs[14], refs[15], refs[0], refs[1], [u.double() for u in units], refs[2:8],
+                           refs[8:14])
+    tu_r = torch.matmul(att_r.unsqueeze(-2), ue_r.transpose(-1, -2)).squeeze(-2)
+    ((x_r * g_x.double()).sum() + (tu_r * g_tu.double()).sum()).backward()
+    del ue_r
+
+    d = torch.device("cuda", 0)
+    params = [t.detach().float().to(d).requires_grad_(True) for t in refs]
+    att_d = att.to(d).requires_grad_(True)
+    link, x = encoder_ops.unit_encoder(env.to(d), params[14], params[15], params[0], params[1], [u.to(d) for u in units],
+                                       params[2:8], params[8:14])
+    assert torch.equal(x.detach().cpu().double(), x_r.detach())
+    tu = encoder_ops.target_unit(att_d, link)
+    ((x * g_x.to(d)).sum() + (tu * g_tu.to(d)).sum()).backward()
+    tol = lambda ref: dict(rtol=0, atol=2e-5 * float(ref.detach().abs().max()))    # noqa: E731
+    torch.testing.assert_close(tu.detach().cpu().double(), tu_r.detach(), **tol(tu_r))
+    torch.testing.assert_close(att_d.grad.cpu().double(), att_r.grad, **tol(att_r.grad))
+    for i, (mine, ref) in enumerate(zip(params, refs)):
+        torch.testing.assert_close(mine.grad.cpu().double(), ref.grad, msg="parameter %d" % i, **tol(ref.grad))

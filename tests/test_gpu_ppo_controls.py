@@ -43,11 +43,12 @@ def _check_stats(got, want):
 
 # ------------------------------------------------------------------------------------------------ kernel vs oracle
 @pytest.mark.parametrize("n_tokens,drop,pad", [(300, None, None), (1000, None, 900), (129, "ability", 100), (5, "x", None),
-                                               (640, "target_unit", 517)])
+                                               (640, "target_unit", 517), (131072, None, None)])
 @pytest.mark.parametrize("value_clip", [None, 0.05])
 def test_stats_and_clipped_value_loss_vs_oracle(n_tokens, drop, pad, value_clip):
     """Several 128-token CTAs, a head without action rows, padding rows: losses, entropies, the diagnostics, dlogits and
-    dvalue of dc_ppo_loss_fwd_bwd_dev against the oracle's autograd (clipped value loss when value_clip is set)."""
+    dvalue of dc_ppo_loss_fwd_bwd_dev against the oracle's autograd (clipped value loss when value_clip is set).
+    131072 tokens are C2's batch: 1024 CTAs meet in the last-CTA ticket and the float64 atomics."""
     from dotaclient_b200 import ops
     e_clip, entropy_coef, vf_coef = 0.2, 5e-4, 0.5
     logits, masks, actions, old, values, adv, ret = P._random_loss_inputs(n_tokens, 11 + n_tokens, drop, pad)
