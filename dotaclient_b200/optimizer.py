@@ -419,19 +419,39 @@ def minibatch_indices(B, num_minibatches, rng):
     return np.array_split(rng.permutation(B), num_minibatches)
 
 
-def padded_segment_offsets(lengths, seq_len):
-    """Row offsets of the scan segments of experience prep under ``mask_padding``: rollout i occupies its padded length
-    ``Lp_i`` (``lengths[i]`` rounded up to a multiple of ``seq_len``) of the rollout-major rows and is split into a real
-    segment of ``lengths[i]`` rows and a padding segment of ``Lp_i - lengths[i]`` rows (possibly empty), so that the real
-    segment ends on the terminal bootstrap of 0.  Returns int64 ``[2R + 1]``: ``0, L_0, Lp_0, Lp_0 + L_1, Lp_0 + Lp_1, ...``."""
-    out = np.zeros(2 * len(lengths) + 1, dtype=np.int64)
-    base = 0
-    for i, L in enumerate(lengths):
+def rollout_segments(lengths, terminal, seq_len, mask_padding):
+    """The scan segments of experience prep.  Rollout i occupies its padded length ``Lp_i`` (``lengths[i]`` rounded up to a
+    multiple of ``seq_len``) of the rollout-major rows.  A terminal rollout without ``mask_padding`` is one segment of
+    ``Lp_i`` rows ending on the terminal bootstrap of 0 (the reference's layout).  Otherwise it is two: its ``lengths[i]``
+    real rows, then its ``Lp_i - lengths[i]`` padding rows (possibly none), which end on 0.  The real segment of a rollout
+    that is not ``terminal[i]`` ends on the bootstrap value of the state its game continues from; that of a terminal one on 0.
+
+    Returns int64 arrays ``(seg_off [n_seg + 1], boot [n_seg], valid_len [n_seg])``: ``boot[s]`` is the index, among the
+    non-terminal rollouts in order, of the one whose bootstrap value ends segment ``s``, or -1 for 0; ``valid_len[s]`` is
+    the number of real steps in segment ``s``."""
+    off, boot, valid = [0], [], []
+    base = n_cut = 0
+    for L, term in zip(lengths, terminal):
         L = int(L)
-        out[2 * i + 1] = base + L
-        base += (L + seq_len - 1) // seq_len * seq_len
-        out[2 * i + 2] = base
-    return out
+        Lp = (L + seq_len - 1) // seq_len * seq_len
+        if term and not mask_padding:
+            off.append(base + Lp)
+            boot.append(-1)
+            valid.append(L)
+        else:
+            off += [base + L, base + Lp]
+            boot += [-1 if term else n_cut, -1]
+            valid += [L, 0]
+        n_cut += not term
+        base += Lp
+    return np.array(off, dtype=np.int64), np.array(boot, dtype=np.int64), np.array(valid, dtype=np.int64)
+
+
+def padded_segment_offsets(lengths, seq_len):
+    """Row offsets of the scan segments of experience prep under ``mask_padding`` for terminal rollouts
+    (``rollout_segments``): a real segment of ``lengths[i]`` rows and a padding segment, so that the real segment ends on
+    the terminal bootstrap of 0.  Returns int64 ``[2R + 1]``: ``0, L_0, Lp_0, Lp_0 + L_1, Lp_0 + Lp_1, ...``."""
+    return rollout_segments(lengths, [True] * len(lengths), seq_len, True)[0]
 
 
 def chunk_valid_lengths(lengths, seq_len):
@@ -460,6 +480,48 @@ def check_behaviour_logp(datas):
             t, h = (int(i) for i in bad.nonzero()[0])
             raise ValueError("%s: 'behaviour_logp' is %r at step %d on head %r, which took an action there"
                              % (who, float(blp[t, h]), t, ops.HEAD_KEYS[h]))
+
+
+def check_continuation(datas, cell, num_layers, hidden_size):
+    """Raises ``ValueError``, naming the rollout's ``game_id`` / ``player_id``, when one of the optional keys of a rollout
+    cut from a longer game is malformed: an ``'initial_hidden'`` that is not the structure ``Policy.init_hidden()`` returns
+    (a ``[num_layers, 1, hidden_size]`` float tensor or array; an ``(h, c)`` pair of them for the LSTM) or that is not
+    finite; a ``'terminal'`` that is not a bool; a non-terminal rollout of no steps.  Also raises when an observation key
+    does not have L rows (terminal) or L + 1 rows (non-terminal: row L is the state the game continues from).  Runs on the
+    host before anything is uploaded."""
+    want = (int(num_layers), 1, int(hidden_size))
+    for d in datas:
+        who = "rollout game_id=%r player_id=%r" % (d.get('game_id'), d.get('player_id'))
+        terminal = d.get('terminal', True)
+        if not isinstance(terminal, (bool, np.bool_)):
+            raise ValueError("%s: 'terminal' must be True or False, got %r" % (who, terminal))
+        L = int(d['rewards'].shape[0])
+        if not terminal and L < 1:
+            raise ValueError("%s: a non-terminal rollout needs at least one step" % who)
+        rows = L if terminal else L + 1
+        for k in Policy.INPUT_KEYS:
+            n = int(d['observations'][k].shape[0])
+            if n != rows:
+                raise ValueError("%s: observations[%r] has %d rows; a %s rollout of %d steps carries %d"
+                                 % (who, k, n, "terminal" if terminal else "non-terminal", L, rows))
+        if 'initial_hidden' not in d:
+            continue
+        h = d['initial_hidden']
+        pair = isinstance(h, (tuple, list))
+        parts = list(h) if pair else [h]
+        if pair != (cell == "lstm") or len(parts) != (2 if cell == "lstm" else 1):
+            raise ValueError("%s: 'initial_hidden' must be %s, as Policy.init_hidden() returns for the %s"
+                             % (who, "an (h, c) pair of [%d, %d, %d] arrays" % want if cell == "lstm"
+                                else "one [%d, %d, %d] array" % want, cell.upper()))
+        for p in parts:
+            if not isinstance(p, (torch.Tensor, np.ndarray)):
+                raise ValueError("%s: 'initial_hidden' holds a %s, not a tensor or an array" % (who, type(p).__name__))
+            t = torch.as_tensor(p)
+            if tuple(t.shape) != want or not t.is_floating_point():
+                raise ValueError("%s: 'initial_hidden' must be float [%d, %d, %d], got %s %s"
+                                 % ((who,) + want + (t.dtype, tuple(t.shape))))
+            if not bool(torch.isfinite(t).all()):
+                raise ValueError("%s: 'initial_hidden' is not finite" % who)
 
 
 class DotaOptimizer:
@@ -694,22 +756,40 @@ class DotaOptimizer:
         time-major ``[L_max, R, ...]`` pass -- encoder chain, recurrence from the zero state, heads, selected log-probs
         (:384-390) -- followed by ONE segmented GAE scan over every rollout's own padded length (:417-421), or with
         ``advantage_estimator='vtrace'`` ONE segmented V-trace scan of the same segments.  With ``mask_padding`` each
-        rollout is two segments, its real steps and its padding (``padded_segment_offsets``), so the terminal bootstrap
+        rollout is two segments, its real steps and its padding (``rollout_segments``), so the terminal bootstrap
         follows the last real step; advantages and returns of padded rows are then zeroed and ``valid [S, B]`` marks the
-        real steps of every chunk.  Returns the raw device tensors; ``experiences_from_rollouts`` / ``batch_from_rollouts``
-        slice them."""
+        real steps of every chunk.
+
+        A rollout cut from a longer game (``check_continuation``) starts the pass from its ``'initial_hidden'`` instead of
+        the zero state.  One that is not ``'terminal'`` is always two segments, and its real segment bootstraps from
+        V(s_L), the critic's value of its extra observation row: ONE more single-step forward of batch R' (the number of
+        such rollouts) from each one's state after its last step, state buffer slot L_i.  The extra row enters neither the
+        main pass nor the batch.  Without either key in any rollout none of this runs.  Returns the raw device tensors;
+        ``experiences_from_rollouts`` / ``batch_from_rollouts`` slice them."""
         S, dev, pol = self.seq_len, self.device, self.policy_base
         R = len(datas)
+        n_layers, H, lstm = pol.num_layers, pol.hidden_size, pol.cell == "lstm"
         vtrace = self.advantage_estimator == 'vtrace'
         if vtrace:
             check_behaviour_logp(datas)                # refused before anything is uploaded
+        check_continuation(datas, pol.cell, n_layers, H)
         Ls = [int(d['rewards'].shape[0]) for d in datas]
         Lps = [(L + S - 1) // S * S for L in Ls]
         Lmax = max(Lps)
         same = all(L == Lmax for L in Ls)
+        terminal = [bool(d.get('terminal', True)) for d in datas]
+        cut = [i for i in range(R) if not terminal[i]]           # the rollouts whose game goes on: bootstrapped from V(s_L)
+        carried = any('initial_hidden' in d for d in datas)
 
         if self._staging_event is not None:
             self._staging_event.synchronize()          # the previous iteration's uploads have left the staging buffers
+
+        def pinned(key, shape, dtype):
+            buf = self._staging.get(key)
+            if buf is None or buf.shape != shape or buf.dtype != dtype:
+                buf = torch.empty(shape, dtype=dtype).pin_memory()
+                self._staging[key] = buf
+            return buf
 
         def batched(group, key, dtype):
             """Rollouts -> one time-major ``[Lmax, R, ...]`` device tensor.  The host side only does contiguous per-rollout
@@ -717,13 +797,9 @@ class DotaOptimizer:
             768-byte-granular scatter, 3x slower) and uploads asynchronously; the transposition to time-major runs on the GPU.
             ``group`` None: a top-level key of the rollout."""
             srcs = [torch.as_tensor(d[group][key] if group else d[key]) for d in datas]
-            shape = (R, Lmax) + tuple(srcs[0].shape[1:])
-            buf = self._staging.get((group, key))
-            if buf is None or buf.shape != shape or buf.dtype != dtype:
-                buf = torch.empty(shape, dtype=dtype).pin_memory()
-                self._staging[(group, key)] = buf
+            buf = pinned((group, key), (R, Lmax) + tuple(srcs[0].shape[1:]), dtype)
             for i, t in enumerate(srcs):
-                buf[i, :Ls[i]].copy_(t)
+                buf[i, :Ls[i]].copy_(t[:Ls[i]])                                        # not the extra row of a cut rollout
                 if Ls[i] < Lmax:
                     buf[i, Ls[i]:].zero_()                                             # zero padding (:367-382)
             return buf.to(dev, non_blocking=True).transpose(0, 1).contiguous()
@@ -732,6 +808,28 @@ class DotaOptimizer:
         masks = {k: batched('masks', k, torch.bool) for k in Policy.OUTPUT_KEYS}
         actions = {k: batched('actions', k, torch.bool) for k in Policy.OUTPUT_KEYS}
         behaviour_logp = batched(None, 'behaviour_logp', torch.float32) if vtrace else None      # [Lmax, R, 5]
+        if carried:                                    # the actors' states entering each rollout, zero where absent
+            buf = pinned(('initial_hidden',), (2 if lstm else 1, n_layers, R, H), torch.float32)
+            buf.zero_()
+            for i, d in enumerate(datas):
+                if 'initial_hidden' in d:
+                    for j, part in enumerate(d['initial_hidden'] if lstm else [d['initial_hidden']]):
+                        buf[j, :, i].copy_(torch.as_tensor(part).reshape(n_layers, H))
+            state0 = buf.to(dev, non_blocking=True)
+        seg_np, boot_src, seg_valid = rollout_segments(Ls, terminal, S, self.mask_padding)
+        if cut:                                        # the observation each cut game continues from: row L_i, [1, R', ...]
+            obs_next = {}
+            for k in Policy.INPUT_KEYS:
+                srcs = [torch.as_tensor(datas[i]['observations'][k])[Ls[i]] for i in cut]
+                buf = pinned(('bootstrap', k), (len(cut),) + tuple(srcs[0].shape), torch.float32)
+                for j, t in enumerate(srcs):
+                    buf[j].copy_(t)
+                obs_next[k] = buf.to(dev, non_blocking=True).unsqueeze(0)
+            # state buffer slot (L_i) and column (i) of every cut rollout's state after its last step, and for every segment
+            # the slot of its bootstrap in [0, b_0, b_1, ...]
+            idx = torch.from_numpy(np.concatenate([[Ls[i] for i in cut], cut, boot_src + 1]).astype(np.int64))
+            idx = idx.pin_memory().to(dev, non_blocking=True)
+            slot_last, col_last, boot_slot = idx[:len(cut)], idx[len(cut):2 * len(cut)], idx[2 * len(cut):]
         self._staging_event = torch.cuda.Event()
         self._staging_event.record()
         rewards_np = np.zeros((R, Lmax, len(REWARD_KEYS)), dtype=np.float32)
@@ -739,13 +837,23 @@ class DotaOptimizer:
             rewards_np[i, :Ls[i]] = np.asarray(d['rewards'], dtype=np.float32)
         with torch.no_grad():
             x, unit_embedding = pol._encode(obs['env'], [obs[k] for k in Policy.INPUT_KEYS[1:]])
-            n_layers = pol.num_layers
-            h0 = torch.zeros((n_layers, R, pol.hidden_size), dtype=torch.float32, device=dev)
-            c0 = torch.zeros_like(h0) if pol.cell == "lstm" else None
+            if carried:
+                h0, c0 = state0[0], (state0[1] if lstm else None)
+            else:
+                h0 = torch.zeros((n_layers, R, H), dtype=torch.float32, device=dev)
+                c0 = torch.zeros_like(h0) if lstm else None
             # every layer's state buffers are kept: the state entering chunk j of rollout i is ybufs[k][j*S, i] per layer k
-            ybufs, cbufs = ops.rnn_stack_forward_states(x.contiguous(), [pol.rnn.layer(k) for k in range(n_layers)],
-                                                        h0, c0, pol.cell)
+            layers = [pol.rnn.layer(k) for k in range(n_layers)]
+            ybufs, cbufs = ops.rnn_stack_forward_states(x.contiguous(), layers, h0, c0, pol.cell)
             logits, values = pol._heads(ybufs[-1][1:], unit_embedding)
+            bootstrap = boot = None
+            if cut:                                    # V(s_L) of every cut rollout: one step of batch R' from slot L_i
+                xb, ue = pol._encode(obs_next['env'], [obs_next[k] for k in Policy.INPUT_KEYS[1:]])
+                hb = ops.stack_layers([yb[slot_last, col_last] for yb in ybufs])
+                cb = ops.stack_layers([c[slot_last, col_last] for c in cbufs]) if lstm else None
+                yb_next, _ = ops.rnn_stack_forward_states(xb.contiguous(), layers, hb, cb, pol.cell)
+                bootstrap = pol._heads(yb_next[-1][1:], ue)[1].reshape(len(cut))
+                boot = torch.cat([bootstrap.new_zeros(1), bootstrap])[boot_slot]          # per segment
             keys = ops.HEAD_KEYS
             old_logp = ops.selected_logp([logits[k] for k in keys], [masks[k] for k in keys],
                                          [actions[k] for k in keys]).view(Lmax, R, 5)        # :387-390
@@ -761,22 +869,21 @@ class DotaOptimizer:
                 rew_c = torch.from_numpy(rewards_np.reshape(R * Lmax, -1)).to(dev, non_blocking=True)
             else:
                 rew_c = torch.from_numpy(np.concatenate([rewards_np[i, :Lps[i]] for i in range(R)])).to(dev)
-            if self.mask_padding:                    # [real | padding] per rollout: the bootstrap of 0 follows step L_i
-                seg = torch.tensor(padded_segment_offsets(Ls, S), dtype=torch.int64, device=dev)
-            else:
-                seg = torch.tensor(np.concatenate([[0], np.cumsum(Lps)]), dtype=torch.int64, device=dev)
+            # [real | padding] per rollout under mask_padding or when cut: the bootstrap follows step L_i
+            seg = torch.tensor(seg_np, dtype=torch.int64, device=dev)
             if vtrace:
                 # heads that took no action carry no behaviour log-prob (old_logp is 0 there too); padding rows are 0 already
                 acted = torch.stack([actions[k].any(dim=-1) for k in keys], dim=-1)
                 behaviour_logp = torch.where(acted, behaviour_logp, 0.0)
-                lens = [n for L in Ls for n in (L, 0)] if self.mask_padding else Ls     # padding segments: no real steps
-                valid_len = torch.tensor(lens, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
+                valid_len = torch.from_numpy(seg_valid).pin_memory().to(dev, non_blocking=True)  # padding: no real steps
                 adv_c, ret_c, self._vtrace_seg_stats = ops.vtrace_scan(
                     rew_c, vals_c, rollout_major(old_logp), rollout_major(behaviour_logp), seg, gamma=self.gamma,
-                    lam=self.gae_lambda, rho_clip=self.vtrace_rho_clip, c_clip=self.vtrace_c_clip, valid_len=valid_len,
-                    stats=True)
+                    lam=self.gae_lambda, rho_clip=self.vtrace_rho_clip, c_clip=self.vtrace_c_clip, boot_value=boot,
+                    valid_len=valid_len, stats=True)
             else:
-                adv_c, ret_c = ops.gae_scan(rew_c, vals_c, seg, gamma=self.gamma, lam=self.gae_lambda)   # :417-421
+                # :417-421; a cut rollout's returns go on past the cut as gamma^(L-t) V(s_L), its advantages from V(s_L)
+                adv_c, ret_c = ops.gae_scan(rew_c, vals_c, seg, gamma=self.gamma, lam=self.gae_lambda, boot_value=boot,
+                                            boot_reward=boot)
             valid = None
             if self.mask_padding:
                 lens = torch.tensor(chunk_valid_lengths(Ls, S), dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
@@ -785,7 +892,8 @@ class DotaOptimizer:
                 adv_c.masked_fill_(~real, 0.0)
                 ret_c.masked_fill_(~real, 0.0)
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
-                    adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same, valid=valid)
+                    adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same, valid=valid,
+                    bootstrap=bootstrap)
 
     def experiences_from_rollouts(self, datas):
         """``experiences_from_rollout`` (:328-430) for all rollouts of an iteration at once: per rollout the result equals a
@@ -1164,6 +1272,9 @@ class DotaOptimizer:
             metrics['ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
         if self.mask_padding:                                              # share of the trained tokens that were padding
             metrics['padding_fraction'] = (n_steps - sum(rollout_lens)) / n_steps
+        n_cut = sum(not r.get('terminal', True) for r in rollouts)
+        if n_cut:                                                          # share of the rollouts cut from a game that goes on
+            metrics['non_terminal_fraction'] = n_cut / len(rollouts)
         if self.advantage_estimator == 'vtrace':                           # read now: the steps have synced the device
             for k, v in self.last_vtrace_stats.items():
                 metrics['vtrace/{}'.format(k)] = v

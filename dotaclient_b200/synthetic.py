@@ -59,6 +59,35 @@ def make_rollout(length, seed, game_id=0, team_id=2, weight_version=1, with_canv
     return data
 
 
+def split_rollout(data, cuts, initial_hiddens=None):
+    """One game's rollout -> the pieces an actor publishing every few steps sends: cut before each step in ``cuts``
+    (increasing, each in ``[1, L)``).  Piece p holds steps ``[a, b)``.  Every piece but the last is ``'terminal': False``
+    and its observations carry ``b - a + 1`` rows: row ``b - a`` is the observation after its last step, which is also the
+    next piece's row 0.  The last piece is ``'terminal': True``.  ``initial_hiddens`` (optional, one entry per piece, None
+    for none) become the pieces' ``'initial_hidden'``: the actor's recurrent state entering the piece's first step."""
+    L = int(data['rewards'].shape[0])
+    bounds = [0] + [int(c) for c in cuts] + [L]
+    if any(b <= a for a, b in zip(bounds, bounds[1:])):
+        raise ValueError("cuts=%r: must increase strictly within [1, %d)" % (list(cuts), L))
+    if initial_hiddens is not None and len(initial_hiddens) != len(bounds) - 1:
+        raise ValueError("initial_hiddens: %d entries for %d pieces" % (len(initial_hiddens), len(bounds) - 1))
+    pieces = []
+    for p, (a, b) in enumerate(zip(bounds, bounds[1:])):
+        last = b == L
+        piece = {k: v for k, v in data.items() if k not in ('observations', 'masks', 'actions', 'rewards', 'behaviour_logp')}
+        piece['observations'] = {k: v[a:b if last else b + 1] for k, v in data['observations'].items()}
+        for k in ('masks', 'actions'):
+            piece[k] = {h: v[a:b] for h, v in data[k].items()}
+        piece['rewards'] = data['rewards'][a:b]
+        if 'behaviour_logp' in data:
+            piece['behaviour_logp'] = data['behaviour_logp'][a:b]
+        piece['terminal'] = last
+        if initial_hiddens is not None and initial_hiddens[p] is not None:
+            piece['initial_hidden'] = initial_hiddens[p]
+        pieces.append(piece)
+    return pieces
+
+
 def rollout_seed(rank, index):
     """SURVEY.md 8(d): ``7 + 1000*rank + i``."""
     return 7 + 1000 * int(rank) + int(index)
