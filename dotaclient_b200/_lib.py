@@ -29,6 +29,9 @@ SIGNATURES = {
     "dc_rnn_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "dc_rnn_seq_fwd": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "dc_rnn_seq_bwd": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "dc_rnn_seq_fwd_reset": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "dc_rnn_seq_bwd_reset": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp,
+                                    _vp]),
     "dc_gemm_tf32x3_supported": (_i32, [_i64, _i32, _i32]),
     "dc_gemm_tf32x3": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _i64, _i32, _i32, _i32, _vp]),
     "dc_gemm_wgrad_workspace_bytes": (_sz, [_i32, _i32]),

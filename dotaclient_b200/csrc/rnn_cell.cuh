@@ -7,6 +7,19 @@
 
 namespace dc_rnn {
 
+// Recurrent-state resets inside a sequence (dc_rnn_seq_fwd_reset / dc_rnn_seq_bwd_reset).  slot [S, B] int32: k = slot[t*B + b]
+// >= 0 replaces the state entering step t of sequence b with row r = k*B + b of the column-local tables
+//   prev [K, B, H]      h (GRU) or c (LSTM): the cell's `prev` operand
+//   pre  [K, B, G*H]    h W_hh^T + b_hh of the reset h: the cell's `pre` operand (forward only)
+// so the mat-vec of the step on the stale state is discarded.  Backward reads `prev` from the table and carries no gradient
+// into step t-1 (neither through W_hh nor the direct dh z / dc f path).  Kernels take it as a template flag: the
+// instantiations without it are the plain recurrence.
+struct Reset {
+    const int *slot;
+    const float *prev;
+    const float *pre;
+};
+
 // Forward step.  gi(g): i2h pre-activation of gate g (x W_ih^T + b_ih); pre(g): h2h pre-activation (W_hh h_{t-1} + b_hh);
 // prev: h_{t-1} (GRU) or c_{t-1} (LSTM).  gi and pre are callables so that each kernel reads its inputs where the cell
 // uses them (keeps register allocation as tight as a hand-inlined cell).  Writes the activated gates to act and what

@@ -87,10 +87,12 @@ struct FwdSmem {
 };
 constexpr int kNP = 2;                                            // (sequence, unit) pairs per thread in the gate phase
 
-template <int G>
+// kReset: resets from rs (rnn_cell.cuh).  The all-gather and the MMAs run unchanged on the stale state; the gate math of a
+// reset token takes pre and prev from the tables.  Each step's reset slots are prefetched with its i2h inputs.
+template <int G, bool kReset = false>
 __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, const float *__restrict__ w_hh,
                                                                    const float *__restrict__ b_hh, float *ybuf, float *cbuf,
-                                                                   int B, int S) {
+                                                                   int B, int S, dc_rnn::Reset rs) {
     constexpr int H = kH, GH = G * kH, NP = kNP;
     extern __shared__ unsigned char smem_raw[];
     unsigned char *base = align1024(smem_raw);
@@ -147,6 +149,7 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
     // gate phase: thread = (unit ul, sequences sb + 16 i)
     const int ul = lane, unit = rank * 32 + ul, sb = warp;
     float bias[G], c_reg[NP], h_reg[NP], cur[NP][G], nxt[NP][G];
+    int cslot[NP], nslot[NP];                                              // reset slots of this step and the next (kReset)
     bool live[NP];
 #pragma unroll
     for (int g = 0; g < G; ++g) bias[g] = __ldg(b_hh + g * H + unit);
@@ -154,6 +157,7 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
     for (int i = 0; i < NP; ++i) {
         const int b = b0 + sb + 16 * i;
         live[i] = b < B;
+        if constexpr (kReset) cslot[i] = nslot[i] = live[i] ? __ldg(rs.slot + b) : -1;
         c_reg[i] = (G == 4 && live[i]) ? cbuf[(size_t)b * H + unit] : 0.f;
         h_reg[i] = (G == 3 && live[i]) ? ybuf[(size_t)b * H + unit] : 0.f;
 #pragma unroll
@@ -205,10 +209,12 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
         // prefetch the next step's i2h pre-activations while the tensor core works
         if (t + 1 < S) {
 #pragma unroll
-            for (int i = 0; i < NP; ++i)
+            for (int i = 0; i < NP; ++i) {
 #pragma unroll
                 for (int g = 0; g < G; ++g)
                     nxt[i][g] = live[i] ? gates[((size_t)(t + 1) * B + b0 + sb + 16 * i) * GH + g * H + unit] : 0.f;
+                if constexpr (kReset) nslot[i] = live[i] ? __ldg(rs.slot + (size_t)(t + 1) * B + b0 + sb + 16 * i) : -1;
+            }
         }
         dc_wgmma_wait0();
         acc_fence(d);
@@ -226,8 +232,15 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
             float pre[G];
 #pragma unroll
             for (int g = 0; g < G; ++g) pre[g] = bias[g] + (scratch[(g * kNB + bb) * 32 + ul] + scratch[((4 + g) * kNB + bb) * 32 + ul]);
+            float prev = G == 3 ? h_reg[i] : c_reg[i];
+            if (kReset && cslot[i] >= 0) {
+                const size_t r = (size_t)cslot[i] * B + b0 + bb;
+#pragma unroll
+                for (int g = 0; g < G; ++g) pre[g] = rs.pre[r * GH + g * H + unit];
+                prev = rs.prev[r * H + unit];
+            }
             const float hnew = dc_rnn::cell_fwd<G>([&](int g) { return cur[i][g]; }, [&](int g) { return pre[g]; },
-                                                   G == 3 ? h_reg[i] : c_reg[i], act[i], aux[i]);
+                                                   prev, act[i], aux[i]);
             if (G == 3) h_reg[i] = hnew;
             else c_reg[i] = aux[i];
             if (live[i]) ybuf[((size_t)(t + 1) * B + b0 + bb) * H + unit] = hnew;  // the slice the other CTAs wait for
@@ -245,6 +258,7 @@ __global__ void __launch_bounds__(kThreads, 1) fwd_cluster_kernel(float *gates, 
             }
 #pragma unroll
             for (int g = 0; g < G; ++g) cur[i][g] = nxt[i][g];
+            if constexpr (kReset) cslot[i] = nslot[i];
         }
         cluster_wait();
     }
@@ -262,12 +276,14 @@ struct BwdSmem {
 
 inline size_t bwd_workspace_bytes(int B) { return (size_t)2 * ((B + kNB - 1) / kNB) * kCL * kNB * kH * sizeof(float); }
 
-template <int G>
+// kReset: resets from rs (rnn_cell.cuh).  A reset token reads prev from the table and puts zero carries and a zero column into
+// the B operand, so every CTA's partial for that sequence -- and so the reduce-scatter into step t-1 -- is exactly zero.
+template <int G, bool kReset = false>
 __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, const float *__restrict__ w_hh, const float *ybuf,
                                                                    float *cbuf, const float *__restrict__ dy,
                                                                    const float *__restrict__ dhn, const float *__restrict__ dcn,
                                                                    float *__restrict__ dh0, float *__restrict__ dc0, float *part,
-                                                                   int B, int S) {
+                                                                   int B, int S, dc_rnn::Reset rs) {
     constexpr int H = kH, GH = G * kH, NP = kNP;
     extern __shared__ unsigned char smem_raw[];
     unsigned char *base = align1024(smem_raw);
@@ -319,10 +335,12 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
     float dh_carry[NP], dc_carry[NP], c_cur[NP];
     // per-step inputs, prefetched one step ahead: saved gates, dy, aux0 (LSTM c_{t-1} | GRU hn), aux1 (GRU h_{t-1})
     float cg[NP][G], cdy[NP], ca0[NP], ca1[NP], ng[NP][G], ndy[NP], na0[NP], na1[NP];
-    auto fetch = [&](int t, float (&fg)[NP][G], float (&fdy)[NP], float (&fa0)[NP], float (&fa1)[NP]) {
+    int cslot[NP], nslot[NP];                                                      // reset slots (kReset)
+    auto fetch = [&](int t, float (&fg)[NP][G], float (&fdy)[NP], float (&fa0)[NP], float (&fa1)[NP], int (&fsl)[NP]) {
 #pragma unroll
         for (int i = 0; i < NP; ++i) {
             const size_t tok = (size_t)t * B + b0 + sb + 16 * i;
+            if constexpr (kReset) fsl[i] = live[i] ? __ldg(rs.slot + tok) : -1;
             if (live[i]) {
 #pragma unroll
                 for (int g = 0; g < G; ++g) fg[i][g] = gates[tok * GH + g * H + unit];
@@ -349,8 +367,8 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
         dc_carry[i] = (G == 4 && live[i] && dcn) ? dcn[(size_t)b * H + unit] : 0.f;
         c_cur[i] = (G == 4 && live[i]) ? cbuf[((size_t)S * B + b) * H + unit] : 0.f;
     }
-    fetch(S - 1, cg, cdy, ca0, ca1);
-    fetch(S - 1, ng, ndy, na0, na1);                                               // (initialises the second buffer)
+    fetch(S - 1, cg, cdy, ca0, ca1, cslot);
+    fetch(S - 1, ng, ndy, na0, na1, nslot);                                        // (initialises the second buffer)
     cluster_barrier();
 
     for (int it = 0; it < S; ++it) {
@@ -373,11 +391,18 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
 #pragma unroll
             for (int g = 0; g < G; ++g) dgi[i][g] = d[g] = 0.f;
             if (live[i]) {
+                float prev = G == 3 ? ca1[i] : ca0[i];                             // h_{t-1} | c_{t-1}
+                if (kReset && cslot[i] >= 0) prev = rs.prev[((size_t)cslot[i] * B + b0 + bb) * H + unit];
                 dh_carry[i] = dc_rnn::cell_bwd<G>([&](int g) { return cg[i][g]; }, G == 3 ? ca0[i] : c_cur[i],   // hn | c_t
-                                                  G == 3 ? ca1[i] : ca0[i], dh, dc_carry[i], dgi[i], d);         // h_{t-1} | c_{t-1}
+                                                  prev, dh, dc_carry[i], dgi[i], d);
                 if (G == 4) c_cur[i] = ca0[i];
             }
             daux[i] = d[2];                                                        // GRU: dghn -> cbuf slot t+1
+            if (kReset && cslot[i] >= 0) {                                         // nothing flows into step t-1
+                dh_carry[i] = dc_carry[i] = 0.f;
+#pragma unroll
+                for (int g = 0; g < G; ++g) d[g] = 0.f;
+            }
             // B operand: row = sequence bb, column kappa = g*32 + ul  ->  K-panel g, 16-byte chunk ul/4, word ul%4
             const int off = swz(bb, ul >> 2) + (ul & 3) * 4;
 #pragma unroll
@@ -413,7 +438,7 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
             for (int g = 0; g < G; ++g) gout[g * H] = dgi[i][g];
             if (G == 3) cbuf[(tok + B) * H + unit] = daux[i];
         }
-        if (t > 0) fetch(t - 1, ng, ndy, na0, na1);
+        if (t > 0) fetch(t - 1, ng, ndy, na0, na1, nslot);
         dc_wgmma_wait0();
         acc_fence(d);
         {   // partial dh_{t-1}[b][k] of this CTA's 128 gate columns -> scratch [buffer][cluster][rank][b][k]
@@ -427,6 +452,7 @@ __global__ void __launch_bounds__(kThreads, 1) bwd_cluster_kernel(float *gates, 
 #pragma unroll
             for (int g = 0; g < G; ++g) cg[i][g] = ng[i][g];
             cdy[i] = ndy[i]; ca0[i] = na0[i]; ca1[i] = na1[i];
+            if constexpr (kReset) cslot[i] = nslot[i];
         }
         cluster_wait();
     }
@@ -465,16 +491,21 @@ inline int launch_cluster(K kern, int B, size_t smem, cudaStream_t st, Args... a
     return DC_OK;
 }
 
+template <bool kReset>
 inline int launch_fwd(int cell, float *gates, const float *w_hh, const float *b_hh, float *ybuf, float *cbuf, int B, int S,
-                      cudaStream_t st) {
-    if (cell == DC_CELL_GRU) return launch_cluster(fwd_cluster_kernel<3>, B, FwdSmem::total, st, gates, w_hh, b_hh, ybuf, cbuf, B, S);
-    return launch_cluster(fwd_cluster_kernel<4>, B, FwdSmem::total, st, gates, w_hh, b_hh, ybuf, cbuf, B, S);
-}
-inline int launch_bwd(int cell, float *gates, const float *w_hh, const float *ybuf, float *cbuf, const float *dy, const float *dhn,
-                      const float *dcn, float *dh0, float *dc0, float *part, int B, int S, cudaStream_t st) {
+                      dc_rnn::Reset rs, cudaStream_t st) {
     if (cell == DC_CELL_GRU)
-        return launch_cluster(bwd_cluster_kernel<3>, B, BwdSmem::total, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, part, B, S);
-    return launch_cluster(bwd_cluster_kernel<4>, B, BwdSmem::total, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, part, B, S);
+        return launch_cluster(fwd_cluster_kernel<3, kReset>, B, FwdSmem::total, st, gates, w_hh, b_hh, ybuf, cbuf, B, S, rs);
+    return launch_cluster(fwd_cluster_kernel<4, kReset>, B, FwdSmem::total, st, gates, w_hh, b_hh, ybuf, cbuf, B, S, rs);
+}
+template <bool kReset>
+inline int launch_bwd(int cell, float *gates, const float *w_hh, const float *ybuf, float *cbuf, const float *dy, const float *dhn,
+                      const float *dcn, float *dh0, float *dc0, float *part, int B, int S, dc_rnn::Reset rs, cudaStream_t st) {
+    if (cell == DC_CELL_GRU)
+        return launch_cluster(bwd_cluster_kernel<3, kReset>, B, BwdSmem::total, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0,
+                              part, B, S, rs);
+    return launch_cluster(bwd_cluster_kernel<4, kReset>, B, BwdSmem::total, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0,
+                          part, B, S, rs);
 }
 
 }  // namespace dc_rnnc

@@ -17,11 +17,11 @@ constexpr int kThreads = 256;
 // slices' partial sums go through shared memory and are added in slice order, so that the result is deterministic.
 __host__ __device__ constexpr int bwd_slices(int H) { return kThreads >= H ? kThreads / H : 1; }
 
-// Forward.  gates [S,B,G,H] (in: x W_ih^T + b_ih; out: activated gates), wT [H, G*H].
-template <int G>
+// Forward.  gates [S,B,G,H] (in: x W_ih^T + b_ih; out: activated gates), wT [H, G*H].  kReset: resets from rs (rnn_cell.cuh).
+template <int G, bool kReset = false>
 __global__ void __launch_bounds__(kThreads) fwd_generic_kernel(float *__restrict__ gates, const float *__restrict__ wT,
                                                                const float *__restrict__ b_hh, float *__restrict__ ybuf,
-                                                               float *__restrict__ cbuf, int B, int S, int H) {
+                                                               float *__restrict__ cbuf, int B, int S, int H, Reset rs) {
     extern __shared__ __align__(16) float smem[];
     float *h_s = smem;                 // [kBT][H]
     float *pre_s = smem + kBT * H;     // [kBT][G*H]
@@ -62,7 +62,15 @@ __global__ void __launch_bounds__(kThreads) fwd_generic_kernel(float *__restrict
             float *g = gates + tok * GH;
             const float *pre = pre_s + b * GH;
             float act[G], aux;
-            const float prev = G == 3 ? h_s[b * H + u] : cbuf[((size_t)t * B + b0 + b) * H + u];
+            float prev = G == 3 ? h_s[b * H + u] : cbuf[((size_t)t * B + b0 + b) * H + u];
+            if constexpr (kReset) {
+                const int k = rs.slot[tok];
+                if (k >= 0) {                   // the mat-vec on the stale state is discarded
+                    const size_t r = (size_t)k * B + b0 + b;
+                    pre = rs.pre + r * GH;
+                    prev = rs.prev[r * H + u];
+                }
+            }
             const float hnew = cell_fwd<G>([&](int q) { return g[q * H + u]; }, [&](int q) { return pre[q * H + u]; }, prev, act, aux);
 #pragma unroll
             for (int q = 0; q < G; ++q) g[q * H + u] = act[q];
@@ -74,13 +82,13 @@ __global__ void __launch_bounds__(kThreads) fwd_generic_kernel(float *__restrict
     }
 }
 
-// Backward.  gates in: activated gates, out: dgi.  w [G*H, H] as stored.
-template <int G>
+// Backward.  gates in: activated gates, out: dgi.  w [G*H, H] as stored.  kReset: resets from rs (rnn_cell.cuh).
+template <int G, bool kReset = false>
 __global__ void __launch_bounds__(kThreads) bwd_generic_kernel(float *__restrict__ gates, const float *__restrict__ w,
                                                                const float *__restrict__ ybuf, float *__restrict__ cbuf,
                                                                const float *__restrict__ dy, const float *__restrict__ dhn,
                                                                const float *__restrict__ dcn, float *__restrict__ dh0,
-                                                               float *__restrict__ dc0, int B, int S, int H) {
+                                                               float *__restrict__ dc0, int B, int S, int H, Reset rs) {
     extern __shared__ __align__(16) float smem[];
     float *dh_s = smem;                    // [kBT][H] recurrent gradient wrt h
     float *dc_s = smem + kBT * H;          // [kBT][H] (LSTM) recurrent gradient wrt c
@@ -106,11 +114,22 @@ __global__ void __launch_bounds__(kThreads) bwd_generic_kernel(float *__restrict
             const float dh = dy[tok * H + u] + dh_s[b * H + u];
             const size_t ci = ((size_t)(t + 1) * B + b0 + b) * H + u;
             float dgi[G], dgh[G];
-            const float prev = G == 3 ? ybuf[tok * H + u] : cbuf[tok * H + u];     // slot t: h_{t-1} | c_{t-1}
+            float prev = G == 3 ? ybuf[tok * H + u] : cbuf[tok * H + u];           // slot t: h_{t-1} | c_{t-1}
+            int k = -1;
+            if constexpr (kReset) {
+                k = rs.slot[tok];
+                if (k >= 0) prev = rs.prev[((size_t)k * B + b0 + b) * H + u];
+            }
             dh_s[b * H + u] = cell_bwd<G>([&](int q) { return g[q * H + u]; }, cbuf[ci], prev, dh, dc_s[b * H + u], dgi, dgh);   // matvec adds on top
 #pragma unroll
             for (int q = 0; q < G; ++q) { g[q * H + u] = dgi[q]; dg[q * H + u] = dgh[q]; }
             if (G == 3) cbuf[ci] = dgh[2];                                            // n-gate part of dgh
+            if (kReset && k >= 0) {             // nothing flows into step t-1: zero carries, zero mat-vec operand
+                dh_s[b * H + u] = 0.f;
+                dc_s[b * H + u] = 0.f;
+#pragma unroll
+                for (int q = 0; q < G; ++q) dg[q * H + u] = 0.f;
+            }
         }
         __syncthreads();
         // dh_{t-1}[b][k] += sum_j dgh[b][j] * W[j][k]
@@ -159,23 +178,26 @@ inline int launch_generic(K kern, int B, size_t smem, cudaStream_t st, Args... a
 }
 
 // workspace: W_hh^T [H, G*H] (the forward reads the transpose so that output columns are contiguous)
+template <bool kReset>
 inline int launch_fwd_generic(int cell, float *gates, const float *w_hh, const float *b_hh, float *ybuf, float *cbuf, int B, int S,
-                              int H, void *workspace, cudaStream_t st) {
+                              int H, void *workspace, Reset rs, cudaStream_t st) {
     const int G = cell == DC_CELL_GRU ? 3 : 4;
     float *wT = reinterpret_cast<float *>(workspace);
     int rc = launch_transpose(w_hh, wT, G * H, H, st);
     if (rc) return rc;
     const size_t smem = (size_t)kBT * (G + 1) * H * sizeof(float);
-    if (G == 3) return launch_generic(fwd_generic_kernel<3>, B, smem, st, gates, wT, b_hh, ybuf, cbuf, B, S, H);
-    return launch_generic(fwd_generic_kernel<4>, B, smem, st, gates, wT, b_hh, ybuf, cbuf, B, S, H);
+    if (G == 3) return launch_generic(fwd_generic_kernel<3, kReset>, B, smem, st, gates, wT, b_hh, ybuf, cbuf, B, S, H, rs);
+    return launch_generic(fwd_generic_kernel<4, kReset>, B, smem, st, gates, wT, b_hh, ybuf, cbuf, B, S, H, rs);
 }
+template <bool kReset>
 inline int launch_bwd_generic(int cell, float *gates, const float *w_hh, const float *ybuf, float *cbuf, const float *dy,
-                              const float *dhn, const float *dcn, float *dh0, float *dc0, int B, int S, int H, cudaStream_t st) {
+                              const float *dhn, const float *dcn, float *dh0, float *dc0, int B, int S, int H, Reset rs,
+                              cudaStream_t st) {
     const int G = cell == DC_CELL_GRU ? 3 : 4;
     const int nslice = bwd_slices(H);
     const size_t smem = ((size_t)kBT * (G + 2) * H + (nslice > 1 ? (size_t)nslice * kBT * H : 0)) * sizeof(float);
-    if (G == 3) return launch_generic(bwd_generic_kernel<3>, B, smem, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H);
-    return launch_generic(bwd_generic_kernel<4>, B, smem, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H);
+    if (G == 3) return launch_generic(bwd_generic_kernel<3, kReset>, B, smem, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, rs);
+    return launch_generic(bwd_generic_kernel<4, kReset>, B, smem, st, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, rs);
 }
 
 }  // namespace dc_rnn

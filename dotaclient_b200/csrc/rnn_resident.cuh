@@ -141,10 +141,12 @@ struct FwdSmem {
 };
 
 // ---- forward --------------------------------------------------------------------------------
-template <int G, int BT>
+// kReset: resets from rs (rnn_cell.cuh): the gate thread of a reset token takes pre and prev from the tables instead of the
+// mat-vec partials and its own h / c.
+template <int G, int BT, bool kReset = false>
 __global__ void __launch_bounds__(G *kH, 1) fwd_resident_kernel(float *__restrict__ gates, const float *__restrict__ wT,
                                                                  const float *__restrict__ b_hh, float *__restrict__ ybuf,
-                                                                 float *__restrict__ cbuf, int B, int S) {
+                                                                 float *__restrict__ cbuf, int B, int S, Reset rs) {
     using SM = FwdSmem<G, BT>;
     constexpr int NT = SM::NT, GH = SM::GH, H = kH;
     static_assert(BT * kH <= G * kH, "one gate thread per (sequence, unit) pair");
@@ -185,6 +187,8 @@ __global__ void __launch_bounds__(G *kH, 1) fwd_resident_kernel(float *__restric
         }
     }
     for (int t = 0; t < S; ++t) {
+        int k = -1;                             // loaded ahead of the mat-vec, read after it
+        if constexpr (kReset) k = live ? __ldg(rs.slot + (size_t)t * B + b0 + ub) : -1;
         matvec_partial<NT, GH, BT>(wr, w_s, in_s, part_s);
         __syncthreads();
         const int st = t % kStages;
@@ -200,11 +204,18 @@ __global__ void __launch_bounds__(G *kH, 1) fwd_resident_kernel(float *__restric
                     for (int ms = 0; ms < 4; ++ms) a += part_s[(ms * BT + ub) * GH + g * H + uu];
                     pre[g] = a;
                 }
+                float prev = G == 3 ? in_s[ub * H + uu] : c_reg;
+                if (kReset && k >= 0) {
+                    const size_t r = (size_t)k * B + b0 + ub;
+#pragma unroll
+                    for (int g = 0; g < G; ++g) pre[g] = rs.pre[r * GH + g * H + uu];
+                    prev = rs.prev[r * H + uu];
+                }
                 const size_t tok = (size_t)t * B + b0 + ub;
                 float *gout = gates + tok * GH;
                 float act[G], aux;
                 const float hnew = cell_fwd<G, false>([&](int g) { return gi[g * H + uu]; }, [&](int g) { return pre[g]; },
-                                               G == 3 ? in_s[ub * H + uu] : c_reg, act, aux);
+                                               prev, act, aux);
                 if (G == 4) c_reg = aux;
 #pragma unroll
                 for (int g = 0; g < G; ++g) gout[g * H + uu] = act[g];
@@ -235,12 +246,14 @@ struct BwdSmem {
     static constexpr size_t total = w_bytes + in_bytes + part_bytes + kStages * stage_floats * 4 + kStages * 8 + 16;
 };
 
-template <int G, int BT>
+// kReset: resets from rs (rnn_cell.cuh): a reset token reads prev from the table and leaves zero carries and a zero mat-vec
+// operand, so step t-1 (or dh0 / dc0) receives exactly nothing from it.
+template <int G, int BT, bool kReset = false>
 __global__ void __launch_bounds__(G *kH, 1) bwd_resident_kernel(float *__restrict__ gates, const float *__restrict__ w,
                                                                  const float *__restrict__ ybuf, float *__restrict__ cbuf,
                                                                  const float *__restrict__ dy, const float *__restrict__ dhn,
                                                                  const float *__restrict__ dcn, float *__restrict__ dh0,
-                                                                 float *__restrict__ dc0, int B, int S) {
+                                                                 float *__restrict__ dc0, int B, int S, Reset rs) {
     using SM = BwdSmem<G, BT>;
     constexpr int NT = SM::NT, GH = SM::GH, H = kH, NMS = SM::NMS;
     static_assert(BT * kH <= G * kH, "one gate thread per (sequence, unit) pair");
@@ -301,6 +314,8 @@ __global__ void __launch_bounds__(G *kH, 1) bwd_resident_kernel(float *__restric
         const int t = S - 1 - it;
         const int st = it % kStages;
         if (unit) {
+            int k = -1;
+            if constexpr (kReset) k = live ? __ldg(rs.slot + (size_t)t * B + b0 + ub) : -1;
             dc_mbar_wait(&bars[st], (it / kStages) & 1);
             if (live) {
                 const float *sg = stage_s + (size_t)st * SM::stage_floats;
@@ -314,11 +329,23 @@ __global__ void __launch_bounds__(G *kH, 1) bwd_resident_kernel(float *__restric
                 auto act = [&](int q) { return g[q * H + uu]; };
                 const float aux1 = sg[BT * (GH + H) + ub * H + uu];                  // LSTM c_{t-1} | GRU hn
                 float dgi[G], dgh[G];
-                if (G == 3) dh_carry = cell_bwd<G>(act, aux1, sg[BT * (GH + 2 * H) + ub * H + uu], dh, dc_carry, dgi, dgh);
-                else dh_carry = cell_bwd<G>(act, c_cur, aux1, dh, dc_carry, dgi, dgh);
+                if constexpr (kReset) {
+                    float prev = G == 3 ? sg[BT * (GH + 2 * H) + ub * H + uu] : aux1;
+                    if (k >= 0) prev = rs.prev[((size_t)k * B + b0 + ub) * H + uu];
+                    dh_carry = cell_bwd<G>(act, G == 3 ? aux1 : c_cur, prev, dh, dc_carry, dgi, dgh);
+                } else {
+                    if (G == 3) dh_carry = cell_bwd<G>(act, aux1, sg[BT * (GH + 2 * H) + ub * H + uu], dh, dc_carry, dgi, dgh);
+                    else dh_carry = cell_bwd<G>(act, c_cur, aux1, dh, dc_carry, dgi, dgh);
+                }
 #pragma unroll
                 for (int q = 0; q < G; ++q) gout[q * H + uu] = dgi[q];
                 if (G == 3) cbuf[(tok + B) * H + uu] = dgh[2];
+                if (kReset && k >= 0) {
+                    dh_carry = 0.f;
+                    dc_carry = 0.f;
+#pragma unroll
+                    for (int q = 0; q < G; ++q) dgh[q] = 0.f;
+                }
 #pragma unroll
                 for (int q = 0; q < G; ++q) dg[q * H + uu] = dgh[q];
                 if (G == 4) c_cur = aux1;
@@ -340,20 +367,20 @@ __global__ void __launch_bounds__(G *kH, 1) bwd_resident_kernel(float *__restric
 
 inline bool resident_supported(int H) { return H == kH; }
 
-template <int G, int BT>
-int launch_fwd_t(float *gates, const float *wT, const float *b_hh, float *ybuf, float *cbuf, int B, int S, cudaStream_t st) {
+template <int G, int BT, bool kReset>
+int launch_fwd_t(float *gates, const float *wT, const float *b_hh, float *ybuf, float *cbuf, int B, int S, Reset rs, cudaStream_t st) {
     const size_t smem = FwdSmem<G, BT>::total;
-    DC_CUDA(cudaFuncSetAttribute(fwd_resident_kernel<G, BT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    fwd_resident_kernel<G, BT><<<(B + BT - 1) / BT, G * kH, smem, st>>>(gates, wT, b_hh, ybuf, cbuf, B, S);
+    DC_CUDA(cudaFuncSetAttribute(fwd_resident_kernel<G, BT, kReset>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    fwd_resident_kernel<G, BT, kReset><<<(B + BT - 1) / BT, G * kH, smem, st>>>(gates, wT, b_hh, ybuf, cbuf, B, S, rs);
     DC_LAUNCH_OK();
     return DC_OK;
 }
-template <int G, int BT>
+template <int G, int BT, bool kReset>
 int launch_bwd_t(float *gates, const float *w, const float *ybuf, float *cbuf, const float *dy, const float *dhn,
-                 const float *dcn, float *dh0, float *dc0, int B, int S, cudaStream_t st) {
+                 const float *dcn, float *dh0, float *dc0, int B, int S, Reset rs, cudaStream_t st) {
     const size_t smem = BwdSmem<G, BT>::total;
-    DC_CUDA(cudaFuncSetAttribute(bwd_resident_kernel<G, BT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    bwd_resident_kernel<G, BT><<<(B + BT - 1) / BT, G * kH, smem, st>>>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S);
+    DC_CUDA(cudaFuncSetAttribute(bwd_resident_kernel<G, BT, kReset>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    bwd_resident_kernel<G, BT, kReset><<<(B + BT - 1) / BT, G * kH, smem, st>>>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, rs);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -363,24 +390,26 @@ int launch_bwd_t(float *gates, const float *w, const float *ybuf, float *cbuf, c
 inline bool small_tile(int B) { return (B + 1) / 2 <= dc_sm_count(); }
 
 // workspace: W_hh^T [H, G*H], the [M, NOUT] operand of the forward mat-vec
+template <bool kReset>
 inline int launch_fwd_resident(int cell, float *gates, const float *w_hh, const float *b_hh, float *ybuf, float *cbuf, int B,
-                               int S, void *workspace, cudaStream_t st) {
+                               int S, void *workspace, Reset rs, cudaStream_t st) {
     float *wT = reinterpret_cast<float *>(workspace);
     int rc = launch_transpose(w_hh, wT, (cell == DC_CELL_GRU ? 3 : 4) * kH, kH, st);
     if (rc) return rc;
     if (cell == DC_CELL_GRU)
-        return small_tile(B) ? launch_fwd_t<3, 2>(gates, wT, b_hh, ybuf, cbuf, B, S, st)
-                             : launch_fwd_t<3, 3>(gates, wT, b_hh, ybuf, cbuf, B, S, st);
-    return small_tile(B) ? launch_fwd_t<4, 2>(gates, wT, b_hh, ybuf, cbuf, B, S, st)
-                         : launch_fwd_t<4, 4>(gates, wT, b_hh, ybuf, cbuf, B, S, st);
+        return small_tile(B) ? launch_fwd_t<3, 2, kReset>(gates, wT, b_hh, ybuf, cbuf, B, S, rs, st)
+                             : launch_fwd_t<3, 3, kReset>(gates, wT, b_hh, ybuf, cbuf, B, S, rs, st);
+    return small_tile(B) ? launch_fwd_t<4, 2, kReset>(gates, wT, b_hh, ybuf, cbuf, B, S, rs, st)
+                         : launch_fwd_t<4, 4, kReset>(gates, wT, b_hh, ybuf, cbuf, B, S, rs, st);
 }
+template <bool kReset>
 inline int launch_bwd_resident(int cell, float *gates, const float *w, const float *ybuf, float *cbuf, const float *dy,
-                               const float *dhn, const float *dcn, float *dh0, float *dc0, int B, int S, cudaStream_t st) {
+                               const float *dhn, const float *dcn, float *dh0, float *dc0, int B, int S, Reset rs, cudaStream_t st) {
     if (cell == DC_CELL_GRU)
-        return small_tile(B) ? launch_bwd_t<3, 2>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, st)
-                             : launch_bwd_t<3, 3>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, st);
-    return small_tile(B) ? launch_bwd_t<4, 2>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, st)
-                         : launch_bwd_t<4, 4>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, st);
+        return small_tile(B) ? launch_bwd_t<3, 2, kReset>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, rs, st)
+                             : launch_bwd_t<3, 3, kReset>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, rs, st);
+    return small_tile(B) ? launch_bwd_t<4, 2, kReset>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, rs, st)
+                         : launch_bwd_t<4, 4, kReset>(gates, w, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, rs, st);
 }
 
 }  // namespace dc_rnn

@@ -1,4 +1,5 @@
-// Entry points of the recurrent core (dc_rnn_seq_fwd / dc_rnn_seq_bwd) and kernel dispatch.
+// Entry points of the recurrent core (dc_rnn_seq_fwd / dc_rnn_seq_bwd, and the _reset variants with recurrent-state resets
+// inside a sequence) and kernel dispatch.
 //
 // Replaces the time loop inside nn.GRU / nn.LSTM (policy.py:66,141).  Layout, saved tensors and
 // in-place reuse of the gate buffer are described in include/dotaclient_b200.h and DESIGN.md.
@@ -27,16 +28,39 @@ static int check_rnn_args(const char *fn, int cell, int B, int S, int H) {
     return DC_OK;
 }
 
+// Dispatch shared by the plain entry points (kReset = false, rs unused) and the _reset ones.
+template <bool kReset>
+static int rnn_fwd(int cell, float *gates, const float *w_hh, const float *b_hh, float *ybuf, float *cbuf, int B, int S, int H,
+                   void *workspace, dc_rnn::Reset rs, cudaStream_t st) {
+    if (dc_rnn::resident_supported(H)) return dc_rnn::launch_fwd_resident<kReset>(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, workspace, rs, st);
+    if (dc_rnnc::cluster_supported(H)) return dc_rnnc::launch_fwd<kReset>(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, rs, st);
+    if (dc_rnns::stepwise_supported(H)) return dc_rnns::launch_fwd<kReset>(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, H, workspace, rs, st);
+    return dc_rnn::launch_fwd_generic<kReset>(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, H, workspace, rs, st);
+}
+
+template <bool kReset>
+static int rnn_bwd(const char *fn, int cell, float *gates, const float *w_hh, const float *ybuf, float *cbuf, const float *dy,
+                   const float *dhn, const float *dcn, float *dh0, float *dc0, int B, int S, int H, void *workspace,
+                   dc_rnn::Reset rs, cudaStream_t st) {
+    if (dc_rnn::resident_supported(H)) return dc_rnn::launch_bwd_resident<kReset>(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, rs, st);
+    if (dc_rnnc::cluster_supported(H)) {
+        DC_REQUIRE(workspace, DC_EINVAL, "%s: the H = 256 kernels need the workspace (dc_rnn_workspace_bytes)", fn);
+        return dc_rnnc::launch_bwd<kReset>(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, reinterpret_cast<float *>(workspace),
+                                           B, S, rs, st);
+    }
+    if (dc_rnns::stepwise_supported(H)) {
+        DC_REQUIRE(workspace, DC_EINVAL, "%s: the step-wise kernels need the workspace (dc_rnn_workspace_bytes)", fn);
+        return dc_rnns::launch_bwd<kReset>(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, workspace, rs, st);
+    }
+    return dc_rnn::launch_bwd_generic<kReset>(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, rs, st);
+}
+
 extern "C" int dc_rnn_seq_fwd(int cell, float *gates, const float *w_hh, const float *b_hh, float *ybuf, float *cbuf,
                               int B, int S, int H, void *workspace, dc_stream_t stream) {
     int rc = check_rnn_args("dc_rnn_seq_fwd", cell, B, S, H);
     if (rc) return rc;
     DC_REQUIRE(gates && w_hh && b_hh && ybuf && cbuf && workspace, DC_EINVAL, "dc_rnn_seq_fwd: null pointer");
-    cudaStream_t st = dc_cu_stream(stream);
-    if (dc_rnn::resident_supported(H)) return dc_rnn::launch_fwd_resident(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, workspace, st);
-    if (dc_rnnc::cluster_supported(H)) return dc_rnnc::launch_fwd(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, st);
-    if (dc_rnns::stepwise_supported(H)) return dc_rnns::launch_fwd(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, H, workspace, st);
-    return dc_rnn::launch_fwd_generic(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, H, workspace, st);
+    return rnn_fwd<false>(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, H, workspace, dc_rnn::Reset{}, dc_cu_stream(stream));
 }
 
 extern "C" int dc_rnn_seq_bwd(int cell, float *gates, const float *w_hh, const float *ybuf, float *cbuf, const float *dy,
@@ -45,15 +69,38 @@ extern "C" int dc_rnn_seq_bwd(int cell, float *gates, const float *w_hh, const f
     int rc = check_rnn_args("dc_rnn_seq_bwd", cell, B, S, H);
     if (rc) return rc;
     DC_REQUIRE(gates && w_hh && ybuf && cbuf && dy, DC_EINVAL, "dc_rnn_seq_bwd: null pointer");
-    cudaStream_t st = dc_cu_stream(stream);
-    if (dc_rnn::resident_supported(H)) return dc_rnn::launch_bwd_resident(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, st);
-    if (dc_rnnc::cluster_supported(H)) {
-        DC_REQUIRE(workspace, DC_EINVAL, "dc_rnn_seq_bwd: the H = 256 kernels need the workspace (dc_rnn_workspace_bytes)");
-        return dc_rnnc::launch_bwd(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, reinterpret_cast<float *>(workspace), B, S, st);
-    }
-    if (dc_rnns::stepwise_supported(H)) {
-        DC_REQUIRE(workspace, DC_EINVAL, "dc_rnn_seq_bwd: the step-wise kernels need the workspace (dc_rnn_workspace_bytes)");
-        return dc_rnns::launch_bwd(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, workspace, st);
-    }
-    return dc_rnn::launch_bwd_generic(cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, st);
+    return rnn_bwd<false>("dc_rnn_seq_bwd", cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, workspace,
+                          dc_rnn::Reset{}, dc_cu_stream(stream));
+}
+
+static int check_reset_args(const char *fn, const int32_t *reset_slot, const float *reset_prev, const float *reset_pre, int K,
+                            bool need_pre) {
+    DC_REQUIRE(reset_slot, DC_EINVAL, "%s: null reset_slot", fn);
+    DC_REQUIRE(K >= 0, DC_EINVAL, "%s: K=%d", fn, K);
+    DC_REQUIRE(K == 0 || (reset_prev && (reset_pre || !need_pre)), DC_EINVAL, "%s: null reset table with K=%d", fn, K);
+    return DC_OK;
+}
+
+extern "C" int dc_rnn_seq_fwd_reset(int cell, float *gates, const float *w_hh, const float *b_hh, float *ybuf, float *cbuf,
+                                    const int32_t *reset_slot, const float *reset_prev, const float *reset_pre, int K, int B,
+                                    int S, int H, void *workspace, dc_stream_t stream) {
+    int rc = check_rnn_args("dc_rnn_seq_fwd_reset", cell, B, S, H);
+    if (rc) return rc;
+    DC_REQUIRE(gates && w_hh && b_hh && ybuf && cbuf && workspace, DC_EINVAL, "dc_rnn_seq_fwd_reset: null pointer");
+    rc = check_reset_args("dc_rnn_seq_fwd_reset", reset_slot, reset_prev, reset_pre, K, true);
+    if (rc) return rc;
+    return rnn_fwd<true>(cell, gates, w_hh, b_hh, ybuf, cbuf, B, S, H, workspace, dc_rnn::Reset{reset_slot, reset_prev, reset_pre},
+                         dc_cu_stream(stream));
+}
+
+extern "C" int dc_rnn_seq_bwd_reset(int cell, float *gates, const float *w_hh, const float *ybuf, float *cbuf, const float *dy,
+                                    const float *dhn, const float *dcn, float *dh0, float *dc0, const int32_t *reset_slot,
+                                    const float *reset_prev, int K, int B, int S, int H, void *workspace, dc_stream_t stream) {
+    int rc = check_rnn_args("dc_rnn_seq_bwd_reset", cell, B, S, H);
+    if (rc) return rc;
+    DC_REQUIRE(gates && w_hh && ybuf && cbuf && dy, DC_EINVAL, "dc_rnn_seq_bwd_reset: null pointer");
+    rc = check_reset_args("dc_rnn_seq_bwd_reset", reset_slot, reset_prev, nullptr, K, false);
+    if (rc) return rc;
+    return rnn_bwd<true>("dc_rnn_seq_bwd_reset", cell, gates, w_hh, ybuf, cbuf, dy, dhn, dcn, dh0, dc0, B, S, H, workspace,
+                         dc_rnn::Reset{reset_slot, reset_prev, nullptr}, dc_cu_stream(stream));
 }

@@ -235,8 +235,29 @@ def _rnn_workspace(cell, B, H, device):
     return ws
 
 
-def _rnn_forward_impl(x, w_ih, w_hh, b_ih, b_hh, h0, c0, cell):
-    """i2h GEMM (wgmma 3xTF32, ``dc_gemm_tf32x3``) + recurrence kernel.  Returns (x2, w_ih, w_hh, gates, ybuf, cbuf)."""
+def _check_reset(reset, S, B, H, cell, device):
+    """``reset`` of ``rnn_sequence`` -> ``(slot [S, B] int32, h_tab [K, B, H], prev_tab [K, B, H])`` (prev: h for the GRU, c
+    for the LSTM), all contiguous; None when there is nothing to reset (None, or K = 0)."""
+    if reset is None:
+        return None
+    slot, h_tab, c_tab = reset
+    _need_cuda(slot, h_tab, c_tab)
+    K = h_tab.shape[0]
+    if slot.shape != (S, B) or slot.dtype != torch.int32:
+        raise ValueError("reset slot must be int32 [%d, %d], got %s %s" % (S, B, slot.dtype, tuple(slot.shape)))
+    if h_tab.shape != (K, B, H) or (cell == "lstm") != (c_tab is not None) or (c_tab is not None and c_tab.shape != (K, B, H)):
+        raise ValueError("reset states must be [K, %d, %d] (h, and c for the LSTM only), got %s / %s"
+                         % (B, H, tuple(h_tab.shape), None if c_tab is None else tuple(c_tab.shape)))
+    if K == 0:
+        return None
+    h_tab = _f32c(h_tab.detach())
+    return slot.contiguous(), h_tab, (h_tab if c_tab is None else _f32c(c_tab.detach()))
+
+
+def _rnn_forward_impl(x, w_ih, w_hh, b_ih, b_hh, h0, c0, cell, reset=None):
+    """i2h GEMM (wgmma 3xTF32, ``dc_gemm_tf32x3``) + recurrence kernel.  Returns (x2, w_ih, w_hh, gates, ybuf, cbuf).
+    ``reset``: the checked operands of ``_check_reset`` or None; the reset rows' h2h pre-activations are computed here, one
+    GEMM of K*B rows, and the recurrence runs through ``dc_rnn_seq_fwd_reset``."""
     _need_cuda(x, w_ih, w_hh, b_ih, b_hh, h0, c0)
     S, B, Hin = x.shape
     H = w_hh.shape[1]
@@ -252,6 +273,16 @@ def _rnn_forward_impl(x, w_ih, w_hh, b_ih, b_hh, h0, c0, cell):
         cbuf[0].copy_(c0.detach().reshape(B, H))
     ws = _rnn_workspace(cell, B, H, x.device)
     lib = _lib.load()
+    if reset is not None:
+        slot, h_tab, prev_tab = reset
+        K = h_tab.shape[0]
+        pre = gemm_tf32x3(h_tab.view(K * B, H), w_hh, b_hh)                  # h_reset W_hh^T + b_hh [K*B, G*H]
+        with PROFILE.span("rnn_fwd", 1, 4 * S * B * ((4 if cell == "lstm" else 3) + 1) * H):
+            _lib.check(lib.dc_rnn_seq_fwd_reset(CELL_ID[cell], gates.data_ptr(), w_hh.data_ptr(), b_hh.data_ptr(),
+                                                ybuf.data_ptr(), cbuf.data_ptr(), slot.data_ptr(), prev_tab.data_ptr(),
+                                                pre.data_ptr(), K, B, S, H, ws.data_ptr(), _lib.stream_ptr()),
+                       "dc_rnn_seq_fwd_reset")
+        return x2, w_ih, w_hh, gates, ybuf, cbuf
     with PROFILE.span("rnn_fwd", 1, 4 * S * B * ((4 if cell == "lstm" else 3) + 1) * H):      # SURVEY.md 8(d)
         _lib.check(lib.dc_rnn_seq_fwd(CELL_ID[cell], gates.data_ptr(), w_hh.data_ptr(), b_hh.data_ptr(),
                                       ybuf.data_ptr(), cbuf.data_ptr(), B, S, H, ws.data_ptr(), _lib.stream_ptr()),
@@ -285,20 +316,52 @@ def stack_layers(states):
     return states[0].unsqueeze(0) if len(states) == 1 else torch.stack(states)
 
 
+def _reset_rows(slot, K):
+    """For every row ``k*B + b`` of a ``[K, B, ...]`` reset table: the token ``t*B + b`` whose ``slot[t, b]`` is k
+    (int64 ``[K*B]``, 0 for unused rows) and whether the row is used (fp32 ``[K*B, 1]``, 1 / 0).  On the device, no sync."""
+    S, B = slot.shape
+    dev = slot.device
+    s = slot.long()
+    b = torch.arange(B, device=dev).expand(S, B)
+    row = torch.where(s >= 0, s * B + b, K * B).reshape(-1)               # carried tokens all land on a spare row K*B
+    tok = torch.arange(S * B, device=dev)
+    idx = torch.zeros(K * B + 1, dtype=torch.int64, device=dev).scatter_(0, row, tok)
+    used = torch.zeros(K * B + 1, dtype=torch.float32, device=dev).scatter_(0, row, torch.ones(S * B, device=dev))
+    return idx[:K * B], used[:K * B].unsqueeze(1)
+
+
+def _gather_rows(srcs, index):
+    """``src[index]`` for every 2-D contiguous ``src`` with a DEVICE int64 ``index`` (one ``dc_gather_columns`` launch on
+    ``[1, N, row]`` views).  The caller guarantees ``0 <= index < N``: the index is made on the device from checked data."""
+    n = index.numel()
+    outs = [torch.empty((n, src.shape[1]), dtype=src.dtype, device=src.device) for src in srcs]
+    descs = [_lib.GatherDesc(src.data_ptr(), out.data_ptr(), 1, src.shape[0], src.shape[1] * src.element_size())
+             for src, out in zip(srcs, outs)]
+    with PROFILE.span("gather_columns", 1):
+        _lib.check(_lib.load().dc_gather_columns((_lib.GatherDesc * len(descs))(*descs), len(descs), index.data_ptr(), n,
+                                                 _lib.stream_ptr()), "dc_gather_columns")
+    return outs
+
+
 class RnnSequence(torch.autograd.Function):
     """Time-major GRU/LSTM layer: i2h GEMM (wgmma 3xTF32) + hand-written recurrence kernels.
 
-    forward(x [S,B,Hin], w_ih [G*H,Hin], w_hh [G*H,H], b_ih, b_hh, h0 [B,H], c0 [B,H]|None, cell)
+    forward(x [S,B,Hin], w_ih [G*H,Hin], w_hh [G*H,H], b_ih, b_hh, h0 [B,H], c0 [B,H]|None, cell, reset=None)
       -> y [S,B,H], h_n [B,H], c_n [B,H] (zeros-size-0 tensor for GRU)
     Semantics of ``torch.nn.GRU/LSTM(batch_first=...)`` as used in ``policy.py:66,141``.
+    ``reset``: None, or ``(slot [S, B] int32, h [K, B, H], c [K, B, H] | None)``: at a token with ``slot[t, b] = k >= 0``
+    the state entering step t of sequence b is replaced by row (k, b) of the tables (``dc_rnn_seq_fwd_reset``).  The
+    tables are data: they get no gradient, like ``h0`` of a training batch.
     """
 
     @staticmethod
-    def forward(ctx, x, w_ih, w_hh, b_ih, b_hh, h0, c0, cell):
+    def forward(ctx, x, w_ih, w_hh, b_ih, b_hh, h0, c0, cell, reset=None):
         S, B, Hin = x.shape
         H = w_hh.shape[1]
-        x2, w_ih, w_hh, gates, ybuf, cbuf = _rnn_forward_impl(x, w_ih, w_hh, b_ih, b_hh, h0, c0, cell)
+        reset = _check_reset(reset, S, B, H, cell, x.device)
+        x2, w_ih, w_hh, gates, ybuf, cbuf = _rnn_forward_impl(x, w_ih, w_hh, b_ih, b_hh, h0, c0, cell, reset)
         ctx.cell, ctx.dims = cell, (S, B, Hin, H, GATES[cell])
+        ctx.reset = reset
         ctx.save_for_backward(x2, w_ih, w_hh, gates, ybuf, cbuf)
         y = ybuf[1:]
         h_n = ybuf[S].clone()
@@ -325,10 +388,19 @@ class RnnSequence(torch.autograd.Function):
         dc0 = torch.empty((B, H), dtype=torch.float32, device=x2.device) if cell == "lstm" else None
         ws = _rnn_workspace(cell, B, H, x2.device)
         lib = _lib.load()
+        reset = ctx.reset
         with PROFILE.span("rnn_bwd", 1, 8 * S * B * ((4 if cell == "lstm" else 3) + 1) * H):
-            _lib.check(lib.dc_rnn_seq_bwd(CELL_ID[cell], gates.data_ptr(), w_hh.data_ptr(), ybuf.data_ptr(),
-                                          cbuf.data_ptr(), dy.data_ptr(), _lib.ptr(dhn), _lib.ptr(dcn), dh0.data_ptr(),
-                                          _lib.ptr(dc0), B, S, H, ws.data_ptr(), _lib.stream_ptr()), "dc_rnn_seq_bwd")
+            if reset is None:
+                _lib.check(lib.dc_rnn_seq_bwd(CELL_ID[cell], gates.data_ptr(), w_hh.data_ptr(), ybuf.data_ptr(),
+                                              cbuf.data_ptr(), dy.data_ptr(), _lib.ptr(dhn), _lib.ptr(dcn), dh0.data_ptr(),
+                                              _lib.ptr(dc0), B, S, H, ws.data_ptr(), _lib.stream_ptr()), "dc_rnn_seq_bwd")
+            else:
+                slot, h_tab, prev_tab = reset
+                _lib.check(lib.dc_rnn_seq_bwd_reset(CELL_ID[cell], gates.data_ptr(), w_hh.data_ptr(), ybuf.data_ptr(),
+                                                    cbuf.data_ptr(), dy.data_ptr(), _lib.ptr(dhn), _lib.ptr(dcn),
+                                                    dh0.data_ptr(), _lib.ptr(dc0), slot.data_ptr(), prev_tab.data_ptr(),
+                                                    h_tab.shape[0], B, S, H, ws.data_ptr(), _lib.stream_ptr()),
+                           "dc_rnn_seq_bwd_reset")
         dgi = gates                                   # [N, G*H], overwritten in place by the kernel
         hprev = ybuf[:S].view(N, H)                   # h_{t-1} for every token (slot t)
         dx = gemm_tf32x3(dgi, w_ih.t().contiguous()).view(S, B, Hin) if ctx.needs_input_grad[0] else None   # dx = dgi W_ih
@@ -342,11 +414,27 @@ class RnnSequence(torch.autograd.Function):
             gemm_wgrad_tf32x3(dgi[:, :2 * H], hprev, want_bias=False, dw_out=dw_hh[:2 * H])
             _, db_n = gemm_wgrad_tf32x3(dghn, hprev, dw_out=dw_hh[2 * H:])
             db_hh = torch.cat([db_ih[:2 * H], db_n])
-        return dx, dw_ih, dw_hh, db_ih, db_hh, dh0, dc0, None
+        if reset is not None:
+            # dW_hh above paired each token's dgh with ybuf[t]; a reset token's step used h_reset: add
+            # dgh_t^T (h_reset - ybuf[t]) over the reset tokens (K*B gathered rows, unused ones weighted 0)
+            slot, h_tab, _ = reset
+            K = h_tab.shape[0]
+            tok, used = _reset_rows(slot, K)
+            srcs = [dgi, hprev] + ([] if cell == "lstm" else [cbuf[1:].view(N, H)])
+            rows = _gather_rows(srcs, tok)
+            diff = (h_tab.view(K * B, H) - rows[1]) * used
+            if cell == "lstm":
+                gemm_wgrad_tf32x3(rows[0], diff, want_bias=False, dw_out=dw_hh, accumulate=True)
+            else:
+                gemm_wgrad_tf32x3(rows[0][:, :2 * H], diff, want_bias=False, dw_out=dw_hh[:2 * H], accumulate=True)
+                gemm_wgrad_tf32x3(rows[2], diff, want_bias=False, dw_out=dw_hh[2 * H:], accumulate=True)
+        return dx, dw_ih, dw_hh, db_ih, db_hh, dh0, dc0, None, None
 
 
-def rnn_sequence(x_tm, w_ih, w_hh, b_ih, b_hh, h0, c0, cell):
-    return RnnSequence.apply(x_tm, w_ih, w_hh, b_ih, b_hh, h0, c0, cell)
+def rnn_sequence(x_tm, w_ih, w_hh, b_ih, b_hh, h0, c0, cell, reset=None):
+    """One recurrent layer (``RnnSequence``); ``reset`` = ``(slot [S, B] int32, h [K, B, H], c [K, B, H] | None)`` restarts
+    the state inside sequences (see ``RnnSequence``), None is the plain recurrence."""
+    return RnnSequence.apply(x_tm, w_ih, w_hh, b_ih, b_hh, h0, c0, cell, reset)
 
 
 # --------------------------------------------------------------------------------------------- PPO loss

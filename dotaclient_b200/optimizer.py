@@ -215,15 +215,20 @@ class ExperienceBatch:
     (``DotaOptimizer(value_clip=...)``) needs; a batch without them has no such entry in ``tensors()``.
     ``valid [S, B]`` (optional, bool) marks the real steps against the zero padding of each rollout's last chunk, which
     ``DotaOptimizer(mask_padding=True)`` leaves out of the loss; like ``old_values`` it is absent from ``tensors()`` when None.
+    A packed batch (``DotaOptimizer(pack_sequences=True)``, ``pack_layout``) holds several rollout tails in one column and
+    carries the recurrent-state resets between them: ``reset_slot [S, B]`` int32 (-1: carry the state; k >= 0: the state
+    entering that step is row (k, column) of the tables), ``reset_h [K, B, L*H]`` and, for the LSTM, ``reset_c`` (every
+    layer's state side by side).  They are gathered column by column like every other field, and absent when None.
     """
-    FIELDS = ("advantages", "returns", "old_logp", "h0", "c0", "old_values", "valid")
+    FIELDS = ("advantages", "returns", "old_logp", "h0", "c0", "old_values", "valid", "reset_slot", "reset_h", "reset_c")
 
     def __init__(self, observations, masks, actions, old_logp, advantages, returns, h0, c0=None, old_values=None,
-                 valid=None):
+                 valid=None, reset_slot=None, reset_h=None, reset_c=None):
         self.observations, self.masks, self.actions = observations, masks, actions
         self.old_logp, self.advantages, self.returns, self.h0, self.c0 = old_logp, advantages, returns, h0, c0
         self.old_values = old_values
         self.valid = valid
+        self.reset_slot, self.reset_h, self.reset_c = reset_slot, reset_h, reset_c
         self._ready = {}        # data_ptr -> event of an upload still to be waited for (``to`` from pinned memory)
         self._slot = None       # the DotaOptimizer input slot whose static buffers these tensors are (``prefetch``)
 
@@ -235,9 +240,15 @@ class ExperienceBatch:
                                {k: fn(v) for k, v in self.actions.items()}, **{f: opt(getattr(self, f)) for f in self.FIELDS})
 
     def graph_key(self):
-        """The shape a captured step graph is specialised to (old_values, valid: one more static input each)."""
+        """The shape a captured step graph is specialised to (old_values, valid, the reset tables of a packed batch: more
+        static inputs)."""
         key = (self.seq_len, self.batch_size, self.old_values is not None)
-        return key if self.valid is None else key + ('valid',)
+        key = key if self.valid is None else key + ('valid',)
+        return key if self.reset_slot is None else key + (('reset', self.reset_h.shape[0]),)
+
+    def reset(self):
+        """The ``reset`` operand of ``Policy._recur`` (None for a batch that is not packed)."""
+        return None if self.reset_slot is None else (self.reset_slot, self.reset_h, self.reset_c)
 
     def wait(self, *tensors):
         """Makes the current stream wait for the uploads of ``tensors`` (None allowed) that are still outstanding; each
@@ -281,7 +292,7 @@ class ExperienceBatch:
             holder, k, _ = item
             if holder is self.observations:
                 return 0 if k == 'env' else 3 + Policy.INPUT_KEYS.index(k)
-            if not isinstance(holder, dict) and k in ('h0', 'c0'):
+            if not isinstance(holder, dict) and k in ('h0', 'c0', 'reset_slot', 'reset_h', 'reset_c'):
                 return 1
             return 100
         moved, ready = {}, {}
@@ -370,13 +381,18 @@ ADVANTAGE_ESTIMATORS = ('gae', 'vtrace')
 
 
 def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
-                       vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False):
+                       vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False, pack_sequences=False):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
-    vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool) and mask_padding a bool.  NaN fails
-    every check."""
+    vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool and
+    pack_sequences a bool that is True only with mask_padding.  NaN fails every check."""
     if not isinstance(mask_padding, bool):
         raise ValueError("mask_padding=%r: must be True or False" % (mask_padding,))
+    if not isinstance(pack_sequences, bool):
+        raise ValueError("pack_sequences=%r: must be True or False" % (pack_sequences,))
+    if pack_sequences and not mask_padding:
+        raise ValueError("pack_sequences=True needs mask_padding=True: without the mask, experience prep gives padded steps "
+                         "advantages and value targets that packing would drop")
     if isinstance(num_minibatches, bool) or not isinstance(num_minibatches, numbers.Integral) or num_minibatches < 1:
         raise ValueError("num_minibatches=%r: the number of minibatches per epoch must be an int >= 1" % (num_minibatches,))
     def number(name, v):
@@ -458,6 +474,102 @@ def chunk_valid_lengths(lengths, seq_len):
     """The real steps of every ``seq_len`` chunk, rollout by rollout and chunk by chunk (the batch's sequence order): chunk
     j of a rollout of length L has ``min(seq_len, L - j * seq_len)``."""
     return [min(seq_len, int(L) - j * seq_len) for L in lengths for j in range((int(L) + seq_len - 1) // seq_len)]
+
+
+class PackLayout(typing.NamedTuple):
+    """The packed training batch of ``pack_layout``: ``B`` columns of ``seq_len`` steps.  For every token (t, c):
+    ``rollout[t, c]`` / ``step[t, c]`` the rollout and its step that the token holds (-1 / -1 for padding), ``reset_slot[t, c]``
+    (int32) -1, or k >= 0 where a tail starts after others in its column (its k-th such tail: row k of the column's reset
+    tables, the state at ``step[t, c]``).  ``h0_rollout[c]`` / ``h0_step[c]``: the state entering column c, state-buffer slot
+    ``h0_step[c]`` of that rollout.  ``K``: the largest number of such mid-column tails in a column.  ``n_full``: the
+    columns 0 .. n_full - 1 hold the full chunks, rollout by rollout, chunk by chunk."""
+    B: int
+    K: int
+    n_full: int
+    rollout: np.ndarray
+    step: np.ndarray
+    reset_slot: np.ndarray
+    h0_rollout: np.ndarray
+    h0_step: np.ndarray
+
+
+def _first_fit_decreasing(tails, seq_len):
+    """Column (0, 1, ...) and offset of every tail ``(length, rollout)`` of ``tails``, placed in the order
+    first-fit-decreasing by length, ties by rollout order, each whole into the first column with room for it."""
+    order = sorted(range(len(tails)), key=lambda j: (-tails[j][0], tails[j][1]))
+    free = np.empty(len(tails), dtype=np.int64)
+    n_col = 0
+    col, off = [0] * len(tails), [0] * len(tails)
+    for j in order:
+        r = tails[j][0]
+        fits = np.flatnonzero(free[:n_col] >= r)
+        c = int(fits[0]) if fits.size else n_col
+        if c == n_col:
+            free[c] = seq_len
+            n_col += 1
+        col[j], off[j] = c, seq_len - int(free[c])
+        free[c] -= r
+    return col, off, n_col
+
+
+def pack_layout(lengths, seq_len):
+    """The packed layout of rollouts of ``lengths`` real steps (``DotaOptimizer(pack_sequences=True)``).  A rollout of L
+    steps has ``L // seq_len`` full chunks, which keep one column each and start from the state at their first step, as in
+    the unpacked batch, and a tail of ``L % seq_len`` steps (none when 0).  The tails are packed whole into shared columns
+    of ``seq_len`` steps, first-fit-decreasing by length with ties broken by rollout order, so the layout depends on the
+    lengths alone.  The first tail of a column starts from the column's initial state; every later one from a reset to the
+    state at its own first step.  So each tail starts from the same state and ends at the same truncation point as in the
+    unpacked batch.  The unused end of a tail column is padding.  Returns a ``PackLayout``."""
+    S = int(seq_len)
+    Ls = [int(L) for L in lengths]
+    segs = [[(i, j * S, S)] for i, L in enumerate(Ls) for j in range(L // S)]            # (rollout, first step, steps)
+    n_full = len(segs)
+    tails = [(L % S, i) for i, L in enumerate(Ls) if L % S]
+    col, off, n_col = _first_fit_decreasing(tails, S)
+    tail_cols = [[] for _ in range(n_col)]
+    for (r, i), c, o in sorted(zip(tails, col, off), key=lambda x: (x[1], x[2])):
+        tail_cols[c].append((i, Ls[i] - r, r))
+    segs += tail_cols
+    B = len(segs)
+    rollout = np.full((S, B), -1, dtype=np.int64)
+    step = np.full((S, B), -1, dtype=np.int64)
+    reset_slot = np.full((S, B), -1, dtype=np.int32)
+    h0_rollout = np.empty(B, dtype=np.int64)
+    h0_step = np.empty(B, dtype=np.int64)
+    K = 0
+    for c, col_segs in enumerate(segs):
+        h0_rollout[c], h0_step[c] = col_segs[0][0], col_segs[0][1]
+        t = 0
+        for k, (i, first, n) in enumerate(col_segs):
+            rollout[t:t + n, c] = i
+            step[t:t + n, c] = np.arange(first, first + n)
+            if k:
+                reset_slot[t, c] = k - 1
+            t += n
+        K = max(K, len(col_segs) - 1)
+    return PackLayout(B, K, n_full, rollout, step, reset_slot, h0_rollout, h0_step)
+
+
+def sequence_count(lengths, seq_len, pack=False):
+    """The number of training sequences that rollouts of ``lengths`` steps make: ``ceil(L / seq_len)`` each, or with
+    ``pack`` the columns of their ``pack_layout``."""
+    unpacked = sum((int(L) + seq_len - 1) // seq_len for L in lengths)
+    if not pack or not unpacked:
+        return unpacked
+    tails = [(int(L) % seq_len, i) for i, L in enumerate(lengths) if int(L) % seq_len]
+    return sum(int(L) // seq_len for L in lengths) + _first_fit_decreasing(tails, seq_len)[2]
+
+
+def check_reset_slots(reset_slot, K):
+    """Raises ``ValueError`` unless every value of the host array ``reset_slot`` lies in [-1, K) and no reset row (k, column)
+    is used twice: the recurrence kernels index the reset tables with them on the device, where they cannot be checked."""
+    rs = np.asarray(reset_slot)
+    if rs.size and (rs.min() < -1 or rs.max() >= K):
+        raise ValueError("reset slots %d..%d outside [-1, %d)" % (rs.min(), rs.max(), K))
+    t, c = np.nonzero(rs >= 0)
+    rows = rs[t, c].astype(np.int64) * rs.shape[1] + c
+    if np.unique(rows).size != rows.size:
+        raise ValueError("a reset row is used by two tokens")
 
 
 def check_behaviour_logp(datas):
@@ -543,15 +655,18 @@ class DotaOptimizer:
                  entropy_coef, vf_coef, run_local, *, hidden_size=256, cell="gru", num_layers=1, mq=None,
                  iterations=100000, rollout_prefetch=0, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1,
                  max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0,
-                 num_minibatches=1, mask_padding=False):
+                 num_minibatches=1, mask_padding=False, pack_sequences=False):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
                              % (num_layers, self.MAX_LAYERS, _lib.MAX_PARAM_TENSORS))
         check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                            vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
-                           mask_padding=mask_padding)
+                           mask_padding=mask_padding, pack_sequences=pack_sequences)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # True: batch_from_rollouts packs the rollouts' tails into shared columns with state resets between them
+        # (pack_layout), so the padding of every rollout's last chunk is not trained on
+        self.pack_sequences = pack_sequences
         # True: the zero padding of each rollout's last chunk counts for nothing -- prep bootstraps at the real end and
         # marks the real steps (ExperienceBatch.valid), the loss leaves padded tokens out of every mean
         self.mask_padding = mask_padding
@@ -934,6 +1049,8 @@ class DotaOptimizer:
         Python objects, no per-sequence re-stacking (an iteration of the stream has ~1000 sequences of 16 steps)."""
         S, pol = self.seq_len, self.policy_base
         p = self._prepare_rollouts(datas)
+        if self.pack_sequences:
+            return self._packed_batch(p)
         R, Lps = len(datas), p['Lps']
         n_chunks = [lp // S for lp in Lps]
 
@@ -957,6 +1074,64 @@ class DotaOptimizer:
         c0 = ops.stack_layers([cb[t_idx, r_idx] for cb in p['cbufs']]) if pol.cell == "lstm" else None
         old_values = chunked(p['values_lr']).contiguous()               # the critic at prep time (value clipping)
         return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values, valid=p['valid'])
+
+    def _packed_batch(self, p):
+        """The packed ``ExperienceBatch`` of ``pack_layout`` from the prepared ``[L_max, R, ...]`` tensors: every field is
+        one token gather per index (``dc_gather_columns`` over ``[1, L_max * R, ...]`` views, and over the rollout-major
+        advantages and returns), so the assembly is a handful of launches whatever the number of sequences.  A padding token
+        reads a padded row of a rollout with a tail: zeros, zero advantage and return, like the padding of the unpacked
+        batch."""
+        S, pol, dev = self.seq_len, self.policy_base, self.device
+        Ls, Lps, Lmax = p['Ls'], p['Lps'], p['Lmax']
+        R = len(Ls)
+        lay = pack_layout(Ls, S)
+        check_reset_slots(lay.reset_slot, lay.K)
+        B = lay.B
+        real = lay.rollout >= 0
+        pad_r = next((i for i, L in enumerate(Ls) if L % S), 0)           # any rollout with a tail has padded rows
+        src_r = np.where(real, lay.rollout, pad_r)
+        src_t = np.where(real, lay.step, Ls[pad_r])
+        base = np.concatenate([[0], np.cumsum(Lps)[:-1]]).astype(np.int64)
+        idx_tm = (src_t * R + src_r).reshape(-1)                          # rows of the time-major [L_max, R] tensors
+        idx_rm = (base[src_r] + src_t).reshape(-1)                        # rows of the rollout-major scan outputs
+
+        def gather(tensors, index, n_src):
+            outs = [torch.empty((S, B) + tuple(t.shape[2:]) if t.dim() >= 2 else (S, B), dtype=t.dtype, device=dev)
+                    for t in tensors]
+            ops.gather_columns([(t.contiguous().view((1, n_src) + tuple(t.shape[2:] if t.dim() >= 2 else ())),
+                                 o.view((1, S * B) + tuple(o.shape[2:]))) for t, o in zip(tensors, outs)], index)
+            return outs
+        keys_o, keys_h = list(p['obs']), list(p['masks'])
+        tm = [p['obs'][k] for k in keys_o] + [p['masks'][k] for k in keys_h] + [p['actions'][k] for k in keys_h] + \
+            [p['old_logp'], p['values_lr']]
+        g = gather(tm, idx_tm, Lmax * R)
+        obs = dict(zip(keys_o, g[:len(keys_o)]))
+        masks = dict(zip(keys_h, g[len(keys_o):len(keys_o) + len(keys_h)]))
+        actions = dict(zip(keys_h, g[len(keys_o) + len(keys_h):len(keys_o) + 2 * len(keys_h)]))
+        old_logp, old_values = g[-2], g[-1]
+        adv, ret = gather([p['adv_c'], p['ret_c']], idx_rm, int(sum(Lps)))
+        # the host layout goes up in one pinned copy: valid, the reset slots and the state-buffer coordinates
+        t_rs, c_rs = np.nonzero(lay.reset_slot >= 0)
+        meta = np.concatenate([real.reshape(-1), lay.reset_slot.reshape(-1), lay.h0_step, lay.h0_rollout,
+                               lay.reset_slot[t_rs, c_rs], c_rs, lay.step[t_rs, c_rs], lay.rollout[t_rs, c_rs]]).astype(np.int64)
+        meta = torch.from_numpy(meta).pin_memory().to(dev, non_blocking=True)
+        n, o = S * B, 2 * S * B
+        valid = meta[:n].view(S, B).bool()
+        reset_slot = meta[n:o].view(S, B).to(torch.int32)
+        h0_t, h0_r = meta[o:o + B], meta[o + B:o + 2 * B]
+        m = len(t_rs)
+        rk, rc, rt, rr = (meta[o + 2 * B + j * m:o + 2 * B + (j + 1) * m] for j in range(4))
+        lstm = pol.cell == "lstm"
+        h0 = ops.stack_layers([yb[h0_t, h0_r] for yb in p['ybufs']])
+        c0 = ops.stack_layers([cb[h0_t, h0_r] for cb in p['cbufs']]) if lstm else None
+
+        def table(bufs):                      # [K, B, L*H]: row (k, c) = every layer's state at the k-th reset of column c
+            tab = torch.zeros((lay.K, B, pol.num_layers * pol.hidden_size), dtype=torch.float32, device=dev)
+            if m:
+                tab[rk, rc] = torch.cat([bf[rt, rr] for bf in bufs], dim=1)
+            return tab
+        return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values, valid=valid,
+                               reset_slot=reset_slot, reset_h=table(p['ybufs']), reset_c=table(p['cbufs']) if lstm else None)
 
     @staticmethod
     def list_of_dicts_to_dict_of_lists(x):
@@ -982,6 +1157,9 @@ class DotaOptimizer:
                              % self.value_clip)
         if self.mask_padding and batch.valid is None:
             raise ValueError("mask_padding=True needs the valid mask of experience prep, and this batch has no valid")
+        if batch.reset_slot is not None and not self.mask_padding:
+            raise ValueError("a packed batch (reset_slot) trains only with mask_padding=True: its padding carries no "
+                             "advantages or value targets")
         t_enter = time.perf_counter()
         self._upload_hparams()
         slot = batch._slot
@@ -1059,9 +1237,9 @@ class DotaOptimizer:
         keys = ops.HEAD_KEYS
         self.flat.zero_grad_detached()                                    # :671 (grads gathered into the flat buffer below)
         hidden = (batch.h0, batch.c0) if self.policy_base.cell == "lstm" else batch.h0
-        batch.wait(batch.observations['env'], batch.h0, batch.c0)
+        batch.wait(batch.observations['env'], batch.h0, batch.c0, batch.reset_slot, batch.reset_h, batch.reset_c)
         # :619 on the module itself: the data-parallel wrapper's hook-driven reduction stays idle, the step reduces below
-        packed, target_unit = self.policy_base._train_forward(batch.observations, hidden, wait=batch.wait)
+        packed, target_unit = self.policy_base._train_forward(batch.observations, hidden, wait=batch.wait, reset=batch.reset())
         valid = batch.valid if self.mask_padding else None
         batch.wait(batch.old_logp, batch.advantages, batch.returns, batch.old_values, valid, *batch.masks.values(),
                    *batch.actions.values(), *batch.observations.values())
@@ -1206,6 +1384,16 @@ class DotaOptimizer:
         for it in range(self.iteration_start, self.iterations):
             self.run_iteration(it)
 
+    def _pulled_sequences(self, rollout_lens, n_seq):
+        """The training sequences of the rollouts pulled so far (``rollout_lens``, the last one just pulled; ``n_seq`` the
+        count before it): the reference's ``ceil(L / seq_len)`` per rollout, or with ``pack_sequences`` the columns of the
+        packed layout -- computed only once the unpacked count reaches ``min_seq_per_epoch``, as it can only be smaller."""
+        S = self.seq_len
+        if not self.pack_sequences:
+            return n_seq + (rollout_lens[-1] + S - 1) // S
+        unpacked = sequence_count(rollout_lens, S)
+        return unpacked if unpacked < self.min_seq_per_epoch else sequence_count(rollout_lens, S, pack=True)
+
     def run_iteration(self, it):
         logger.info('iteration {}/{}'.format(it, self.iterations))
         experiences, subrewards, rollout_lens, weight_ages = [], [], [], []
@@ -1213,17 +1401,18 @@ class DotaOptimizer:
         xp_waits = 0
         # The reference pulls and prepares rollouts one at a time until it holds min_seq_per_epoch sequences (:448-466).  The
         # number of sequences a rollout yields is known from its length alone, so the SAME rollouts are pulled here first and
-        # then prepared together in one batched pass (experiences_from_rollouts).
+        # then prepared together in one batched pass (experiences_from_rollouts).  With pack_sequences the count is that of
+        # the packed layout, so every rank still holds at least min_seq_per_epoch sequences.
         rollouts, n_seq = [], 0
         while n_seq < self.min_seq_per_epoch:                             # :448
             start_xp_wait = time.time()
             rollout, rollout_subrewards, rollout_len, weight_version, _ = self._next_rollout()
             xp_waits += time.time() - start_xp_wait
             rollouts.append(rollout)
-            n_seq += (rollout_len + self.seq_len - 1) // self.seq_len
             subrewards.append(rollout_subrewards)
             rollout_lens.append(rollout_len)
             weight_ages.append(it - weight_version)
+            n_seq = self._pulled_sequences(rollout_lens, n_seq)
         batch = self.batch_from_rollouts(rollouts)                        # prepared + stacked once, reused by every epoch
         time_xp = time.time() - start_xp
         # a stream of rollouts gives every iteration its own batch size: capturing a graph per shape would cost more than the
@@ -1272,6 +1461,8 @@ class DotaOptimizer:
             metrics['ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
         if self.mask_padding:                                              # share of the trained tokens that were padding
             metrics['padding_fraction'] = (n_steps - sum(rollout_lens)) / n_steps
+        if self.pack_sequences:                                            # share of the sequences packing saved
+            metrics['packing_saved_fraction'] = 1.0 - batch.batch_size / sequence_count(rollout_lens, self.seq_len)
         n_cut = sum(not r.get('terminal', True) for r in rollouts)
         if n_cut:                                                          # share of the rollouts cut from a game that goes on
             metrics['non_terminal_fraction'] = n_cut / len(rollouts)
@@ -1401,10 +1592,10 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          pretrained_model, mq_prefetch_count, log_dir, entropy_coef, vf_coef, run_local,
          hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
          value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
-         mask_padding=False):
+         mask_padding=False, pack_sequences=False):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
-                       mask_padding=mask_padding)                                        # before any process-group setup
+                       mask_padding=mask_padding, pack_sequences=pack_sequences)         # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -1415,7 +1606,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         run_local=run_local, hidden_size=hidden_size, cell=cell, num_layers=num_layers, gamma=gamma,
         gae_lambda=gae_lambda, clip_range=clip_range, max_grad_norm=max_grad_norm, value_clip=value_clip,
         advantage_estimator=advantage_estimator, vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip,
-        num_minibatches=num_minibatches, mask_padding=mask_padding)
+        num_minibatches=num_minibatches, mask_padding=mask_padding, pack_sequences=pack_sequences)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -1430,7 +1621,8 @@ def default_log_dir():
 def build_arg_parser():
     """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell``, ``--num-layers`` and the PPO
     settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm``, ``--value-clip``,
-    ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches`` and ``--mask-padding``."""
+    ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches``, ``--mask-padding`` and
+    ``--pack-sequences``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -1464,6 +1656,9 @@ def build_arg_parser():
     p.add_argument("--mask-padding", action="store_true",
                    help="leave the zero padding of each rollout's last chunk out of GAE / V-trace and the loss "
                         "(reference: padding is trained on)")
+    p.add_argument("--pack-sequences", action="store_true",
+                   help="pack the rollouts' last partial chunks into shared sequences with recurrent-state resets, so "
+                        "padding is not trained on (needs --mask-padding)")
     return p
 
 
@@ -1478,6 +1673,6 @@ if __name__ == '__main__':
              num_layers=args.num_layers, gamma=args.gamma, gae_lambda=args.gae_lambda, clip_range=args.clip_range,
              max_grad_norm=args.max_grad_norm, value_clip=args.value_clip, advantage_estimator=args.advantage_estimator,
              vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip, num_minibatches=args.num_minibatches,
-             mask_padding=args.mask_padding)
+             mask_padding=args.mask_padding, pack_sequences=args.pack_sequences)
     except KeyboardInterrupt:
         pass

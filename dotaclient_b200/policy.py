@@ -133,12 +133,13 @@ class Policy(nn.Module):
         so ``DotaOptimizer.train`` pays no transposes.  ``observations`` is a dict keyed by INPUT_KEYS."""
         return self._run(tuple(observations[k] for k in self.INPUT_KEYS), hidden, time_major=True)
 
-    def _train_forward(self, observations, hidden, wait=None):
+    def _train_forward(self, observations, hidden, wait=None, reset=None):
         """The training step's forward on time-major inputs -> (the packed ``[S, B, ops.PACK_WIDTH]`` output of the four
         small heads and the value head, target-unit logits ``[S, B, 40]``): the tensors the fused PPO loss reads and
-        backward starts from.  ``wait`` (see ``encoder_ops.unit_encoder``) lets the observations arrive while it runs."""
+        backward starts from.  ``wait`` (see ``encoder_ops.unit_encoder``) lets the observations arrive while it runs.
+        ``reset``: recurrent-state resets inside the sequences (``_recur``)."""
         x, unit_embedding = self._encode(observations['env'], [observations[k] for k in self.INPUT_KEYS[1:]], wait=wait)
-        y, _ = self._recur(x.contiguous(), hidden)
+        y, _ = self._recur(x.contiguous(), hidden, reset)
         return self._head_outputs(y, unit_embedding)
 
     # ------------------------------------------------------------------ implementation
@@ -152,18 +153,27 @@ class Policy(nn.Module):
             [l.weight for l in layers], [l.bias for l in layers], wait=wait)
         return ops.linear(x, self.affine_pre_rnn.weight, self.affine_pre_rnn.bias, relu=True), unit_embedding
 
-    def _recur(self, x_tm, hidden):
+    def _recur(self, x_tm, hidden, reset=None):
         """x_tm ``[S, B, H]`` time-major -> y_tm ``[S, B, H]``, new hidden in torch's ``[L, B, H]`` form.
 
         One ``ops.rnn_sequence`` (i2h GEMM + width-selected recurrence kernel) per layer, as ``nn.GRU(num_layers=L)``
         stacks them: layer k reads layer k-1's output sequence, a view of that layer's state buffer (no copy), so
-        autograd chains the backward through layer k's ``dx``."""
+        autograd chains the backward through layer k's ``dx``.
+
+        ``reset``: None, or ``(slot [S, B] int32, h [K, B, L*H], c [K, B, L*H] | None)`` (``ExperienceBatch.reset_*``): at
+        a token with ``slot[t, b] = k >= 0`` every layer's state entering step t is replaced by its ``H``-wide slice of row
+        (k, b) of the tables."""
         r = self.rnn
         lstm = self.cell == "lstm"
+        H = self.hidden_size
         h0, c0 = hidden if lstm else (hidden, None)
         y, hs, cs = x_tm, [], []
         for k in range(self.num_layers):
-            y, hn, cn = ops.rnn_sequence(y, *r.layer(k), h0[k], c0[k] if lstm else None, self.cell)
+            rk = None
+            if reset is not None:
+                slot, rh, rc = reset
+                rk = (slot, rh[:, :, k * H:(k + 1) * H].contiguous(), rc[:, :, k * H:(k + 1) * H].contiguous() if lstm else None)
+            y, hn, cn = ops.rnn_sequence(y, *r.layer(k), h0[k], c0[k] if lstm else None, self.cell, rk)
             hs.append(hn)
             cs.append(cn)
         h_n = ops.stack_layers(hs)

@@ -142,6 +142,32 @@ int dc_rnn_seq_bwd(int cell, float *gates, const float *w_hh, const float *ybuf,
                    const float *dy, const float *dhn, const float *dcn, float *dh0, float *dc0,
                    int B, int S, int H, void *workspace, dc_stream_t stream);
 
+/* Same recurrence with recurrent-state RESETS inside a sequence: several segments (e.g. the tails of different rollouts
+ * packed into one training sequence) share one column, and each later segment restarts from its own state.
+ *   reset_slot [S, B] int32   k = reset_slot[t*B + b]: -1 carries the state; k >= 0 replaces the state entering step t of
+ *                             sequence b (at t = 0 it overrides h_0 / c_0) with row k*B + b of the tables below
+ *   reset_prev [K, B, H]      GRU: the reset h; LSTM: the reset c (the cell's previous-state operand)
+ *   reset_pre  [K, B, G*H]    forward only: h_reset W_hh^T + b_hh of the reset h (the caller computes it once, a GEMM of
+ *                             K*B rows)
+ *   K >= 0                    rows per column of the tables (NULL tables are allowed when K = 0)
+ * Forward: at a reset token the cell reads its h2h pre-activation from reset_pre and its previous state from reset_prev; the
+ * step's mat-vec on the stale state is discarded.  The saved tensors keep their meaning (ybuf slot t+1 = h_t, the GRU's cbuf
+ * aux = the W_hn h + b_hn the cell used).  Backward: at a reset token prev comes from reset_prev and no gradient flows into
+ * step t-1 (neither through W_hh nor through the direct dh z / dc f path); a reset at t = 0 leaves dh0 / dc0 zero for b.
+ * The weight gradient dW_hh = dgh^T ybuf[:S] that the caller forms is then wrong at the reset tokens by
+ * dgh_t^T (h_reset - ybuf[t]): the caller adds that correction.  db_hh needs none.  The reset states get no gradient.
+ * Every design (H = 128, 256, other multiples of 128, generic) has a reset instantiation; the plain entry points above run
+ * the instantiations without it.  With every slot at -1 the results are bit-identical to dc_rnn_seq_fwd / _bwd.
+ * Preconditions the library cannot check (the slots are on the device): -1 <= reset_slot < K.  Checked before any CUDA
+ * call: the arguments of dc_rnn_seq_fwd / _bwd, reset_slot != NULL, K >= 0, non-null tables when K > 0 -> DC_EINVAL. */
+int dc_rnn_seq_fwd_reset(int cell, float *gates, const float *w_hh, const float *b_hh, float *ybuf, float *cbuf,
+                         const int32_t *reset_slot, const float *reset_prev, const float *reset_pre, int K,
+                         int B, int S, int H, void *workspace, dc_stream_t stream);
+int dc_rnn_seq_bwd_reset(int cell, float *gates, const float *w_hh, const float *ybuf, float *cbuf,
+                         const float *dy, const float *dhn, const float *dcn, float *dh0, float *dc0,
+                         const int32_t *reset_slot, const float *reset_prev, int K,
+                         int B, int S, int H, void *workspace, dc_stream_t stream);
+
 /* ---- fp32-accurate tensor-core GEMM (wgmma, 3xTF32) ---------------------------------------
  * C[M,N] = A[M,K] * B[N,K]^T (+ bias[N]) (ReLU if relu != 0); row-major fp32 with leading dimensions lda/ldb/ldc.
  * Replaces the library SGEMM of the input-to-hidden projection inside nn.GRU / nn.LSTM (policy.py:66,141:
