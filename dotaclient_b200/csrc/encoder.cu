@@ -5,62 +5,26 @@
 //
 //   env_fwd / env_bwd   relu(env W_e^T + b_e), 3 -> 128, written into / read from columns [0,128) of the concatenated
 //                       [N, 896] pre-rnn input row (no torch.cat), policy.py:55,97
-//   unit_basic_fwd      relu(units W_b^T + b_b)            [R,12] -> [R,128]     (K = 12: not a tensor-core shape)
 //   unit_basic reduce   fixed-order sum of the dW_b / db_b partials of the fused data-gradient kernel (gemm_tf32x3.cu)
 //   target_unit_q_fwd   logits[n,u] = <att[n] W_g, basic[n,u]> + <att[n], b_g>: the head WITHOUT the [N,40,128] embedding
 //   target_unit_q_bwd   s_g[n] = sum_u dlogits[n,u] basic_g[n,u] (-> d_att and the head's share of dW_g as token-level GEMMs)
-// The max-pool over a group's units lives in the embedding GEMM's epilogue (dc_gemm_unit_max) and its backward routing is
+// The basic layer relu(units W_b^T + b_b) ([R,12] -> [R,128], K = 12: not a tensor-core shape) has no kernel of its own: the
+// embedding GEMM's producers (dc_unit_embed_fwd) and the target-unit head rebuild it from the raw unit features
+// (unit_basic.cuh).  The max-pool over a group's units lives in the embedding GEMM's epilogue and its backward routing is
 // generated inside the weight- / data-gradient kernels (dc_unit_wgrad_routed, dc_unit_dgrad_fused), all in gemm_tf32x3.cu.
 //
 // Thread mapping everywhere: one warp per row of 128 channels, lane l owns channels 4l..4l+3 -> every global access
 // is a fully coalesced 512-byte row segment (16 bytes per lane).
 #include "dc_common.cuh"
+#include "unit_basic.cuh"
 
 namespace {
 
 constexpr int kC = 128;          // embedding width (policy.py:56-63)
-constexpr int kIn = 12;          // unit feature count (policy.py:56)
+constexpr int kIn = kUnitFeatures;
 constexpr int kWarps = 8;
 constexpr int kThreadsE = kWarps * 32;
 constexpr int kMaxUnits = 40;
-
-// ---- relu(units W_b^T + b_b) -------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreadsE) unit_basic_fwd_kernel(const float *__restrict__ units,
-                                                                   const float *__restrict__ w_b,
-                                                                   const float *__restrict__ b_b,
-                                                                   float *__restrict__ basic, int64_t R) {
-    __shared__ float s_u[kWarps][32][kIn];                        // 32 rows of raw features per warp per iteration
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    // weights as channel PAIRS: w2[p][k] = (W_b[4l+2p][k], W_b[4l+2p+1][k])
-    float2 w2[2][kIn], b2[2];
-#pragma unroll
-    for (int p = 0; p < 2; ++p) {
-        b2[p] = make_float2(b_b[lane * 4 + 2 * p], b_b[lane * 4 + 2 * p + 1]);
-#pragma unroll
-        for (int k = 0; k < kIn; ++k) w2[p][k] = make_float2(w_b[(lane * 4 + 2 * p) * kIn + k], w_b[(lane * 4 + 2 * p + 1) * kIn + k]);
-    }
-    const int64_t rows_per_iter = (int64_t)gridDim.x * kWarps * 32;
-    for (int64_t base = ((int64_t)blockIdx.x * kWarps + warp) * 32; base < R; base += rows_per_iter) {
-        const int nrows = (int)min((int64_t)32, R - base);
-        // stage 32 x 12 contiguous floats (coalesced), then every lane reads each row as a broadcast
-        float *su = &s_u[warp][0][0];
-        for (int i = lane; i < nrows * kIn; i += 32) su[i] = units[base * kIn + i];
-        __syncwarp();
-        for (int r = 0; r < nrows; ++r) {
-            float2 a0 = b2[0], a1 = b2[1];
-#pragma unroll
-            for (int k = 0; k < kIn; ++k) {
-                const float u = s_u[warp][r][k];
-                const float2 uu = make_float2(u, u);
-                a0 = dc_ffma2(uu, w2[0][k], a0);
-                a1 = dc_ffma2(uu, w2[1][k], a1);
-            }
-            *reinterpret_cast<float4 *>(basic + (base + r) * kC + lane * 4) =
-                make_float4(fmaxf(a0.x, 0.f), fmaxf(a0.y, 0.f), fmaxf(a1.x, 0.f), fmaxf(a1.y, 0.f));
-        }
-        __syncwarp();
-    }
-}
 
 // ---- dW_b, db_b: fixed-order sum of the [128][13] partials of dc_unit_dgrad_fused (12 weight-gradient columns + the bias gradient)
 __global__ void unit_basic_bwd_reduce_kernel(const float *__restrict__ partial, int nblocks, float *__restrict__ dw_b,
@@ -189,86 +153,140 @@ __global__ void __launch_bounds__(256) env_bwd_reduce_kernel(const float *__rest
 // ---- target-unit head without the unit embedding ------------------------------------------------------------------------
 // logits[n,u] = <att[n], W_g basic[n,u] + b_g> = <att[n] W_g, basic[n,u]> + <att[n], b_g> (policy.py:144-153; algebra pinned in
 // tests/test_oracle.py): with q[n, g*128 + j] = (att W_g)[n, j] and q[n, 768 + g] = <att[n], b_g> from ONE small GEMM over tokens,
-// the head reads the stored `basic` rows and the [N, 40, 128] embedding is never materialised.
-struct BasicPtrs { const float *p[6]; };
-__constant__ int kGroupUnits[6] = {1, 5, 16, 16, 1, 1};
-__constant__ int kGroupOffset[6] = {0, 1, 6, 22, 38, 39};
+// the head rebuilds the `basic` rows from the raw unit features and the [N, 40, 128] embedding is never materialised.
+// A warp owns one token at a time (grid-stride over tokens, so that a lane loads the W_b rows of its 4 channels once): the
+// token's 40 raw unit rows (1.9 KB) are staged in the warp's shared-memory slot, every lane reads a row as a broadcast and
+// regenerates its 4 channels in registers -- 20 KB per token that are not read from HBM, for 48 FMAs per lane and row.
+struct UnitPtrs { const float *p[6]; };
+__host__ __device__ constexpr int group_units(int g) { return g == 1 ? 5 : (g == 2 || g == 3) ? 16 : 1; }
+__host__ __device__ constexpr int group_offset(int g) { return g == 0 ? 0 : g == 1 ? 1 : g == 2 ? 6 : g == 3 ? 22 : g == 4 ? 38 : 39; }
+constexpr int kTokenU4 = kMaxUnits * kIn / 4;                      // 16-byte pieces of a token's raw unit rows
 
-__global__ void __launch_bounds__(kThreadsE) target_unit_q_fwd_kernel(const float *__restrict__ q, int ld_q, BasicPtrs basics,
-                                                                      float *__restrict__ logits, int64_t N) {
-    const int lane = threadIdx.x & 31;
-    const int64_t n = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
-    if (n >= N) return;
-    const float *qrow = q + n * ld_q;
-    float mine = 0.f, mine_hi = 0.f;                              // lane u keeps logit u (u < 32), lanes 0..7 also u+32
+// W_b / b_b of the lane's channels 4l..4l+3
+__device__ __forceinline__ void load_basic_weights(float (&w)[4][kIn], float (&b)[4], const float *__restrict__ w_b,
+                                                   const float *__restrict__ b_b, int lane) {
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        b[c] = __ldg(b_b + 4 * lane + c);
+#pragma unroll
+        for (int k = 0; k < kIn; ++k) w[c][k] = __ldg(w_b + (4 * lane + c) * kIn + k);
+    }
+}
+
+// token n's unit rows, group after group (row off_g + u at su + 3 (off_g + u)); the caller brackets it with __syncwarp()
+__device__ __forceinline__ void stage_token_units(float4 *su, const UnitPtrs &units, int64_t n, int lane) {
 #pragma unroll
     for (int g = 0; g < 6; ++g) {
-        const float4 a = __ldg(reinterpret_cast<const float4 *>(qrow + g * kC) + lane);
-        const float c = __ldg(qrow + 6 * kC + g);
-        const int nu = kGroupUnits[g], off = kGroupOffset[g];
-        const float4 *row = reinterpret_cast<const float4 *>(basics.p[g] + n * nu * kC) + lane;
-        for (int u = 0; u < nu; ++u) {
-            const float4 v = __ldg(row + u * (kC / 4));
-            float d = v.x * a.x + v.y * a.y + v.z * a.z + v.w * a.w;
-            d = dc_warp_sum(d) + c;
-            const int o = off + u;
-            if (o < 32) { if (lane == o) mine = d; } else { if (lane == o - 32) mine_hi = d; }
-        }
+        const int cnt = 3 * group_units(g);
+        const float4 *src = reinterpret_cast<const float4 *>(units.p[g]) + n * cnt;
+        for (int j = lane; j < cnt; j += 32) su[3 * group_offset(g) + j] = __ldg(src + j);
     }
-    logits[n * kMaxUnits + lane] = mine;
-    if (lane < kMaxUnits - 32) logits[n * kMaxUnits + 32 + lane] = mine_hi;
+}
+
+// the lane's 4 channels of the basic row whose raw features are at `row`
+__device__ __forceinline__ float4 basic_row(const float4 *row, const float (&w)[4][kIn], const float (&b)[4]) {
+    const float4 u0 = row[0], u1 = row[1], u2 = row[2];
+    const float u[kIn] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w, u2.x, u2.y, u2.z, u2.w};
+    return make_float4(dc_unit_basic(u, w[0], b[0]), dc_unit_basic(u, w[1], b[1]), dc_unit_basic(u, w[2], b[2]),
+                       dc_unit_basic(u, w[3], b[3]));
+}
+
+__global__ void __launch_bounds__(kThreadsE) target_unit_q_fwd_kernel(const float *__restrict__ q, int ld_q, UnitPtrs units,
+                                                                      const float *__restrict__ w_b, const float *__restrict__ b_b,
+                                                                      float *__restrict__ logits, int64_t N) {
+    __shared__ float4 s_u[kWarps][kTokenU4];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float w[4][kIn], b[4];
+    load_basic_weights(w, b, w_b, b_b, lane);
+    float4 *su = s_u[warp];
+    for (int64_t n = (int64_t)blockIdx.x * kWarps + warp; n < N; n += (int64_t)gridDim.x * kWarps) {
+        const float *qrow = q + n * ld_q;
+        __syncwarp();                                              // the previous token's rows have been read
+        stage_token_units(su, units, n, lane);
+        __syncwarp();
+        float mine = 0.f, mine_hi = 0.f;                          // lane u keeps logit u (u < 32), lanes 0..7 also u+32
+#pragma unroll
+        for (int g = 0; g < 6; ++g) {
+            const float4 a = __ldg(reinterpret_cast<const float4 *>(qrow + g * kC) + lane);
+            const float c = __ldg(qrow + 6 * kC + g);
+            const int nu = group_units(g), off = group_offset(g);
+            for (int u = 0; u < nu; ++u) {
+                const float4 v = basic_row(su + 3 * (off + u), w, b);
+                float d = v.x * a.x + v.y * a.y + v.z * a.z + v.w * a.w;
+                d = dc_warp_sum(d) + c;
+                const int o = off + u;
+                if (o < 32) { if (lane == o) mine = d; } else { if (lane == o - 32) mine_hi = d; }
+            }
+        }
+        logits[n * kMaxUnits + lane] = mine;
+        if (lane < kMaxUnits - 32) logits[n * kMaxUnits + 32 + lane] = mine_hi;
+    }
 }
 
 // s[n, g*128 + j] = sum_u dlogits[n, off_g + u] basic_g[n,u,j],  s[n, 768 + g] = sum_u dlogits[n, off_g + u]  (zeros elsewhere):
 // d_att = s [W_0 | ... | W_5 | b_0..b_5]^T is then one GEMM over tokens.  Tokens that did not use the head write zeros, read nothing.
-__global__ void __launch_bounds__(kThreadsE) target_unit_q_bwd_kernel(const float *__restrict__ dlogits, BasicPtrs basics,
+__global__ void __launch_bounds__(kThreadsE) target_unit_q_bwd_kernel(const float *__restrict__ dlogits, UnitPtrs units,
+                                                                      const float *__restrict__ w_b, const float *__restrict__ b_b,
                                                                       float *__restrict__ s, int ld_s, int64_t N) {
-    const int lane = threadIdx.x & 31;
-    const int64_t n = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
-    if (n >= N) return;
-    const float g_lo = dlogits[n * kMaxUnits + lane];
-    const float g_hi = lane < kMaxUnits - 32 ? dlogits[n * kMaxUnits + 32 + lane] : 0.f;
-    const bool any = __any_sync(0xffffffffu, g_lo != 0.f || g_hi != 0.f);
-    float4 *srow = reinterpret_cast<float4 *>(s + n * ld_s) + lane;
+    __shared__ float4 s_u[kWarps][kTokenU4];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float w[4][kIn], b[4];
+    load_basic_weights(w, b, w_b, b_b, lane);
+    float4 *su = s_u[warp];
     const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (!any) {
+    for (int64_t n = (int64_t)blockIdx.x * kWarps + warp; n < N; n += (int64_t)gridDim.x * kWarps) {
+        const float g_lo = dlogits[n * kMaxUnits + lane];
+        const float g_hi = lane < kMaxUnits - 32 ? dlogits[n * kMaxUnits + 32 + lane] : 0.f;
+        const bool any = __any_sync(0xffffffffu, g_lo != 0.f || g_hi != 0.f);
+        float4 *srow = reinterpret_cast<float4 *>(s + n * ld_s) + lane;
+        if (!any) {
 #pragma unroll
-        for (int g = 0; g < 7; ++g) srow[g * (kC / 4)] = zero;
-        return;
-    }
-    float sig[6];
-#pragma unroll
-    for (int g = 0; g < 6; ++g) {
-        const int nu = kGroupUnits[g], off = kGroupOffset[g];
-        const float4 *row = reinterpret_cast<const float4 *>(basics.p[g] + n * nu * kC) + lane;
-        float4 acc = zero;
-        float sg = 0.f;
-        for (int u = 0; u < nu; ++u) {
-            const int o = off + u;
-            const float gv = __shfl_sync(0xffffffffu, o < 32 ? g_lo : g_hi, o & 31);
-            const float4 v = __ldg(row + u * (kC / 4));
-            acc.x = fmaf(gv, v.x, acc.x); acc.y = fmaf(gv, v.y, acc.y); acc.z = fmaf(gv, v.z, acc.z); acc.w = fmaf(gv, v.w, acc.w);
-            sg += gv;
+            for (int g = 0; g < 7; ++g) srow[g * (kC / 4)] = zero;
+            continue;
         }
-        srow[g * (kC / 4)] = acc;
-        sig[g] = sg;
+        __syncwarp();
+        stage_token_units(su, units, n, lane);
+        __syncwarp();
+        float sig[6];
+#pragma unroll
+        for (int g = 0; g < 6; ++g) {
+            const int nu = group_units(g), off = group_offset(g);
+            float4 acc = zero;
+            float sg = 0.f;
+            for (int u = 0; u < nu; ++u) {
+                const int o = off + u;
+                const float gv = __shfl_sync(0xffffffffu, o < 32 ? g_lo : g_hi, o & 31);
+                const float4 v = basic_row(su + 3 * o, w, b);
+                acc.x = fmaf(gv, v.x, acc.x); acc.y = fmaf(gv, v.y, acc.y); acc.z = fmaf(gv, v.z, acc.z); acc.w = fmaf(gv, v.w, acc.w);
+                sg += gv;
+            }
+            srow[g * (kC / 4)] = acc;
+            sig[g] = sg;
+        }
+        float4 tail = zero;                                        // columns 768..895: the six sums, then zeros
+        if (lane == 0) tail = make_float4(sig[0], sig[1], sig[2], sig[3]);
+        if (lane == 1) tail = make_float4(sig[4], sig[5], 0.f, 0.f);
+        srow[6 * (kC / 4)] = tail;
     }
-    float4 tail = zero;                                            // columns 768..895: the six sums, then zeros
-    if (lane == 0) tail = make_float4(sig[0], sig[1], sig[2], sig[3]);
-    if (lane == 1) tail = make_float4(sig[4], sig[5], 0.f, 0.f);
-    srow[6 * (kC / 4)] = tail;
+}
+
+// Grid of the two head kernels: one warp per token, at most as many blocks as are resident at once (per_sm per SM).
+static unsigned head_grid(int per_sm, int64_t N) {
+    const int64_t want = (N + kWarps - 1) / kWarps, cap = (int64_t)(per_sm < 1 ? 1 : per_sm) * dc_sm_count();
+    return (unsigned)(want < cap ? want : cap);
+}
+
+// the six unit arrays of the head: non-null, 16-byte aligned (rows are read as 3 x 16 bytes)
+static int unit_ptrs(const float *const units[6], UnitPtrs *up, const char *who) {
+    DC_REQUIRE(units != nullptr, DC_EINVAL, "%s: units is NULL", who);
+    for (int g = 0; g < 6; ++g) {
+        DC_REQUIRE(units[g] && ((uintptr_t)units[g] & 15) == 0, DC_EINVAL, "%s: units[%d] null / not 16-byte aligned", who, g);
+        up->p[g] = units[g];
+    }
+    return DC_OK;
 }
 
 }  // namespace
-
-extern "C" int dc_unit_basic_fwd(const float *units, const float *w_b, const float *b_b, float *basic, int64_t R,
-                                 dc_stream_t stream) {
-    DC_REQUIRE(units && w_b && b_b && basic && R > 0, DC_EINVAL, "dc_unit_basic_fwd: bad arguments");
-    DC_REQUIRE(((uintptr_t)basic & 15) == 0, DC_EINVAL, "dc_unit_basic_fwd: output must be 16-byte aligned");
-    unit_basic_fwd_kernel<<<4 * dc_sm_count(), kThreadsE, 0, dc_cu_stream(stream)>>>(units, w_b, b_b, basic, R);
-    DC_LAUNCH_OK();
-    return DC_OK;
-}
 
 extern "C" size_t dc_unit_basic_bwd_workspace_bytes(void) { return (size_t)4 * 1024 * kC * (kIn + 1) * sizeof(float); }
 
@@ -304,30 +322,30 @@ extern "C" int dc_env_bwd(const float *d_out, const float *out, int ld, const fl
     return DC_OK;
 }
 
-extern "C" int dc_target_unit_q_fwd(const float *q, int ld_q, const float *const basics[6], float *logits, int64_t N,
-                                    dc_stream_t stream) {
-    DC_REQUIRE(q && basics && logits && N > 0 && ld_q >= 7 * kC && ld_q % 4 == 0, DC_EINVAL, "dc_target_unit_q_fwd: bad arguments");
-    BasicPtrs bp;
-    for (int g = 0; g < 6; ++g) {
-        DC_REQUIRE(basics[g] && ((uintptr_t)basics[g] & 15) == 0, DC_EINVAL, "dc_target_unit_q_fwd: basic[%d] null / unaligned", g);
-        bp.p[g] = basics[g];
-    }
+extern "C" int dc_target_unit_q_fwd(const float *q, int ld_q, const float *const units[6], const float *w_b, const float *b_b,
+                                    float *logits, int64_t N, dc_stream_t stream) {
+    DC_REQUIRE(q && w_b && b_b && logits && N > 0 && ld_q >= 7 * kC && ld_q % 4 == 0, DC_EINVAL, "dc_target_unit_q_fwd: bad arguments");
+    UnitPtrs up;
+    const int rc = unit_ptrs(units, &up, "dc_target_unit_q_fwd");
+    if (rc != DC_OK) return rc;
     DC_REQUIRE(((uintptr_t)q & 15) == 0, DC_EINVAL, "dc_target_unit_q_fwd: alignment");
-    target_unit_q_fwd_kernel<<<(unsigned)((N + kWarps - 1) / kWarps), kThreadsE, 0, dc_cu_stream(stream)>>>(q, ld_q, bp, logits, N);
+    int per_sm = 0;
+    DC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, target_unit_q_fwd_kernel, kThreadsE, 0));
+    target_unit_q_fwd_kernel<<<head_grid(per_sm, N), kThreadsE, 0, dc_cu_stream(stream)>>>(q, ld_q, up, w_b, b_b, logits, N);
     DC_LAUNCH_OK();
     return DC_OK;
 }
 
-extern "C" int dc_target_unit_q_bwd(const float *dlogits, const float *const basics[6], float *s, int ld_s, int64_t N,
-                                    dc_stream_t stream) {
-    DC_REQUIRE(dlogits && basics && s && N > 0 && ld_s >= 7 * kC && ld_s % 4 == 0, DC_EINVAL, "dc_target_unit_q_bwd: bad arguments");
-    BasicPtrs bp;
-    for (int g = 0; g < 6; ++g) {
-        DC_REQUIRE(basics[g] && ((uintptr_t)basics[g] & 15) == 0, DC_EINVAL, "dc_target_unit_q_bwd: basic[%d] null / unaligned", g);
-        bp.p[g] = basics[g];
-    }
+extern "C" int dc_target_unit_q_bwd(const float *dlogits, const float *const units[6], const float *w_b, const float *b_b, float *s,
+                                    int ld_s, int64_t N, dc_stream_t stream) {
+    DC_REQUIRE(dlogits && w_b && b_b && s && N > 0 && ld_s >= 7 * kC && ld_s % 4 == 0, DC_EINVAL, "dc_target_unit_q_bwd: bad arguments");
+    UnitPtrs up;
+    const int rc = unit_ptrs(units, &up, "dc_target_unit_q_bwd");
+    if (rc != DC_OK) return rc;
     DC_REQUIRE(((uintptr_t)s & 15) == 0, DC_EINVAL, "dc_target_unit_q_bwd: alignment");
-    target_unit_q_bwd_kernel<<<(unsigned)((N + kWarps - 1) / kWarps), kThreadsE, 0, dc_cu_stream(stream)>>>(dlogits, bp, s, ld_s, N);
+    int per_sm = 0;
+    DC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, target_unit_q_bwd_kernel, kThreadsE, 0));
+    target_unit_q_bwd_kernel<<<head_grid(per_sm, N), kThreadsE, 0, dc_cu_stream(stream)>>>(dlogits, up, w_b, b_b, s, ld_s, N);
     DC_LAUNCH_OK();
     return DC_OK;
 }

@@ -51,11 +51,15 @@ def _wgrad_workspace(No, Ni, device):
     return ws
 
 
-# The unit embedding [N, 40, 128] (policy.py:130-131) is never materialised in the forward pass.  Its two consumers are
-#   * the max-pool: fused into the epilogue of the embedding GEMM (dc_gemm_unit_max: max + arg-max per token and channel; the
-#     1-unit groups are plain GEMMs writing their slot of the pre-rnn row; the enemy-tower embedding is not needed at all in
-#     forward because policy.py:127 takes that slot's maximum from the enemy non-heroes);
-#   * the target-unit head, which is linear in it: logits[n,u] = <att[n] W_g, basic[n,u]> + <att[n], b_g>  (TargetUnit below).
+# The unit embedding [N, 40, 128] (policy.py:130-131) is never materialised in the forward pass, and the basic layer
+# basic = relu(units W_b^T + b_b) that feeds it is rebuilt from the 12 raw features of a unit wherever it is read.  The consumers are
+#   * the max-pool: one launch per group (dc_unit_embed_fwd) whose producers generate `basic` into the embedding GEMM's operand
+#     ring and whose epilogue keeps max + arg-max per token and channel; for the 1-unit groups the plain epilogue writes the
+#     group's slot of the pre-rnn row.  The enemy-tower group runs nothing in forward because policy.py:127 takes that slot's
+#     maximum from the enemy non-heroes.  `basic` of groups 0-4 is stored by the same launch only when a backward may follow:
+#     the weight gradients below read it;
+#   * the target-unit head, which is linear in it: logits[n,u] = <att[n] W_g, basic[n,u]> + <att[n], b_g>  (TargetUnit below,
+#     `basic` regenerated from the raw features in the head kernels).
 # In backward the embedding's gradient d_emb[n,u,:] has two sources -- the head (rank 1: dlogits[n,u] * att[n,:], arrives first) and the
 # max-pool routing R (d_xmax[n,:] to the arg-max unit of every channel; arrives with the pre-rnn gradient, after the recurrence).
 # TargetUnit parks (dlogits, att, s) in the `link` cell the two Functions of one graph share; UnitEncoder.backward then needs no
@@ -79,12 +83,13 @@ class UnitEncoder(torch.autograd.Function):
     followed by the six group maxima, written in place by the kernels (no cat, no ``[N, 40, 128]`` embedding).
 
     maxima slot 5 (enemy towers) is a copy of slot 3 (enemy non-heroes): the reference's ``policy.py:127``.
-    ``link`` (a dict) receives the per-group ``basic`` activations and the embedding weights for the target-unit head.
-    ``wait``: see ``unit_encoder``.
+    ``link`` (a dict) receives the raw unit features, the basic layer's and the embedding weights for the target-unit head.
+    ``wait``: see ``unit_encoder``.  ``need_grad``: a backward may follow, so the basic activations of groups 0-4 are stored
+    for the weight gradients (without it nothing of the basic layer reaches HBM).
     """
 
     @staticmethod
-    def forward(ctx, link, wait, env, w_e, b_e, w_b, b_b, *rest):
+    def forward(ctx, link, wait, need_grad, env, w_e, b_e, w_b, b_b, *rest):
         units, weights, biases = rest[:6], rest[6:12], rest[12:18]
         ctx.link = link
         _need_cuda(env, w_b, *units)
@@ -111,24 +116,23 @@ class UnitEncoder(torch.autograd.Function):
         basics = []
         for g, n_u in enumerate(UNITS):
             R = N * n_u
-            basic = torch.empty((R, C), dtype=torch.float32, device=dev)
             if wait is not None:                      # this group's observations may still be in flight over PCIe
                 wait(units[g])
-            with PROFILE.span("unit_basic_fwd", 1, 4 * R * (12 + C)):
-                _lib.check(lib.dc_unit_basic_fwd(units[g].data_ptr(), w_b.data_ptr(), b_b.data_ptr(), basic.data_ptr(), R, st),
-                           "dc_unit_basic_fwd")
-            if n_u > 1:                               # embedding GEMM with the max-pool in its epilogue
-                copy = _ptr(xcat, 6 * C) if g == 3 else None
-                with PROFILE.span("gemm_unit_max", 1, 4 * (R * C + C * C + N * C) + N * C):
-                    _lib.check(lib.dc_gemm_unit_max(basic.data_ptr(), weights[g].data_ptr(), biases[g].data_ptr(),
-                                                    _ptr(xcat, (g + 1) * C), copy, XCAT, argmax[g].data_ptr(), N, n_u, st),
-                               "dc_gemm_unit_max")
-            elif g < 5:                               # one unit: the embedding IS the maximum -> straight into its slot
-                with PROFILE.span("gemm_tf32x3", 1, 4 * (2 * R * C + C * C)):
-                    _lib.check(lib.dc_gemm_tf32x3(basic.data_ptr(), C, weights[g].data_ptr(), C, biases[g].data_ptr(),
-                                                  _ptr(xcat, (g + 1) * C), XCAT, R, C, C, 0, st), "dc_gemm_tf32x3")
+            if g == 5:                                # policy.py:127: the enemy-tower maximum is never used
+                continue
+            # basic layer + embedding GEMM in one launch: the max-pool epilogue, or for one unit the embedding IS the maximum
+            # and goes straight into its slot
+            basic = torch.empty((R, C), dtype=torch.float32, device=dev) if need_grad else None
+            copy = _ptr(xcat, 6 * C) if g == 3 else None
+            am = argmax[g].data_ptr() if n_u > 1 else None
+            nbytes = 4 * (R * 12 + (R * C if need_grad else 0) + C * C + N * C) + (N * C if n_u > 1 else 0)
+            with PROFILE.span("gemm_unit_max" if n_u > 1 else "gemm_tf32x3", 1, nbytes):
+                _lib.check(lib.dc_unit_embed_fwd(units[g].data_ptr(), w_b.data_ptr(), b_b.data_ptr(), _lib.ptr(basic),
+                                                 weights[g].data_ptr(), biases[g].data_ptr(), _ptr(xcat, (g + 1) * C), copy, XCAT,
+                                                 am, N, n_u, st), "dc_unit_embed_fwd")
             basics.append(basic)
-        link["basics"], link["weights"], link["biases"] = basics, weights, biases
+        link["units"], link["w_b"], link["b_b"] = units, w_b, b_b
+        link["weights"], link["biases"] = weights, biases
         ctx.N = N
         ctx.lead = lead
         ctx.save_for_backward(argmax, *units, *basics, *weights, env2, xcat, w_b, b_b)
@@ -137,8 +141,8 @@ class UnitEncoder(torch.autograd.Function):
     @staticmethod
     def backward(ctx, d_xcat):
         saved = ctx.saved_tensors
-        argmax, units, basics, weights, env2, xcat = saved[0], saved[1:7], saved[7:13], saved[13:19], saved[19], saved[20]
-        w_b, b_b = saved[21], saved[22]
+        argmax, units, basics, weights, env2, xcat = saved[0], saved[1:7], saved[7:12], saved[12:18], saved[18], saved[19]
+        w_b, b_b = saved[20], saved[21]
         N = ctx.N
         lib = _lib.load()
         st = _lib.stream_ptr()
@@ -189,7 +193,7 @@ class UnitEncoder(torch.autograd.Function):
             dw_all += dw_head[:, :6 * C].reshape(C, 6, C).permute(1, 0, 2)
             db_all += dw_head[:, 6 * C:6 * C + 6].t()
         dws, dbs = list(dw_all.unbind(0)), list(db_all.unbind(0))
-        return (None, None, None, dw_e, db_e, dw_b, db_b) + (None,) * 6 + tuple(dws) + tuple(dbs)
+        return (None, None, None, None, dw_e, db_e, dw_b, db_b) + (None,) * 6 + tuple(dws) + tuple(dbs)
 
 
 QW = 7 * C     # width of the head's token-level operands: six groups x 128 channels + one block carrying the six bias dots
@@ -198,14 +202,15 @@ QW = 7 * C     # width of the head's token-level operands: six groups x 128 chan
 class TargetUnit(torch.autograd.Function):
     """``logits[..., u] = <attention, unit_embedding[..., u, :]>`` (``policy.py:152-153``) WITHOUT the embedding:
     ``<att, W_g basic_u + b_g> = <att W_g, basic_u> + <att, b_g>``.  One GEMM over tokens produces ``q = att [W_0|..|W_5|b]``
-    ``[N, 896]``, a bandwidth kernel dots it with the stored ``basic`` rows.  Backward: ``s_g = sum_u dlogits_u basic_u`` (same
-    kernel shape), ``d_att = s [W_0|..|W_5|b]^T`` (one GEMM); the gradient towards the embedding weights and the basic layer
-    is finished by ``UnitEncoder.backward`` from (dlogits, att, s) parked in ``link``."""
+    ``[N, 896]``, a kernel dots it with the ``basic`` rows it rebuilds from the raw unit features.  Backward: ``s_g = sum_u
+    dlogits_u basic_u`` (same kernel shape), ``d_att = s [W_0|..|W_5|b]^T`` (one GEMM); the gradient towards the embedding
+    weights and the basic layer is finished by ``UnitEncoder.backward`` from (dlogits, att, s) parked in ``link``."""
 
     @staticmethod
     def forward(ctx, att, link):
         _need_cuda(att)
-        basics, weights, biases = link["basics"], link["weights"], link["biases"]
+        units, w_b, b_b = link["units"], link["w_b"], link["b_b"]
+        weights, biases = link["weights"], link["biases"]
         lead = att.shape[:-1]
         N = att.numel() // C
         att2 = _f32c(att.detach()).reshape(N, C)
@@ -215,24 +220,24 @@ class TargetUnit(torch.autograd.Function):
         bm = torch.cat(list(weights) + [bias_block], dim=1)                  # [128, 896]: bm[c, g*128+j] = W_g[c,j], bm[c, 768+g] = b_g[c]
         q = gemm_tf32x3(att2, bm.t().contiguous())                           # [N, 896] = att [W_0 | ... | W_5 | b]
         logits = torch.empty((N, MAX_UNITS), dtype=torch.float32, device=dev)
-        with PROFILE.span("target_unit_fwd", 1, 4 * N * (MAX_UNITS * C + QW + MAX_UNITS)):
-            _lib.check(_lib.load().dc_target_unit_q_fwd(q.data_ptr(), QW, _ptr6(basics), logits.data_ptr(), N, _lib.stream_ptr()),
-                       "dc_target_unit_q_fwd")
-        ctx.save_for_backward(att2, bm, *basics)
+        with PROFILE.span("target_unit_fwd", 1, 4 * N * (MAX_UNITS * 12 + QW + MAX_UNITS)):
+            _lib.check(_lib.load().dc_target_unit_q_fwd(q.data_ptr(), QW, _ptr6(units), w_b.data_ptr(), b_b.data_ptr(),
+                                                        logits.data_ptr(), N, _lib.stream_ptr()), "dc_target_unit_q_fwd")
+        ctx.save_for_backward(att2, bm, w_b, b_b, *units)
         ctx.link = link
         ctx.att_shape = att.shape
         return logits.view(*lead, MAX_UNITS)
 
     @staticmethod
     def backward(ctx, dlogits):
-        att2, bm = ctx.saved_tensors[:2]
-        basics = ctx.saved_tensors[2:]
+        att2, bm, w_b, b_b = ctx.saved_tensors[:4]
+        units = ctx.saved_tensors[4:]
         N = att2.shape[0]
         dl = _f32c(dlogits).reshape(N, MAX_UNITS)
         s = torch.empty((N, QW), dtype=torch.float32, device=att2.device)
         with PROFILE.span("target_unit_bwd", 1):       # bytes depend on how many tokens used the head (others are skipped)
-            _lib.check(_lib.load().dc_target_unit_q_bwd(dl.data_ptr(), _ptr6(basics), s.data_ptr(), QW, N, _lib.stream_ptr()),
-                       "dc_target_unit_q_bwd")
+            _lib.check(_lib.load().dc_target_unit_q_bwd(dl.data_ptr(), _ptr6(units), w_b.data_ptr(), b_b.data_ptr(), s.data_ptr(),
+                                                        QW, N, _lib.stream_ptr()), "dc_target_unit_q_bwd")
         d_att = gemm_tf32x3(s, bm)                                          # [N, 128] = s [W_0 | ... | W_5 | b]^T
         ctx.link["pending"] = (dl, att2, s)                                  # consumed by UnitEncoder.backward
         return d_att.view(ctx.att_shape), None
@@ -243,7 +248,9 @@ def unit_encoder(env, w_e, b_e, w_b, b_b, units, weights, biases, wait=None):
     the current stream wait for an input still being uploaded: it is called for ``env`` and for each unit group right
     before their first kernel, so the upload of group g+1 overlaps the kernels of group g."""
     link = {}
-    xcat = UnitEncoder.apply(link, wait, env, w_e, b_e, w_b, b_b, *units, *weights, *biases)
+    tensors = (env, w_e, b_e, w_b, b_b, *units, *weights, *biases)
+    need_grad = torch.is_grad_enabled() and any(t.requires_grad for t in tensors)
+    xcat = UnitEncoder.apply(link, wait, need_grad, *tensors)
     return link, xcat
 
 

@@ -190,13 +190,9 @@ size_t dc_gemm_wgrad_workspace_bytes(int No, int Ni);
 int dc_gemm_wgrad_tf32x3(const float *dY, int ldy, const float *X, int ldx, int64_t T, int No, int Ni,
                          float *dW, int ldw, float *db, int accumulate, void *workspace, dc_stream_t stream);
 
-/* ---- unit encoder / target-unit head: the bandwidth-bound pieces ------------------------------
- * (policy.py:99-136,144-153; the 128x128 embedding GEMMs themselves are dc_gemm_tf32x3 for the 1-unit groups and
- * dc_gemm_unit_max for the others)
- *   dc_unit_basic_fwd   basic[R,128] = relu(units[R,12] W_b^T + b_b)            policy.py:100,105,...
- */
-int dc_unit_basic_fwd(const float *units, const float *w_b, const float *b_b, float *basic, int64_t R,
-                      dc_stream_t stream);
+/* ---- unit encoder / target-unit head ------------------------------------------------------------
+ * (policy.py:99-136,144-153).  The basic layer basic[R,128] = relu(units[R,12] W_b^T + b_b) (policy.py:100,105,...) is
+ * rebuilt from the raw unit features by every kernel that reads it, bit for bit the same value everywhere. */
 size_t dc_unit_basic_bwd_workspace_bytes(void);   /* partial sums of dW_b / db_b: the workspace of dc_unit_dgrad_fused */
 /* Environment encoder (policy.py:55,97): out[n*ld_out + c] = relu(env[n,:3] . W_e[c,:] + b_e[c]), c < 128 -- written into
  * columns [0,128) of the concatenated pre-rnn input row (ld_out = 896), so the reference's torch.cat (policy.py:129-136)
@@ -211,12 +207,22 @@ int dc_env_bwd(const float *d_out, const float *out, int ld, const float *env, f
  * argmax[n*128 + c] (first maximum wins, like torch.max); the embedding itself is never stored.  n_units = 5 or 16. */
 int dc_gemm_unit_max(const float *basic, const float *w, const float *bias, float *xmax, float *xmax_copy, int ld_x,
                      uint8_t *argmax, int64_t n_tokens, int n_units, dc_stream_t stream);
+/* One unit-embedding group's forward in one launch: the basic layer of units [N*n_units, 12] (w_b [128,12], b_b [128]) is
+ * generated inside the embedding GEMM and, when basic_out is not NULL, also stored there ([N*n_units, 128], what the weight
+ * gradients read).  n_units 5, 16: the max-pool epilogue of dc_gemm_unit_max (xmax, xmax_copy, argmax; same results bit for
+ * bit as dc_gemm_unit_max on the stored basic).  n_units 1: xmax[n*ld_x + c] = (basic W^T)[n,c] + b[c], argmax and
+ * xmax_copy NULL.  units, basic_out, w, bias, xmax, xmax_copy 16-byte aligned; ld_x >= 128, a multiple of 4. */
+int dc_unit_embed_fwd(const float *units, const float *w_b, const float *b_b, float *basic_out, const float *w, const float *bias,
+                      float *xmax, float *xmax_copy, int ld_x, uint8_t *argmax, int64_t n_tokens, int n_units, dc_stream_t stream);
 /* Target-unit head without the embedding (policy.py:144-153): logits[n,u] = <q[n, g*128 ..], basic_g[n,u,:]> + q[n, 768+g]
- * with q = att [W_0|...|W_5|b_0..b_5] (ld_q >= 896) and basics[g] = the [N*units_g, 128] basic activations of group g
- * (units 1,5,16,16,1,1).  Backward: s[n, g*128 + j] = sum_u dlogits[n,u] basic_g[n,u,j], s[n, 768+g] = sum_u dlogits[n,u]
- * (zeros in 774..895), so that d_att = s [W_0|...|W_5|b]^T is one GEMM. */
-int dc_target_unit_q_fwd(const float *q, int ld_q, const float *const basics[6], float *logits, int64_t N, dc_stream_t stream);
-int dc_target_unit_q_bwd(const float *dlogits, const float *const basics[6], float *s, int ld_s, int64_t N, dc_stream_t stream);
+ * with q = att [W_0|...|W_5|b_0..b_5] (ld_q >= 896) and basic_g = relu(units[g] W_b^T + b_b) rebuilt from the raw unit
+ * features units[g] [N*units_g, 12] (units 1,5,16,16,1,1; 16-byte aligned).  Backward: s[n, g*128 + j] = sum_u dlogits[n,u]
+ * basic_g[n,u,j], s[n, 768+g] = sum_u dlogits[n,u] (zeros in 774..895), so that d_att = s [W_0|...|W_5|b]^T is one GEMM;
+ * tokens whose dlogits row is all zero get a zero row of s. */
+int dc_target_unit_q_fwd(const float *q, int ld_q, const float *const units[6], const float *w_b, const float *b_b, float *logits,
+                         int64_t N, dc_stream_t stream);
+int dc_target_unit_q_bwd(const float *dlogits, const float *const units[6], const float *w_b, const float *b_b, float *s, int ld_s,
+                         int64_t N, dc_stream_t stream);
 /* Backward of one unit-embedding layer WITHOUT the dense [N*units, 128] gradient of the embedding (what the reference's autograd
  * materialises behind policy.py:100-127,152-153).  R[(n,u), c] = (argmax[n*128 + c] == u) ? d_xmax[n*ld_dx + c] (+ d_xmax2[..]) : 0 is
  * the max-pool routing, generated inside the kernels.
@@ -226,7 +232,7 @@ int dc_target_unit_q_bwd(const float *dlogits, const float *const basics[6], flo
  *                         G[(n,u), j] = (basic[(n,u), j] > 0) * sum_c (R[(n,u), c] + dlogits[n*ld_dl + u] att[n*128 + c]) W[c, j]:
  *                         the whole gradient of the embedding (routing + the target-unit head's rank-1 part) is generated inside
  *                         the kernel; w_t = W^T [128,128]; the ReLU mask is recomputed from units/w_b/b_b (bit-identical to
- *                         dc_unit_basic_fwd); dlogits (already offset to the group's first unit) and att [N,128] are NULL when the
+ *                         the forward value); dlogits (already offset to the group's first unit) and att [N,128] are NULL when the
  *                         head was not used; d_xmax NULL = no routing (the enemy-tower layer, policy.py:127).  n_units = 1, 5 or
  *                         16; units, att, d_xmax 16-byte aligned; workspace: dc_unit_basic_bwd_workspace_bytes().
  * The head's share of dW / db is a token-level product (att^T s, s from dc_target_unit_q_bwd) the caller adds. */
