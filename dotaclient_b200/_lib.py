@@ -54,6 +54,8 @@ SIGNATURES = {
                                        _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "dc_ppo_loss_fwd_bwd_masked": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
                                           _vp, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "dc_ppo_loss_fwd_bwd_joint": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
+                                         _vp, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "dc_selected_logp": (_i32, [_ptr5, _ptr5, _ptr5, _i64, _vp, _vp]),
     "dc_select_actions": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _vp, _i64, _vp, _vp, _vp]),
     "dc_grad_flags": (_i32, [_vp, _i64, _vp, _i32, _vp, _vp]),
@@ -72,6 +74,7 @@ HP_LR, HP_E_CLIP, HP_ENTROPY_COEF, HP_VF_COEF, HP_MAX_GRAD_NORM, HP_VALUE_CLIP =
 # the PPO diagnostics written by dc_ppo_loss_fwd_bwd_dev (DC_STAT_* in include/dotaclient_b200.h)
 PPO_STATS_SLOTS = 16
 STAT_APPROX_KL, STAT_CLIP_FRACTION, STAT_EXPLAINED_VAR = 0, 6, 12
+STAT_JOINT_APPROX_KL, STAT_JOINT_CLIP_FRACTION = 13, 14     # dc_ppo_loss_fwd_bwd_joint only
 VTRACE_STATS_SLOTS = 8      # per-segment fp64 sums written by dc_vtrace_scan (DC_VTRACE_STATS_SLOTS)
 GATHER_MAX_TENSORS = 32     # descriptors per dc_gather_columns call (DC_GATHER_MAX_TENSORS)
 MAX_PARAM_TENSORS = 96      # kMaxSeg of csrc/grad_finish.cu: parameter tensors dc_grad_flags / dc_grad_finish can handle

@@ -25,9 +25,16 @@
 // value loss and its 1/N, the diagnostics -- and receives exactly zero gradient.  The statistics pass counts the valid
 // tokens into the workspace (n_valid); with valid == NULL every token counts and the arithmetic is the unmasked one.
 //
+// The `_joint` entry point (kJoint) clips the ratio of the whole hierarchical action instead of each head's:
+// log r_t = sum over the heads with an action row at t of (logp_new - old_logp), one clipped surrogate per token, averaged
+// over the T_a counting tokens with at least one action row (counted by the statistics pass).  One thread makes two sweeps
+// over its token's heads in the shared-memory tile: (1) log-sum-exp, selected log-prob, entropy, per-head diagnostics and
+// the joint log-ratio; (2) every head's dlogits row from the joint ratio's gradient.  Entropy and value terms are per head,
+// as in the default objective.
+//
 // Algorithmic HBM bytes per token: logits 260 + masks 65 + actions 65 + old 20 + adv/ret/value 12
 // read, dlogits 260 + dvalue 4 written = 686 (+ 69 for the statistics pass, + 4 for the old value when the value loss
-// is clipped, + 1 in each pass for `valid` when given).
+// is clipped, + 1 in each pass for `valid` when given).  The joint ratio reads and writes the same bytes.
 #include "dc_common.cuh"
 
 namespace {
@@ -66,11 +73,13 @@ struct HeadPtrs {
 constexpr int kStats = 2 * kHeads + 4;
 constexpr int kStKl = 0, kStClip = kHeads, kStD = 2 * kHeads, kStD2 = kStD + 1, kStR = kStD + 2, kStR2 = kStD + 3;
 constexpr int kTokD = 2 * kHeads, kTokR = kTokD + 1, kTokRows = kTokR + 1;   // rows of the per-token staging
+// joint ratio only: two more staging rows and sums after the above (k3 KL and clip flag of the joint ratio)
+constexpr int kTokJoint = kTokRows, kJointStats = 2;
 static_assert(2 * kHeads + 3 < DC_PPO_STATS_SLOTS, "stats output too small");
 
 // Workspace layout (DC_PPO_WORKSPACE_BYTES, zeroed per call)
 struct Workspace {
-    double pol[kHeads];   // sum over action rows of min(surr1, surr2)
+    double pol[kHeads];   // sum over action rows of min(surr1, surr2); joint ratio: pol[0] sums over the T_a tokens
     double ent[kHeads];   // sum over masked entries of -p*logp
     double vl;            // sum (ret - v)^2, or of the clipped value loss term
     double adv_sum, adv_sq;
@@ -79,6 +88,8 @@ struct Workspace {
     unsigned long long n_valid;   // tokens that count (all N when no valid mask is given)
     unsigned ticket_stats, ticket_loss;
     float adv_mean, adv_std;
+    unsigned long long n_joint;      // joint ratio: T_a, the tokens that count with at least one action row
+    double st_joint[kJointStats];    // joint ratio: sums over the T_a tokens of its k3 KL and of its clip flag
 };
 static_assert(sizeof(Workspace) <= DC_PPO_WORKSPACE_BYTES, "workspace too small");
 
@@ -156,6 +167,8 @@ __device__ __forceinline__ T block_sum(T v, T *scratch) {
 }
 
 // ---- pass 1: counts + advantage statistics ------------------------------------------------
+// kJoint: also counts T_a (tokens that count with an action row in any head) into ws->n_joint
+template <bool kJoint>
 __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const float *__restrict__ adv,
                                                            const uint8_t *__restrict__ valid, int64_t N,
                                                            Workspace *ws, int32_t *n_actions_out) {
@@ -187,10 +200,13 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
 #pragma unroll
     for (int h = 0; h < kHeads; ++h) tot[h] = __syncthreads_count(has[h]);
     const int n_live = __syncthreads_count(live);
+    int n_joint = 0;
+    if constexpr (kJoint) n_joint = __syncthreads_count(has[0] | has[1] | has[2] | has[3] | has[4]);
     if (threadIdx.x == 0) {
         atomicAdd(&ws->adv_sum, sa);
         atomicAdd(&ws->adv_sq, sq);
         atomicAdd(&ws->n_valid, (unsigned long long)n_live);
+        if (kJoint && n_joint) atomicAdd(&ws->n_joint, (unsigned long long)n_joint);
 #pragma unroll
         for (int h = 0; h < kHeads; ++h)
             if (tot[h]) atomicAdd(&ws->cnt[h], tot[h]);
@@ -294,7 +310,90 @@ __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, con
     }
 }
 
-template <bool kSelectOnly>
+// Joint ratio, sweep 1 over head H of one token: masked log-softmax, entropy and the per-head diagnostics as head_token,
+// and the head's term lp[a] - old_lp of the joint log-ratio.  Sets bit H of in_s when the head has an action row here.
+template <int H>
+__device__ __forceinline__ void joint_head_fwd(const float *lrow, const uint8_t *mrow, const uint8_t *arow, float old_lp,
+                                               int n_h, float e_clip, float &ent_acc, float *kl_out, float *clip_out,
+                                               float &log_r, int &in_s) {
+    constexpr int N = head_n(H);
+    float l[N], e[N];
+    int mask_any = 0, a_idx = -1;
+    float se = 0.f;
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+        l[j] = lrow[j];
+        const int m = mrow[j];
+        mask_any |= m;
+        e[j] = m ? __expf(l[j]) : 0.f;
+        se += e[j];
+        if (arow[j]) a_idx = j;
+    }
+    if (n_h == 0 || (!mask_any && a_idx < 0)) return;     // skipped as in head_token
+    const float lse = logf(se);
+    const float inv_se = 1.0f / se;
+    float ent_row = 0.f, lpa = 0.f;
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+        const float lp = l[j] - lse;
+        if (mrow[j]) ent_row -= (e[j] * inv_se) * lp;
+        if (j == a_idx) lpa = lp;
+    }
+    ent_acc += ent_row;
+    if (a_idx >= 0) {
+        const float lr = lpa - old_lp;
+        *kl_out = expm1f(lr) - lr;
+        *clip_out = fabsf(__expf(lr) - 1.0f) > e_clip ? 1.f : 0.f;
+        log_r += lr;                      // head order 0..4, fp32
+        in_s |= 1 << H;
+    }
+}
+
+// Joint ratio, sweep 2 over head H: the dlogits row, with g_lp = d loss / d lp[a] of the joint surrogate (the same for
+// every head with an action row) and the head's entropy term, recomputed from the tile exactly as sweep 1 computed it.
+template <int H>
+__device__ __forceinline__ void joint_head_bwd(float *lrow, const uint8_t *mrow, const uint8_t *arow, int n_h, float g_lp,
+                                               float entropy_coef) {
+    constexpr int N = head_n(H);
+    float l[N], e[N];
+    int mask_any = 0, a_idx = -1;
+    float se = 0.f;
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+        l[j] = lrow[j];
+        const int m = mrow[j];
+        mask_any |= m;
+        e[j] = m ? __expf(l[j]) : 0.f;
+        se += e[j];
+        if (arow[j]) a_idx = j;
+    }
+    if (n_h == 0 || (!mask_any && a_idx < 0)) {
+#pragma unroll
+        for (int j = 0; j < N; ++j) lrow[j] = 0.f;
+        return;
+    }
+    const float lse = logf(se);
+    const float inv_se = 1.0f / se;
+    float ent_row = 0.f;
+    float p[N], lp[N];
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+        lp[j] = l[j] - lse;
+        p[j] = e[j] * inv_se;
+        if (mrow[j]) ent_row -= p[j] * lp[j];
+    }
+    if (a_idx < 0) g_lp = 0.f;
+    const float ce = entropy_coef > 0.f ? entropy_coef / (float)n_h : 0.f;
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+        float g = -g_lp * p[j];
+        if (j == a_idx) g += g_lp;
+        if (mrow[j]) g += ce * p[j] * (lp[j] + ent_row);
+        lrow[j] = g;
+    }
+}
+
+template <bool kSelectOnly, bool kJoint>
 __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const float *__restrict__ old_logp,
                                                           const float *__restrict__ adv_raw,
                                                           const float *__restrict__ ret,
@@ -306,16 +405,19 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
                                                           float *__restrict__ dvalue, float *__restrict__ out,
                                                           float *__restrict__ stats, Workspace *ws,
                                                           float *__restrict__ logp_out) {
+    static_assert(!(kSelectOnly && kJoint), "the joint ratio is a loss");
+    constexpr int kRows = kTokRows + (kJoint ? kJointStats : 0);
+    constexpr int kSums = kStats + (kJoint ? kJointStats : 0);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *s_logits = reinterpret_cast<float *>(smem_raw);
     float *s_old = s_logits + kLogitFloats;
     uint8_t *s_mask = reinterpret_cast<uint8_t *>(s_old + kOldFloats);
     uint8_t *s_act = s_mask + kByteTile;
     __shared__ float s_red[kTile / 32];
-    // per-token diagnostics (rows kStKl.., kStClip.., then ret - v and ret), staged here rather than held in registers
-    // across the head loop, and their block sums
-    __shared__ float s_tok[kTokRows][kTile];
-    __shared__ double s_st[kStats];
+    // per-token diagnostics (rows kStKl.., kStClip.., then ret - v and ret, then the joint ratio's), staged here rather
+    // than held in registers across the head loop, and their block sums
+    __shared__ float s_tok[kRows][kTile];
+    __shared__ double s_st[kSums];
     __shared__ bool s_last;
 
     // hyper-parameters from the device block when given, rounded to the types of the scalar arguments
@@ -349,7 +451,7 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
     float vl = 0.f;
     if (!kSelectOnly) {
 #pragma unroll
-        for (int i = 0; i < kTokRows; ++i) s_tok[i][t] = 0.f;     // rows without an action (and dead threads) count 0
+        for (int i = 0; i < kRows; ++i) s_tok[i][t] = 0.f;        // rows without an action (and dead threads) count 0
     }
     int cnt[kHeads] = {0, 0, 0, 0, 0};
     float adv_n = 0.f;
@@ -365,6 +467,38 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
     }
     if (live) {
         float lp_sel[kHeads];
+        if constexpr (kJoint) {
+            float log_r = 0.f;
+            int in_s = 0;
+#define DC_JHEAD(H)                                                                                                 \
+            joint_head_fwd<H>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H),    \
+                              s_act + byte_off(H) + t * head_n(H), s_old[t * 5 + H], use ? cnt[H] : 0, e_clip,       \
+                              ent[H], &s_tok[kStKl + H][t], &s_tok[kStClip + H][t], log_r, in_s);
+            DC_JHEAD(0) DC_JHEAD(1) DC_JHEAD(2) DC_JHEAD(3) DC_JHEAD(4)
+#undef DC_JHEAD
+            float g_lp = 0.f;                 // d loss / d lp[a], the same for every head in S_t
+            if (in_s) {                       // S_t not empty (so the token counts and T_a >= 1)
+                const float ratio = __expf(log_r);
+                s_tok[kTokJoint][t] = expm1f(log_r) - log_r;
+                s_tok[kTokJoint + 1][t] = fabsf(ratio - 1.0f) > e_clip ? 1.f : 0.f;
+                const float lo = 1.0f - e_clip, hi = 1.0f + e_clip;
+                const float s1 = ratio * adv_n;
+                const float s2 = fminf(fmaxf(ratio, lo), hi) * adv_n;
+                pol[0] += fminf(s1, s2);
+                // the same autograd rules as head_token: ties of torch.min split, clamp passes inside [lo, hi]
+                const float g1 = s1 < s2 ? 1.f : (s1 == s2 ? 0.5f : 0.f);
+                const float g2 = s2 < s1 ? 1.f : (s1 == s2 ? 0.5f : 0.f);
+                const float in_range = (ratio >= lo && ratio <= hi) ? 1.f : 0.f;
+                g_lp = -1.0f / (float)ws->n_joint * adv_n * (g1 + g2 * in_range) * ratio;
+            }
+            // sweep 2 re-reads the tile: without this the compiler keeps every head's sweep-1 values live instead
+            asm volatile("" ::: "memory");
+#define DC_JHEAD(H)                                                                                                 \
+            joint_head_bwd<H>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H),    \
+                              s_act + byte_off(H) + t * head_n(H), use ? cnt[H] : 0, g_lp, entropy_coef);
+            DC_JHEAD(0) DC_JHEAD(1) DC_JHEAD(2) DC_JHEAD(3) DC_JHEAD(4)
+#undef DC_JHEAD
+        } else {
 #define DC_HEAD(H)                                                                                              \
         head_token<H, true>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H),  \
                             s_act + byte_off(H) + t * head_n(H), kSelectOnly ? 0.f : s_old[t * 5 + H], adv_n,   \
@@ -372,6 +506,7 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
                             &s_tok[kStClip + H][t], kSelectOnly ? &lp_sel[H] : nullptr);
         DC_HEAD(0) DC_HEAD(1) DC_HEAD(2) DC_HEAD(3) DC_HEAD(4)
 #undef DC_HEAD
+        }
         if (kSelectOnly) {
 #pragma unroll
             for (int h = 0; h < kHeads; ++h) logp_out[(t0 + t) * 5 + h] = lp_sel[h];
@@ -418,8 +553,8 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
     sums[2 * kHeads] = block_sum(vl, s_red);
     if (stats) {    // the diagnostics (s_tok is complete: block_sum synchronised the block): one warp per sum, in float64
         const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-        for (int i = warp; i < kStats; i += kTile / 32) {
-            const int row = i < kStD ? i : (i < kStR ? kTokD : kTokR);
+        for (int i = warp; i < kSums; i += kTile / 32) {
+            const int row = (kJoint && i >= kStats) ? kTokJoint + (i - kStats) : (i < kStD ? i : (i < kStR ? kTokD : kTokR));
             const bool square = i == kStD2 || i == kStR2;
             double s = 0.0;
             for (int j = lane; j < kTile; j += 32) {
@@ -441,6 +576,10 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         if (stats) {
             for (int i = 0; i < kStats; ++i)
                 if (s_st[i] != 0.0) atomicAdd(&ws->st[i], s_st[i]);
+            if constexpr (kJoint) {
+                for (int i = 0; i < kJointStats; ++i)
+                    if (s_st[kStats + i] != 0.0) atomicAdd(&ws->st_joint[i], s_st[kStats + i]);
+            }
         }
         __threadfence();
         s_last = atomicAdd(&ws->ticket_loss, 1u) == gridDim.x - 1;
@@ -452,14 +591,19 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         float policy = 0.f, entropy = 0.f;
         for (int h = 0; h < kHeads; ++h) {
             const int n = w->cnt[h];
-            const float pl = n ? (float)(-w->pol[h] / (double)n) : 0.f;     // optimizer.py:641 / :628
+            const float pl = (!kJoint && n) ? (float)(-w->pol[h] / (double)n) : 0.f;     // optimizer.py:641 / :628
             const float en = n ? (float)(w->ent[h] / (double)n) : 0.f;      // optimizer.py:646 / :629
             out[9 + h] = pl;
             out[4 + h] = en;
             policy += pl;
             entropy += en;
         }
-        policy /= (float)kHeads;                                            // optimizer.py:650
+        if constexpr (kJoint) {                                             // -(1/T_a) sum_t min(r A, clip(r) A); 0 if T_a = 0
+            const unsigned long long n_a = w->n_joint;
+            policy = n_a ? (float)(-w->pol[0] / (double)n_a) : 0.f;
+        } else {
+            policy /= (float)kHeads;                                        // optimizer.py:650
+        }
         const float e_loss = entropy_coef > 0.f ? -entropy_coef * entropy : 0.f;
         const double n_tok_d = (double)w->n_valid;                          // N, or N_v under a valid mask
         const float v_loss = vf_coef > 0.f ? vf_coef * (0.5f * (float)(w->vl / n_tok_d)) : 0.f;
@@ -491,6 +635,11 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             const double var_d = w->st[kStD2] / n - md * md, var_r = w->st[kStR2] / n - mr * mr;
             stats[DC_STAT_EXPLAINED_VAR] = var_r > 0.0 ? (float)(1.0 - var_d / var_r) : __int_as_float(0x7fc00000);
             for (int i = DC_STAT_EXPLAINED_VAR + 1; i < DC_PPO_STATS_SLOTS; ++i) stats[i] = 0.f;
+            if constexpr (kJoint) {
+                const unsigned long long n_a = w->n_joint;
+                stats[DC_STAT_JOINT_APPROX_KL] = n_a ? (float)(w->st_joint[0] / (double)n_a) : 0.f;
+                stats[DC_STAT_JOINT_CLIP_FRACTION] = n_a ? (float)(w->st_joint[1] / (double)n_a) : 0.f;
+            }
         }
     }
 }
@@ -503,13 +652,14 @@ int check_heads(const float *const logits[], const uint8_t *const masks[], const
 
 // Both launches of one loss evaluation.  hparams == nullptr: e_clip / entropy_coef / vf_coef are the scalar arguments and
 // the value loss is not clipped; otherwise they come from the device block.  stats == nullptr skips the diagnostics.
+// joint: the joint-ratio instantiations of both kernels.
 int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
                     const uint8_t *const masks[DC_NUM_HEADS], const uint8_t *const actions[DC_NUM_HEADS],
                     const float *old_logp, const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
                     const float *old_value, const uint8_t *valid, int64_t N, float e_clip, float entropy_coef, float vf_coef,
                     const double *hparams, float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
                     float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions, void *workspace,
-                    dc_stream_t stream) {
+                    dc_stream_t stream, bool joint = false) {
     DC_REQUIRE(N > 0, DC_EINVAL, "dc_ppo_loss_fwd_bwd: N=%lld", (long long)N);
     DC_REQUIRE(check_heads(logits, masks, actions) && old_logp && adv_raw && ret && value && dvalue && out &&
                    n_actions && workspace && ld_logits && ld_dlogits, DC_EINVAL, "dc_ppo_loss_fwd_bwd: null pointer");
@@ -526,14 +676,25 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
     Workspace *ws = reinterpret_cast<Workspace *>(workspace);
     DC_CUDA(cudaMemsetAsync(ws, 0, sizeof(Workspace), st));
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
-    ppo_stats_kernel<<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
+    if (joint) {
+        ppo_stats_kernel<true><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
+        DC_LAUNCH_OK();
+        DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)kSmemBytes));
+        ppo_loss_kernel<false, true><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
+                                                                        entropy_coef, vf_coef, old_value, valid, hparams,
+                                                                        dvalue, out, stats, ws, nullptr);
+        DC_LAUNCH_OK();
+        return DC_OK;
+    }
+    ppo_stats_kernel<false><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
     DC_LAUNCH_OK();
     // per-device attribute: set on every call (a process-wide "done" flag breaks the second GPU of a process)
-    DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
-    DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
-    ppo_loss_kernel<false><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
-                                                              entropy_coef, vf_coef, old_value, valid, hparams, dvalue, out,
-                                                              stats, ws, nullptr);
+    DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+    DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+    ppo_loss_kernel<false, false><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
+                                                                     entropy_coef, vf_coef, old_value, valid, hparams,
+                                                                     dvalue, out, stats, ws, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -580,6 +741,20 @@ extern "C" int dc_ppo_loss_fwd_bwd_masked(const float *const logits[DC_NUM_HEADS
                            workspace, stream);
 }
 
+extern "C" int dc_ppo_loss_fwd_bwd_joint(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                                         const uint8_t *const masks[DC_NUM_HEADS],
+                                         const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
+                                         const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                                         const float *old_value, const uint8_t *valid, int64_t N, const double *hparams,
+                                         float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                                         float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
+                                         void *workspace, dc_stream_t stream) {
+    DC_REQUIRE(hparams, DC_EINVAL, "dc_ppo_loss_fwd_bwd_joint: null hyper-parameter block");
+    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, old_value, valid,
+                           N, 0.f, 0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions,
+                           workspace, stream, true);
+}
+
 extern "C" int dc_ppo_loss_fwd_bwd(const float *const logits[DC_NUM_HEADS], const uint8_t *const masks[DC_NUM_HEADS],
                                    const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
                                    const float *adv_raw, const float *ret, const float *value, int64_t N,
@@ -603,9 +778,9 @@ extern "C" int dc_selected_logp(const float *const logits[DC_NUM_HEADS], const u
     }
     hp.ld_v = 1; hp.ld_dv = 1;
     // per-device attribute: set on every call (a process-wide "done" flag breaks the second GPU of a process)
-    DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+    DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
-    ppo_loss_kernel<true><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
+    ppo_loss_kernel<true, false><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
         hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
         nullptr, logp_out);
     DC_LAUNCH_OK();

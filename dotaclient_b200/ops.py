@@ -448,8 +448,11 @@ def hparam_block(device, lr=0.0, e_clip=0.0, entropy_coef=0.0, vf_coef=0.0, max_
     return torch.tensor(vals, dtype=torch.float64, device=device)
 
 
-def _ppo_dev_args(hparams, old_value, stats, N, dev, valid=None):
-    """Checks the extra operands of ``dc_ppo_loss_fwd_bwd_dev`` / ``_masked``; allocates ``stats`` when not given."""
+def _ppo_dev_args(hparams, old_value, stats, N, dev, valid=None, joint=False):
+    """Checks the extra operands of ``dc_ppo_loss_fwd_bwd_dev`` / ``_masked`` / ``_joint``; allocates ``stats`` when not
+    given."""
+    if joint and hparams is None:
+        raise ValueError("the joint-ratio PPO loss needs the device hyper-parameter block (hparams=)")
     if hparams is None:
         raise ValueError("the valid mask of the PPO loss needs the device hyper-parameter block (hparams=)")
     _need_cuda(hparams, old_value, valid)
@@ -469,21 +472,24 @@ def _ppo_dev_args(hparams, old_value, stats, N, dev, valid=None):
 
 
 def _ppo_dev_call(lib, lptr, ld_l, masks, actions, old_logp, adv_raw, ret, value_ptr, ld_v, old_value, valid, N, hparams,
-                  dptr, ld_d, dvalue_ptr, ld_dv, out, stats, n_actions, ws):
-    """``dc_ppo_loss_fwd_bwd_dev``, or ``dc_ppo_loss_fwd_bwd_masked`` when a valid mask is given."""
+                  dptr, ld_d, dvalue_ptr, ld_dv, out, stats, n_actions, ws, joint=False):
+    """``dc_ppo_loss_fwd_bwd_dev``, or ``dc_ppo_loss_fwd_bwd_masked`` when a valid mask is given, or
+    ``dc_ppo_loss_fwd_bwd_joint`` (valid or not) when ``joint``."""
     head = (lptr, ld_l, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(),
             value_ptr, ld_v, _lib.ptr(old_value))
     tail = (N, hparams.data_ptr(), dptr, ld_d, dvalue_ptr, ld_dv, out.data_ptr(), stats.data_ptr(), n_actions.data_ptr(),
             ws.data_ptr(), _lib.stream_ptr())
     with PROFILE.span("ppo_loss", 2):
-        if valid is None:
+        if joint:
+            _lib.check(lib.dc_ppo_loss_fwd_bwd_joint(*head, _lib.ptr(valid), *tail), "dc_ppo_loss_fwd_bwd_joint")
+        elif valid is None:
             _lib.check(lib.dc_ppo_loss_fwd_bwd_dev(*head, *tail), "dc_ppo_loss_fwd_bwd_dev")
         else:
             _lib.check(lib.dc_ppo_loss_fwd_bwd_masked(*head, valid.data_ptr(), *tail), "dc_ppo_loss_fwd_bwd_masked")
 
 
 def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_clip, entropy_coef, vf_coef, hparams=None,
-                     old_value=None, stats=None, valid=None):
+                     old_value=None, stats=None, valid=None, joint=False):
     """Fused PPO loss + gradients (``optimizer.py:587-589,621-665`` and their backward).
 
     logits/masks/actions: sequences of 5 tensors [..., n_h] in HEAD_KEYS order (any leading dims,
@@ -496,6 +502,9 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     [``_lib.PPO_STATS_SLOTS``]; the return value gains that tensor as a fifth element.
     ``valid`` [...] bool (needs ``hparams``): tokens where it is False count for nothing and get zero gradients
     (``dc_ppo_loss_fwd_bwd_masked``); None is the unmasked loss.
+    ``joint`` (needs ``hparams``): one clipped PPO ratio per token, of the whole hierarchical action, instead of one per
+    head (``dc_ppo_loss_fwd_bwd_joint``, with or without ``valid``); ``stats`` then also holds the joint ratio's KL and
+    clip fraction (``_lib.STAT_JOINT_APPROX_KL`` / ``STAT_JOINT_CLIP_FRACTION``).
     """
     logits = [_f32c(l.detach()) for l in logits]
     _need_cuda(*logits)
@@ -514,11 +523,11 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     n_actions = torch.empty(5, dtype=torch.int32, device=dev)
     ws = torch.empty(_lib.PPO_WORKSPACE_BYTES, dtype=torch.uint8, device=dev)
     lib = _lib.load()
-    if hparams is not None or valid is not None:
-        old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid)
+    if hparams is not None or valid is not None or joint:
+        old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid, joint)
         ld = (ctypes.c_int64 * 5)(*HEAD_SIZES)
         _ppo_dev_call(lib, _lib.ptr5(logits), ld, masks, actions, old_logp, adv_raw, ret, value.data_ptr(), 1, old_value,
-                      valid, N, hparams, _lib.ptr5(dlogits), ld, dvalue.data_ptr(), 1, out, stats, n_actions, ws)
+                      valid, N, hparams, _lib.ptr5(dlogits), ld, dvalue.data_ptr(), 1, out, stats, n_actions, ws, joint)
         return out, n_actions, dlogits, dvalue, stats
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd(_lib.ptr5(logits), _lib.ptr5(masks), _lib.ptr5(actions),
@@ -710,14 +719,14 @@ PACK_WIDTH = 128
 
 
 def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e_clip, entropy_coef, vf_coef, hparams=None,
-                    old_value=None, stats=None, valid=None):
+                    old_value=None, stats=None, valid=None, joint=False):
     """Fused PPO loss where the four small heads and the value head are column ranges of ONE packed ``[N,128]``
     tensor-core GEMM output (``PACK_COLS``) and the target-unit logits are a separate ``[N,40]`` tensor.
 
     Returns (out[16], n_actions[5], d_packed [N,128], d_logits_tu [N,40]): the gradients go straight back into the two
     producers, so no slice/cat kernels run and the five tiny K=131072 weight-gradient GEMMs become one wgmma wgrad.
-    ``hparams`` / ``old_value`` / ``stats`` / ``valid``: as ``ppo_loss_fwd_bwd`` (the fifth element of the result is then
-    ``stats``).
+    ``hparams`` / ``old_value`` / ``stats`` / ``valid`` / ``joint``: as ``ppo_loss_fwd_bwd`` (the fifth element of the
+    result is then ``stats``).
     """
     _need_cuda(packed, logits_tu)
     p2 = _f32c(packed.detach()).reshape(-1, PACK_WIDTH)
@@ -740,10 +749,10 @@ def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e
     dptr = _lib._ptr5(col(d_packed, "enum"), col(d_packed, "x"), col(d_packed, "y"), d_tu.data_ptr(), col(d_packed, "ability"))
     ld = (c.c_int64 * 5)(PACK_WIDTH, PACK_WIDTH, PACK_WIDTH, 40, PACK_WIDTH)
     lib = _lib.load()
-    if hparams is not None or valid is not None:
-        old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid)
+    if hparams is not None or valid is not None or joint:
+        old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid, joint)
         _ppo_dev_call(lib, lptr, ld, masks, actions, old_logp, adv_raw, ret, col(p2, "value"), PACK_WIDTH, old_value, valid,
-                      N, hparams, dptr, ld, col(d_packed, "value"), PACK_WIDTH, out, stats, n_actions, ws)
+                      N, hparams, dptr, ld, col(d_packed, "value"), PACK_WIDTH, out, stats, n_actions, ws, joint)
         return out, n_actions, d_packed.view_as(packed), d_tu.view_as(logits_tu), stats
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd_strided(lptr, ld, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(),

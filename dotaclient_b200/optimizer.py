@@ -378,14 +378,21 @@ def all_gather(t):                                                        # :193
 
 # ------------------------------------------------------------------------------------------ optimizer
 ADVANTAGE_ESTIMATORS = ('gae', 'vtrace')
+# 'per_head': the reference's objective, one clipped ratio per action head; 'joint': one clipped ratio per step, of the
+# whole hierarchical action (the product of the sampled heads' probabilities)
+POLICY_RATIOS = ('per_head', 'joint')
 
 
 def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
-                       vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False, pack_sequences=False):
+                       vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False, pack_sequences=False,
+                       policy_ratio='per_head'):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
-    vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool and
-    pack_sequences a bool that is True only with mask_padding.  NaN fails every check."""
+    vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool,
+    pack_sequences a bool that is True only with mask_padding and policy_ratio one of ``POLICY_RATIOS``.  NaN fails every
+    check."""
+    if not isinstance(policy_ratio, str) or policy_ratio not in POLICY_RATIOS:
+        raise ValueError("policy_ratio=%r: must be one of %s" % (policy_ratio, ", ".join(POLICY_RATIOS)))
     if not isinstance(mask_padding, bool):
         raise ValueError("mask_padding=%r: must be True or False" % (mask_padding,))
     if not isinstance(pack_sequences, bool):
@@ -655,15 +662,18 @@ class DotaOptimizer:
                  entropy_coef, vf_coef, run_local, *, hidden_size=256, cell="gru", num_layers=1, mq=None,
                  iterations=100000, rollout_prefetch=0, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1,
                  max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0,
-                 num_minibatches=1, mask_padding=False, pack_sequences=False):
+                 num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head'):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
                              % (num_layers, self.MAX_LAYERS, _lib.MAX_PARAM_TENSORS))
         check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                            vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
-                           mask_padding=mask_padding, pack_sequences=pack_sequences)
+                           mask_padding=mask_padding, pack_sequences=pack_sequences, policy_ratio=policy_ratio)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # 'joint': the loss clips one PPO ratio per step, of the whole hierarchical action (log r = sum over the sampled
+        # heads of logp_new - logp_old), averaged over the steps with an action; 'per_head': the reference's five ratios
+        self.policy_ratio = policy_ratio
         # True: batch_from_rollouts packs the rollouts' tails into shared columns with state resets between them
         # (pack_layout), so the padding of every rollout's last chunk is not trained on
         self.pack_sequences = pack_sequences
@@ -1181,7 +1191,7 @@ class DotaOptimizer:
         torch.cuda.current_stream().synchronize()      # the step's single host sync (result read-back)
         res = host.clone()
         keys = ops.HEAD_KEYS
-        self.last_ppo_stats = self._ppo_stats_dict(res[_lib.LOSS_SLOTS + 4:].tolist())
+        self.last_ppo_stats = self._ppo_stats_dict(res[_lib.LOSS_SLOTS + 4:].tolist(), joint=self.policy_ratio == 'joint')
         if res[_lib.LOSS_SLOTS + 3] != 0:               # :667-669, :678-679 (parameters were left untouched)
             if math.isnan(float(res[0])):
                 raise ValueError('loss={}, policy_loss={}, entropy_loss={}, value_loss={}'.format(
@@ -1205,12 +1215,15 @@ class DotaOptimizer:
                 'c_clip_fraction': s[4] / n}
 
     @staticmethod
-    def _ppo_stats_dict(st):
+    def _ppo_stats_dict(st, joint=False):
         out = {'approx_kl': st[_lib.STAT_APPROX_KL], 'clip_fraction': st[_lib.STAT_CLIP_FRACTION]}
         for h, k in enumerate(ops.HEAD_KEYS):
             out['approx_kl/' + k] = st[_lib.STAT_APPROX_KL + 1 + h]
             out['clip_fraction/' + k] = st[_lib.STAT_CLIP_FRACTION + 1 + h]
         out['explained_variance'] = st[_lib.STAT_EXPLAINED_VAR]
+        if joint:                   # the ratio the joint objective clips, over the steps with an action
+            out['approx_kl/joint'] = st[_lib.STAT_JOINT_APPROX_KL]
+            out['clip_fraction/joint'] = st[_lib.STAT_JOINT_CLIP_FRACTION]
         return out
 
     def _upload_hparams(self):
@@ -1244,11 +1257,13 @@ class DotaOptimizer:
         batch.wait(batch.old_logp, batch.advantages, batch.returns, batch.old_values, valid, *batch.masks.values(),
                    *batch.actions.values(), *batch.observations.values())
         # e_clip / entropy_coef / vf_coef / value_clip are read from the device block (_upload_hparams); padded tokens
-        # (valid = False) count for nothing under mask_padding
+        # (valid = False) count for nothing under mask_padding; the policy ratio is fixed per optimizer, so a captured
+        # graph of the step keeps it
         out, n_actions, d_packed, d_tu, _ = ops.ppo_loss_packed(
             packed, target_unit, [batch.masks[k] for k in keys], [batch.actions[k] for k in keys],
             batch.old_logp, batch.advantages, batch.returns, self.e_clip, self.entropy_coef, self.vf_coef,
-            hparams=self._hparams_dev, old_value=batch.old_values, stats=self._ppo_stats, valid=valid)
+            hparams=self._hparams_dev, old_value=batch.old_values, stats=self._ppo_stats, valid=valid,
+            joint=self.policy_ratio == 'joint')
         self._n_actions[:5].copy_(n_actions)
         torch.autograd.backward([packed, target_unit], [d_packed, d_tu])                                # :672
         # drop every reference into this step's autograd graph before the gradient finish: it holds the saved activations
@@ -1592,10 +1607,11 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          pretrained_model, mq_prefetch_count, log_dir, entropy_coef, vf_coef, run_local,
          hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
          value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
-         mask_padding=False, pack_sequences=False):
+         mask_padding=False, pack_sequences=False, policy_ratio='per_head'):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
-                       mask_padding=mask_padding, pack_sequences=pack_sequences)         # before any process-group setup
+                       mask_padding=mask_padding, pack_sequences=pack_sequences,
+                       policy_ratio=policy_ratio)                                         # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -1606,7 +1622,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         run_local=run_local, hidden_size=hidden_size, cell=cell, num_layers=num_layers, gamma=gamma,
         gae_lambda=gae_lambda, clip_range=clip_range, max_grad_norm=max_grad_norm, value_clip=value_clip,
         advantage_estimator=advantage_estimator, vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip,
-        num_minibatches=num_minibatches, mask_padding=mask_padding, pack_sequences=pack_sequences)
+        num_minibatches=num_minibatches, mask_padding=mask_padding, pack_sequences=pack_sequences,
+        policy_ratio=policy_ratio)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -1621,8 +1638,8 @@ def default_log_dir():
 def build_arg_parser():
     """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell``, ``--num-layers`` and the PPO
     settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm``, ``--value-clip``,
-    ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches``, ``--mask-padding`` and
-    ``--pack-sequences``."""
+    ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches``, ``--mask-padding``,
+    ``--pack-sequences`` and ``--policy-ratio``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -1659,6 +1676,9 @@ def build_arg_parser():
     p.add_argument("--pack-sequences", action="store_true",
                    help="pack the rollouts' last partial chunks into shared sequences with recurrent-state resets, so "
                         "padding is not trained on (needs --mask-padding)")
+    p.add_argument("--policy-ratio", type=str, choices=POLICY_RATIOS, default='per_head',
+                   help="'joint' clips one PPO ratio per step, of the whole hierarchical action, instead of one per head "
+                        "(reference: per_head)")
     return p
 
 
@@ -1673,6 +1693,6 @@ if __name__ == '__main__':
              num_layers=args.num_layers, gamma=args.gamma, gae_lambda=args.gae_lambda, clip_range=args.clip_range,
              max_grad_norm=args.max_grad_norm, value_clip=args.value_clip, advantage_estimator=args.advantage_estimator,
              vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip, num_minibatches=args.num_minibatches,
-             mask_padding=args.mask_padding, pack_sequences=args.pack_sequences)
+             mask_padding=args.mask_padding, pack_sequences=args.pack_sequences, policy_ratio=args.policy_ratio)
     except KeyboardInterrupt:
         pass

@@ -302,12 +302,14 @@ int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEADS], const i
  *       6 clip fraction (share of action rows with |r-1| > e_clip), the same mean; 7..11 per head;
  *       12 explained variance 1 - Var(ret - v) / Var(ret) over all N tokens, padding included (NaN if Var(ret) = 0;
  *          over the valid tokens only under dc_ppo_loss_fwd_bwd_masked);
- *       13..15 zero.
+ *       13..15 zero (dc_ppo_loss_fwd_bwd_joint: 13, 14 see there).
  */
 #define DC_PPO_STATS_SLOTS 16
 #define DC_STAT_APPROX_KL 0
 #define DC_STAT_CLIP_FRACTION 6
 #define DC_STAT_EXPLAINED_VAR 12
+#define DC_STAT_JOINT_APPROX_KL 13
+#define DC_STAT_JOINT_CLIP_FRACTION 14
 int dc_ppo_loss_fwd_bwd_dev(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
                             const uint8_t *const masks[DC_NUM_HEADS],
                             const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
@@ -337,6 +339,30 @@ int dc_ppo_loss_fwd_bwd_masked(const float *const logits[DC_NUM_HEADS], const in
                                float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
                                float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
                                void *workspace, dc_stream_t stream);
+
+/* Same arguments as dc_ppo_loss_fwd_bwd_masked (valid may be NULL), with the PPO ratio of the whole hierarchical action
+ * instead of one ratio per head (no counterpart in the reference, optimizer.py:621-650).  Per token t that counts, S_t is
+ * the set of heads with an action row at t and T_a the number of counting tokens with S_t not empty:
+ *   log r_t = sum over h in S_t, in head order, of (logp_new[t,h,a_h] - old_logp[t,h])   (fp32; old_logp of a head not
+ *             in S_t is ignored)
+ *   policy  = -(1/T_a) sum_t min(r_t A_t, clamp(r_t, 1-eps, 1+eps) A_t)                  (0 when T_a = 0)
+ * A_t is normalised as by dc_ppo_loss_fwd_bwd_masked.  d loss / d logp_new[t,h,a_h] is the same for every h in S_t,
+ * -(1/T_a) A_t (g1 + g2 [r_t in range]) r_t with the autograd rules of torch.min and clamp, and reaches the logits
+ * through each head's masked log-softmax.  The entropy term, the value loss (clipped or not), n_actions, the skipping of a
+ * head without action rows and the empty-mask rows are as in dc_ppo_loss_fwd_bwd_masked.
+ *   out: 1 is the joint policy loss (not divided by 5), and 0 also adds it; 9..13 (policy per head) are 0.
+ *   stats: 0..12 as dc_ppo_loss_fwd_bwd_dev (per-head KL / clip fraction of the per-head ratios); 13 the k3 KL and 14 the
+ *          clip fraction of the joint ratio, averaged over the T_a tokens (0 when T_a = 0); 15 zero.
+ * Algorithmic bytes: as dc_ppo_loss_fwd_bwd_masked; the statistics pass also counts T_a.
+ */
+int dc_ppo_loss_fwd_bwd_joint(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                              const uint8_t *const masks[DC_NUM_HEADS],
+                              const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
+                              const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                              const float *old_value, const uint8_t *valid, int64_t N, const double *hparams,
+                              float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                              float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
+                              void *workspace, dc_stream_t stream);
 
 /* Log-prob of the taken action per head, [N,5] dense (0 where the head took no action):
  * the no-grad half of experiences_from_rollout (optimizer.py:387-390). */
