@@ -107,7 +107,10 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(float *__restrict__ para
     __syncthreads();
     if (s_nan) return;                                   // ValueError path: leave parameters untouched
     const float coef = s_coef;
-    const float beta1 = (float)beta1_d, beta2 = (float)beta2_d, eps = (float)eps_d;
+    // 1 - beta rounded from float64, as torch receives it (a Python float): 1 - (float)0.999 in fp32 would be 1.3e-5
+    // off 0.001 and move the first updates of a fresh state by ~6e-6 relative
+    const float beta2 = (float)beta2_d, eps = (float)eps_d;
+    const float one_m_beta1 = (float)(1.0 - beta1_d), one_m_beta2 = (float)(1.0 - beta2_d);
     const int64_t stride = (int64_t)gridDim.x * kThreads;
     // per-tensor scalars once per block (thread p -> tensor p): the float64 pow() calls are ~100 instructions each and were
     // being repeated by every thread for every tensor (0.10 ms for a 1 MB parameter set)
@@ -127,8 +130,8 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(float *__restrict__ para
         for (int64_t i = lo + (int64_t)blockIdx.x * kThreads + threadIdx.x; i < hi; i += stride) {
             const float gi = g[i] * coef;
             g[i] = gi;                                   // clipped gradient stays visible in .grad
-            const float mi = m[i] + (gi - m[i]) * (1.0f - beta1);          // exp_avg.lerp_(grad, 1-beta1)
-            const float vi = v[i] * beta2 + (1.0f - beta2) * gi * gi;      // mul_(beta2).addcmul_(g, g, 1-beta2)
+            const float mi = m[i] + (gi - m[i]) * one_m_beta1;             // exp_avg.lerp_(grad, 1-beta1)
+            const float vi = v[i] * beta2 + one_m_beta2 * gi * gi;         // mul_(beta2).addcmul_(g, g, 1-beta2)
             m[i] = mi;
             v[i] = vi;
             const float denom = sqrtf(vi) / bc2_sqrt + eps;

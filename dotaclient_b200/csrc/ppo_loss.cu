@@ -9,7 +9,7 @@
 //   :672      loss.backward() down to d loss / d logits and d loss / d value
 //
 // Two launches.  (1) ppo_stats_kernel: per-head action-row counts and sum / sum-of-squares of
-// the raw advantage (float64) -- the counts are needed as divisors by every gradient.
+// the raw advantage (float64) -- the counts are needed as divisors by every gradient -- and the first counting token.
 // (2) ppo_loss_kernel: one thread per token; a 128-token tile of every head's logits / masks /
 // actions is staged through shared memory with coalesced 16-byte loads (rows are 12..160 bytes,
 // so per-thread row reads from global would waste most of every sector), the tile is overwritten
@@ -90,6 +90,7 @@ struct Workspace {
     float adv_mean, adv_std;
     unsigned long long n_joint;      // joint ratio: T_a, the tokens that count with at least one action row
     double st_joint[kJointStats];    // joint ratio: sums over the T_a tokens of its k3 KL and of its clip flag
+    unsigned long long first_rev;    // N - (index of the first token that counts); 0 when no token counts
 };
 static_assert(sizeof(Workspace) <= DC_PPO_WORKSPACE_BYTES, "workspace too small");
 
@@ -175,13 +176,16 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
     __shared__ __align__(16) uint8_t s_act[kByteTile];
     __shared__ double s_red[kTile / 32];
     __shared__ bool s_last;
+    __shared__ int s_first;
     const int64_t t0 = (int64_t)blockIdx.x * kTile;
     const int count = (int)min((int64_t)kTile, N - t0);
+    if (threadIdx.x == 0) s_first = kTile;
 #pragma unroll
     for (int h = 0; h < kHeads; ++h) stage_bytes(s_act + byte_off(h), hp.actions[h] + t0 * head_n(h), count * head_n(h));
     __syncthreads();
     // a token that does not count (valid = 0) adds nothing to the sums and the action counts
     const bool live = threadIdx.x < count && (valid == nullptr || valid[t0 + threadIdx.x] != 0);
+    if (live) atomicMin(&s_first, (int)threadIdx.x);
     double a = 0.0;
     if (live) a = (double)adv[t0 + threadIdx.x];
     int has[kHeads];
@@ -207,6 +211,7 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
         atomicAdd(&ws->adv_sq, sq);
         atomicAdd(&ws->n_valid, (unsigned long long)n_live);
         if (kJoint && n_joint) atomicAdd(&ws->n_joint, (unsigned long long)n_joint);
+        if (s_first < kTile) atomicMax(&ws->first_rev, (unsigned long long)(N - (t0 + s_first)));
 #pragma unroll
         for (int h = 0; h < kHeads; ++h)
             if (tot[h]) atomicAdd(&ws->cnt[h], tot[h]);
@@ -532,8 +537,17 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
                 vl = d * d;                                                 // optimizer.py:660
             }
             dvalue[(t0 + t) * hp.ld_dv] = vf_coef > 0.f ? vf_coef * g / (float)ws->n_valid : 0.f;   // N_v, or N unmasked
-            s_tok[kTokD][t] = d;
-            s_tok[kTokR][t] = r;
+            // the explained-variance sums run on values shifted by the first counting token's: constant returns then sum
+            // to exactly zero variance (unshifted, the rounding of the float64 sums of r^2 leaves a variance of either
+            // sign), and near-constant ones keep their digits; r - shift is exact for r within a factor 2 of the shift
+            float shift_r = 0.f, shift_d = 0.f;
+            if (stats) {
+                const int64_t tf = N - (int64_t)ws->first_rev;    // this token counts, so first_rev > 0
+                shift_r = ret[tf];
+                shift_d = shift_r - value[tf * hp.ld_v];
+            }
+            s_tok[kTokD][t] = d - shift_d;
+            s_tok[kTokR][t] = r - shift_r;
         }
     }
     if (kSelectOnly) return;
@@ -628,8 +642,8 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             }
             stats[DC_STAT_APPROX_KL] = used ? kl_sum / (float)used : 0.f;
             stats[DC_STAT_CLIP_FRACTION] = used ? clip_sum / (float)used : 0.f;
-            // 1 - Var(ret - v) / Var(ret) over the tokens that count (population variances); NaN when the returns are
-            // constant
+            // 1 - Var(ret - v) / Var(ret) over the tokens that count (population variances, from the shifted sums);
+            // NaN when the returns are constant
             const double n = n_tok_d;
             const double md = w->st[kStD] / n, mr = w->st[kStR] / n;
             const double var_d = w->st[kStD2] / n - md * md, var_r = w->st[kStR2] / n - mr * mr;
