@@ -42,8 +42,11 @@ SIGNATURES = {
     "dc_env_bwd": (_i32, [_vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp]),
     "dc_unit_wgrad_routed": (_i32, [_vp, _vp, _i32, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp]),
     "dc_unit_dgrad_fused": (_i32, [_vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp]),
+    "dc_unit_dgrad_fused_mask": (_i32, [_vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _i32, _vp,
+                                        _vp]),
     "dc_gemm_unit_max": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _vp, _i64, _i32, _vp]),
     "dc_unit_embed_fwd": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i64, _i32, _vp]),
+    "dc_unit_embed_fwd_mask": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i64, _i32, _vp]),
     "dc_target_unit_q_fwd": (_i32, [_vp, _i32, _c.c_void_p * 6, _vp, _vp, _vp, _i64, _vp]),
     "dc_target_unit_q_bwd": (_i32, [_vp, _c.c_void_p * 6, _vp, _vp, _vp, _i32, _i64, _vp]),
     "dc_ppo_loss_fwd_bwd": (_i32, [_ptr5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _ptr5, _vp, _vp,

@@ -56,8 +56,8 @@ def _wgrad_workspace(No, Ni, device):
 #   * the max-pool: one launch per group (dc_unit_embed_fwd) whose producers generate `basic` into the embedding GEMM's operand
 #     ring and whose epilogue keeps max + arg-max per token and channel; for the 1-unit groups the plain epilogue writes the
 #     group's slot of the pre-rnn row.  The enemy-tower group runs nothing in forward because policy.py:127 takes that slot's
-#     maximum from the enemy non-heroes.  `basic` of groups 0-4 is stored by the same launch only when a backward may follow:
-#     the weight gradients below read it;
+#     maximum from the enemy non-heroes.  `basic` of groups 0-4 and its ReLU mask (16 bytes per unit row) are stored by the same
+#     launch only when a backward may follow: the weight gradients below read `basic`, the data gradient the mask;
 #   * the target-unit head, which is linear in it: logits[n,u] = <att[n] W_g, basic[n,u]> + <att[n], b_g>  (TargetUnit below,
 #     `basic` regenerated from the raw features in the head kernels).
 # In backward the embedding's gradient d_emb[n,u,:] has two sources -- the head (rank 1: dlogits[n,u] * att[n,:], arrives first) and the
@@ -66,8 +66,9 @@ def _wgrad_workspace(No, Ni, device):
 # dense [N, 40, 128] tensor at all:
 #   dW_g  = R^T basic_g  (dc_unit_wgrad_routed: R generated in the dY^T producer)  +  att^T s_g   (one token-level GEMM for all groups,
 #           s_g = sum_u dlogits_u basic_u from dc_target_unit_q_bwd; its bias block gives the head's share of db_g)
-#   dW_b += (relu'(.) (R + dlogits x att) W_g)^T units   (dc_unit_dgrad_fused: d_emb generated in the producers, the ReLU mask
-#           recomputed and dW_b reduced in the epilogue) -- d_basic never exists either.
+#   dW_b += (relu'(.) (R + dlogits x att) W_g)^T units   (dc_unit_dgrad_fused_mask: d_emb generated in the producers, the ReLU mask
+#           the forward stored -- recomputed for the enemy towers, which have no forward launch -- and dW_b as a second tensor-core
+#           product from the masked accumulator) -- d_basic never exists either.
 
 
 def _ptr(t, float_offset=0):
@@ -85,7 +86,7 @@ class UnitEncoder(torch.autograd.Function):
     maxima slot 5 (enemy towers) is a copy of slot 3 (enemy non-heroes): the reference's ``policy.py:127``.
     ``link`` (a dict) receives the raw unit features, the basic layer's and the embedding weights for the target-unit head.
     ``wait``: see ``unit_encoder``.  ``need_grad``: a backward may follow, so the basic activations of groups 0-4 are stored
-    for the weight gradients (without it nothing of the basic layer reaches HBM).
+    for the weight gradients and their ReLU masks for the data gradient (without it nothing of the basic layer reaches HBM).
     """
 
     @staticmethod
@@ -113,7 +114,7 @@ class UnitEncoder(torch.autograd.Function):
             wait(env2)
         with PROFILE.span("env_fwd", 1, 4 * N * (3 + C)):
             _lib.check(lib.dc_env_fwd(env2.data_ptr(), w_e.data_ptr(), b_e.data_ptr(), xcat.data_ptr(), XCAT, N, st), "dc_env_fwd")
-        basics = []
+        basics, masks = [], []
         for g, n_u in enumerate(UNITS):
             R = N * n_u
             if wait is not None:                      # this group's observations may still be in flight over PCIe
@@ -123,26 +124,28 @@ class UnitEncoder(torch.autograd.Function):
             # basic layer + embedding GEMM in one launch: the max-pool epilogue, or for one unit the embedding IS the maximum
             # and goes straight into its slot
             basic = torch.empty((R, C), dtype=torch.float32, device=dev) if need_grad else None
+            mask = torch.empty((R, 4), dtype=torch.int32, device=dev) if need_grad else None     # bit j/4 of word j%4 of row r: basic[r, j] > 0
             copy = _ptr(xcat, 6 * C) if g == 3 else None
             am = argmax[g].data_ptr() if n_u > 1 else None
-            nbytes = 4 * (R * 12 + (R * C if need_grad else 0) + C * C + N * C) + (N * C if n_u > 1 else 0)
+            nbytes = 4 * (R * 12 + (R * C + R * 4 if need_grad else 0) + C * C + N * C) + (N * C if n_u > 1 else 0)
             with PROFILE.span("gemm_unit_max" if n_u > 1 else "gemm_tf32x3", 1, nbytes):
-                _lib.check(lib.dc_unit_embed_fwd(units[g].data_ptr(), w_b.data_ptr(), b_b.data_ptr(), _lib.ptr(basic),
-                                                 weights[g].data_ptr(), biases[g].data_ptr(), _ptr(xcat, (g + 1) * C), copy, XCAT,
-                                                 am, N, n_u, st), "dc_unit_embed_fwd")
+                _lib.check(lib.dc_unit_embed_fwd_mask(units[g].data_ptr(), w_b.data_ptr(), b_b.data_ptr(), _lib.ptr(basic), _lib.ptr(mask),
+                                                      weights[g].data_ptr(), biases[g].data_ptr(), _ptr(xcat, (g + 1) * C), copy, XCAT,
+                                                      am, N, n_u, st), "dc_unit_embed_fwd_mask")
             basics.append(basic)
+            masks.append(mask)
         link["units"], link["w_b"], link["b_b"] = units, w_b, b_b
         link["weights"], link["biases"] = weights, biases
         ctx.N = N
         ctx.lead = lead
-        ctx.save_for_backward(argmax, *units, *basics, *weights, env2, xcat, w_b, b_b)
+        ctx.save_for_backward(argmax, *units, *basics, *weights, env2, xcat, w_b, b_b, *masks)
         return xcat.view(*lead, XCAT)
 
     @staticmethod
     def backward(ctx, d_xcat):
         saved = ctx.saved_tensors
         argmax, units, basics, weights, env2, xcat = saved[0], saved[1:7], saved[7:12], saved[12:18], saved[18], saved[19]
-        w_b, b_b = saved[20], saved[21]
+        w_b, b_b, masks = saved[20], saved[21], saved[22:27]
         N = ctx.N
         lib = _lib.load()
         st = _lib.stream_ptr()
@@ -178,12 +181,14 @@ class UnitEncoder(torch.autograd.Function):
                     _lib.check(lib.dc_gemm_wgrad_tf32x3(dx, XCAT, basics[g].data_ptr(), C, R, C, C, dw_all[g].data_ptr(), C,
                                                         db_all[g].data_ptr(), 0, ws_w.data_ptr(), st), "dc_gemm_wgrad_tf32x3")
             wt = weights[g].t().contiguous()
-            with PROFILE.span("unit_dgrad_fused", 2, N * (4 * C + C) * (1 if routed else 0) + 4 * R * 12 + (4 * N * (C + n_u) if dl is not None else 0)):
-                _lib.check(lib.dc_unit_dgrad_fused(dx, dx2, XCAT, argmax[g].data_ptr() if (routed and n_u > 1) else None,
-                                                   None if dl is None else _ptr(dl, off), MAX_UNITS, None if att is None else att.data_ptr(),
-                                                   wt.data_ptr(), units[g].data_ptr(), w_b.data_ptr(), b_b.data_ptr(), N, n_u,
-                                                   dw_b.data_ptr(), db_b.data_ptr(), 1 if g > 0 else 0, ws_b.data_ptr(), st),
-                           "dc_unit_dgrad_fused")
+            mask = masks[g] if routed else None           # the enemy towers have no forward launch: their mask is recomputed
+            with PROFILE.span("unit_dgrad_fused", 2, N * (4 * C + C) * (1 if routed else 0) + 4 * R * 12 + (16 * R if routed else 0)
+                              + (4 * N * (C + n_u) if dl is not None else 0)):
+                _lib.check(lib.dc_unit_dgrad_fused_mask(dx, dx2, XCAT, argmax[g].data_ptr() if (routed and n_u > 1) else None,
+                                                        None if dl is None else _ptr(dl, off), MAX_UNITS, None if att is None else att.data_ptr(),
+                                                        wt.data_ptr(), units[g].data_ptr(), _lib.ptr(mask), w_b.data_ptr(), b_b.data_ptr(),
+                                                        N, n_u, dw_b.data_ptr(), db_b.data_ptr(), 1 if g > 0 else 0, ws_b.data_ptr(), st),
+                           "dc_unit_dgrad_fused_mask")
         if dl is not None:
             # the head's share of every dW_g and db_g in ONE token-level product: att^T [s_0 | ... | s_5 | sum_u dlogits]
             dw_head = torch.empty((C, QW), dtype=torch.float32, device=dev)

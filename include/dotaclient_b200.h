@@ -214,6 +214,11 @@ int dc_gemm_unit_max(const float *basic, const float *w, const float *bias, floa
  * xmax_copy NULL.  units, basic_out, w, bias, xmax, xmax_copy 16-byte aligned; ld_x >= 128, a multiple of 4. */
 int dc_unit_embed_fwd(const float *units, const float *w_b, const float *b_b, float *basic_out, const float *w, const float *bias,
                       float *xmax, float *xmax_copy, int ld_x, uint8_t *argmax, int64_t n_tokens, int n_units, dc_stream_t stream);
+/* dc_unit_embed_fwd that also stores the basic layer's ReLU mask when mask_out is not NULL: mask_out[row*4 + c%4] bit c/4
+ * = (basic[row][c] > 0), 16 bytes per unit row ([N*n_units][4] words, 16-byte aligned) -- what dc_unit_dgrad_fused_mask reads. */
+int dc_unit_embed_fwd_mask(const float *units, const float *w_b, const float *b_b, float *basic_out, uint32_t *mask_out, const float *w,
+                           const float *bias, float *xmax, float *xmax_copy, int ld_x, uint8_t *argmax, int64_t n_tokens, int n_units,
+                           dc_stream_t stream);
 /* Target-unit head without the embedding (policy.py:144-153): logits[n,u] = <q[n, g*128 ..], basic_g[n,u,:]> + q[n, 768+g]
  * with q = att [W_0|...|W_5|b_0..b_5] (ld_q >= 896) and basic_g = relu(units[g] W_b^T + b_b) rebuilt from the raw unit
  * features units[g] [N*units_g, 12] (units 1,5,16,16,1,1; 16-byte aligned).  Backward: s[n, g*128 + j] = sum_u dlogits[n,u]
@@ -235,6 +240,9 @@ int dc_target_unit_q_bwd(const float *dlogits, const float *const units[6], cons
  *                         the forward value); dlogits (already offset to the group's first unit) and att [N,128] are NULL when the
  *                         head was not used; d_xmax NULL = no routing (the enemy-tower layer, policy.py:127).  n_units = 1, 5 or
  *                         16; units, att, d_xmax 16-byte aligned; workspace: dc_unit_basic_bwd_workspace_bytes().
+ *   dc_unit_dgrad_fused_mask  the same with the ReLU mask read from `mask` (the words dc_unit_embed_fwd_mask stored for these
+ *                         unit rows, 16-byte aligned) instead of recomputed; mask NULL = dc_unit_dgrad_fused.  dW_b / db_b are
+ *                         bitwise the same either way.
  * The head's share of dW / db is a token-level product (att^T s, s from dc_target_unit_q_bwd) the caller adds. */
 int dc_unit_wgrad_routed(const float *d_xmax, const float *d_xmax2, int ld_dx, const uint8_t *argmax, const float *basic,
                          int64_t n_tokens, int n_units, float *dW, float *db, void *workspace, dc_stream_t stream);
@@ -242,6 +250,10 @@ int dc_unit_dgrad_fused(const float *d_xmax, const float *d_xmax2, int ld_dx, co
                         int ld_dl, const float *att, const float *w_t, const float *units, const float *w_b,
                         const float *b_b, int64_t n_tokens, int n_units, float *dw_b, float *db_b, int accumulate,
                         void *workspace, dc_stream_t stream);
+int dc_unit_dgrad_fused_mask(const float *d_xmax, const float *d_xmax2, int ld_dx, const uint8_t *argmax, const float *dlogits,
+                             int ld_dl, const float *att, const float *w_t, const float *units, const uint32_t *mask, const float *w_b,
+                             const float *b_b, int64_t n_tokens, int n_units, float *dw_b, float *db_b, int accumulate,
+                             void *workspace, dc_stream_t stream);
 
 /* ---- fused PPO loss + gradient ----------------------------------------------------------
  * Replaces optimizer.py:587-589 (advantage normalisation) and :621-665 (masked log-softmax x5,
