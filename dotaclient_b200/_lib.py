@@ -59,6 +59,9 @@ SIGNATURES = {
                                           _vp, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "dc_ppo_loss_fwd_bwd_joint": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
                                          _vp, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "dc_value_norm_stats": (_i32, [_vp, _vp, _i64, _vp, _vp]),
+    "dc_value_denorm": (_i32, [_vp, _i64, _i64, _f64, _f64, _vp, _vp]),
+    "dc_value_head_rescale": (_i32, [_vp, _i64, _vp, _f64, _f64, _f64, _f64, _vp]),
     "dc_selected_logp": (_i32, [_ptr5, _ptr5, _ptr5, _i64, _vp, _vp]),
     "dc_select_actions": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _vp, _i64, _vp, _vp, _vp]),
     "dc_grad_flags": (_i32, [_vp, _i64, _vp, _i32, _vp, _vp]),
@@ -74,6 +77,7 @@ LOSS_SLOTS = 16
 # the device hyper-parameter block of the `_dev` entry points (fp64, DC_HP_* in include/dotaclient_b200.h)
 HPARAM_SLOTS = 8
 HP_LR, HP_E_CLIP, HP_ENTROPY_COEF, HP_VF_COEF, HP_MAX_GRAD_NORM, HP_VALUE_CLIP = range(6)
+HP_VALUE_NORM_MEAN, HP_VALUE_NORM_STD = 6, 7       # value normalisation (mu, sigma); sigma 0 = off
 # the PPO diagnostics written by dc_ppo_loss_fwd_bwd_dev (DC_STAT_* in include/dotaclient_b200.h)
 PPO_STATS_SLOTS = 16
 STAT_APPROX_KL, STAT_CLIP_FRACTION, STAT_EXPLAINED_VAR = 0, 6, 12

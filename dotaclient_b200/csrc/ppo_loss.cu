@@ -32,6 +32,11 @@
 // the joint log-ratio; (2) every head's dlogits row from the joint ratio's gradient.  Entropy and value terms are per head,
 // as in the default objective.
 //
+// Value normalisation (PopArt): when hparams[DC_HP_VALUE_NORM_STD] = sigma > 0 the value head's output is in normalised
+// units, and every raw value target r (and, for the clipped value loss, every raw old value) is read as
+// fp32((r - mu) / sigma), computed in float64.  The value loss, dvalue and the explained-variance sums then run in
+// normalised units.  No extra bytes; slot 7 = 0 runs the plain arithmetic.
+//
 // Algorithmic HBM bytes per token: logits 260 + masks 65 + actions 65 + old 20 + adv/ret/value 12
 // read, dlogits 260 + dvalue 4 written = 686 (+ 69 for the statistics pass, + 4 for the old value when the value loss
 // is clipped, + 1 in each pass for `valid` when given).  The joint ratio reads and writes the same bytes.
@@ -154,6 +159,11 @@ __device__ __forceinline__ void stage_bytes(uint8_t *dst, const uint8_t *__restr
     } else {
         for (int idx = threadIdx.x; idx < total; idx += kTile) dst[idx] = src[idx];
     }
+}
+
+// (x - mu) / sigma in float64, rounded once to fp32: a raw value target in the units of a normalised value head
+__device__ __forceinline__ float vn_normalise(float x, double mu, double sigma) {
+    return (float)__ddiv_rn(__dsub_rn((double)x, mu), sigma);
 }
 
 template <typename T>
@@ -427,12 +437,16 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
 
     // hyper-parameters from the device block when given, rounded to the types of the scalar arguments
     float value_clip = 0.f;
+    double vn_mu = 0.0, vn_sigma = 0.0;     // value normalisation: sigma > 0 turns it on
     if (!kSelectOnly && hparams) {
         e_clip = (float)hparams[DC_HP_E_CLIP];
         entropy_coef = (float)hparams[DC_HP_ENTROPY_COEF];
         vf_coef = (float)hparams[DC_HP_VF_COEF];
         value_clip = (float)hparams[DC_HP_VALUE_CLIP];
+        vn_mu = hparams[DC_HP_VALUE_NORM_MEAN];
+        vn_sigma = hparams[DC_HP_VALUE_NORM_STD];
     }
+    const bool vnorm = vn_sigma > 0.0;
     const bool clip_value = old_value != nullptr && value_clip > 0.f;
 
     const int64_t t0 = (int64_t)blockIdx.x * kTile;
@@ -518,13 +532,15 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         } else if (!use) {              // masked out: zero gradient rows (head_token with a count of 0), zero dvalue
             dvalue[(t0 + t) * hp.ld_dv] = 0.f;
         } else {
-            const float v = value[(t0 + t) * hp.ld_v], r = ret[t0 + t];
+            // under value normalisation the head's output v is in normalised units: the raw target (and the raw old value)
+            // are brought to them here, in float64 and rounded once; x - 0 and x / 1 are exact, so (0, 1) changes no bit
+            const float v = value[(t0 + t) * hp.ld_v], r = vnorm ? vn_normalise(ret[t0 + t], vn_mu, vn_sigma) : ret[t0 + t];
             const float d = r - v;
             float g = v - r;                                                // d value_loss / d v, up to vf_coef / N
             if (clip_value) {
                 // PPO2: max((v - R)^2, (v_old + clip(v - v_old, -eps, eps) - R)^2); autograd of torch.maximum (ties split
                 // the gradient in half) and of clamp (passes it inside [-eps, eps])
-                const float vo = old_value[t0 + t];
+                const float vo = vnorm ? vn_normalise(old_value[t0 + t], vn_mu, vn_sigma) : old_value[t0 + t];
                 const float dv = v - vo;
                 const float dc = (vo + fminf(fmaxf(dv, -value_clip), value_clip)) - r;
                 const float l1 = d * d, l2 = dc * dc;
@@ -543,7 +559,7 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             float shift_r = 0.f, shift_d = 0.f;
             if (stats) {
                 const int64_t tf = N - (int64_t)ws->first_rev;    // this token counts, so first_rev > 0
-                shift_r = ret[tf];
+                shift_r = vnorm ? vn_normalise(ret[tf], vn_mu, vn_sigma) : ret[tf];
                 shift_d = shift_r - value[tf * hp.ld_v];
             }
             s_tok[kTokD][t] = d - shift_d;

@@ -438,14 +438,62 @@ def rnn_sequence(x_tm, w_ih, w_hh, b_ih, b_hh, h0, c0, cell, reset=None):
 
 
 # --------------------------------------------------------------------------------------------- PPO loss
-def hparam_block(device, lr=0.0, e_clip=0.0, entropy_coef=0.0, vf_coef=0.0, max_grad_norm=0.0, value_clip=None):
+def hparam_block(device, lr=0.0, e_clip=0.0, entropy_coef=0.0, vf_coef=0.0, max_grad_norm=0.0, value_clip=None,
+                 value_norm=None):
     """A device hyper-parameter block (``_lib.HPARAM_SLOTS`` fp64) holding the given values, for the ``hparams=``
-    argument of ``ppo_loss_fwd_bwd`` / ``ppo_loss_packed`` / ``grad_finish``."""
+    argument of ``ppo_loss_fwd_bwd`` / ``ppo_loss_packed`` / ``grad_finish``.  ``value_norm=(mu, sigma)`` makes the loss
+    normalise the raw value targets as ``(r - mu) / sigma`` (sigma > 0); None leaves slots 6 and 7 at 0 (off)."""
     vals = [0.0] * _lib.HPARAM_SLOTS
     vals[_lib.HP_LR], vals[_lib.HP_E_CLIP], vals[_lib.HP_ENTROPY_COEF] = float(lr), float(e_clip), float(entropy_coef)
     vals[_lib.HP_VF_COEF], vals[_lib.HP_MAX_GRAD_NORM] = float(vf_coef), float(max_grad_norm)
     vals[_lib.HP_VALUE_CLIP] = float(value_clip or 0.0)
+    if value_norm is not None:
+        vals[_lib.HP_VALUE_NORM_MEAN], vals[_lib.HP_VALUE_NORM_STD] = float(value_norm[0]), float(value_norm[1])
     return torch.tensor(vals, dtype=torch.float64, device=device)
+
+
+# --------------------------------------------------------------------------------------------- value normalisation
+def value_norm_stats(x, valid=None):
+    """``[count, sum x, sum x^2]`` (fp64 device tensor, no sync) over the elements of ``x`` (fp32) where ``valid`` (bool,
+    same number of elements, or None: all) is True -- ``dc_value_norm_stats``, bitwise reproducible."""
+    _need_cuda(x, valid)
+    x = _f32c(x).reshape(-1)
+    if valid is not None:
+        valid = _u8(valid).reshape(-1)
+        assert valid.numel() == x.numel(), "valid has %d elements for %d values" % (valid.numel(), x.numel())
+    out = torch.empty(3, dtype=torch.float64, device=x.device)
+    with PROFILE.span("value_norm_stats", 1, 4 * x.numel() + (0 if valid is None else x.numel())):
+        _lib.check(_lib.load().dc_value_norm_stats(x.data_ptr(), _lib.ptr(valid), x.numel(), out.data_ptr(),
+                                                   _lib.stream_ptr()), "dc_value_norm_stats")
+    return out
+
+
+def value_denorm(v, mu, sigma):
+    """``fp32(mu + sigma * v)`` computed in float64 (``dc_value_denorm``): a contiguous fp32 tensor of ``v``'s shape.
+    ``v`` may be a strided view whose elements lie at one stride, such as the value column of the packed head GEMM."""
+    _need_cuda(v)
+    flat = v.detach().reshape(-1)
+    if flat.dtype != torch.float32:
+        flat = flat.float()
+    n = flat.numel()
+    ld = flat.stride(0) if n > 1 else 1
+    out = torch.empty(v.shape, dtype=torch.float32, device=v.device)
+    with PROFILE.span("value_denorm", 1, 8 * n):
+        _lib.check(_lib.load().dc_value_denorm(flat.data_ptr(), ld, n, float(mu), float(sigma), out.data_ptr(),
+                                               _lib.stream_ptr()), "dc_value_denorm")
+    return out
+
+
+def value_head_rescale(weight, bias, old, new):
+    """The POP step in place on a value head's fp32 ``weight`` (contiguous, any shape) and ``bias`` (one element):
+    ``sigma v + mu`` is preserved when the statistics move from ``old = (mu, sigma)`` to ``new``
+    (``dc_value_head_rescale``)."""
+    _need_cuda(weight, bias)
+    assert weight.dtype == torch.float32 and bias.dtype == torch.float32 and weight.is_contiguous() and bias.numel() == 1
+    with PROFILE.span("value_head_rescale", 1, 8 * (weight.numel() + 1)):
+        _lib.check(_lib.load().dc_value_head_rescale(weight.data_ptr(), weight.numel(), bias.data_ptr(), float(old[0]),
+                                                     float(old[1]), float(new[0]), float(new[1]), _lib.stream_ptr()),
+                   "dc_value_head_rescale")
 
 
 def _ppo_dev_args(hparams, old_value, stats, N, dev, valid=None, joint=False):

@@ -385,12 +385,17 @@ POLICY_RATIOS = ('per_head', 'joint')
 
 def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
                        vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False, pack_sequences=False,
-                       policy_ratio='per_head'):
+                       policy_ratio='per_head', value_norm=False, value_norm_decay=0.99):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
     vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool,
-    pack_sequences a bool that is True only with mask_padding and policy_ratio one of ``POLICY_RATIOS``.  NaN fails every
-    check."""
+    pack_sequences a bool that is True only with mask_padding, policy_ratio one of ``POLICY_RATIOS``, value_norm a bool
+    and 0 <= value_norm_decay < 1.  NaN fails every check."""
+    if not isinstance(value_norm, bool):
+        raise ValueError("value_norm=%r: must be True or False" % (value_norm,))
+    if isinstance(value_norm_decay, bool) or not isinstance(value_norm_decay, numbers.Real) \
+            or not 0.0 <= float(value_norm_decay) < 1.0:
+        raise ValueError("value_norm_decay=%r: the decay of the value statistics must be in [0, 1)" % (value_norm_decay,))
     if not isinstance(policy_ratio, str) or policy_ratio not in POLICY_RATIOS:
         raise ValueError("policy_ratio=%r: must be one of %s" % (policy_ratio, ", ".join(POLICY_RATIOS)))
     if not isinstance(mask_padding, bool):
@@ -422,6 +427,26 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
         raise ValueError("vtrace_rho_clip=%r: the V-trace rho truncation must be > 0" % (vtrace_rho_clip,))
     if not number('vtrace_c_clip', vtrace_c_clip) > 0.0:
         raise ValueError("vtrace_c_clip=%r: the V-trace c truncation must be > 0" % (vtrace_c_clip,))
+
+
+def value_norm_moments(state, min_std):
+    """(mu, sigma) of the value statistics ``state = (m, q, w)`` (float64 EMAs of the target mean and mean square, and
+    their debias weight): (0, 1) while w = 0, else mu = m / w and sigma = max(sqrt(max(q / w - mu^2, 0)), min_std)."""
+    m, q, w = state
+    if w == 0.0:
+        return 0.0, 1.0
+    mu = m / w
+    return mu, max(math.sqrt(max(q / w - mu * mu, 0.0)), min_std)
+
+
+def value_norm_update(state, n, s1, s2, decay):
+    """The value statistics after one batch of ``n`` targets with sum ``s1`` and sum of squares ``s2`` (float64):
+    m <- d m + (1 - d) s1 / n, q <- d q + (1 - d) s2 / n, w <- d w + (1 - d).  ``n`` = 0 leaves ``state`` as it is."""
+    if n <= 0:
+        return state
+    m, q, w = state
+    d = float(decay)
+    return d * m + (1.0 - d) * (s1 / n), d * q + (1.0 - d) * (s2 / n), d * w + (1.0 - d)
 
 
 def check_minibatch_count(num_minibatches, min_seq_per_epoch):
@@ -647,6 +672,9 @@ class DotaOptimizer:
     MODEL_FILENAME_FMT = "model_%09d.pt"
     ADAM_FILENAME_FMT = "adam_%09d.state"         # extension: Adam moments of the same iteration (torch.optim.Adam layout)
     ADAM_FILES_KEPT = 3
+    # extension: the value statistics and the normalised value head of the same iteration (value_norm=True)
+    VALUE_NORM_FILENAME_FMT = "value_norm_%09d.state"
+    VALUE_NORM_MIN_STD = 1e-2       # floor of the value statistics' sigma: bounds the value head's rescale factor
     BUCKET_NAME = 'dotaservice'
     MODEL_HISTOGRAM_FREQ = 128
     MAX_GRAD_NORM = 0.5
@@ -662,15 +690,24 @@ class DotaOptimizer:
                  entropy_coef, vf_coef, run_local, *, hidden_size=256, cell="gru", num_layers=1, mq=None,
                  iterations=100000, rollout_prefetch=0, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1,
                  max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0,
-                 num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head'):
+                 num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False,
+                 value_norm_decay=0.99):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
                              % (num_layers, self.MAX_LAYERS, _lib.MAX_PARAM_TENSORS))
         check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                            vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
-                           mask_padding=mask_padding, pack_sequences=pack_sequences, policy_ratio=policy_ratio)
+                           mask_padding=mask_padding, pack_sequences=pack_sequences, policy_ratio=policy_ratio,
+                           value_norm=value_norm, value_norm_decay=value_norm_decay)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # True: PopArt.  The critic learns (R - mu) / sigma, with (mu, sigma) from running statistics of the value targets
+        # (_value_norm = (m, q, w), updated once per prepared batch); the value head is rescaled at every update so that
+        # sigma v + mu does not move.  policy_base's `value` output is then sigma^-1 (V - mu); prep, the batch, the
+        # published model and agents see V.
+        self.value_norm = value_norm
+        self.value_norm_decay = float(value_norm_decay)
+        self._value_norm = (0.0, 0.0, 0.0)
         # 'joint': the loss clips one PPO ratio per step, of the whole hierarchical action (log r = sum over the sampled
         # heads of logp_new - logp_old), averaged over the steps with an action; 'per_head': the reference's five ratios
         self.policy_ratio = policy_ratio
@@ -731,6 +768,10 @@ class DotaOptimizer:
             # loaded into num_layers=2) sets the layers it has and leaves rnn.*_l1 ... at their seeded initial values; its
             # Adam moments (keyed by parameter index) do not fit the new layout and are not restored (below)
             self.policy_base.load_state_dict(torch.load(pretrained_model, map_location='cpu'), strict=False)
+            if self.checkpoint:
+                # before the data-parallel wrapper broadcasts the weights: the normalised head must be in place
+                self._restore_value_norm(os.path.join(os.path.dirname(pretrained_model),
+                                                      self.VALUE_NORM_FILENAME_FMT % (self.iteration_start - 1)))
 
         self.policy_base.to(self.device)
         self.flat = FlatParameterSpace(self.policy_base, self.device)
@@ -807,6 +848,28 @@ class DotaOptimizer:
         it = torch.tensor([self.iteration_start], dtype=torch.int64, device=self.device)
         dist.broadcast(it, 0)
         self.iteration_start = int(it.item())
+        if self.value_norm:                 # the value statistics (the normalised head travels with the weights)
+            vn = torch.tensor(self._value_norm, dtype=torch.float64, device=self.device)
+            dist.broadcast(vn, 0)
+            self._value_norm = tuple(vn.tolist())
+
+    def _restore_value_norm(self, path):
+        """Resume with ``value_norm``: the statistics and the exact normalised value head from ``path`` (written by
+        ``upload_model`` next to the weights).  Without the file -- e.g. a model trained without the feature -- the
+        statistics start at identity and the head stays as loaded, which is then already in raw units.  Without the feature
+        the file is ignored."""
+        if not os.path.isfile(path):
+            return
+        if not self.value_norm:
+            logger.warning('Ignoring %s: value_norm is off, so the value head stays in the raw units it was published in',
+                           path)
+            return
+        logger.info('Restoring the value statistics and the normalised value head from {}'.format(path))
+        st = torch.load(path, map_location='cpu')
+        self._value_norm = (float(st['m']), float(st['q']), float(st['w']))
+        with torch.no_grad():
+            self.policy_base.affine_value.weight.copy_(st['weight'])
+            self.policy_base.affine_value.bias.copy_(st['bias'])
 
     # -- checkpoints (:287-308, :697-723) --------------------------------------------------------
     @staticmethod
@@ -826,6 +889,13 @@ class DotaOptimizer:
             return
         buffer = io.BytesIO()
         state_dict = {k: v.detach().cpu().clone() for k, v in self.policy_base.state_dict().items()}
+        if self.value_norm:
+            # the published head is the denormalised one, sigma W and sigma b + mu (float64, rounded once): plain Policy
+            # users and agents read raw-scale values, and the state_dict keeps its keys and shapes
+            mu, sigma = self._value_norm_moments()
+            w_n, b_n = state_dict['affine_value.weight'], state_dict['affine_value.bias']
+            state_dict['affine_value.weight'] = (sigma * w_n.double()).float()
+            state_dict['affine_value.bias'] = (sigma * b_n.double() + mu).float()
         torch.save(obj=state_dict, f=buffer)                              # same bytes-format as :705-709
         state_dict_b = buffer.getvalue()
         if self.checkpoint:
@@ -834,9 +904,16 @@ class DotaOptimizer:
             # extension (SURVEY.md 8(f)3): the Adam moments next to the weights, in torch.optim.Adam's own format.  The name
             # does not end in .pt, so the reference's "latest *.pt" scan and its agents never see it.
             torch.save(self.optimizer.state_dict(), os.path.join(self.log_dir, self.ADAM_FILENAME_FMT % version))
-            stale = sorted(f for f in os.listdir(self.log_dir) if re.fullmatch(r'adam_\d{9}\.state', f))[:-self.ADAM_FILES_KEPT]
-            for f in stale:                                                 # resume only ever needs the newest: bound the disk growth
-                os.remove(os.path.join(self.log_dir, f))
+            side = [r'adam_\d{9}\.state']
+            if self.value_norm:             # the statistics and the exact normalised head, for resume
+                m, q, w = self._value_norm
+                torch.save({'m': m, 'q': q, 'w': w, 'weight': w_n, 'bias': b_n},
+                           os.path.join(self.log_dir, self.VALUE_NORM_FILENAME_FMT % version))
+                side.append(r'value_norm_\d{9}\.state')
+            for pattern in side:            # resume only ever needs the newest: bound the disk growth
+                stale = sorted(f for f in os.listdir(self.log_dir) if re.fullmatch(pattern, f))[:-self.ADAM_FILES_KEPT]
+                for f in stale:
+                    os.remove(os.path.join(self.log_dir, f))
         self.mq.publish_model(msg=state_dict_b, hdr={'version': version})   # :716
 
     # -- experience intake (:314-430) -------------------------------------------------------------
@@ -889,7 +966,12 @@ class DotaOptimizer:
         the zero state.  One that is not ``'terminal'`` is always two segments, and its real segment bootstraps from
         V(s_L), the critic's value of its extra observation row: ONE more single-step forward of batch R' (the number of
         such rollouts) from each one's state after its last step, state buffer slot L_i.  The extra row enters neither the
-        main pass nor the batch.  Without either key in any rollout none of this runs.  Returns the raw device tensors;
+        main pass nor the batch.  Without either key in any rollout none of this runs.
+
+        With ``value_norm`` the values and bootstraps read from the normalised head are denormalised first, so the scans,
+        ``Sequence.values`` and the batch stay in raw units; at the end the value statistics take this batch's targets and
+        the value head is rescaled (``_update_value_norm``).  Data-parallel, that update all-reduces across the ranks, so
+        prep is then a collective: every rank must prepare a batch for each iteration.  Returns the raw device tensors;
         ``experiences_from_rollouts`` / ``batch_from_rollouts`` slice them."""
         S, dev, pol = self.seq_len, self.device, self.policy_base
         R = len(datas)
@@ -971,6 +1053,9 @@ class DotaOptimizer:
             layers = [pol.rnn.layer(k) for k in range(n_layers)]
             ybufs, cbufs = ops.rnn_stack_forward_states(x.contiguous(), layers, h0, c0, pol.cell)
             logits, values = pol._heads(ybufs[-1][1:], unit_embedding)
+            # value_norm: the head is normalised; everything prep makes from it is in raw units, V = mu + sigma v with the
+            # statistics this forward ran under (denormalised from the packed column into a contiguous [Lmax, R] tensor)
+            vn = self._value_norm_moments() if self.value_norm else None
             bootstrap = boot = None
             if cut:                                    # V(s_L) of every cut rollout: one step of batch R' from slot L_i
                 xb, ue = pol._encode(obs_next['env'], [obs_next[k] for k in Policy.INPUT_KEYS[1:]])
@@ -978,12 +1063,14 @@ class DotaOptimizer:
                 cb = ops.stack_layers([c[slot_last, col_last] for c in cbufs]) if lstm else None
                 yb_next, _ = ops.rnn_stack_forward_states(xb.contiguous(), layers, hb, cb, pol.cell)
                 bootstrap = pol._heads(yb_next[-1][1:], ue)[1].reshape(len(cut))
+                if vn is not None:
+                    bootstrap = ops.value_denorm(bootstrap, *vn)
                 boot = torch.cat([bootstrap.new_zeros(1), bootstrap])[boot_slot]          # per segment
             keys = ops.HEAD_KEYS
             old_logp = ops.selected_logp([logits[k] for k in keys], [masks[k] for k in keys],
                                          [actions[k] for k in keys]).view(Lmax, R, 5)        # :387-390
             # GAE per rollout over ITS padded length: back-to-back segments, rollout-major
-            values_lr = values.reshape(Lmax, R)
+            values_lr = values.reshape(Lmax, R) if vn is None else ops.value_denorm(values, *vn).view(Lmax, R)
 
             def rollout_major(t):                    # [Lmax, R, ...] -> the rows of every rollout's padded length in turn
                 if same:
@@ -1016,6 +1103,8 @@ class DotaOptimizer:
                 real = valid.t().reshape(-1)                                                      # rollout-major rows
                 adv_c.masked_fill_(~real, 0.0)
                 ret_c.masked_fill_(~real, 0.0)
+            if self.value_norm:                        # the statistics of this batch's raw targets, then the POP rescale
+                self._update_value_norm(ret_c, real if self.mask_padding else None)
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
                     adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same, valid=valid,
                     bootstrap=bootstrap)
@@ -1214,6 +1303,33 @@ class DotaOptimizer:
         return {'mean_log_rho': s[1] / n, 'mean_clipped_rho': s[2] / n, 'rho_clip_fraction': s[3] / n,
                 'c_clip_fraction': s[4] / n}
 
+    def _value_norm_moments(self):
+        return value_norm_moments(self._value_norm, self.VALUE_NORM_MIN_STD)
+
+    @property
+    def value_norm_stats(self):
+        """With ``value_norm``: ``{'mean': mu, 'std': sigma, 'weight': w}`` of the value statistics the next step trains
+        under (w = 0: no update yet, identity); None when the feature is off."""
+        if not self.value_norm:
+            return None
+        mu, sigma = self._value_norm_moments()
+        return {'mean': mu, 'std': sigma, 'weight': self._value_norm[2]}
+
+    def _update_value_norm(self, ret, valid):
+        """The end of experience prep under ``value_norm``: the batch's (n, sum R, sum R^2) over the tokens the value loss
+        averages over (``valid`` rows, or all), summed over the ranks with one all-reduce when data-parallel (a collective:
+        every rank's prep must reach it), one host sync, the statistics update, and the POP rescale of the value head."""
+        st = ops.value_norm_stats(ret, valid)
+        if is_distributed():
+            dist.all_reduce(st)
+        n, s1, s2 = st.tolist()
+        old = self._value_norm_moments()
+        self._value_norm = value_norm_update(self._value_norm, n, s1, s2, self.value_norm_decay)
+        new = self._value_norm_moments()
+        if new != old:
+            head = self.policy_base.affine_value
+            ops.value_head_rescale(head.weight.data, head.bias.data, old, new)
+
     @staticmethod
     def _ppo_stats_dict(st, joint=False):
         out = {'approx_kl': st[_lib.STAT_APPROX_KL], 'clip_fraction': st[_lib.STAT_CLIP_FRACTION]}
@@ -1231,13 +1347,15 @@ class DotaOptimizer:
         current stream, before the step is launched or replayed (never inside a captured graph), and only when a value
         changed (with the value head's has-gradient flag, which follows vf_coef).  The pinned source is free to rewrite: the
         previous step's copy completed before that step's result was read back."""
+        # value_norm: the statistics of the last prep (mu, sigma), which the loss normalises the raw targets with; off: 0, 0
+        mu, sigma = self._value_norm_moments() if self.value_norm else (0.0, 0.0)
         vals = (float(self.learning_rate), float(self.e_clip), float(self.entropy_coef), float(self.vf_coef),
-                float(self.MAX_GRAD_NORM), float(self.value_clip or 0.0))
+                float(self.MAX_GRAD_NORM), float(self.value_clip or 0.0), mu, sigma)
         if vals == self._hparams_uploaded:
             return
         h = self._hparams_host.numpy()
         for slot, v in zip((_lib.HP_LR, _lib.HP_E_CLIP, _lib.HP_ENTROPY_COEF, _lib.HP_VF_COEF, _lib.HP_MAX_GRAD_NORM,
-                            _lib.HP_VALUE_CLIP), vals):
+                            _lib.HP_VALUE_CLIP, _lib.HP_VALUE_NORM_MEAN, _lib.HP_VALUE_NORM_STD), vals):
             h[slot] = v
         self._hparams_dev.copy_(self._hparams_host, non_blocking=True)
         # the value head has a gradient only while the value loss is on (optimizer.py:660-662): with vf_coef = 0 the
@@ -1484,6 +1602,9 @@ class DotaOptimizer:
         if self.advantage_estimator == 'vtrace':                           # read now: the steps have synced the device
             for k, v in self.last_vtrace_stats.items():
                 metrics['vtrace/{}'.format(k)] = v
+        if self.value_norm:                                                # the statistics this iteration trained under
+            st = self.value_norm_stats
+            metrics['value_norm/mean'], metrics['value_norm/std'] = st['mean'], st['std']
         logger.info('steps_per_s={:.2f}, avg_weight_age={:.1f}, loss={:.4f}, entropy={:.3f}'.format(
             metrics[self.SPEED_KEY], float(metrics['avg_weight_age']), float(metrics['loss/sum']), float(metrics['entropy'])))
         if self.checkpoint:
@@ -1607,11 +1728,12 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          pretrained_model, mq_prefetch_count, log_dir, entropy_coef, vf_coef, run_local,
          hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
          value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
-         mask_padding=False, pack_sequences=False, policy_ratio='per_head'):
+         mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False, value_norm_decay=0.99):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                        mask_padding=mask_padding, pack_sequences=pack_sequences,
-                       policy_ratio=policy_ratio)                                         # before any process-group setup
+                       policy_ratio=policy_ratio, value_norm=value_norm,
+                       value_norm_decay=value_norm_decay)                                 # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -1623,7 +1745,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         gae_lambda=gae_lambda, clip_range=clip_range, max_grad_norm=max_grad_norm, value_clip=value_clip,
         advantage_estimator=advantage_estimator, vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip,
         num_minibatches=num_minibatches, mask_padding=mask_padding, pack_sequences=pack_sequences,
-        policy_ratio=policy_ratio)
+        policy_ratio=policy_ratio, value_norm=value_norm, value_norm_decay=value_norm_decay)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -1639,7 +1761,7 @@ def build_arg_parser():
     """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell``, ``--num-layers`` and the PPO
     settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm``, ``--value-clip``,
     ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches``, ``--mask-padding``,
-    ``--pack-sequences`` and ``--policy-ratio``."""
+    ``--pack-sequences``, ``--policy-ratio``, ``--value-norm`` and ``--value-norm-decay``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -1679,6 +1801,11 @@ def build_arg_parser():
     p.add_argument("--policy-ratio", type=str, choices=POLICY_RATIOS, default='per_head',
                    help="'joint' clips one PPO ratio per step, of the whole hierarchical action, instead of one per head "
                         "(reference: per_head)")
+    p.add_argument("--value-norm", action="store_true",
+                   help="PopArt: train the critic on returns normalised by running statistics, rescaling the value head "
+                        "so that its unnormalised output is preserved (reference: raw returns)")
+    p.add_argument("--value-norm-decay", type=float, default=0.99,
+                   help="decay of the running value statistics per prepared batch, in [0, 1)")
     return p
 
 
@@ -1693,6 +1820,7 @@ if __name__ == '__main__':
              num_layers=args.num_layers, gamma=args.gamma, gae_lambda=args.gae_lambda, clip_range=args.clip_range,
              max_grad_norm=args.max_grad_norm, value_clip=args.value_clip, advantage_estimator=args.advantage_estimator,
              vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip, num_minibatches=args.num_minibatches,
-             mask_padding=args.mask_padding, pack_sequences=args.pack_sequences, policy_ratio=args.policy_ratio)
+             mask_padding=args.mask_padding, pack_sequences=args.pack_sequences, policy_ratio=args.policy_ratio,
+             value_norm=args.value_norm, value_norm_decay=args.value_norm_decay)
     except KeyboardInterrupt:
         pass

@@ -302,7 +302,9 @@ int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEADS], const i
 #define DC_HP_ENTROPY_COEF 2
 #define DC_HP_VF_COEF 3
 #define DC_HP_MAX_GRAD_NORM 4  /* global gradient-norm clip                                        */
-#define DC_HP_VALUE_CLIP 5     /* PPO2 value clip range; <= 0: unclipped value loss. Slots 6, 7: 0 */
+#define DC_HP_VALUE_CLIP 5     /* PPO2 value clip range; <= 0: unclipped value loss                 */
+#define DC_HP_VALUE_NORM_MEAN 6 /* value normalisation mu (read only when slot 7 > 0)               */
+#define DC_HP_VALUE_NORM_STD 7  /* value normalisation sigma; <= 0: off (the plain value loss)      */
 
 /* Loss + gradient as dc_ppo_loss_fwd_bwd_strided, hyper-parameters from `hparams` [DC_HPARAM_SLOTS] (device), plus:
  *   old_value [N] fp32 or NULL: critic values at experience prep.  When hparams[DC_HP_VALUE_CLIP] = eps > 0 and
@@ -315,6 +317,11 @@ int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEADS], const i
  *       12 explained variance 1 - Var(ret - v) / Var(ret) over all N tokens, padding included (NaN if Var(ret) = 0;
  *          over the valid tokens only under dc_ppo_loss_fwd_bwd_masked);
  *       13..15 zero (dc_ppo_loss_fwd_bwd_joint: 13, 14 see there).
+ * Value normalisation (PopArt; this entry point, _masked and _joint): when hparams[DC_HP_VALUE_NORM_STD] = sigma > 0, the
+ *   value head's output `value` is in normalised units and the raw targets are read as r_n = fp32((r - mu) / sigma) and,
+ *   for the clipped value loss, v_old,n = fp32((v_old - mu) / sigma), both computed in float64 with
+ *   mu = hparams[DC_HP_VALUE_NORM_MEAN].  The value loss, dvalue and the explained-variance sums use them in place of r and
+ *   v_old.  Slot 7 = 0 runs the plain arithmetic; (mu, sigma) = (0, 1) gives the same bits, as x - 0 and x / 1 are exact.
  */
 #define DC_PPO_STATS_SLOTS 16
 #define DC_STAT_APPROX_KL 0
@@ -375,6 +382,26 @@ int dc_ppo_loss_fwd_bwd_joint(const float *const logits[DC_NUM_HEADS], const int
                               float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
                               float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
                               void *workspace, dc_stream_t stream);
+
+/* ---- value normalisation (PopArt, van Hasselt et al. 2016) --------------------------------------------------------
+ * No counterpart in the reference, whose critic learns raw returns (optimizer.py:660).
+ *   dc_value_norm_stats    out[3] fp64 (device) = count, sum x, sum x^2 over the x[i] [N] with valid[i] != 0 (valid NULL:
+ *                          all N), in float64.  Deterministic: one CTA, a fixed-order two-stage reduction without
+ *                          atomics, so two calls give the same bits.  N = 0 writes zeros.
+ *   dc_value_denorm        out[i] = fp32(mu + sigma * v[i * ld_v]) for i < N, computed in float64 (out contiguous [N]):
+ *                          the raw-scale values of a normalised head, e.g. from the value column (pitch 128) of the packed
+ *                          head GEMM.  sigma > 0.
+ *   dc_value_head_rescale  in place on the value head's weight w [n] and bias b [1] (fp32), computed in float64 and rounded
+ *                          once: w = w sigma_old / sigma_new, b = (sigma_old b + mu_old - mu_new) / sigma_new, so that
+ *                          sigma v + mu is unchanged when the statistics move from (mu_old, sigma_old) to (mu_new,
+ *                          sigma_new).  Both sigmas > 0.
+ * Checked before any CUDA call: N >= 0 / n >= 1, ld_v >= 1, non-null pointers where there is work, finite statistics with
+ * positive sigmas -> DC_EINVAL.
+ */
+int dc_value_norm_stats(const float *x, const uint8_t *valid, int64_t N, double *out, dc_stream_t stream);
+int dc_value_denorm(const float *v, int64_t ld_v, int64_t N, double mu, double sigma, float *out, dc_stream_t stream);
+int dc_value_head_rescale(float *w, int64_t n, float *b, double mu_old, double sigma_old, double mu_new, double sigma_new,
+                          dc_stream_t stream);
 
 /* Log-prob of the taken action per head, [N,5] dense (0 where the head took no action):
  * the no-grad half of experiences_from_rollout (optimizer.py:387-390). */
