@@ -5,11 +5,13 @@
 // implies (1 -> x and y, 2 -> target_unit, 3 -> ability; 0 = no-op).  For an in-process pool of agents that is
 // launch-latency work; here one thread handles one agent end to end.
 //
-// torch.multinomial's RNG stream cannot be reproduced on a GPU, so what is pinned against the oracle is the INDEX
+// torch.multinomial's RNG stream cannot be reproduced on a GPU, so what is held to the oracle is the INDEX
 // FUNCTION (oracle/ref_policy.py:sample_index): inverse CDF over the masked probabilities for a caller-supplied uniform
 // u in [0,1) -- fp32, sequential accumulation in index order, first valid index whose cumulative mass exceeds
 // u * total, falling back to the last valid index.  The log-probability of the chosen entry comes back too (it is what
-// the optimizer later recomputes as old_logp, optimizer.py:386-398).
+// the optimizer later recomputes as old_logp, optimizer.py:386-398).  expf and this sequential normaliser round
+// differently from torch's exp and sum, which can move a cumulative boundary by a few ulp: a u that close to a boundary
+// may take the adjacent legal index, so the two agree only outside that band.
 #include "dc_common.cuh"
 
 namespace {

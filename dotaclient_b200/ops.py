@@ -741,7 +741,9 @@ def select_actions(logits, masks, u):
 
     ``logits`` / ``masks``: five ``[A, n_h]`` tensors in ``HEAD_KEYS`` order (rows may be strided column slices);
     ``u``: ``[A, 5]`` uniforms in [0, 1).  Returns ``(chosen [A,5] int32, logp [A,5] fp32)``; ``chosen`` is -1 for the
-    sub-heads the sampled enum does not use.  The index function is pinned to ``oracle.ref_policy.sample_index``."""
+    sub-heads the sampled enum does not use.  The index function is ``oracle.ref_policy.sample_index``'s inverse CDF; the
+    two differ in fp32 rounding (CUDA ``expf`` and a sequential normaliser against torch's), so they can take adjacent legal
+    indices when u lies within that rounding of a cumulative boundary."""
     _need_cuda(u, *logits, *masks)
     A = u.shape[0]
     ls, lds, ms = [], [], []

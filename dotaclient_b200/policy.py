@@ -249,7 +249,8 @@ class Policy(nn.Module):
     def select_actions_batched(cls, heads_logits, masks, u=None):
         """``select_actions`` for a whole pool of agents in ONE kernel launch (``csrc/actor.cu``): ``heads_logits`` /
         ``masks`` are ``{head: [A, n]}`` CUDA tensors (``[A, 1, n]`` accepted), ``u`` optional ``[A, 5]`` uniforms (drawn with
-        ``torch.rand`` if omitted).  Returns ``({head: int32 [A]} with -1 where the head was not sampled, logp [A, 5])``."""
+        ``torch.rand`` if omitted).  Returns ``({head: int32 [A]} with -1 where the head was not sampled, logp [A, 5])``.  The picks
+        are ``oracle.ref_policy.sample_index``'s up to fp32 rounding near a cumulative boundary (see ``act_batched``)."""
         A = heads_logits['enum'].shape[0]
         dev = heads_logits['enum'].device
         if u is None:
@@ -266,7 +267,9 @@ class Policy(nn.Module):
         ``hidden``: ``[L, A, H]`` (``(h, c)`` for the LSTM; L = ``num_layers``); ``observations``: ``{key: [A, ...]}`` (what ``single`` takes, with
         a leading agent dimension); ``masks``: ``{head: [A, n]}`` legal-action masks (``action_masks``); ``u``: optional
         ``[A, 5]`` uniforms.  Returns ``(chosen {head: int32 [A], -1 = not sampled}, logp [A, 5], logits {head: [A, n]},
-        value [A], new hidden)``.  Index selection is bit-exact against ``oracle.ref_policy.sample_index``.
+        value [A], new hidden)``.  Index selection is ``oracle.ref_policy.sample_index``'s inverse CDF up to fp32 rounding: the two
+        agree unless u lies within the rounding band of a cumulative boundary (a few 1e-6 for logits of order 1, up to about
+        5e-5 at |logit| 60), where either may take the adjacent legal index.
 
         Row ``a`` of ``logp`` (log-probability of each sampled head in ``ops.HEAD_KEYS`` order, 0 for heads not sampled) is
         the ``behaviour_logp`` row of this step in agent ``a``'s rollout: what ``DotaOptimizer(advantage_estimator='vtrace')``

@@ -443,9 +443,9 @@ int dc_grad_finish_dev(float *flat_param, float *flat_grad, float *exp_avg, floa
  * (policy.py:23-33 MaskedCategorical, :169-178 masked_softmax, :190-216 sample_action/select_actions; caller agent.py:578-674)
  * Heads in DC order (enum 4, x 9, y 9, target_unit 40, ability 3).  logits[h]: A rows with pitch ld[h] floats;
  * masks[h]: [A, n_h] bytes (0/1); u: [A,5] uniforms in [0,1) supplied by the caller (torch.multinomial's RNG stream cannot
- * be reproduced, so the pinned contract is the index function: inverse CDF over the masked probabilities, fp32, sequential
- * in index order -- oracle/ref_policy.py:sample_index).  chosen[A,5]: enum first, then x,y (enum 1) / target_unit (2) /
- * ability (3); -1 for heads that were not sampled.  logp[A,5] (nullable): log-probability of each chosen entry. */
+ * be reproduced, so the contract is the index function: inverse CDF over the masked probabilities, fp32, sequential
+ * in index order -- oracle/ref_policy.py:sample_index, up to fp32 rounding near a cumulative boundary).  chosen[A,5]:
+ * enum first, then x,y (enum 1) / target_unit (2) / ability (3); -1 for heads that were not sampled.  logp[A,5] (nullable): log-probability of each chosen entry. */
 int dc_select_actions(const float *const logits[DC_NUM_HEADS], const int64_t ld[DC_NUM_HEADS],
                       const uint8_t *const masks[DC_NUM_HEADS], const float *u, int64_t A, int32_t *chosen,
                       float *logp, dc_stream_t stream);

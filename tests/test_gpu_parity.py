@@ -7,7 +7,9 @@ Tolerances (fp32 SIMT kernels vs torch-CPU fp32 oracle; stated per test):
   recurrence backward    rtol 2e-4 / atol 2e-6 on dgi-derived gradients
   loss terms, entropies  rtol 1e-4, atol 1e-6
   parameter gradients    rtol 2e-3 on per-tensor norms, cosine >= 0.9999 on sampled tensors
-  integer work           bit-exact (n_actions, action-index selection)
+  integer work           bit-exact (n_actions); action-index selection equal to sample_index on the random u used here
+                         (a u within fp32 rounding of a cumulative boundary may take the adjacent index:
+                         test_gpu_actor_fp64.py)
 """
 import copy
 import os
@@ -674,7 +676,7 @@ def test_act_batched_pool_matches_per_agent_single(tmp_path):
             for k in HEADS:
                 torch.testing.assert_close(logits[k][a].cpu(), lo[k][0, 0], rtol=1e-4, atol=3e-5)
             torch.testing.assert_close(value[a].cpu(), vo[0, 0, 0], rtol=1e-4, atol=3e-5)
-            e = sample_index(logits["enum"][a].cpu(), masks["enum"][a], float(u[a, 0]))      # the index function on OUR logits: bit-exact
+            e = sample_index(logits["enum"][a].cpu(), masks["enum"][a], float(u[a, 0]))      # the index function on OUR logits
             assert int(chosen["enum"][a]) == e
             for h, k in enumerate(HEADS):
                 if k == "enum":

@@ -21,6 +21,14 @@ max|gpu - f64| / max|f64| in brackets):
     generic   (H 192, fp32 FMA)          4.6 /  4.7 /  25  (1.2e-5)
     saturating inputs (H 128 / 256)      8.7 /  6.2 /  13  (4.6e-4, at a torch fp32 error of 1.1e-4)
 The forwards with TF32-rounded W_hh give ratios of 96 to 284, so the forward K of 16 rejects them with a margin of 6.
+
+The edge cases, same columns (the TF32-rounded forward's ratios last):
+    resident-b512-gru (3-sequence tiles, ragged last tile)   3.8 / 3.5 / 12 (4.5e-6)   TF32 191-219
+    resident S 1 / S 3 (fewer steps than kStages = 4)         5.1 / 5.1 / 4.1 (5.9e-7)  TF32 200-400
+    cluster B 1 (S 16) / B 33 (S 1)                           11  / 11  / 8.8 (1.3e-6)  TF32 47-568
+    step-wise B 1 (S 16) / B 129 (S 1)                        8.6 / 22  / 11  (3.2e-6)  TF32 125-345
+    generic B 5 (S 2)                                         4.7 / 5.1 / 3.8 (7.5e-7)  TF32 233-319
+The smallest TF32 ratio, 47 (cluster B 1, c_n), still clears the forward K by a factor of 3.
 The weight gradients of the tensor-core designs sum thousands of tokens of h2h gradients whose error is larger than
 torch's, hence their floor of 5e-4.  The superposition residual reaches 3.0e-4 of max|dW| (step-wise, 524288 tokens).
 """
@@ -36,20 +44,34 @@ SUPERPOSE = 1e-3                   # dense == R-only + complement weight gradien
 
 # (case id, cell, B, S, H, sampled rows R, saturating inputs, TF32 sensitivity run)
 CASES = [
-    # resident, H 128: 2-sequence tiles (B <= 264) on 128 CTAs; 4-sequence tiles above
+    # resident, H 128: 2-sequence tiles (B <= 264) on 128 CTAs; 3-sequence (GRU) / 4-sequence (LSTM) tiles above
     ("resident-b256-gru", "gru", 256, 512, 128, (0, 1, 2, 127, 128, 129, 254, 255), False, True),
     ("resident-b256-lstm", "lstm", 256, 512, 128, (0, 1, 2, 127, 128, 129, 254, 255), False, True),
     ("resident-b512-lstm", "lstm", 512, 512, 128, (0, 3, 4, 255, 256, 259, 508, 511), False, False),
+    # 3-sequence GRU tiles (B > 2 * SMs): 170 full tiles and a last tile holding rows 510 and 511
+    ("resident-b512-gru", "gru", 512, 512, 128, (0, 2, 3, 254, 255, 509, 510, 511), False, True),
+    # fewer steps than the kStages = 4 prefetch ring: the prologue and refill guards
+    ("resident-s1-gru", "gru", 256, 1, 128, (0, 1, 2, 127, 128, 129, 254, 255), False, True),
+    ("resident-s1-lstm", "lstm", 256, 1, 128, (0, 1, 2, 127, 128, 129, 254, 255), False, True),
+    ("resident-s3-gru", "gru", 256, 3, 128, (0, 1, 2, 127, 128, 129, 254, 255), False, True),
+    ("resident-s3-lstm", "lstm", 256, 3, 128, (0, 1, 2, 127, 128, 129, 254, 255), False, True),
     # cluster, H 256: 32 sequences per 8-CTA cluster; 16 clusters, and a last cluster holding 20 of its 32 rows
     ("cluster-b512-gru", "gru", 512, 512, 256, (0, 31, 32, 255, 256, 480, 481, 511), False, True),
     ("cluster-b512-lstm", "lstm", 512, 512, 256, (0, 31, 32, 255, 256, 480, 481, 511), False, True),
     ("cluster-b500-gru", "gru", 500, 512, 256, (0, 31, 32, 255, 256, 479, 480, 499), False, False),
     ("cluster-b500-lstm", "lstm", 500, 512, 256, (0, 31, 32, 255, 256, 479, 480, 499), False, False),
+    # one live row in a cluster, one row past a cluster at a single step
+    ("cluster-b1-lstm", "lstm", 1, 16, 256, (0,), False, True),
+    ("cluster-b33-s1-gru", "gru", 33, 1, 256, (0, 1, 30, 31, 32), False, True),
     # step-wise, H 512: 128-row M tiles of the per-step split-K GEMM; C4's B 512 x S 1024, and a ragged last M tile
     ("stepwise-b512-lstm", "lstm", 512, 1024, 512, (0, 127, 128, 255, 256, 383, 384, 511), False, True),
     ("stepwise-b300-gru", "gru", 300, 256, 512, (0, 127, 128, 255, 256, 257, 298, 299), False, True),
+    # one live row in an M tile, one row past an M tile at a single step
+    ("stepwise-b1-gru", "gru", 1, 16, 512, (0,), False, True),
+    ("stepwise-b129-s1-lstm", "lstm", 129, 1, 512, (0, 1, 126, 127, 128), False, True),
     # generic, H 192: 4-sequence CTAs
     ("generic-b256-lstm", "lstm", 256, 512, 192, (0, 3, 4, 127, 128, 131, 252, 255), False, True),
+    ("generic-b5-s2-gru", "gru", 5, 2, 192, (0, 3, 4), False, True),
     # saturated gates (|pre-activation| 30..100) and an LSTM forget bias of +5
     ("saturating-h128-gru", "gru", 256, 512, 128, (0, 1, 2, 127, 128, 129, 254, 255), True, False),
     ("saturating-h128-lstm", "lstm", 256, 512, 128, (0, 1, 2, 127, 128, 129, 254, 255), True, False),
