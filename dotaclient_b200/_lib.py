@@ -59,6 +59,9 @@ SIGNATURES = {
                                           _vp, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "dc_ppo_loss_fwd_bwd_joint": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
                                          _vp, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "dc_ppo_loss_fwd_bwd_kl": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
+                                      _vp, _i32, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dc_selected_logp_rows": (_i32, [_ptr5, _ptr5, _ptr5, _i64, _vp, _vp, _vp]),
     "dc_value_norm_stats": (_i32, [_vp, _vp, _i64, _vp, _vp]),
     "dc_value_denorm": (_i32, [_vp, _i64, _i64, _f64, _f64, _vp, _vp]),
     "dc_value_head_rescale": (_i32, [_vp, _i64, _vp, _f64, _f64, _f64, _f64, _vp]),
@@ -69,19 +72,25 @@ SIGNATURES = {
                               _vp, _vp]),
     "dc_grad_finish_dev": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _vp, _f64, _f64, _f64, _vp, _vp, _vp,
                                   _vp]),
+    "dc_grad_finish_kl": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _vp, _f64, _f64, _f64, _vp, _vp, _vp,
+                                 _vp]),
 }
 
 PPO_WORKSPACE_BYTES = 512
 FINISH_WORKSPACE_BYTES = 1024
 LOSS_SLOTS = 16
 # the device hyper-parameter block of the `_dev` entry points (fp64, DC_HP_* in include/dotaclient_b200.h)
-HPARAM_SLOTS = 8
+HPARAM_SLOTS = 10
 HP_LR, HP_E_CLIP, HP_ENTROPY_COEF, HP_VF_COEF, HP_MAX_GRAD_NORM, HP_VALUE_CLIP = range(6)
 HP_VALUE_NORM_MEAN, HP_VALUE_NORM_STD = 6, 7       # value normalisation (mu, sigma); sigma 0 = off
+HP_KL_COEF, HP_KL_STOP = 8, 9                      # KL control: penalty beta, early-stop limit (0 = none)
 # the PPO diagnostics written by dc_ppo_loss_fwd_bwd_dev (DC_STAT_* in include/dotaclient_b200.h)
-PPO_STATS_SLOTS = 16
+PPO_STATS_SLOTS = 24
 STAT_APPROX_KL, STAT_CLIP_FRACTION, STAT_EXPLAINED_VAR = 0, 6, 12
 STAT_JOINT_APPROX_KL, STAT_JOINT_CLIP_FRACTION = 13, 14     # dc_ppo_loss_fwd_bwd_joint only
+STAT_KL, STAT_KL_PENALTY = 16, 22                           # dc_ppo_loss_fwd_bwd_kl only (17..21: KL per head)
+KL_ROW_FLOATS = 65          # entries of one token's masked log-prob row over the five heads (DC_KL_ROW_FLOATS)
+FINISH_KL_METRICS = 6       # metrics of dc_grad_finish_kl: the four of dc_grad_finish, the all-ranks KL, the skip flag
 VTRACE_STATS_SLOTS = 8      # per-segment fp64 sums written by dc_vtrace_scan (DC_VTRACE_STATS_SLOTS)
 GATHER_MAX_TENSORS = 32     # descriptors per dc_gather_columns call (DC_GATHER_MAX_TENSORS)
 MAX_PARAM_TENSORS = 96      # kMaxSeg of csrc/grad_finish.cu: parameter tensors dc_grad_flags / dc_grad_finish can handle

@@ -12,6 +12,8 @@
 // (B) clip coefficient + Adam in one elementwise sweep, (C) step counters + metrics.
 // dc_grad_finish_dev reads lr and the clip norm from the device hyper-parameter block (DC_HPARAM_SLOTS) in (B).
 // HBM-bound elementwise work: 4 B read + 4 B written per element in A, 16 B read + 12 B written in B.
+// dc_grad_finish_kl also reads the all-reduced (sum_t KL_t, T_a) behind the flags in (B): above hparams[DC_HP_KL_STOP] the
+// step is skipped like the NaN path (no parameter, moment or counter changes), and (C) reports the KL and the skip.
 #include "dc_common.cuh"
 
 namespace {
@@ -24,6 +26,8 @@ struct FinishWs {
     float clip_coef;
     int nan_flag;
     float mean_norm, total_norm;
+    float kl;             // dc_grad_finish_kl: the all-ranks KL
+    int kl_skip;          // dc_grad_finish_kl: 1 when the KL exceeded the limit and the step was skipped
 };
 static_assert(sizeof(FinishWs) <= DC_FINISH_WORKSPACE_BYTES, "finish workspace too small");
 
@@ -89,7 +93,8 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(float *__restrict__ para
                                                         const int64_t *__restrict__ seg_hi, int n_seg, int64_t total,
                                                         double lr, double beta1_d, double beta2_d, double eps_d,
                                                         float max_norm, const double *__restrict__ hparams,
-                                                        const float *__restrict__ loss_out, FinishWs *ws) {
+                                                        const float *__restrict__ loss_out, FinishWs *ws,
+                                                        const float *__restrict__ kl) {
     __shared__ float s_coef;
     __shared__ int s_nan;
     if (hparams) {                                       // the device block overrides the scalar arguments
@@ -102,10 +107,17 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(float *__restrict__ para
         finish_scalars(g + total, n_seg, ws, loss_out, max_norm, coef, nf, mn, tn);
         s_coef = coef;
         s_nan = nf;
+        if (kl) {    // KL early stop: kl = (sum_t KL_t, T_a) summed over the ranks; a limit <= 0 (or no block) is none
+            const double n_a = (double)kl[1], k = n_a > 0.0 ? (double)kl[0] / n_a : 0.0;
+            const double limit = hparams ? hparams[DC_HP_KL_STOP] : 0.0;
+            const int skip = limit > 0.0 && k > limit;
+            s_nan |= skip;
+            if (blockIdx.x == 0) { ws->kl = (float)k; ws->kl_skip = skip; }
+        }
         if (blockIdx.x == 0) { ws->clip_coef = coef; ws->nan_flag = nf; ws->mean_norm = mn; ws->total_norm = tn; }
     }
     __syncthreads();
-    if (s_nan) return;                                   // ValueError path: leave parameters untouched
+    if (s_nan) return;                                   // ValueError path (or a KL skip): leave parameters untouched
     const float coef = s_coef;
     // 1 - beta rounded from float64, as torch receives it (a Python float): 1 - (float)0.999 in fp32 would be 1.3e-5
     // off 0.001 and move the first updates of a fresh state by ~6e-6 relative
@@ -140,22 +152,28 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(float *__restrict__ para
     }
 }
 
-__global__ void finish_tail_kernel(int32_t *steps, const float *g_tail, int n_seg, const FinishWs *ws, float *metrics) {
+__global__ void finish_tail_kernel(int32_t *steps, const float *g_tail, int n_seg, const FinishWs *ws, float *metrics,
+                                   bool kl) {
     const int p = threadIdx.x;
     const int nan_flag = ws->nan_flag;
-    if (p < n_seg && !nan_flag && g_tail[p] > 0.f) steps[p] += 1;
+    const int skip = kl ? ws->kl_skip : 0;
+    if (p < n_seg && !nan_flag && !skip && g_tail[p] > 0.f) steps[p] += 1;
     if (p == 0) {
         metrics[0] = ws->mean_norm;                      // grad_norm 'unclipped'
         metrics[1] = ws->mean_norm * ws->clip_coef;      // grad_norm 'clipped'
         metrics[2] = ws->total_norm;
         metrics[3] = nan_flag ? 1.0f : 0.0f;
+        if (kl) {
+            metrics[4] = ws->kl;
+            metrics[5] = skip ? 1.0f : 0.0f;
+        }
     }
 }
 
 int launch_finish(float *flat_param, float *flat_grad, float *exp_avg, float *exp_avg_sq, int32_t *steps,
                   const int64_t *seg_lo, const int64_t *seg_hi, int n_seg, int64_t total, double lr, double beta1, double beta2,
                   double adam_eps, double max_norm, const double *hparams, const float *loss_out, float *metrics,
-                  void *workspace, dc_stream_t stream) {
+                  void *workspace, dc_stream_t stream, bool kl = false) {
     DC_REQUIRE(flat_param && flat_grad && exp_avg && exp_avg_sq && steps && seg_lo && seg_hi && metrics && workspace,
                DC_EINVAL, "dc_grad_finish: null pointer");
     DC_REQUIRE(n_seg > 0 && n_seg <= kMaxSeg && total > 0, DC_EINVAL, "dc_grad_finish: n_seg=%d total=%lld", n_seg,
@@ -167,9 +185,10 @@ int launch_finish(float *flat_param, float *flat_grad, float *exp_avg, float *ex
     grad_sumsq_kernel<<<blocks, kThreads, 0, st>>>(flat_grad, seg_lo, seg_hi, n_seg, total, ws);
     DC_LAUNCH_OK();
     adam_kernel<<<blocks, kThreads, 0, st>>>(flat_param, flat_grad, exp_avg, exp_avg_sq, steps, seg_lo, seg_hi, n_seg, total,
-                                             lr, beta1, beta2, adam_eps, (float)max_norm, hparams, loss_out, ws);
+                                             lr, beta1, beta2, adam_eps, (float)max_norm, hparams, loss_out, ws,
+                                             kl ? flat_grad + total + n_seg : nullptr);
     DC_LAUNCH_OK();
-    finish_tail_kernel<<<1, kMaxSeg, 0, st>>>(steps, flat_grad + total, n_seg, ws, metrics);
+    finish_tail_kernel<<<1, kMaxSeg, 0, st>>>(steps, flat_grad + total, n_seg, ws, metrics, kl);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -203,4 +222,14 @@ extern "C" int dc_grad_finish_dev(float *flat_param, float *flat_grad, float *ex
     DC_REQUIRE(hparams, DC_EINVAL, "dc_grad_finish_dev: null hyper-parameter block");
     return launch_finish(flat_param, flat_grad, exp_avg, exp_avg_sq, steps, seg_lo, seg_hi, n_seg, total, 0.0, beta1, beta2,
                          adam_eps, 0.0, hparams, loss_out, metrics, workspace, stream);
+}
+
+extern "C" int dc_grad_finish_kl(float *flat_param, float *flat_grad, float *exp_avg, float *exp_avg_sq, int32_t *steps,
+                                 const int64_t *seg_lo, const int64_t *seg_hi, const int32_t *seg_head, int n_seg,
+                                 int64_t total, const double *hparams, double beta1, double beta2, double adam_eps,
+                                 const float *loss_out, float *metrics, void *workspace, dc_stream_t stream) {
+    (void)seg_head;
+    DC_REQUIRE(hparams, DC_EINVAL, "dc_grad_finish_kl: null hyper-parameter block");
+    return launch_finish(flat_param, flat_grad, exp_avg, exp_avg_sq, steps, seg_lo, seg_hi, n_seg, total, 0.0, beta1, beta2,
+                         adam_eps, 0.0, hparams, loss_out, metrics, workspace, stream, true);
 }

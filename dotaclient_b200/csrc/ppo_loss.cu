@@ -40,6 +40,20 @@
 // Algorithmic HBM bytes per token: logits 260 + masks 65 + actions 65 + old 20 + adv/ret/value 12
 // read, dlogits 260 + dvalue 4 written = 686 (+ 69 for the statistics pass, + 4 for the old value when the value loss
 // is clipped, + 1 in each pass for `valid` when given).  The joint ratio reads and writes the same bytes.
+//
+// KL control (`dc_ppo_loss_fwd_bwd_kl`, kKl): the loss also reads every head's full masked log-prob row of the prep-time
+// policy ([N, 65], written by `dc_selected_logp_rows`, 0 at illegal entries) and adds beta * KL, with
+//   KL = (1 / T_a) sum_t sum_{h in S_t} sum_{a legal} p_old(a) (log p_old(a) - log p(a)),
+// and its gradient (beta / T_a)(p(a) - p_old(a)) to the legal entries of every dlogits row in S_t.  Both come out of the
+// loop that already writes that row from p and log p, so the only new work is one exp per legal entry.  beta = 0 skips
+// the gradient term and the loss term, so the results are those of the instantiation without kKl, bit for bit.  The
+// statistics pass counts T_a (as for the joint ratio), and the last CTA writes (sum_t KL_t, T_a) to `kl_out`.
+// The old rows are staged through shared memory as one contiguous [128, 65] tile (33,280 bytes, 16-byte loads; a pitch
+// of 65 floats keeps per-thread row reads conflict-free).  Read per thread from global instead, a warp's 32 rows would
+// sit 260 bytes apart, every load instruction would touch 32 sectors and the whole tile would have to stay in L1 across
+// the five heads.  Staging takes the CTA from 53.5 KB to 86 KB of dynamic shared memory: ptxas gives the loss kernel
+// about 160 registers, which already limits it to 3 CTAs per SM, and 86 KB + the static rows still allow 2.  The extra
+// HBM traffic is 260 B / token read (686 + 260 = 946 B / token for the loss pass).
 #include "dc_common.cuh"
 
 namespace {
@@ -63,6 +77,12 @@ constexpr int kLogitFloats = logit_off(kHeads);      // 67 * 128
 constexpr int kOldFloats = 5 * kTile;
 constexpr int kByteTile = byte_off(kHeads);          // 65 * 128
 constexpr size_t kSmemBytes = (size_t)(kLogitFloats + kOldFloats) * 4 + 2 * (size_t)kByteTile;
+// KL control: the prep-time log-prob rows, [N, 65] in head order, staged contiguously after the byte tiles
+constexpr int kRowFloats = DC_KL_ROW_FLOATS;
+__host__ __device__ constexpr int row_col(int h) { return byte_off(h) / kTile; }   // first column of head h in a row
+static_assert(kRowFloats == byte_off(kHeads) / kTile, "a log-prob row holds every head's entries");
+static_assert(kSmemBytes % 16 == 0, "the old-row tile is 16-byte aligned");
+constexpr size_t kSmemBytesKl = kSmemBytes + (size_t)kTile * kRowFloats * 4;
 
 struct HeadPtrs {
     const float *logits[kHeads];
@@ -80,7 +100,10 @@ constexpr int kStKl = 0, kStClip = kHeads, kStD = 2 * kHeads, kStD2 = kStD + 1, 
 constexpr int kTokD = 2 * kHeads, kTokR = kTokD + 1, kTokRows = kTokR + 1;   // rows of the per-token staging
 // joint ratio only: two more staging rows and sums after the above (k3 KL and clip flag of the joint ratio)
 constexpr int kTokJoint = kTokRows, kJointStats = 2;
+// KL control only: one staging row and sum per head of the exact KL of that head's row (after the joint rows, if any)
+constexpr int kKlStats = kHeads;
 static_assert(2 * kHeads + 3 < DC_PPO_STATS_SLOTS, "stats output too small");
+static_assert(DC_STAT_KL_PENALTY < DC_PPO_STATS_SLOTS, "stats output too small");
 
 // Workspace layout (DC_PPO_WORKSPACE_BYTES, zeroed per call)
 struct Workspace {
@@ -96,6 +119,7 @@ struct Workspace {
     unsigned long long n_joint;      // joint ratio: T_a, the tokens that count with at least one action row
     double st_joint[kJointStats];    // joint ratio: sums over the T_a tokens of its k3 KL and of its clip flag
     unsigned long long first_rev;    // N - (index of the first token that counts); 0 when no token counts
+    double st_kl[kKlStats];          // KL control: per head, the sum over its action rows of the exact KL of the row
 };
 static_assert(sizeof(Workspace) <= DC_PPO_WORKSPACE_BYTES, "workspace too small");
 
@@ -178,7 +202,8 @@ __device__ __forceinline__ T block_sum(T v, T *scratch) {
 }
 
 // ---- pass 1: counts + advantage statistics ------------------------------------------------
-// kJoint: also counts T_a (tokens that count with an action row in any head) into ws->n_joint
+// kJoint (the joint ratio, and KL control): also counts T_a (tokens that count with an action row in any head) into
+// ws->n_joint
 template <bool kJoint>
 __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const float *__restrict__ adv,
                                                            const uint8_t *__restrict__ valid, int64_t N,
@@ -244,10 +269,14 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
 }
 
 // ---- pass 2: loss + gradient --------------------------------------------------------------
-template <int H, bool kGrad>
+// kKl, loss: `orow` is the token's prep-time log-prob row of head H; the exact KL of the row goes to *kl_row_out (when
+// the head has an action row here) and, with kl_scale = beta / T_a > 0, its gradient joins the dlogits row.
+// kKl, select (logp_out given): the full masked log-prob row overwrites the logits row in the tile, 0 at illegal entries.
+template <int H, bool kGrad, bool kKl = false>
 __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, const uint8_t *arow, float old_lp,
                                            float adv_n, int n_h, float e_clip, float entropy_coef, float &pol_acc,
-                                           float &ent_acc, float *kl_out, float *clip_out, float *logp_out) {
+                                           float &ent_acc, float *kl_out, float *clip_out, float *logp_out,
+                                           const float *orow = nullptr, float kl_scale = 0.f, float *kl_row_out = nullptr) {
     constexpr int N = head_n(H);
     float l[N], e[N];
     int mask_any = 0, a_idx = -1;
@@ -270,6 +299,10 @@ __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, con
             lp = la - logf(se);
         }
         *logp_out = lp;
+        if (kKl) {   // the same expression as the selected entry, so row[a] == *logp_out bit for bit
+#pragma unroll
+            for (int j = 0; j < N; ++j) lrow[j] = mrow[j] ? l[j] - logf(se) : 0.f;
+        }
         return;
     }
     // A head nobody used this batch is skipped entirely (optimizer.py:627-630); a row with an
@@ -315,13 +348,20 @@ __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, con
     }
     if (kGrad) {
         const float ce = entropy_coef > 0.f ? entropy_coef / (float)n_h : 0.f;   // optimizer.py:652-656
+        float kl_row = 0.f;
 #pragma unroll
         for (int j = 0; j < N; ++j) {
             float g = -g_lp * p[j];                       // through logsumexp (masked entries only: p = 0 outside)
             if (j == a_idx) g += g_lp;
             if (mrow[j]) g += ce * p[j] * (lp[j] + ent_row);   // d(-coef * entropy)/d logit
+            if (kKl && a_idx >= 0 && mrow[j]) {          // KL(p_old || p) of a row in S_t, and beta / T_a (p - p_old)
+                const float lo = orow[j], po = __expf(lo);
+                kl_row += po * (lo - lp[j]);
+                if (kl_scale > 0.f) g += kl_scale * (p[j] - po);
+            }
             lrow[j] = g;
         }
+        if (kKl && a_idx >= 0) *kl_row_out = kl_row;
     }
 }
 
@@ -366,9 +406,11 @@ __device__ __forceinline__ void joint_head_fwd(const float *lrow, const uint8_t 
 
 // Joint ratio, sweep 2 over head H: the dlogits row, with g_lp = d loss / d lp[a] of the joint surrogate (the same for
 // every head with an action row) and the head's entropy term, recomputed from the tile exactly as sweep 1 computed it.
-template <int H>
+// kKl: the head's exact KL and its gradient, as in head_token.
+template <int H, bool kKl = false>
 __device__ __forceinline__ void joint_head_bwd(float *lrow, const uint8_t *mrow, const uint8_t *arow, int n_h, float g_lp,
-                                               float entropy_coef) {
+                                               float entropy_coef, const float *orow = nullptr, float kl_scale = 0.f,
+                                               float *kl_row_out = nullptr) {
     constexpr int N = head_n(H);
     float l[N], e[N];
     int mask_any = 0, a_idx = -1;
@@ -399,16 +441,25 @@ __device__ __forceinline__ void joint_head_bwd(float *lrow, const uint8_t *mrow,
     }
     if (a_idx < 0) g_lp = 0.f;
     const float ce = entropy_coef > 0.f ? entropy_coef / (float)n_h : 0.f;
+    float kl_row = 0.f;
 #pragma unroll
     for (int j = 0; j < N; ++j) {
         float g = -g_lp * p[j];
         if (j == a_idx) g += g_lp;
         if (mrow[j]) g += ce * p[j] * (lp[j] + ent_row);
+        if (kKl && a_idx >= 0 && mrow[j]) {
+            const float lo = orow[j], po = __expf(lo);
+            kl_row += po * (lo - lp[j]);
+            if (kl_scale > 0.f) g += kl_scale * (p[j] - po);
+        }
         lrow[j] = g;
     }
+    if (kKl && a_idx >= 0) *kl_row_out = kl_row;
 }
 
-template <bool kSelectOnly, bool kJoint>
+// kSelectOnly && kKl: the selected log-probs and, written through hp.dlogits (column ranges of the [N, 65] rows), every
+// head's masked log-prob row.  !kSelectOnly && kKl: the loss with the KL penalty (old_rows, kl_out).
+template <bool kSelectOnly, bool kJoint, bool kKl = false>
 __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const float *__restrict__ old_logp,
                                                           const float *__restrict__ adv_raw,
                                                           const float *__restrict__ ret,
@@ -419,15 +470,20 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
                                                           const double *__restrict__ hparams,
                                                           float *__restrict__ dvalue, float *__restrict__ out,
                                                           float *__restrict__ stats, Workspace *ws,
-                                                          float *__restrict__ logp_out) {
+                                                          float *__restrict__ logp_out,
+                                                          const float *__restrict__ old_rows, float *__restrict__ kl_out) {
     static_assert(!(kSelectOnly && kJoint), "the joint ratio is a loss");
-    constexpr int kRows = kTokRows + (kJoint ? kJointStats : 0);
-    constexpr int kSums = kStats + (kJoint ? kJointStats : 0);
+    constexpr bool kKlLoss = kKl && !kSelectOnly;
+    constexpr int kTokKl = kTokRows + (kJoint ? kJointStats : 0);
+    constexpr int kRows = kTokKl + (kKlLoss ? kKlStats : 0);
+    constexpr int kSumKl = kStats + (kJoint ? kJointStats : 0);
+    constexpr int kSums = kSumKl + (kKlLoss ? kKlStats : 0);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *s_logits = reinterpret_cast<float *>(smem_raw);
     float *s_old = s_logits + kLogitFloats;
     uint8_t *s_mask = reinterpret_cast<uint8_t *>(s_old + kOldFloats);
     uint8_t *s_act = s_mask + kByteTile;
+    float *s_orows = reinterpret_cast<float *>(smem_raw + kSmemBytes);    // kKlLoss: [kTile][65] prep-time log-prob rows
     __shared__ float s_red[kTile / 32];
     // per-token diagnostics (rows kStKl.., kStClip.., then ret - v and ret, then the joint ratio's), staged here rather
     // than held in registers across the head loop, and their block sums
@@ -438,6 +494,7 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
     // hyper-parameters from the device block when given, rounded to the types of the scalar arguments
     float value_clip = 0.f;
     double vn_mu = 0.0, vn_sigma = 0.0;     // value normalisation: sigma > 0 turns it on
+    float kl_coef = 0.f;                    // KL control: beta
     if (!kSelectOnly && hparams) {
         e_clip = (float)hparams[DC_HP_E_CLIP];
         entropy_coef = (float)hparams[DC_HP_ENTROPY_COEF];
@@ -445,6 +502,7 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         value_clip = (float)hparams[DC_HP_VALUE_CLIP];
         vn_mu = hparams[DC_HP_VALUE_NORM_MEAN];
         vn_sigma = hparams[DC_HP_VALUE_NORM_STD];
+        if (kKlLoss) kl_coef = (float)hparams[DC_HP_KL_COEF];
     }
     const bool vnorm = vn_sigma > 0.0;
     const bool clip_value = old_value != nullptr && value_clip > 0.f;
@@ -462,6 +520,9 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         stage_bytes(s_mask + byte_off(h), hp.masks[h] + t0 * head_n(h), count * head_n(h));
         stage_bytes(s_act + byte_off(h), hp.actions[h] + t0 * head_n(h), count * head_n(h));
     }
+    if (kKlLoss)      // contiguous rows: a byte copy of the tile with 16-byte loads
+        stage_bytes(reinterpret_cast<uint8_t *>(s_orows), reinterpret_cast<const uint8_t *>(old_rows + t0 * kRowFloats),
+                    count * kRowFloats * 4);
     __syncthreads();
 
     const int t = threadIdx.x;
@@ -484,6 +545,15 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             adv_n = __fdiv_rn(__fsub_rn(adv_raw[t0 + t], ws->adv_mean), __fadd_rn(ws->adv_std, 1.1920928955078125e-07f));
         }
     }
+    // KL control: beta / T_a, the weight of (p - p_old) in the dlogits rows of S_t; 0 (no gradient term) when beta = 0
+    float kl_scale = 0.f;
+    if (kKlLoss && kl_coef > 0.f) {
+        const unsigned long long n_a = ws->n_joint;
+        if (n_a) kl_scale = kl_coef / (float)n_a;
+    }
+    // KL control: this token's entry in the staging row of head 0's KL (head H's is H rows further).  Without kKl those
+    // rows do not exist and nothing is staged there.
+    float *const s_kl_tok = kKlLoss ? &s_tok[0][0] + kTokKl * kTile + t : nullptr;
     if (live) {
         float lp_sel[kHeads];
         if constexpr (kJoint) {
@@ -513,16 +583,20 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             // sweep 2 re-reads the tile: without this the compiler keeps every head's sweep-1 values live instead
             asm volatile("" ::: "memory");
 #define DC_JHEAD(H)                                                                                                 \
-            joint_head_bwd<H>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H),    \
-                              s_act + byte_off(H) + t * head_n(H), use ? cnt[H] : 0, g_lp, entropy_coef);
+            joint_head_bwd<H, kKlLoss>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H), \
+                                       s_act + byte_off(H) + t * head_n(H), use ? cnt[H] : 0, g_lp, entropy_coef,       \
+                                       s_orows + t * kRowFloats + row_col(H), kl_scale,                                 \
+                                       kKlLoss ? s_kl_tok + (H) * kTile : nullptr);
             DC_JHEAD(0) DC_JHEAD(1) DC_JHEAD(2) DC_JHEAD(3) DC_JHEAD(4)
 #undef DC_JHEAD
         } else {
 #define DC_HEAD(H)                                                                                              \
-        head_token<H, true>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H),  \
-                            s_act + byte_off(H) + t * head_n(H), kSelectOnly ? 0.f : s_old[t * 5 + H], adv_n,   \
-                            use ? cnt[H] : 0, e_clip, entropy_coef, pol[H], ent[H], &s_tok[kStKl + H][t],       \
-                            &s_tok[kStClip + H][t], kSelectOnly ? &lp_sel[H] : nullptr);
+        head_token<H, true, kKl>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H), \
+                                 s_act + byte_off(H) + t * head_n(H), kSelectOnly ? 0.f : s_old[t * 5 + H], adv_n,   \
+                                 use ? cnt[H] : 0, e_clip, entropy_coef, pol[H], ent[H], &s_tok[kStKl + H][t],       \
+                                 &s_tok[kStClip + H][t], kSelectOnly ? &lp_sel[H] : nullptr,                         \
+                                 s_orows + t * kRowFloats + row_col(H), kl_scale,                                    \
+                                 kKlLoss ? s_kl_tok + (H) * kTile : nullptr);
         DC_HEAD(0) DC_HEAD(1) DC_HEAD(2) DC_HEAD(3) DC_HEAD(4)
 #undef DC_HEAD
         }
@@ -566,109 +640,139 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             s_tok[kTokR][t] = r - shift_r;
         }
     }
-    if (kSelectOnly) return;
+    if (kSelectOnly && !kKl) return;
     __syncthreads();
     unstage_rows_f32<4, 5>(hp.dlogits[0], hp.ld_d[0], t0, s_logits + logit_off(0), count);
     unstage_rows_f32<9, 9>(hp.dlogits[1], hp.ld_d[1], t0, s_logits + logit_off(1), count);
     unstage_rows_f32<9, 9>(hp.dlogits[2], hp.ld_d[2], t0, s_logits + logit_off(2), count);
     unstage_rows_f32<40, 41>(hp.dlogits[3], hp.ld_d[3], t0, s_logits + logit_off(3), count);
     unstage_rows_f32<3, 3>(hp.dlogits[4], hp.ld_d[4], t0, s_logits + logit_off(4), count);
-
-    float sums[2 * kHeads + 1];
+    if constexpr (!kSelectOnly) {   // kKl select: the log-prob rows went out through hp.dlogits; nothing else to do
+        float sums[2 * kHeads + 1];
 #pragma unroll
-    for (int h = 0; h < kHeads; ++h) {
-        sums[h] = block_sum(pol[h], s_red);
-        sums[kHeads + h] = block_sum(ent[h], s_red);
-    }
-    sums[2 * kHeads] = block_sum(vl, s_red);
-    if (stats) {    // the diagnostics (s_tok is complete: block_sum synchronised the block): one warp per sum, in float64
-        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-        for (int i = warp; i < kSums; i += kTile / 32) {
-            const int row = (kJoint && i >= kStats) ? kTokJoint + (i - kStats) : (i < kStD ? i : (i < kStR ? kTokD : kTokR));
-            const bool square = i == kStD2 || i == kStR2;
-            double s = 0.0;
-            for (int j = lane; j < kTile; j += 32) {
-                const double v = (double)s_tok[row][j];
-                s += square ? v * v : v;
+        for (int h = 0; h < kHeads; ++h) {
+            sums[h] = block_sum(pol[h], s_red);
+            sums[kHeads + h] = block_sum(ent[h], s_red);
+        }
+        sums[2 * kHeads] = block_sum(vl, s_red);
+        // the diagnostics (s_tok is complete: block_sum synchronised the block): one warp per sum, in float64.  KL control
+        // needs its sums for kl_out whether or not the diagnostics are asked for.
+        if (stats || kKlLoss) {
+            const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+            for (int i = warp; i < kSums; i += kTile / 32) {
+                const int row = (kKlLoss && i >= kSumKl) ? kTokKl + (i - kSumKl)
+                              : (kJoint && i >= kStats) ? kTokJoint + (i - kStats) : (i < kStD ? i : (i < kStR ? kTokD : kTokR));
+                const bool square = i == kStD2 || i == kStR2;
+                double s = 0.0;
+                for (int j = lane; j < kTile; j += 32) {
+                    const double v = (double)s_tok[row][j];
+                    s += square ? v * v : v;
+                }
+                s = dc_warp_sum(s);
+                if (lane == 0) s_st[i] = s;
             }
-            s = dc_warp_sum(s);
-            if (lane == 0) s_st[i] = s;
+            __syncthreads();
+        }
+        if (threadIdx.x == 0) {
+#pragma unroll
+            for (int h = 0; h < kHeads; ++h) {
+                if (sums[h] != 0.f) atomicAdd(&ws->pol[h], (double)sums[h]);
+                if (sums[kHeads + h] != 0.f) atomicAdd(&ws->ent[h], (double)sums[kHeads + h]);
+            }
+            atomicAdd(&ws->vl, (double)sums[2 * kHeads]);
+            if (stats) {
+                for (int i = 0; i < kStats; ++i)
+                    if (s_st[i] != 0.0) atomicAdd(&ws->st[i], s_st[i]);
+                if constexpr (kJoint) {
+                    for (int i = 0; i < kJointStats; ++i)
+                        if (s_st[kStats + i] != 0.0) atomicAdd(&ws->st_joint[i], s_st[kStats + i]);
+                }
+            }
+            if constexpr (kKlLoss) {
+                for (int i = 0; i < kKlStats; ++i)
+                    if (s_st[kSumKl + i] != 0.0) atomicAdd(&ws->st_kl[i], s_st[kSumKl + i]);
+            }
+            __threadfence();
+            s_last = atomicAdd(&ws->ticket_loss, 1u) == gridDim.x - 1;
         }
         __syncthreads();
-    }
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int h = 0; h < kHeads; ++h) {
-            if (sums[h] != 0.f) atomicAdd(&ws->pol[h], (double)sums[h]);
-            if (sums[kHeads + h] != 0.f) atomicAdd(&ws->ent[h], (double)sums[kHeads + h]);
-        }
-        atomicAdd(&ws->vl, (double)sums[2 * kHeads]);
-        if (stats) {
-            for (int i = 0; i < kStats; ++i)
-                if (s_st[i] != 0.0) atomicAdd(&ws->st[i], s_st[i]);
-            if constexpr (kJoint) {
-                for (int i = 0; i < kJointStats; ++i)
-                    if (s_st[kStats + i] != 0.0) atomicAdd(&ws->st_joint[i], s_st[kStats + i]);
-            }
-        }
-        __threadfence();
-        s_last = atomicAdd(&ws->ticket_loss, 1u) == gridDim.x - 1;
-    }
-    __syncthreads();
-    if (s_last && threadIdx.x == 0) {
-        __threadfence();
-        volatile Workspace *w = ws;
-        float policy = 0.f, entropy = 0.f;
-        for (int h = 0; h < kHeads; ++h) {
-            const int n = w->cnt[h];
-            const float pl = (!kJoint && n) ? (float)(-w->pol[h] / (double)n) : 0.f;     // optimizer.py:641 / :628
-            const float en = n ? (float)(w->ent[h] / (double)n) : 0.f;      // optimizer.py:646 / :629
-            out[9 + h] = pl;
-            out[4 + h] = en;
-            policy += pl;
-            entropy += en;
-        }
-        if constexpr (kJoint) {                                             // -(1/T_a) sum_t min(r A, clip(r) A); 0 if T_a = 0
-            const unsigned long long n_a = w->n_joint;
-            policy = n_a ? (float)(-w->pol[0] / (double)n_a) : 0.f;
-        } else {
-            policy /= (float)kHeads;                                        // optimizer.py:650
-        }
-        const float e_loss = entropy_coef > 0.f ? -entropy_coef * entropy : 0.f;
-        const double n_tok_d = (double)w->n_valid;                          // N, or N_v under a valid mask
-        const float v_loss = vf_coef > 0.f ? vf_coef * (0.5f * (float)(w->vl / n_tok_d)) : 0.f;
-        out[0] = policy + e_loss + v_loss;                                  // optimizer.py:665
-        out[1] = policy;
-        out[2] = e_loss;
-        out[3] = v_loss;
-        out[14] = w->adv_mean;
-        out[15] = w->adv_std;
-        if (stats) {
-            float kl_sum = 0.f, clip_sum = 0.f;
-            int used = 0;
-            for (int h = 0; h < kHeads; ++h) {      // a head without action rows reports 0 and is left out of the mean
+        if (s_last && threadIdx.x == 0) {
+            __threadfence();
+            volatile Workspace *w = ws;
+            float policy = 0.f, entropy = 0.f;
+            for (int h = 0; h < kHeads; ++h) {
                 const int n = w->cnt[h];
-                const float kl_h = n ? (float)(w->st[kStKl + h] / (double)n) : 0.f;
-                const float clip_h = n ? (float)(w->st[kStClip + h] / (double)n) : 0.f;
-                stats[DC_STAT_APPROX_KL + 1 + h] = kl_h;
-                stats[DC_STAT_CLIP_FRACTION + 1 + h] = clip_h;
-                kl_sum += kl_h;
-                clip_sum += clip_h;
-                used += n > 0;
+                const float pl = (!kJoint && n) ? (float)(-w->pol[h] / (double)n) : 0.f;     // optimizer.py:641 / :628
+                const float en = n ? (float)(w->ent[h] / (double)n) : 0.f;      // optimizer.py:646 / :629
+                out[9 + h] = pl;
+                out[4 + h] = en;
+                policy += pl;
+                entropy += en;
             }
-            stats[DC_STAT_APPROX_KL] = used ? kl_sum / (float)used : 0.f;
-            stats[DC_STAT_CLIP_FRACTION] = used ? clip_sum / (float)used : 0.f;
-            // 1 - Var(ret - v) / Var(ret) over the tokens that count (population variances, from the shifted sums);
-            // NaN when the returns are constant
-            const double n = n_tok_d;
-            const double md = w->st[kStD] / n, mr = w->st[kStR] / n;
-            const double var_d = w->st[kStD2] / n - md * md, var_r = w->st[kStR2] / n - mr * mr;
-            stats[DC_STAT_EXPLAINED_VAR] = var_r > 0.0 ? (float)(1.0 - var_d / var_r) : __int_as_float(0x7fc00000);
-            for (int i = DC_STAT_EXPLAINED_VAR + 1; i < DC_PPO_STATS_SLOTS; ++i) stats[i] = 0.f;
-            if constexpr (kJoint) {
+            if constexpr (kJoint) {                                             // -(1/T_a) sum_t min(r A, clip(r) A); 0 if T_a = 0
                 const unsigned long long n_a = w->n_joint;
-                stats[DC_STAT_JOINT_APPROX_KL] = n_a ? (float)(w->st_joint[0] / (double)n_a) : 0.f;
-                stats[DC_STAT_JOINT_CLIP_FRACTION] = n_a ? (float)(w->st_joint[1] / (double)n_a) : 0.f;
+                policy = n_a ? (float)(-w->pol[0] / (double)n_a) : 0.f;
+            } else {
+                policy /= (float)kHeads;                                        // optimizer.py:650
+            }
+            const float e_loss = entropy_coef > 0.f ? -entropy_coef * entropy : 0.f;
+            const double n_tok_d = (double)w->n_valid;                          // N, or N_v under a valid mask
+            const float v_loss = vf_coef > 0.f ? vf_coef * (0.5f * (float)(w->vl / n_tok_d)) : 0.f;
+            out[0] = policy + e_loss + v_loss;                                  // optimizer.py:665
+            out[1] = policy;
+            out[2] = e_loss;
+            out[3] = v_loss;
+            out[14] = w->adv_mean;
+            out[15] = w->adv_std;
+            if (stats) {
+                float kl_sum = 0.f, clip_sum = 0.f;
+                int used = 0;
+                for (int h = 0; h < kHeads; ++h) {      // a head without action rows reports 0 and is left out of the mean
+                    const int n = w->cnt[h];
+                    const float kl_h = n ? (float)(w->st[kStKl + h] / (double)n) : 0.f;
+                    const float clip_h = n ? (float)(w->st[kStClip + h] / (double)n) : 0.f;
+                    stats[DC_STAT_APPROX_KL + 1 + h] = kl_h;
+                    stats[DC_STAT_CLIP_FRACTION + 1 + h] = clip_h;
+                    kl_sum += kl_h;
+                    clip_sum += clip_h;
+                    used += n > 0;
+                }
+                stats[DC_STAT_APPROX_KL] = used ? kl_sum / (float)used : 0.f;
+                stats[DC_STAT_CLIP_FRACTION] = used ? clip_sum / (float)used : 0.f;
+                // 1 - Var(ret - v) / Var(ret) over the tokens that count (population variances, from the shifted sums);
+                // NaN when the returns are constant
+                const double n = n_tok_d;
+                const double md = w->st[kStD] / n, mr = w->st[kStR] / n;
+                const double var_d = w->st[kStD2] / n - md * md, var_r = w->st[kStR2] / n - mr * mr;
+                stats[DC_STAT_EXPLAINED_VAR] = var_r > 0.0 ? (float)(1.0 - var_d / var_r) : __int_as_float(0x7fc00000);
+                for (int i = DC_STAT_EXPLAINED_VAR + 1; i < DC_PPO_STATS_SLOTS; ++i) stats[i] = 0.f;
+                if constexpr (kJoint) {
+                    const unsigned long long n_a = w->n_joint;
+                    stats[DC_STAT_JOINT_APPROX_KL] = n_a ? (float)(w->st_joint[0] / (double)n_a) : 0.f;
+                    stats[DC_STAT_JOINT_CLIP_FRACTION] = n_a ? (float)(w->st_joint[1] / (double)n_a) : 0.f;
+                }
+            }
+            if constexpr (kKlLoss) {
+                // KL = (1 / T_a) sum_t KL_t (0 when T_a = 0); the penalty beta KL joins the total loss only when beta > 0, so
+                // beta = 0 leaves out[0] as the instantiation without the penalty computes it
+                const unsigned long long n_a = w->n_joint;
+                double kl_sum = 0.0;
+                for (int h = 0; h < kHeads; ++h) kl_sum += w->st_kl[h];
+                const float kl = n_a ? (float)(kl_sum / (double)n_a) : 0.f;
+                const float penalty = kl_coef > 0.f ? kl_coef * kl : 0.f;
+                if (kl_coef > 0.f) out[0] = out[0] + penalty;
+                if (stats) {
+                    stats[DC_STAT_KL] = kl;
+                    for (int h = 0; h < kHeads; ++h) {       // over the head's action rows; 0 for a head without any
+                        const int n = w->cnt[h];
+                        stats[DC_STAT_KL + 1 + h] = n ? (float)(w->st_kl[h] / (double)n) : 0.f;
+                    }
+                    stats[DC_STAT_KL_PENALTY] = penalty;
+                }
+                if (kl_out) {       // this rank's (sum_t KL_t, T_a): summed over the ranks by the gradient all-reduce
+                    kl_out[0] = (float)kl_sum;
+                    kl_out[1] = (float)n_a;
+                }
             }
         }
     }
@@ -689,7 +793,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
                     const float *old_value, const uint8_t *valid, int64_t N, float e_clip, float entropy_coef, float vf_coef,
                     const double *hparams, float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
                     float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions, void *workspace,
-                    dc_stream_t stream, bool joint = false) {
+                    dc_stream_t stream, bool joint = false, const float *old_rows = nullptr, float *kl_out = nullptr) {
     DC_REQUIRE(N > 0, DC_EINVAL, "dc_ppo_loss_fwd_bwd: N=%lld", (long long)N);
     DC_REQUIRE(check_heads(logits, masks, actions) && old_logp && adv_raw && ret && value && dvalue && out &&
                    n_actions && workspace && ld_logits && ld_dlogits, DC_EINVAL, "dc_ppo_loss_fwd_bwd: null pointer");
@@ -706,6 +810,16 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
     Workspace *ws = reinterpret_cast<Workspace *>(workspace);
     DC_CUDA(cudaMemsetAsync(ws, 0, sizeof(Workspace), st));
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
+    if (old_rows) {             // KL control, either ratio mode; the statistics pass counts T_a
+        ppo_stats_kernel<true><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
+        DC_LAUNCH_OK();
+        auto kern = joint ? ppo_loss_kernel<false, true, true> : ppo_loss_kernel<false, false, true>;
+        DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytesKl));
+        kern<<<blocks, kTile, kSmemBytesKl, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip, entropy_coef, vf_coef, old_value,
+                                                  valid, hparams, dvalue, out, stats, ws, nullptr, old_rows, kl_out);
+        DC_LAUNCH_OK();
+        return DC_OK;
+    }
     if (joint) {
         ppo_stats_kernel<true><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
         DC_LAUNCH_OK();
@@ -713,7 +827,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
                                      (int)kSmemBytes));
         ppo_loss_kernel<false, true><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
                                                                         entropy_coef, vf_coef, old_value, valid, hparams,
-                                                                        dvalue, out, stats, ws, nullptr);
+                                                                        dvalue, out, stats, ws, nullptr, nullptr, nullptr);
         DC_LAUNCH_OK();
         return DC_OK;
     }
@@ -724,7 +838,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
     DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     ppo_loss_kernel<false, false><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
                                                                      entropy_coef, vf_coef, old_value, valid, hparams,
-                                                                     dvalue, out, stats, ws, nullptr);
+                                                                     dvalue, out, stats, ws, nullptr, nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -812,7 +926,45 @@ extern "C" int dc_selected_logp(const float *const logits[DC_NUM_HEADS], const u
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
     ppo_loss_kernel<true, false><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
         hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-        nullptr, logp_out);
+        nullptr, logp_out, nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
+}
+
+extern "C" int dc_selected_logp_rows(const float *const logits[DC_NUM_HEADS], const uint8_t *const masks[DC_NUM_HEADS],
+                                     const uint8_t *const actions[DC_NUM_HEADS], int64_t N, float *logp_out,
+                                     float *logp_rows, dc_stream_t stream) {
+    DC_REQUIRE(N > 0, DC_EINVAL, "dc_selected_logp_rows: N=%lld", (long long)N);
+    DC_REQUIRE(check_heads(logits, masks, actions) && logp_out && logp_rows, DC_EINVAL,
+               "dc_selected_logp_rows: null pointer");
+    HeadPtrs hp;
+    for (int h = 0; h < kHeads; ++h) {      // head h's entries are columns row_col(h).. of the [N, 65] rows
+        hp.logits[h] = logits[h]; hp.masks[h] = masks[h]; hp.actions[h] = actions[h];
+        hp.dlogits[h] = logp_rows + row_col(h);
+        hp.ld_l[h] = head_n(h); hp.ld_d[h] = kRowFloats;
+    }
+    hp.ld_v = 1; hp.ld_dv = 1;
+    DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)kSmemBytes));
+    const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
+    ppo_loss_kernel<true, false, true><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
+        hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+        nullptr, logp_out, nullptr, nullptr);
+    DC_LAUNCH_OK();
+    return DC_OK;
+}
+
+extern "C" int dc_ppo_loss_fwd_bwd_kl(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                                      const uint8_t *const masks[DC_NUM_HEADS], const uint8_t *const actions[DC_NUM_HEADS],
+                                      const float *old_logp, const float *old_log_probs, const float *adv_raw,
+                                      const float *ret, const float *value, int64_t ld_value, const float *old_value,
+                                      const uint8_t *valid, int64_t N, const double *hparams, int joint,
+                                      float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                                      float *dvalue, int64_t ld_dvalue, float *out, float *stats, float *kl_out,
+                                      int32_t *n_actions, void *workspace, dc_stream_t stream) {
+    DC_REQUIRE(hparams, DC_EINVAL, "dc_ppo_loss_fwd_bwd_kl: null hyper-parameter block");
+    DC_REQUIRE(old_log_probs, DC_EINVAL, "dc_ppo_loss_fwd_bwd_kl: null old_log_probs");
+    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, old_value, valid,
+                           N, 0.f, 0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions,
+                           workspace, stream, joint != 0, old_log_probs, kl_out);
 }

@@ -27,10 +27,14 @@ def head_dependency(param_name):
 
 
 class FlatParameterSpace:
-    """Re-homes ``module``'s parameters (in ``named_parameters()`` order == the reference's all-reduce order)."""
-    ALIGN = 64      # floats
+    """Re-homes ``module``'s parameters (in ``named_parameters()`` order == the reference's all-reduce order).
 
-    def __init__(self, module, device=None):
+    ``kl_tail=True`` (KL control) gives ``grad_full`` two more floats after the has-grad flags, ``kl_tail``: the PPO loss
+    writes the rank's (sum_t KL_t, T_a) there, so the one gradient all-reduce also sums them over the ranks."""
+    ALIGN = 64      # floats
+    KL_TAIL = 2
+
+    def __init__(self, module, device=None, kl_tail=False):
         named = [(n, p) for n, p in module.named_parameters() if p.requires_grad]
         if not named:
             raise ValueError("module has no trainable parameters")
@@ -51,9 +55,11 @@ class FlatParameterSpace:
         offs = starts + [cursor]                       # kept for compatibility: offs[i] = start of tensor i
         self.param = torch.zeros(self.total, dtype=torch.float32, device=device)
         # gradient buffer carries n_seg extra slots: per-parameter has-grad flags / counts (distributed.py:36-37)
-        self.grad_full = torch.zeros(self.total + self.n_seg, dtype=torch.float32, device=device)
+        extra = self.KL_TAIL if kl_tail else 0
+        self.grad_full = torch.zeros(self.total + self.n_seg + extra, dtype=torch.float32, device=device)
         self.grad = self.grad_full[:self.total]
-        self.flags = self.grad_full[self.total:]
+        self.flags = self.grad_full[self.total:self.total + self.n_seg]
+        self.kl_tail = self.grad_full[self.total + self.n_seg:] if kl_tail else None
         for p, lo, hi in zip(self.params, self.starts, self.ends):
             self.param[lo:hi].copy_(p.data.reshape(-1))
             p.data = self.param[lo:hi].view(p.shape)

@@ -439,16 +439,19 @@ def rnn_sequence(x_tm, w_ih, w_hh, b_ih, b_hh, h0, c0, cell, reset=None):
 
 # --------------------------------------------------------------------------------------------- PPO loss
 def hparam_block(device, lr=0.0, e_clip=0.0, entropy_coef=0.0, vf_coef=0.0, max_grad_norm=0.0, value_clip=None,
-                 value_norm=None):
+                 value_norm=None, kl_coef=0.0, kl_stop=None):
     """A device hyper-parameter block (``_lib.HPARAM_SLOTS`` fp64) holding the given values, for the ``hparams=``
     argument of ``ppo_loss_fwd_bwd`` / ``ppo_loss_packed`` / ``grad_finish``.  ``value_norm=(mu, sigma)`` makes the loss
-    normalise the raw value targets as ``(r - mu) / sigma`` (sigma > 0); None leaves slots 6 and 7 at 0 (off)."""
+    normalise the raw value targets as ``(r - mu) / sigma`` (sigma > 0); None leaves slots 6 and 7 at 0 (off).
+    ``kl_coef`` is the KL penalty's beta and ``kl_stop`` the KL limit of the finish (None: no limit); only the KL entry
+    points read them."""
     vals = [0.0] * _lib.HPARAM_SLOTS
     vals[_lib.HP_LR], vals[_lib.HP_E_CLIP], vals[_lib.HP_ENTROPY_COEF] = float(lr), float(e_clip), float(entropy_coef)
     vals[_lib.HP_VF_COEF], vals[_lib.HP_MAX_GRAD_NORM] = float(vf_coef), float(max_grad_norm)
     vals[_lib.HP_VALUE_CLIP] = float(value_clip or 0.0)
     if value_norm is not None:
         vals[_lib.HP_VALUE_NORM_MEAN], vals[_lib.HP_VALUE_NORM_STD] = float(value_norm[0]), float(value_norm[1])
+    vals[_lib.HP_KL_COEF], vals[_lib.HP_KL_STOP] = float(kl_coef), float(kl_stop or 0.0)
     return torch.tensor(vals, dtype=torch.float64, device=device)
 
 
@@ -519,16 +522,35 @@ def _ppo_dev_args(hparams, old_value, stats, N, dev, valid=None, joint=False):
     return old_value, stats, valid
 
 
+def _kl_args(old_log_probs, kl_out, N):
+    """Checks the extra operands of ``dc_ppo_loss_fwd_bwd_kl``: ``old_log_probs`` [..., 65] fp32 (contiguous) and
+    ``kl_out`` (2 fp32, or None)."""
+    _need_cuda(old_log_probs, kl_out)
+    old_log_probs = _f32c(old_log_probs)
+    assert old_log_probs.numel() == N * _lib.KL_ROW_FLOATS, "old_log_probs has %d elements for %d tokens" % (
+        old_log_probs.numel(), N)
+    if kl_out is not None:
+        assert kl_out.dtype == torch.float32 and kl_out.numel() == 2 and kl_out.is_contiguous()
+    return old_log_probs
+
+
 def _ppo_dev_call(lib, lptr, ld_l, masks, actions, old_logp, adv_raw, ret, value_ptr, ld_v, old_value, valid, N, hparams,
-                  dptr, ld_d, dvalue_ptr, ld_dv, out, stats, n_actions, ws, joint=False):
+                  dptr, ld_d, dvalue_ptr, ld_dv, out, stats, n_actions, ws, joint=False, old_log_probs=None, kl_out=None):
     """``dc_ppo_loss_fwd_bwd_dev``, or ``dc_ppo_loss_fwd_bwd_masked`` when a valid mask is given, or
-    ``dc_ppo_loss_fwd_bwd_joint`` (valid or not) when ``joint``."""
+    ``dc_ppo_loss_fwd_bwd_joint`` (valid or not) when ``joint``; ``dc_ppo_loss_fwd_bwd_kl`` (either ratio mode) when
+    ``old_log_probs`` is given."""
     head = (lptr, ld_l, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(),
             value_ptr, ld_v, _lib.ptr(old_value))
     tail = (N, hparams.data_ptr(), dptr, ld_d, dvalue_ptr, ld_dv, out.data_ptr(), stats.data_ptr(), n_actions.data_ptr(),
             ws.data_ptr(), _lib.stream_ptr())
-    with PROFILE.span("ppo_loss", 2):
-        if joint:
+    with PROFILE.span("ppo_loss", 2, _lib.KL_ROW_FLOATS * 4 * N if old_log_probs is not None else 0):
+        if old_log_probs is not None:
+            _lib.check(lib.dc_ppo_loss_fwd_bwd_kl(
+                lptr, ld_l, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(), old_log_probs.data_ptr(),
+                adv_raw.data_ptr(), ret.data_ptr(), value_ptr, ld_v, _lib.ptr(old_value), _lib.ptr(valid), N,
+                hparams.data_ptr(), 1 if joint else 0, dptr, ld_d, dvalue_ptr, ld_dv, out.data_ptr(), stats.data_ptr(),
+                _lib.ptr(kl_out), n_actions.data_ptr(), ws.data_ptr(), _lib.stream_ptr()), "dc_ppo_loss_fwd_bwd_kl")
+        elif joint:
             _lib.check(lib.dc_ppo_loss_fwd_bwd_joint(*head, _lib.ptr(valid), *tail), "dc_ppo_loss_fwd_bwd_joint")
         elif valid is None:
             _lib.check(lib.dc_ppo_loss_fwd_bwd_dev(*head, *tail), "dc_ppo_loss_fwd_bwd_dev")
@@ -537,7 +559,7 @@ def _ppo_dev_call(lib, lptr, ld_l, masks, actions, old_logp, adv_raw, ret, value
 
 
 def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_clip, entropy_coef, vf_coef, hparams=None,
-                     old_value=None, stats=None, valid=None, joint=False):
+                     old_value=None, stats=None, valid=None, joint=False, old_log_probs=None, kl_out=None):
     """Fused PPO loss + gradients (``optimizer.py:587-589,621-665`` and their backward).
 
     logits/masks/actions: sequences of 5 tensors [..., n_h] in HEAD_KEYS order (any leading dims,
@@ -553,6 +575,9 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     ``joint`` (needs ``hparams``): one clipped PPO ratio per token, of the whole hierarchical action, instead of one per
     head (``dc_ppo_loss_fwd_bwd_joint``, with or without ``valid``); ``stats`` then also holds the joint ratio's KL and
     clip fraction (``_lib.STAT_JOINT_APPROX_KL`` / ``STAT_JOINT_CLIP_FRACTION``).
+    ``old_log_probs`` [..., 65] (needs ``hparams``): the prep-time masked log-prob rows (``selected_logp_rows``); the loss
+    then adds the KL penalty ``hparams[HP_KL_COEF] * KL`` (``dc_ppo_loss_fwd_bwd_kl``, either ratio mode), ``stats``
+    also holds the exact KL (``_lib.STAT_KL``...), and ``kl_out`` (2 fp32, or None) receives (sum_t KL_t, T_a).
     """
     logits = [_f32c(l.detach()) for l in logits]
     _need_cuda(*logits)
@@ -571,11 +596,16 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     n_actions = torch.empty(5, dtype=torch.int32, device=dev)
     ws = torch.empty(_lib.PPO_WORKSPACE_BYTES, dtype=torch.uint8, device=dev)
     lib = _lib.load()
-    if hparams is not None or valid is not None or joint:
+    if hparams is not None or valid is not None or joint or old_log_probs is not None:
+        if old_log_probs is not None and hparams is None:
+            raise ValueError("the KL penalty needs the device hyper-parameter block (hparams=)")
         old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid, joint)
+        if old_log_probs is not None:
+            old_log_probs = _kl_args(old_log_probs, kl_out, N)
         ld = (ctypes.c_int64 * 5)(*HEAD_SIZES)
         _ppo_dev_call(lib, _lib.ptr5(logits), ld, masks, actions, old_logp, adv_raw, ret, value.data_ptr(), 1, old_value,
-                      valid, N, hparams, _lib.ptr5(dlogits), ld, dvalue.data_ptr(), 1, out, stats, n_actions, ws, joint)
+                      valid, N, hparams, _lib.ptr5(dlogits), ld, dvalue.data_ptr(), 1, out, stats, n_actions, ws, joint,
+                      old_log_probs, kl_out)
         return out, n_actions, dlogits, dvalue, stats
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd(_lib.ptr5(logits), _lib.ptr5(masks), _lib.ptr5(actions),
@@ -601,6 +631,25 @@ def selected_logp(logits, masks, actions):
     return out
 
 
+def selected_logp_rows(logits, masks, actions):
+    """``selected_logp``'s dense [N,5] log-probs (the same bits) and every head's full masked log-prob row, [N,65] in head
+    order with 0 at illegal entries -- the prep-time distribution the KL penalty compares against
+    (``dc_selected_logp_rows``)."""
+    logits = [_f32c(l.detach()) for l in logits]
+    _need_cuda(*logits)
+    N = logits[0].numel() // HEAD_SIZES[0]
+    masks = [_u8(m) for m in masks]
+    actions = [_u8(a) for a in actions]
+    dev = logits[0].device
+    out = torch.empty((N, 5), dtype=torch.float32, device=dev)
+    rows = torch.empty((N, _lib.KL_ROW_FLOATS), dtype=torch.float32, device=dev)
+    with PROFILE.span("selected_logp_rows", 1, 4 * N * _lib.KL_ROW_FLOATS):
+        _lib.check(_lib.load().dc_selected_logp_rows(_lib.ptr5(logits), _lib.ptr5(masks), _lib.ptr5(actions), N,
+                                                     out.data_ptr(), rows.data_ptr(), _lib.stream_ptr()),
+                   "dc_selected_logp_rows")
+    return out, rows
+
+
 # --------------------------------------------------------------------------------------------- grad finish
 def grad_flags(flat_grad, total, seg_head, n_actions):
     lib = _lib.load()
@@ -610,20 +659,28 @@ def grad_flags(flat_grad, total, seg_head, n_actions):
 
 
 def grad_finish(flat_param, flat_grad, exp_avg, exp_avg_sq, steps, seg_lo, seg_hi, seg_head, total, lr, betas, eps,
-                max_norm, loss_out, metrics, workspace, hparams=None):
+                max_norm, loss_out, metrics, workspace, hparams=None, kl=False):
     """Count-divide, grad norms, clip and Adam on the flat buffers.  With ``hparams`` (a device block, ``hparam_block``)
-    ``lr`` and ``max_norm`` are read from it on the device (``dc_grad_finish_dev``) and the arguments are ignored."""
+    ``lr`` and ``max_norm`` are read from it on the device (``dc_grad_finish_dev``) and the arguments are ignored.
+    ``kl`` (needs ``hparams``): ``flat_grad`` carries the all-reduced (sum_t KL_t, T_a) behind the flags, the step is
+    skipped when that KL exceeds the block's KL limit, and ``metrics`` (``_lib.FINISH_KL_METRICS``) also gets the KL and
+    the skip flag (``dc_grad_finish_kl``)."""
     lib = _lib.load()
+    if kl and hparams is None:
+        raise ValueError("the KL early stop needs the device hyper-parameter block (hparams=)")
     if hparams is not None:
         _need_cuda(hparams)
         assert hparams.dtype == torch.float64 and hparams.numel() == _lib.HPARAM_SLOTS and hparams.is_contiguous()
+        if kl:
+            n_seg = seg_head.numel()
+            assert flat_grad.numel() >= total + n_seg + 2 and metrics.numel() >= _lib.FINISH_KL_METRICS
         with PROFILE.span("grad_finish", 3):
-            _lib.check(lib.dc_grad_finish_dev(flat_param.data_ptr(), flat_grad.data_ptr(), exp_avg.data_ptr(),
+            _lib.check((lib.dc_grad_finish_kl if kl else lib.dc_grad_finish_dev)(flat_param.data_ptr(), flat_grad.data_ptr(), exp_avg.data_ptr(),
                                               exp_avg_sq.data_ptr(), steps.data_ptr(), seg_lo.data_ptr(), seg_hi.data_ptr(),
                                               seg_head.data_ptr(), seg_head.numel(), total, hparams.data_ptr(),
                                               float(betas[0]), float(betas[1]), float(eps), _lib.ptr(loss_out),
                                               metrics.data_ptr(), workspace.data_ptr(), _lib.stream_ptr()),
-                       "dc_grad_finish_dev")
+                       "dc_grad_finish_kl" if kl else "dc_grad_finish_dev")
         return
     with PROFILE.span("grad_finish", 3):
         _lib.check(lib.dc_grad_finish(flat_param.data_ptr(), flat_grad.data_ptr(), exp_avg.data_ptr(),
@@ -769,14 +826,14 @@ PACK_WIDTH = 128
 
 
 def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e_clip, entropy_coef, vf_coef, hparams=None,
-                    old_value=None, stats=None, valid=None, joint=False):
+                    old_value=None, stats=None, valid=None, joint=False, old_log_probs=None, kl_out=None):
     """Fused PPO loss where the four small heads and the value head are column ranges of ONE packed ``[N,128]``
     tensor-core GEMM output (``PACK_COLS``) and the target-unit logits are a separate ``[N,40]`` tensor.
 
     Returns (out[16], n_actions[5], d_packed [N,128], d_logits_tu [N,40]): the gradients go straight back into the two
     producers, so no slice/cat kernels run and the five tiny K=131072 weight-gradient GEMMs become one wgmma wgrad.
-    ``hparams`` / ``old_value`` / ``stats`` / ``valid`` / ``joint``: as ``ppo_loss_fwd_bwd`` (the fifth element of the
-    result is then ``stats``).
+    ``hparams`` / ``old_value`` / ``stats`` / ``valid`` / ``joint`` / ``old_log_probs`` / ``kl_out``: as
+    ``ppo_loss_fwd_bwd`` (the fifth element of the result is then ``stats``).
     """
     _need_cuda(packed, logits_tu)
     p2 = _f32c(packed.detach()).reshape(-1, PACK_WIDTH)
@@ -799,10 +856,15 @@ def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e
     dptr = _lib._ptr5(col(d_packed, "enum"), col(d_packed, "x"), col(d_packed, "y"), d_tu.data_ptr(), col(d_packed, "ability"))
     ld = (c.c_int64 * 5)(PACK_WIDTH, PACK_WIDTH, PACK_WIDTH, 40, PACK_WIDTH)
     lib = _lib.load()
-    if hparams is not None or valid is not None or joint:
+    if hparams is not None or valid is not None or joint or old_log_probs is not None:
+        if old_log_probs is not None and hparams is None:
+            raise ValueError("the KL penalty needs the device hyper-parameter block (hparams=)")
         old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid, joint)
+        if old_log_probs is not None:
+            old_log_probs = _kl_args(old_log_probs, kl_out, N)
         _ppo_dev_call(lib, lptr, ld, masks, actions, old_logp, adv_raw, ret, col(p2, "value"), PACK_WIDTH, old_value, valid,
-                      N, hparams, dptr, ld, col(d_packed, "value"), PACK_WIDTH, out, stats, n_actions, ws, joint)
+                      N, hparams, dptr, ld, col(d_packed, "value"), PACK_WIDTH, out, stats, n_actions, ws, joint,
+                      old_log_probs, kl_out)
         return out, n_actions, d_packed.view_as(packed), d_tu.view_as(logits_tu), stats
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd_strided(lptr, ld, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(),

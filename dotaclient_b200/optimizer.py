@@ -170,7 +170,7 @@ class Sequence:
     """
 
     def __init__(self, game_id, weight_version, team_id, observations, actions, masks, values, rewards, hidden,
-                 log_probs_sel=None, old_logp=None, valid=None):
+                 log_probs_sel=None, old_logp=None, valid=None, old_log_probs=None):
         self.game_id = game_id
         self.weight_version = weight_version
         self.team_id = team_id
@@ -183,6 +183,7 @@ class Sequence:
         self._log_probs_sel = log_probs_sel
         self.old_logp = old_logp
         self.valid = valid          # [S] bool, real steps vs zero padding (set by prep under DotaOptimizer(mask_padding=True))
+        self.old_log_probs = old_log_probs  # [S, 65] prep-time masked log-prob rows (set by prep under KL control)
         self.advantages = None
         self.returns = None
 
@@ -219,14 +220,19 @@ class ExperienceBatch:
     carries the recurrent-state resets between them: ``reset_slot [S, B]`` int32 (-1: carry the state; k >= 0: the state
     entering that step is row (k, column) of the tables), ``reset_h [K, B, L*H]`` and, for the LSTM, ``reset_c`` (every
     layer's state side by side).  They are gathered column by column like every other field, and absent when None.
+    ``old_log_probs [S, B, 65]`` (optional) are every head's full masked log-prob rows at experience prep, in head order
+    with 0 at illegal entries, which the KL penalty and the KL early stop (``DotaOptimizer(kl_coef=..., kl_stop=...)``)
+    compare against; absent from ``tensors()`` when None.
     """
-    FIELDS = ("advantages", "returns", "old_logp", "h0", "c0", "old_values", "valid", "reset_slot", "reset_h", "reset_c")
+    FIELDS = ("advantages", "returns", "old_logp", "h0", "c0", "old_values", "valid", "reset_slot", "reset_h", "reset_c",
+              "old_log_probs")
 
     def __init__(self, observations, masks, actions, old_logp, advantages, returns, h0, c0=None, old_values=None,
-                 valid=None, reset_slot=None, reset_h=None, reset_c=None):
+                 valid=None, reset_slot=None, reset_h=None, reset_c=None, old_log_probs=None):
         self.observations, self.masks, self.actions = observations, masks, actions
         self.old_logp, self.advantages, self.returns, self.h0, self.c0 = old_logp, advantages, returns, h0, c0
         self.old_values = old_values
+        self.old_log_probs = old_log_probs
         self.valid = valid
         self.reset_slot, self.reset_h, self.reset_c = reset_slot, reset_h, reset_c
         self._ready = {}        # data_ptr -> event of an upload still to be waited for (``to`` from pinned memory)
@@ -240,11 +246,12 @@ class ExperienceBatch:
                                {k: fn(v) for k, v in self.actions.items()}, **{f: opt(getattr(self, f)) for f in self.FIELDS})
 
     def graph_key(self):
-        """The shape a captured step graph is specialised to (old_values, valid, the reset tables of a packed batch: more
-        static inputs)."""
+        """The shape a captured step graph is specialised to (old_values, valid, the reset tables of a packed batch, the
+        old log-prob rows: more static inputs)."""
         key = (self.seq_len, self.batch_size, self.old_values is not None)
         key = key if self.valid is None else key + ('valid',)
-        return key if self.reset_slot is None else key + (('reset', self.reset_h.shape[0]),)
+        key = key if self.reset_slot is None else key + (('reset', self.reset_h.shape[0]),)
+        return key if self.old_log_probs is None else key + ('old_log_probs',)
 
     def reset(self):
         """The ``reset`` operand of ``Policy._recur`` (None for a batch that is not packed)."""
@@ -349,8 +356,11 @@ class ExperienceBatch:
         valid = None
         if all(getattr(e, 'valid', None) is not None for e in experiences):
             valid = stack([torch.as_tensor(e.valid).reshape(-1).bool() for e in experiences])
+        old_log_probs = None
+        if all(getattr(e, 'old_log_probs', None) is not None for e in experiences):
+            old_log_probs = stack([torch.as_tensor(e.old_log_probs).float() for e in experiences])
         return ExperienceBatch(obs, masks, actions, old, adv, ret, h0.detach(), None if c0 is None else c0.detach(),
-                               old_values=old_values, valid=valid)
+                               old_values=old_values, valid=valid, old_log_probs=old_log_probs)
 
 
 class _CapturedStep(typing.NamedTuple):
@@ -385,12 +395,14 @@ POLICY_RATIOS = ('per_head', 'joint')
 
 def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
                        vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False, pack_sequences=False,
-                       policy_ratio='per_head', value_norm=False, value_norm_decay=0.99):
+                       policy_ratio='per_head', value_norm=False, value_norm_decay=0.99, kl_coef=0.0, kl_target=None,
+                       kl_stop=None):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
     vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool,
     pack_sequences a bool that is True only with mask_padding, policy_ratio one of ``POLICY_RATIOS``, value_norm a bool
-    and 0 <= value_norm_decay < 1.  NaN fails every check."""
+    and 0 <= value_norm_decay < 1, finite kl_coef >= 0, kl_target None or finite > 0 (and then kl_coef > 0), kl_stop None
+    or finite > 0.  NaN fails every check."""
     if not isinstance(value_norm, bool):
         raise ValueError("value_norm=%r: must be True or False" % (value_norm,))
     if isinstance(value_norm_decay, bool) or not isinstance(value_norm_decay, numbers.Real) \
@@ -427,6 +439,27 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
         raise ValueError("vtrace_rho_clip=%r: the V-trace rho truncation must be > 0" % (vtrace_rho_clip,))
     if not number('vtrace_c_clip', vtrace_c_clip) > 0.0:
         raise ValueError("vtrace_c_clip=%r: the V-trace c truncation must be > 0" % (vtrace_c_clip,))
+    if not 0.0 <= number('kl_coef', kl_coef) < math.inf:
+        raise ValueError("kl_coef=%r: the KL penalty coefficient must be finite and >= 0" % (kl_coef,))
+    if kl_target is not None:
+        if not 0.0 < number('kl_target', kl_target) < math.inf:
+            raise ValueError("kl_target=%r: the KL target must be finite and > 0 (or None: a fixed kl_coef)" % (kl_target,))
+        if not float(kl_coef) > 0.0:
+            raise ValueError("kl_target=%r needs kl_coef > 0: the adaptive coefficient starts from kl_coef and only "
+                             "doubles or halves it" % (kl_target,))
+    if kl_stop is not None and not 0.0 < number('kl_stop', kl_stop) < math.inf:
+        raise ValueError("kl_stop=%r: the KL limit must be finite and > 0 (or None: no early stop)" % (kl_stop,))
+
+
+def kl_coef_update(kl_coef, kl, kl_target):
+    """The adaptive KL coefficient after an iteration whose steps measured a mean KL of ``kl`` (Schulman et al. 2017,
+    section 4): doubled when kl > 1.5 kl_target, halved when kl < kl_target / 1.5, unchanged otherwise (the boundaries
+    included)."""
+    if kl > 1.5 * kl_target:
+        return kl_coef * 2.0
+    if kl < kl_target / 1.5:
+        return kl_coef / 2.0
+    return kl_coef
 
 
 def value_norm_moments(state, min_std):
@@ -674,6 +707,7 @@ class DotaOptimizer:
     ADAM_FILES_KEPT = 3
     # extension: the value statistics and the normalised value head of the same iteration (value_norm=True)
     VALUE_NORM_FILENAME_FMT = "value_norm_%09d.state"
+    KL_COEF_FILENAME_FMT = "kl_coef_%09d.state"     # the adaptive KL coefficient of the same iteration (kl_target)
     VALUE_NORM_MIN_STD = 1e-2       # floor of the value statistics' sigma: bounds the value head's rescale factor
     BUCKET_NAME = 'dotaservice'
     MODEL_HISTOGRAM_FREQ = 128
@@ -691,7 +725,7 @@ class DotaOptimizer:
                  iterations=100000, rollout_prefetch=0, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1,
                  max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0,
                  num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False,
-                 value_norm_decay=0.99):
+                 value_norm_decay=0.99, kl_coef=0.0, kl_target=None, kl_stop=None):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
@@ -699,8 +733,18 @@ class DotaOptimizer:
         check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                            vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                            mask_padding=mask_padding, pack_sequences=pack_sequences, policy_ratio=policy_ratio,
-                           value_norm=value_norm, value_norm_decay=value_norm_decay)
+                           value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
+                           kl_stop=kl_stop)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # KL control: the loss adds kl_coef * KL(pi_prep || pi), the exact KL over the legal actions of every sampled head,
+        # and a step whose all-ranks KL exceeds kl_stop is skipped and ends the iteration's updates.  kl_target adapts
+        # kl_coef once per iteration.  kl_control fixes at construction whether prep stores the old distribution and the
+        # step runs the KL kernels; kl_coef and kl_stop can then be scheduled like the other hyper-parameters.
+        self.kl_coef = float(kl_coef)
+        self.kl_target = None if kl_target is None else float(kl_target)
+        self.kl_stop = None if kl_stop is None else float(kl_stop)
+        self.kl_control = self.kl_coef > 0.0 or self.kl_stop is not None
+        self.last_kl_updates = None         # (updates run, updates skipped) of the last train_epochs under kl_stop
         # True: PopArt.  The critic learns (R - mu) / sigma, with (mu, sigma) from running statistics of the value targets
         # (_value_norm = (m, q, w), updated once per prepared batch); the value head is rescaled at every update so that
         # sigma v + mu does not move.  policy_base's `value` output is then sigma^-1 (V - mu); prep, the batch, the
@@ -772,9 +816,11 @@ class DotaOptimizer:
                 # before the data-parallel wrapper broadcasts the weights: the normalised head must be in place
                 self._restore_value_norm(os.path.join(os.path.dirname(pretrained_model),
                                                       self.VALUE_NORM_FILENAME_FMT % (self.iteration_start - 1)))
+                self._restore_kl_coef(os.path.join(os.path.dirname(pretrained_model),
+                                                   self.KL_COEF_FILENAME_FMT % (self.iteration_start - 1)))
 
         self.policy_base.to(self.device)
-        self.flat = FlatParameterSpace(self.policy_base, self.device)
+        self.flat = FlatParameterSpace(self.policy_base, self.device, kl_tail=self.kl_control)
         if is_distributed():
             self.policy = DistributedDataParallelSparseParamCPU(self.policy_base, flat_space=self.flat)   # :268-269
         else:
@@ -795,9 +841,11 @@ class DotaOptimizer:
                     logger.warning('Not restoring Adam state from %s (%s): the moments start from zero', adam_file, e)
         self._sync_resume_state()
         self._n_actions = torch.zeros(8, dtype=torch.int32, device=self.device)   # + value-head flag (_upload_hparams)
-        # grad-norm metrics and PPO diagnostics side by side: the step reads both back with one copy
-        self._result_dev = torch.zeros(4 + _lib.PPO_STATS_SLOTS, dtype=torch.float32, device=self.device)
-        self._metrics, self._ppo_stats = self._result_dev[:4], self._result_dev[4:]
+        # grad-norm metrics and PPO diagnostics side by side: the step reads both back with one copy.  KL control: two more
+        # metrics, the all-ranks KL and the skip flag of dc_grad_finish_kl
+        self._n_metrics = _lib.FINISH_KL_METRICS if self.kl_control else 4
+        self._result_dev = torch.zeros(self._n_metrics + _lib.PPO_STATS_SLOTS, dtype=torch.float32, device=self.device)
+        self._metrics, self._ppo_stats = self._result_dev[:self._n_metrics], self._result_dev[self._n_metrics:]
         self._finish_ws = torch.zeros(_lib.FINISH_WORKSPACE_BYTES, dtype=torch.uint8, device=self.device)
         # learning_rate, e_clip, entropy_coef, vf_coef, MAX_GRAD_NORM and value_clip are read by the step's kernels from this
         # device block, rewritten from the pinned host copy before every step: a captured graph of the step holds the
@@ -806,7 +854,8 @@ class DotaOptimizer:
         self._hparams_dev = torch.zeros(_lib.HPARAM_SLOTS, dtype=torch.float64, device=self.device)
         self._hparams_uploaded = None       # the values the device block holds
         self.last_ppo_stats = None          # approx_kl, clip_fraction (and per head), explained_variance of the last step
-        self._host_result = torch.zeros(_lib.LOSS_SLOTS + 4 + _lib.PPO_STATS_SLOTS, dtype=torch.float32).pin_memory()
+        self._host_result = torch.zeros(_lib.LOSS_SLOTS + self._n_metrics + _lib.PPO_STATS_SLOTS,
+                                        dtype=torch.float32).pin_memory()
         self.last_step_launch_estimate = 0
         self._staging, self._staging_event = {}, None    # pinned host staging of the batched experience prep
         # rollout_prefetch > 0: a background thread pulls and unpickles up to that many rollouts ahead (same order, same
@@ -852,6 +901,21 @@ class DotaOptimizer:
             vn = torch.tensor(self._value_norm, dtype=torch.float64, device=self.device)
             dist.broadcast(vn, 0)
             self._value_norm = tuple(vn.tolist())
+        if self.kl_target is not None:      # the adaptive KL coefficient
+            kc = torch.tensor([self.kl_coef], dtype=torch.float64, device=self.device)
+            dist.broadcast(kc, 0)
+            self.kl_coef = float(kc.item())
+
+    def _restore_kl_coef(self, path):
+        """Resume with ``kl_target``: the adaptive KL coefficient from ``path`` (written by ``upload_model``).  Without the
+        file the coefficient starts from ``kl_coef``; without ``kl_target`` the file is ignored."""
+        if not os.path.isfile(path):
+            return
+        if self.kl_target is None:
+            logger.warning('Ignoring %s: kl_target is off, so kl_coef stays at %r', path, self.kl_coef)
+            return
+        logger.info('Restoring the adaptive KL coefficient from {}'.format(path))
+        self.kl_coef = float(torch.load(path, map_location='cpu')['kl_coef'])
 
     def _restore_value_norm(self, path):
         """Resume with ``value_norm``: the statistics and the exact normalised value head from ``path`` (written by
@@ -910,6 +974,9 @@ class DotaOptimizer:
                 torch.save({'m': m, 'q': q, 'w': w, 'weight': w_n, 'bias': b_n},
                            os.path.join(self.log_dir, self.VALUE_NORM_FILENAME_FMT % version))
                 side.append(r'value_norm_\d{9}\.state')
+            if self.kl_target is not None:  # the adaptive KL coefficient the next iteration trains with, for resume
+                torch.save({'kl_coef': self.kl_coef}, os.path.join(self.log_dir, self.KL_COEF_FILENAME_FMT % version))
+                side.append(r'kl_coef_\d{9}\.state')
             for pattern in side:            # resume only ever needs the newest: bound the disk growth
                 stale = sorted(f for f in os.listdir(self.log_dir) if re.fullmatch(pattern, f))[:-self.ADAM_FILES_KEPT]
                 for f in stale:
@@ -1067,8 +1134,14 @@ class DotaOptimizer:
                     bootstrap = ops.value_denorm(bootstrap, *vn)
                 boot = torch.cat([bootstrap.new_zeros(1), bootstrap])[boot_slot]          # per segment
             keys = ops.HEAD_KEYS
-            old_logp = ops.selected_logp([logits[k] for k in keys], [masks[k] for k in keys],
-                                         [actions[k] for k in keys]).view(Lmax, R, 5)        # :387-390
+            old_log_probs = None
+            if self.kl_control:                        # and every head's full masked log-prob row, for the KL terms
+                old_logp, old_log_probs = ops.selected_logp_rows([logits[k] for k in keys], [masks[k] for k in keys],
+                                                                 [actions[k] for k in keys])
+                old_logp, old_log_probs = old_logp.view(Lmax, R, 5), old_log_probs.view(Lmax, R, _lib.KL_ROW_FLOATS)
+            else:
+                old_logp = ops.selected_logp([logits[k] for k in keys], [masks[k] for k in keys],
+                                             [actions[k] for k in keys]).view(Lmax, R, 5)        # :387-390
             # GAE per rollout over ITS padded length: back-to-back segments, rollout-major
             values_lr = values.reshape(Lmax, R) if vn is None else ops.value_denorm(values, *vn).view(Lmax, R)
 
@@ -1107,7 +1180,7 @@ class DotaOptimizer:
                 self._update_value_norm(ret_c, real if self.mask_padding else None)
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
                     adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same, valid=valid,
-                    bootstrap=bootstrap)
+                    bootstrap=bootstrap, old_log_probs=old_log_probs)
 
     def experiences_from_rollouts(self, datas):
         """``experiences_from_rollout`` (:328-430) for all rollouts of an iteration at once: per rollout the result equals a
@@ -1134,7 +1207,8 @@ class DotaOptimizer:
                                masks={k: v[sl, i] for k, v in masks.items()},
                                values=p['values_lr'][sl, i].reshape(1, S, 1), rewards=p['rewards_np'][i, sl], hidden=hid,
                                old_logp=p['old_logp'][sl, i],
-                               valid=None if p['valid'] is None else p['valid'][:, col + j])
+                               valid=None if p['valid'] is None else p['valid'][:, col + j],
+                               old_log_probs=None if p['old_log_probs'] is None else p['old_log_probs'][sl, i])
                 seq.advantages = p['adv_c'][base + j * S: base + (j + 1) * S]
                 seq.returns = p['ret_c'][base + j * S: base + (j + 1) * S]
                 sequences.append(seq)
@@ -1172,7 +1246,9 @@ class DotaOptimizer:
         h0 = ops.stack_layers([yb[t_idx, r_idx] for yb in p['ybufs']])
         c0 = ops.stack_layers([cb[t_idx, r_idx] for cb in p['cbufs']]) if pol.cell == "lstm" else None
         old_values = chunked(p['values_lr']).contiguous()               # the critic at prep time (value clipping)
-        return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values, valid=p['valid'])
+        old_log_probs = None if p['old_log_probs'] is None else chunked(p['old_log_probs']).contiguous()
+        return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values, valid=p['valid'],
+                               old_log_probs=old_log_probs)
 
     def _packed_batch(self, p):
         """The packed ``ExperienceBatch`` of ``pack_layout`` from the prepared ``[L_max, R, ...]`` tensors: every field is
@@ -1201,13 +1277,16 @@ class DotaOptimizer:
                                  o.view((1, S * B) + tuple(o.shape[2:]))) for t, o in zip(tensors, outs)], index)
             return outs
         keys_o, keys_h = list(p['obs']), list(p['masks'])
+        kl_rows = [] if p['old_log_probs'] is None else [p['old_log_probs']]
         tm = [p['obs'][k] for k in keys_o] + [p['masks'][k] for k in keys_h] + [p['actions'][k] for k in keys_h] + \
-            [p['old_logp'], p['values_lr']]
+            [p['old_logp'], p['values_lr']] + kl_rows
         g = gather(tm, idx_tm, Lmax * R)
         obs = dict(zip(keys_o, g[:len(keys_o)]))
         masks = dict(zip(keys_h, g[len(keys_o):len(keys_o) + len(keys_h)]))
         actions = dict(zip(keys_h, g[len(keys_o) + len(keys_h):len(keys_o) + 2 * len(keys_h)]))
-        old_logp, old_values = g[-2], g[-1]
+        n_tm = len(keys_o) + 2 * len(keys_h)
+        old_logp, old_values = g[n_tm], g[n_tm + 1]
+        old_log_probs = g[n_tm + 2] if kl_rows else None
         adv, ret = gather([p['adv_c'], p['ret_c']], idx_rm, int(sum(Lps)))
         # the host layout goes up in one pinned copy: valid, the reset slots and the state-buffer coordinates
         t_rs, c_rs = np.nonzero(lay.reset_slot >= 0)
@@ -1230,7 +1309,8 @@ class DotaOptimizer:
                 tab[rk, rc] = torch.cat([bf[rt, rr] for bf in bufs], dim=1)
             return tab
         return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values, valid=valid,
-                               reset_slot=reset_slot, reset_h=table(p['ybufs']), reset_c=table(p['cbufs']) if lstm else None)
+                               reset_slot=reset_slot, reset_h=table(p['ybufs']), reset_c=table(p['cbufs']) if lstm else None,
+                               old_log_probs=old_log_probs)
 
     @staticmethod
     def list_of_dicts_to_dict_of_lists(x):
@@ -1245,7 +1325,9 @@ class DotaOptimizer:
         A device-resident batch of a shape seen before is replayed from a CUDA graph of the whole step (forward, loss,
         backward, all-reduce, finish: ~80 kernel launches -> one graph launch); batches still in flight from the host
         (``prefetch``) run the same kernels launch by launch so that the upload overlaps them.  Either way the step uses
-        the current ``learning_rate``, ``e_clip``, ``entropy_coef``, ``vf_coef``, ``MAX_GRAD_NORM`` and ``value_clip``.
+        the current ``learning_rate``, ``e_clip``, ``entropy_coef``, ``vf_coef``, ``MAX_GRAD_NORM`` and ``value_clip``
+        (and under KL control ``kl_coef`` and ``kl_stop``).  A step that ``kl_stop`` skips returns normally, with the
+        parameters, Adam moments and step counters unchanged; ``last_ppo_stats['kl_skipped']`` is then 1.
         """
         if isinstance(experiences, ExperienceBatch):
             batch = experiences if experiences.advantages.is_cuda else experiences.to(self.device)
@@ -1256,6 +1338,12 @@ class DotaOptimizer:
                              % self.value_clip)
         if self.mask_padding and batch.valid is None:
             raise ValueError("mask_padding=True needs the valid mask of experience prep, and this batch has no valid")
+        if not self.kl_control and (self.kl_coef or self.kl_stop is not None):
+            raise ValueError("kl_coef=%r / kl_stop=%r: KL control is off for this optimizer (construct it with kl_coef > 0 "
+                             "or kl_stop set, so that prep stores the old distribution)" % (self.kl_coef, self.kl_stop))
+        if self.kl_control and batch.old_log_probs is None:
+            raise ValueError("kl_coef=%r / kl_stop=%r need the log-prob rows of experience prep, and this batch has no "
+                             "old_log_probs" % (self.kl_coef, self.kl_stop))
         if batch.reset_slot is not None and not self.mask_padding:
             raise ValueError("a packed batch (reset_slot) trains only with mask_padding=True: its padding carries no "
                              "advantages or value targets")
@@ -1280,7 +1368,11 @@ class DotaOptimizer:
         torch.cuda.current_stream().synchronize()      # the step's single host sync (result read-back)
         res = host.clone()
         keys = ops.HEAD_KEYS
-        self.last_ppo_stats = self._ppo_stats_dict(res[_lib.LOSS_SLOTS + 4:].tolist(), joint=self.policy_ratio == 'joint')
+        self.last_ppo_stats = self._ppo_stats_dict(res[_lib.LOSS_SLOTS + self._n_metrics:].tolist(),
+                                                   joint=self.policy_ratio == 'joint', kl=self.kl_control)
+        if self.kl_control:             # the all-ranks KL of the finish, and whether it skipped the update
+            self.last_ppo_stats['kl_all_ranks'] = float(res[_lib.LOSS_SLOTS + 4])
+            self.last_ppo_stats['kl_skipped'] = float(res[_lib.LOSS_SLOTS + 5])
         if res[_lib.LOSS_SLOTS + 3] != 0:               # :667-669, :678-679 (parameters were left untouched)
             if math.isnan(float(res[0])):
                 raise ValueError('loss={}, policy_loss={}, entropy_loss={}, value_loss={}'.format(
@@ -1331,7 +1423,7 @@ class DotaOptimizer:
             ops.value_head_rescale(head.weight.data, head.bias.data, old, new)
 
     @staticmethod
-    def _ppo_stats_dict(st, joint=False):
+    def _ppo_stats_dict(st, joint=False, kl=False):
         out = {'approx_kl': st[_lib.STAT_APPROX_KL], 'clip_fraction': st[_lib.STAT_CLIP_FRACTION]}
         for h, k in enumerate(ops.HEAD_KEYS):
             out['approx_kl/' + k] = st[_lib.STAT_APPROX_KL + 1 + h]
@@ -1340,6 +1432,11 @@ class DotaOptimizer:
         if joint:                   # the ratio the joint objective clips, over the steps with an action
             out['approx_kl/joint'] = st[_lib.STAT_JOINT_APPROX_KL]
             out['clip_fraction/joint'] = st[_lib.STAT_JOINT_CLIP_FRACTION]
+        if kl:                      # the exact KL to the prep-time policy (this rank), per head, and the penalty beta KL
+            out['kl'] = st[_lib.STAT_KL]
+            for h, k in enumerate(ops.HEAD_KEYS):
+                out['kl/' + k] = st[_lib.STAT_KL + 1 + h]
+            out['kl_penalty'] = st[_lib.STAT_KL_PENALTY]
         return out
 
     def _upload_hparams(self):
@@ -1349,13 +1446,16 @@ class DotaOptimizer:
         previous step's copy completed before that step's result was read back."""
         # value_norm: the statistics of the last prep (mu, sigma), which the loss normalises the raw targets with; off: 0, 0
         mu, sigma = self._value_norm_moments() if self.value_norm else (0.0, 0.0)
+        # KL control: the penalty's beta and the early-stop limit (None: 0, no limit)
         vals = (float(self.learning_rate), float(self.e_clip), float(self.entropy_coef), float(self.vf_coef),
-                float(self.MAX_GRAD_NORM), float(self.value_clip or 0.0), mu, sigma)
+                float(self.MAX_GRAD_NORM), float(self.value_clip or 0.0), mu, sigma, float(self.kl_coef),
+                float(self.kl_stop or 0.0))
         if vals == self._hparams_uploaded:
             return
         h = self._hparams_host.numpy()
         for slot, v in zip((_lib.HP_LR, _lib.HP_E_CLIP, _lib.HP_ENTROPY_COEF, _lib.HP_VF_COEF, _lib.HP_MAX_GRAD_NORM,
-                            _lib.HP_VALUE_CLIP, _lib.HP_VALUE_NORM_MEAN, _lib.HP_VALUE_NORM_STD), vals):
+                            _lib.HP_VALUE_CLIP, _lib.HP_VALUE_NORM_MEAN, _lib.HP_VALUE_NORM_STD, _lib.HP_KL_COEF,
+                            _lib.HP_KL_STOP), vals):
             h[slot] = v
         self._hparams_dev.copy_(self._hparams_host, non_blocking=True)
         # the value head has a gradient only while the value loss is on (optimizer.py:660-662): with vf_coef = 0 the
@@ -1372,8 +1472,9 @@ class DotaOptimizer:
         # :619 on the module itself: the data-parallel wrapper's hook-driven reduction stays idle, the step reduces below
         packed, target_unit = self.policy_base._train_forward(batch.observations, hidden, wait=batch.wait, reset=batch.reset())
         valid = batch.valid if self.mask_padding else None
-        batch.wait(batch.old_logp, batch.advantages, batch.returns, batch.old_values, valid, *batch.masks.values(),
-                   *batch.actions.values(), *batch.observations.values())
+        old_log_probs = batch.old_log_probs if self.kl_control else None
+        batch.wait(batch.old_logp, batch.advantages, batch.returns, batch.old_values, valid, old_log_probs,
+                   *batch.masks.values(), *batch.actions.values(), *batch.observations.values())
         # e_clip / entropy_coef / vf_coef / value_clip are read from the device block (_upload_hparams); padded tokens
         # (valid = False) count for nothing under mask_padding; the policy ratio is fixed per optimizer, so a captured
         # graph of the step keeps it
@@ -1381,7 +1482,7 @@ class DotaOptimizer:
             packed, target_unit, [batch.masks[k] for k in keys], [batch.actions[k] for k in keys],
             batch.old_logp, batch.advantages, batch.returns, self.e_clip, self.entropy_coef, self.vf_coef,
             hparams=self._hparams_dev, old_value=batch.old_values, stats=self._ppo_stats, valid=valid,
-            joint=self.policy_ratio == 'joint')
+            joint=self.policy_ratio == 'joint', old_log_probs=old_log_probs, kl_out=self.flat.kl_tail)
         self._n_actions[:5].copy_(n_actions)
         torch.autograd.backward([packed, target_unit], [d_packed, d_tu])                                # :672
         # drop every reference into this step's autograd graph before the gradient finish: it holds the saved activations
@@ -1394,7 +1495,7 @@ class DotaOptimizer:
         ops.grad_finish(self.flat.param, self.flat.grad_full, self.exp_avg, self.exp_avg_sq, self.adam_steps,
                         self.flat.seg_lo, self.flat.seg_hi, self.flat.seg_head, self.flat.total, self.learning_rate, self.ADAM_BETAS,
                         self.ADAM_EPS, self.MAX_GRAD_NORM, out, self._metrics, self._finish_ws,
-                        hparams=self._hparams_dev)                                                  # :674-681
+                        hparams=self._hparams_dev, kl=self.kl_control)                              # :674-681
         return out, self._metrics
 
     # -- CUDA graph of the step ----------------------------------------------------------------------
@@ -1495,13 +1596,16 @@ class DotaOptimizer:
         per minibatch -- forward, loss (advantages normalised over the minibatch), backward, all-reduce, clip, Adam.  With
         one minibatch every epoch trains on ``batch`` itself, as the reference does (:469).  Returns the per-step lists
         ``(losses, entropies, grad_norms, ppo_stats)``.  Raises ``ValueError`` when the batch has fewer sequences than
-        minibatches."""
+        minibatches.  Under ``kl_stop`` the first step whose all-ranks KL exceeds the limit is skipped and ends the
+        iteration's updates (the shuffles of the epochs not run are not drawn); its results are the last in the lists, and
+        ``last_kl_updates`` holds (updates run, updates skipped)."""
         M = self.num_minibatches
         if batch.batch_size < M:
             raise ValueError("the batch has %d sequences, fewer than num_minibatches=%d" % (batch.batch_size, M))
         if M > 1 and not batch.advantages.is_cuda:
             batch = batch.to(self.device)                  # uploaded once; the minibatches are gathered on the device
         losses, entropies, grad_norms, ppo_stats = [], [], [], []
+        stopped = False
         for ep in range(self.epochs):                                      # :469
             self.mq.process_data_events()
             for idx in minibatch_indices(batch.batch_size, M, self.minibatch_rng):
@@ -1510,6 +1614,14 @@ class DotaOptimizer:
                 entropies.append(entropy_d)
                 grad_norms.append(grad_norm_d)
                 ppo_stats.append(self.last_ppo_stats)
+                if self.kl_control and self.last_ppo_stats['kl_skipped']:
+                    stopped = True
+                    break
+            if stopped:
+                break
+        if self.kl_control:
+            run = len(losses) - (1 if stopped else 0)
+            self.last_kl_updates = (run, self.epochs * M - run)
         return losses, entropies, grad_norms, ppo_stats
 
     # -- iteration driver (:436-579) ----------------------------------------------------------------
@@ -1590,8 +1702,20 @@ class DotaOptimizer:
             metrics['grad_norm/{}'.format(k)] = v.mean()
         for k, v in reward_dict.items():
             metrics['reward_per_sec/{}'.format(k)] = v
-        for k in ppo_stats[0]:                                             # means over the steps
-            metrics['ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
+        # means over the steps.  Under kl_stop they include the step that was skipped: its losses, grad norms and statistics were
+        # measured at the parameters it left unchanged, and its KL is the measurement that stopped the iteration
+        for k in ppo_stats[0]:
+            if k not in ('kl_all_ranks', 'kl_skipped'):
+                metrics['ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
+        if self.kl_control:
+            # d: the mean over the steps (a skipped one included) of the all-ranks KL, the same number on every rank, so
+            # the adaptive coefficient stays identical across ranks
+            d = float(np.mean([s['kl_all_ranks'] for s in ppo_stats]))
+            metrics['kl/coef'], metrics['kl/all_ranks'] = self.kl_coef, d
+            if self.kl_stop is not None:
+                metrics['kl/updates_run'], metrics['kl/updates_skipped'] = self.last_kl_updates
+            if self.kl_target is not None:                                 # for the next iteration (saved with the model)
+                self.kl_coef = kl_coef_update(self.kl_coef, d, self.kl_target)
         if self.mask_padding:                                              # share of the trained tokens that were padding
             metrics['padding_fraction'] = (n_steps - sum(rollout_lens)) / n_steps
         if self.pack_sequences:                                            # share of the sequences packing saved
@@ -1728,12 +1852,14 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          pretrained_model, mq_prefetch_count, log_dir, entropy_coef, vf_coef, run_local,
          hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
          value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
-         mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False, value_norm_decay=0.99):
+         mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False, value_norm_decay=0.99,
+         kl_coef=0.0, kl_target=None, kl_stop=None):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                        mask_padding=mask_padding, pack_sequences=pack_sequences,
                        policy_ratio=policy_ratio, value_norm=value_norm,
-                       value_norm_decay=value_norm_decay)                                 # before any process-group setup
+                       value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
+                       kl_stop=kl_stop)                                                   # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -1745,7 +1871,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         gae_lambda=gae_lambda, clip_range=clip_range, max_grad_norm=max_grad_norm, value_clip=value_clip,
         advantage_estimator=advantage_estimator, vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip,
         num_minibatches=num_minibatches, mask_padding=mask_padding, pack_sequences=pack_sequences,
-        policy_ratio=policy_ratio, value_norm=value_norm, value_norm_decay=value_norm_decay)
+        policy_ratio=policy_ratio, value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef,
+        kl_target=kl_target, kl_stop=kl_stop)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -1761,7 +1888,8 @@ def build_arg_parser():
     """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell``, ``--num-layers`` and the PPO
     settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm``, ``--value-clip``,
     ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches``, ``--mask-padding``,
-    ``--pack-sequences``, ``--policy-ratio``, ``--value-norm`` and ``--value-norm-decay``."""
+    ``--pack-sequences``, ``--policy-ratio``, ``--value-norm``, ``--value-norm-decay``, ``--kl-coef``, ``--kl-target`` and
+    ``--kl-stop``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -1806,6 +1934,12 @@ def build_arg_parser():
                         "so that its unnormalised output is preserved (reference: raw returns)")
     p.add_argument("--value-norm-decay", type=float, default=0.99,
                    help="decay of the running value statistics per prepared batch, in [0, 1)")
+    p.add_argument("--kl-coef", type=float, default=0.0,
+                   help="coefficient of a penalty on the exact KL to the policy that prepared the batch (0: off)")
+    p.add_argument("--kl-target", type=float, default=None,
+                   help="adapt --kl-coef once per iteration: doubled above 1.5x this KL, halved below it / 1.5")
+    p.add_argument("--kl-stop", type=float, default=None,
+                   help="skip a step whose KL to the prep-time policy exceeds this, and the rest of the iteration's steps")
     return p
 
 
@@ -1821,6 +1955,7 @@ if __name__ == '__main__':
              max_grad_norm=args.max_grad_norm, value_clip=args.value_clip, advantage_estimator=args.advantage_estimator,
              vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip, num_minibatches=args.num_minibatches,
              mask_padding=args.mask_padding, pack_sequences=args.pack_sequences, policy_ratio=args.policy_ratio,
-             value_norm=args.value_norm, value_norm_decay=args.value_norm_decay)
+             value_norm=args.value_norm, value_norm_decay=args.value_norm_decay, kl_coef=args.kl_coef,
+             kl_target=args.kl_target, kl_stop=args.kl_stop)
     except KeyboardInterrupt:
         pass

@@ -296,7 +296,7 @@ int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEADS], const i
  * entry point uses: e_clip, entropy_coef, vf_coef, value_clip to float, lr to double, max_grad_norm to float, so at the
  * same values the results are bit-identical to dc_ppo_loss_fwd_bwd_strided / dc_grad_finish.
  */
-#define DC_HPARAM_SLOTS 8
+#define DC_HPARAM_SLOTS 10
 #define DC_HP_LR 0             /* Adam learning rate                                               */
 #define DC_HP_E_CLIP 1         /* PPO ratio clip range epsilon                                     */
 #define DC_HP_ENTROPY_COEF 2
@@ -305,6 +305,8 @@ int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEADS], const i
 #define DC_HP_VALUE_CLIP 5     /* PPO2 value clip range; <= 0: unclipped value loss                 */
 #define DC_HP_VALUE_NORM_MEAN 6 /* value normalisation mu (read only when slot 7 > 0)               */
 #define DC_HP_VALUE_NORM_STD 7  /* value normalisation sigma; <= 0: off (the plain value loss)      */
+#define DC_HP_KL_COEF 8        /* KL penalty coefficient beta (read by dc_ppo_loss_fwd_bwd_kl only) */
+#define DC_HP_KL_STOP 9        /* KL limit of dc_grad_finish_kl; <= 0: no limit                    */
 
 /* Loss + gradient as dc_ppo_loss_fwd_bwd_strided, hyper-parameters from `hparams` [DC_HPARAM_SLOTS] (device), plus:
  *   old_value [N] fp32 or NULL: critic values at experience prep.  When hparams[DC_HP_VALUE_CLIP] = eps > 0 and
@@ -316,19 +318,21 @@ int dc_ppo_loss_fwd_bwd_strided(const float *const logits[DC_NUM_HEADS], const i
  *       6 clip fraction (share of action rows with |r-1| > e_clip), the same mean; 7..11 per head;
  *       12 explained variance 1 - Var(ret - v) / Var(ret) over all N tokens, padding included (NaN if Var(ret) = 0;
  *          over the valid tokens only under dc_ppo_loss_fwd_bwd_masked);
- *       13..15 zero (dc_ppo_loss_fwd_bwd_joint: 13, 14 see there).
+ *       13..23 zero (dc_ppo_loss_fwd_bwd_joint: 13, 14 see there; dc_ppo_loss_fwd_bwd_kl: 16..22 see there).
  * Value normalisation (PopArt; this entry point, _masked and _joint): when hparams[DC_HP_VALUE_NORM_STD] = sigma > 0, the
  *   value head's output `value` is in normalised units and the raw targets are read as r_n = fp32((r - mu) / sigma) and,
  *   for the clipped value loss, v_old,n = fp32((v_old - mu) / sigma), both computed in float64 with
  *   mu = hparams[DC_HP_VALUE_NORM_MEAN].  The value loss, dvalue and the explained-variance sums use them in place of r and
  *   v_old.  Slot 7 = 0 runs the plain arithmetic; (mu, sigma) = (0, 1) gives the same bits, as x - 0 and x / 1 are exact.
  */
-#define DC_PPO_STATS_SLOTS 16
+#define DC_PPO_STATS_SLOTS 24
 #define DC_STAT_APPROX_KL 0
 #define DC_STAT_CLIP_FRACTION 6
 #define DC_STAT_EXPLAINED_VAR 12
 #define DC_STAT_JOINT_APPROX_KL 13
 #define DC_STAT_JOINT_CLIP_FRACTION 14
+#define DC_STAT_KL 16           /* dc_ppo_loss_fwd_bwd_kl: exact KL; 17..21 per head                  */
+#define DC_STAT_KL_PENALTY 22   /* dc_ppo_loss_fwd_bwd_kl: beta * KL, the term added to the loss      */
 int dc_ppo_loss_fwd_bwd_dev(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
                             const uint8_t *const masks[DC_NUM_HEADS],
                             const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
@@ -371,7 +375,7 @@ int dc_ppo_loss_fwd_bwd_masked(const float *const logits[DC_NUM_HEADS], const in
  * head without action rows and the empty-mask rows are as in dc_ppo_loss_fwd_bwd_masked.
  *   out: 1 is the joint policy loss (not divided by 5), and 0 also adds it; 9..13 (policy per head) are 0.
  *   stats: 0..12 as dc_ppo_loss_fwd_bwd_dev (per-head KL / clip fraction of the per-head ratios); 13 the k3 KL and 14 the
- *          clip fraction of the joint ratio, averaged over the T_a tokens (0 when T_a = 0); 15 zero.
+ *          clip fraction of the joint ratio, averaged over the T_a tokens (0 when T_a = 0); 15..23 zero.
  * Algorithmic bytes: as dc_ppo_loss_fwd_bwd_masked; the statistics pass also counts T_a.
  */
 int dc_ppo_loss_fwd_bwd_joint(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
@@ -382,6 +386,40 @@ int dc_ppo_loss_fwd_bwd_joint(const float *const logits[DC_NUM_HEADS], const int
                               float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
                               float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions,
                               void *workspace, dc_stream_t stream);
+
+/* ---- KL control: a penalty on the exact KL to the prep-time policy, and an early stop at a KL limit ----------------------
+ * No counterpart in the reference.  For a token t that counts (valid, or every token), S_t is the set of heads with an
+ * action row at t and T_a the number of counting tokens with S_t not empty.  p_old is the masked softmax of experience
+ * prep and p the current one, both over the legal entries of the head's mask, in the reference's form:
+ *   KL_t = sum over h in S_t, a legal, of p_old(a) (log p_old(a) - log p(a)),    KL = (1 / T_a) sum_t KL_t (0 if T_a = 0)
+ *   loss += beta KL,   dlogits[t, h, a] += (beta / T_a)(p(a) - p_old(a)) for a legal (0 elsewhere)
+ * with beta = hparams[DC_HP_KL_COEF].  One definition for both ratio modes.
+ *
+ * dc_selected_logp_rows: dc_selected_logp's [N,5] output, bit for bit, plus logp_rows [N, DC_KL_ROW_FLOATS] fp32, every
+ *   head's full masked log-prob row in head order (columns 0-3 enum, 4-12 x, 13-21 y, 22-61 target_unit, 62-64 ability),
+ *   0 at illegal entries.  The selected entry of a row equals logp_out bit for bit.
+ * dc_ppo_loss_fwd_bwd_kl: the arguments of dc_ppo_loss_fwd_bwd_masked (valid may be NULL), plus
+ *   old_log_probs [N, DC_KL_ROW_FLOATS]  the rows dc_selected_logp_rows wrote at prep
+ *   joint          0: the per-head ratios of dc_ppo_loss_fwd_bwd_masked; 1: the joint ratio of dc_ppo_loss_fwd_bwd_joint
+ *   kl_out [2] fp32 or NULL  this call's (sum_t KL_t, T_a), e.g. the two floats behind the has-grad flags of the flat
+ *                  gradient (dc_grad_finish_kl), so that the gradient all-reduce sums them over the ranks
+ *   stats: as the entry point of the chosen ratio mode, plus DC_STAT_KL = KL, 17..21 the per-head KL (sum over the head's
+ *          action rows of its row's KL, over their count; 0 for a head without any), DC_STAT_KL_PENALTY = beta KL.
+ *   With beta = 0 the loss, dlogits, dvalue and the other stats are those of _masked / _joint bit for bit.
+ * Algorithmic bytes: those of the ratio mode's entry point + 260 per token (the old rows).  Checked before any CUDA call:
+ * the arguments of _masked, a non-null hparams and old_log_probs -> DC_EINVAL.
+ */
+#define DC_KL_ROW_FLOATS 65
+int dc_selected_logp_rows(const float *const logits[DC_NUM_HEADS], const uint8_t *const masks[DC_NUM_HEADS],
+                          const uint8_t *const actions[DC_NUM_HEADS], int64_t N, float *logp_out, float *logp_rows,
+                          dc_stream_t stream);
+int dc_ppo_loss_fwd_bwd_kl(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                           const uint8_t *const masks[DC_NUM_HEADS], const uint8_t *const actions[DC_NUM_HEADS],
+                           const float *old_logp, const float *old_log_probs, const float *adv_raw, const float *ret,
+                           const float *value, int64_t ld_value, const float *old_value, const uint8_t *valid, int64_t N,
+                           const double *hparams, int joint, float *const dlogits[DC_NUM_HEADS],
+                           const int64_t ld_dlogits[DC_NUM_HEADS], float *dvalue, int64_t ld_dvalue, float *out,
+                           float *stats, float *kl_out, int32_t *n_actions, void *workspace, dc_stream_t stream);
 
 /* ---- value normalisation (PopArt, van Hasselt et al. 2016) --------------------------------------------------------
  * No counterpart in the reference, whose critic learns raw returns (optimizer.py:660).
@@ -438,6 +476,16 @@ int dc_grad_finish_dev(float *flat_param, float *flat_grad, float *exp_avg, floa
                        int64_t total, const double *hparams, double beta1, double beta2, double adam_eps,
                        const float *loss_out, float *metrics, void *workspace, dc_stream_t stream);
 #define DC_FINISH_WORKSPACE_BYTES 1024
+/* dc_grad_finish_dev with the KL early stop.  flat_grad holds two more floats after the n_seg flags: the all-reduced
+ * (sum_t KL_t, T_a) that dc_ppo_loss_fwd_bwd_kl wrote (kl_out) on every rank.  KL = sum / T_a (0 when T_a = 0).  When
+ * hparams[DC_HP_KL_STOP] > 0 and KL exceeds it, the step is skipped: parameters, moments and step counters are left
+ * untouched, as on the NaN path, but it is not an error.  Every rank reads the same all-reduced numbers, so every rank
+ * makes the same decision.  metrics [DC_FINISH_KL_METRICS]: 0..3 as dc_grad_finish, 4 KL, 5 skipped (1) or not (0). */
+#define DC_FINISH_KL_METRICS 6
+int dc_grad_finish_kl(float *flat_param, float *flat_grad, float *exp_avg, float *exp_avg_sq,
+                      int32_t *steps, const int64_t *seg_lo, const int64_t *seg_hi, const int32_t *seg_head, int n_seg,
+                      int64_t total, const double *hparams, double beta1, double beta2, double adam_eps,
+                      const float *loss_out, float *metrics, void *workspace, dc_stream_t stream);
 
 /* ---- actor side: hierarchical action selection for a batch of A agents in one launch ----------------
  * (policy.py:23-33 MaskedCategorical, :169-178 masked_softmax, :190-216 sample_action/select_actions; caller agent.py:578-674)
