@@ -5,6 +5,8 @@ i.e. the same order as an fp32 SIMT GEMM and ~1000x tighter than single-pass TF3
 import pytest
 import torch
 
+from test_gpu_rnn_fp64 import tf32_rna
+
 pytestmark = pytest.mark.gpu
 
 
@@ -83,3 +85,40 @@ def test_gemm_wgrad_tf32x3_matches_fp64(T, No, Ni):
     ops.gemm_wgrad_tf32x3(big[:, 128:], x.to(d), want_bias=False, dw_out=acc, accumulate=True)
     ref2 = base.cpu().double() + big[:, 128:].cpu().double().t() @ x.double()
     assert (acc.cpu().double() - ref2).abs().max().item() <= 3e-6 * max(scale, 1.0) * 4
+
+
+DENSE_K896_BOUND = (96.0, 2e-6)     # K, FLOOR of max|gpu - f64| <= K * max|torch32 - f64| + FLOOR * max|f64|
+
+
+@pytest.mark.parametrize("kind", ["normal", "coherent"])
+@pytest.mark.parametrize("M,N", [(131072, 128), (524288, 512)])
+def test_gemm_tf32x3_k896_at_benchmark_rows(M, N, kind):
+    """The pre-RNN forward (K = 896, the ring kernel gemm_tf32x3_kernel) at c2's and c4's rows, against float64 on a sample
+    of rows (tile boundaries included); coherent: A = ReLU(normal), as the encoder's outputs are.  Its accumulation length
+    is the model's fixed K, so the error does not grow with M.  Measured on one H100 80GB HBM3 (700 W power limit), the
+    ratio max|gpu - f64| / max|torch32 - f64| (torch fp32 on the CPU) and max|gpu - f64| / max|f64|:
+        M 131072, N 128   normal 20.0 (6.1e-6)   coherent 27.3 (6.5e-6)
+        M 524288, N 512   normal 15.3 (6.2e-6)   coherent 27.7 (8.3e-6)
+    K = 96 leaves a margin of 3.5 over the largest ratio.  Single-pass TF32 (operands rounded by tf32_rna, exact sums)
+    exceeds the bound 7.0 to 11.8 times."""
+    from dotaclient_b200 import ops
+    d = torch.device("cuda", 0)
+    g = torch.Generator(device=d).manual_seed(M + N + (kind == "coherent"))
+    a = torch.randn(M, 896, generator=g, device=d)
+    if kind == "coherent":
+        a = torch.relu(a)
+    b = torch.randn(N, 896, generator=g, device=d) / 896 ** 0.5
+    out = ops.gemm_tf32x3(a, b)
+    rows = torch.tensor(sorted({0, 1, 127, 128, 255, 256, M // 2, M - 129, M - 128, M - 1}
+                               | set(torch.randint(0, M, (54,), generator=torch.Generator().manual_seed(M)).tolist())))
+    a_s, b_c = a[rows.to(d)].cpu(), b.cpu()
+    f64 = a_s.double() @ b_c.double().t()
+    f32 = (a_s @ b_c.t()).double()
+    tf = tf32_rna(a_s).double() @ tf32_rna(b_c).double().t()
+    err = (out[rows.to(d)].cpu().double() - f64).abs().max().item()
+    cal, ref = (f32 - f64).abs().max().item(), f64.abs().max().item()
+    lim = DENSE_K896_BOUND[0] * cal + DENSE_K896_BOUND[1] * ref
+    print("\nK 896 M %d N %d %s: ratio to fp32 %.1f, max|err|/max|f64| %.2e, tf32 %.1fx the bound"
+          % (M, N, kind, err / cal, err / ref, (tf - f64).abs().max().item() / lim))
+    assert err <= lim, (err, cal, ref)
+    assert (tf - f64).abs().max().item() > lim
