@@ -25,6 +25,9 @@ SIGNATURES = {
     "dc_device_info": (_i32, [_c.POINTER(_i32)] * 3),
     "dc_gae_scan": (_i32, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _vp, _vp, _vp]),
     "dc_vtrace_scan": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _f64, _f64, _vp, _vp, _vp, _vp]),
+    "dc_gae_scan_indexed": (_i32, [_vp, _i32, _vp, _i64, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _vp, _vp, _vp]),
+    "dc_vtrace_scan_indexed": (_i32, [_vp, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _f64, _f64, _vp,
+                                      _vp, _vp, _vp]),
     "dc_gather_columns": (_i32, [_c.POINTER(GatherDesc), _i32, _vp, _i64, _vp]),
     "dc_rnn_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "dc_rnn_seq_fwd": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),

@@ -11,6 +11,13 @@
 // fp32 with the three roundings numpy applies (no FMA contraction).
 //
 // HBM traffic: (4*n_sub + 4) read + 8 written bytes per row -- 16 B/row with pre-summed rewards.
+//
+// kIndexed (dc_gae_scan_indexed): the rows stay rollout-major for the rewards, the segments and the bootstraps, but the
+// values are read from, and the outputs written to, a token layout of their own: row r reads values[tok[r] * ld_values]
+// and writes adv[tok[r]], ret[tok[r]].  tok[r] < 0 reads a value of 0 and writes nothing.  This lets the advantages of a
+// training batch ([S, B], one rollout spread over several columns or sharing one) be recomputed where the batch holds
+// them, from values read where the head GEMM wrote them.  (4*n_sub + 8 + 4) read + 8 written bytes per row; the value
+// and output accesses are gathers.  The arithmetic is the non-indexed kernel's.
 #include "dc_common.cuh"
 #include "np_sum.cuh"
 
@@ -18,13 +25,15 @@ namespace {
 
 using dc::np_sum_row;
 
+template <bool kIndexed>
 __global__ void __launch_bounds__(128) gae_scan_kernel(const float *__restrict__ rewards, int n_sub,
                                                         const float *__restrict__ values,
                                                         const int64_t *__restrict__ seg_off, int n_seg,
                                                         const float *__restrict__ boot_value,
                                                         const float *__restrict__ boot_reward, double gamma,
                                                         double lam, float *__restrict__ adv,
-                                                        float *__restrict__ ret) {
+                                                        float *__restrict__ ret, const int64_t *__restrict__ tok,
+                                                        int64_t ld_values) {
     const int lane = threadIdx.x & 31;
     const int seg = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (seg >= n_seg) return;
@@ -43,8 +52,14 @@ __global__ void __launch_bounds__(128) gae_scan_kernel(const float *__restrict__
         const int64_t row = end - 32 + lane;
         const bool ok = row >= lo;
         float v = 0.f, r = 0.f;
+        int64_t t = row;  // where the row's value and outputs live (the row itself unless kIndexed)
         if (ok) {
-            v = values[row];
+            if constexpr (kIndexed) {
+                t = tok[row];
+                if (t >= 0) v = values[t * ld_values];
+            } else {
+                v = values[row];
+            }
             r = np_sum_row(rewards + row * (int64_t)n_sub, n_sub);
         }
         float v_next = __shfl_down_sync(0xffffffffu, v, 1);
@@ -62,7 +77,11 @@ __global__ void __launch_bounds__(128) gae_scan_kernel(const float *__restrict__
         }
         a += pa * carry_a;
         q += pr * carry_r;
-        if (ok) { adv[row] = (float)a; ret[row] = (float)q; }
+        if constexpr (kIndexed) {
+            if (ok && t >= 0) { adv[t] = (float)a; ret[t] = (float)q; }
+        } else {
+            if (ok) { adv[row] = (float)a; ret[row] = (float)q; }
+        }
         carry_a = __shfl_sync(0xffffffffu, a, 0);
         carry_r = __shfl_sync(0xffffffffu, q, 0);
         v_after = __shfl_sync(0xffffffffu, v, 0);
@@ -78,8 +97,24 @@ extern "C" int dc_gae_scan(const float *rewards, int n_sub, const float *values,
     if (n_seg == 0) return DC_OK;
     DC_REQUIRE(rewards && values && seg_off && adv && ret, DC_EINVAL, "dc_gae_scan: null pointer");
     const int warps = 4;
-    gae_scan_kernel<<<(n_seg + warps - 1) / warps, warps * 32, 0, dc_cu_stream(stream)>>>(
-        rewards, n_sub, values, seg_off, n_seg, boot_value, boot_reward, gamma, lam, adv, ret);
+    gae_scan_kernel<false><<<(n_seg + warps - 1) / warps, warps * 32, 0, dc_cu_stream(stream)>>>(
+        rewards, n_sub, values, seg_off, n_seg, boot_value, boot_reward, gamma, lam, adv, ret, nullptr, 1);
+    DC_LAUNCH_OK();
+    return DC_OK;
+}
+
+extern "C" int dc_gae_scan_indexed(const float *rewards, int n_sub, const float *values, int64_t ld_values,
+                                   const int64_t *tok, const int64_t *seg_off, int n_seg, const float *boot_value,
+                                   const float *boot_reward, double gamma, double lam, float *adv, float *ret,
+                                   dc_stream_t stream) {
+    DC_REQUIRE(n_seg >= 0 && n_sub >= 1 && n_sub < 128, DC_EINVAL, "dc_gae_scan_indexed: n_seg=%d n_sub=%d", n_seg,
+               n_sub);
+    DC_REQUIRE(ld_values >= 1, DC_EINVAL, "dc_gae_scan_indexed: ld_values=%lld must be >= 1", (long long)ld_values);
+    if (n_seg == 0) return DC_OK;
+    DC_REQUIRE(rewards && values && tok && seg_off && adv && ret, DC_EINVAL, "dc_gae_scan_indexed: null pointer");
+    const int warps = 4;
+    gae_scan_kernel<true><<<(n_seg + warps - 1) / warps, warps * 32, 0, dc_cu_stream(stream)>>>(
+        rewards, n_sub, values, seg_off, n_seg, boot_value, boot_reward, gamma, lam, adv, ret, tok, ld_values);
     DC_LAUNCH_OK();
     return DC_OK;
 }

@@ -17,6 +17,12 @@
 //
 // HBM traffic per row: 4*n_sub + 4 + 2*20 bytes read, 8 written.  The two [rows, 5] log-prob inputs are read as one
 // contiguous 640-byte block per tile each (coalesced) through shared memory.
+//
+// kIndexed (dc_vtrace_scan_indexed): as gae_scan_kernel<true>, row r reads its value at values[tok[r] * ld_values] and
+// its target log-probs at logp_target[tok[r] * 5 + h], and writes pg_adv[tok[r]], vs[tok[r]]; tok[r] < 0 reads 0 for
+// both and writes nothing.  Rewards, segments, bootstraps, behaviour log-probs and valid_len stay rollout-major.  Each
+// lane stages its own row's five target log-probs into the same shared-memory tile, so the arithmetic is unchanged.
+// (4*n_sub + 8 + 4 + 2*20) bytes read, 8 written per row.
 #include "dc_common.cuh"
 #include "np_sum.cuh"
 
@@ -26,12 +32,14 @@ constexpr int kWarps = 4;
 constexpr int kHeads = DC_NUM_HEADS;
 constexpr int kTileLp = 32 * kHeads;   // log-prob floats per 32-row tile
 
+template <bool kIndexed>
 __global__ void __launch_bounds__(kWarps * 32) vtrace_scan_kernel(
     const float *__restrict__ rewards, int n_sub, const float *__restrict__ values,
     const float *__restrict__ logp_target, const float *__restrict__ logp_behaviour,
     const int64_t *__restrict__ seg_off, int n_seg, const int64_t *__restrict__ valid_len,
     const float *__restrict__ boot_value, double gamma, double lam, double rho_clip, double c_clip,
-    float *__restrict__ pg_adv, float *__restrict__ vs_out, double *__restrict__ seg_stats) {
+    float *__restrict__ pg_adv, float *__restrict__ vs_out, double *__restrict__ seg_stats,
+    const int64_t *__restrict__ tok, int64_t ld_values) {
     __shared__ float s_lt[kWarps][kTileLp];
     __shared__ float s_lb[kWarps][kTileLp];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -54,15 +62,25 @@ __global__ void __launch_bounds__(kWarps * 32) vtrace_scan_kernel(
             const int e = j * 32 + lane;
             const int64_t idx = base * kHeads + e;
             const bool in = idx >= lo * kHeads;
-            s_lt[warp][e] = in ? logp_target[idx] : 0.f;
+            if constexpr (!kIndexed) s_lt[warp][e] = in ? logp_target[idx] : 0.f;
             s_lb[warp][e] = in ? logp_behaviour[idx] : 0.f;
+        }
+        int64_t t = -1;  // kIndexed: the token of this lane's row, where its value, target log-probs and outputs live
+        if constexpr (kIndexed) {
+            t = base + lane >= lo ? tok[base + lane] : -1;
+#pragma unroll
+            for (int h = 0; h < kHeads; ++h) s_lt[warp][lane * kHeads + h] = t >= 0 ? logp_target[t * kHeads + h] : 0.f;
         }
         __syncwarp();
         const int64_t row = base + lane;
         const bool ok = row >= lo;
         double v = 0.0, r = 0.0, logrho = 0.0;
         if (ok) {
-            v = (double)values[row];
+            if constexpr (kIndexed) {
+                if (t >= 0) v = (double)values[t * ld_values];
+            } else {
+                v = (double)values[row];
+            }
             r = (double)dc::np_sum_row(rewards + row * (int64_t)n_sub, n_sub);
 #pragma unroll
             for (int h = 0; h < kHeads; ++h)
@@ -87,8 +105,15 @@ __global__ void __launch_bounds__(kWarps * 32) vtrace_scan_kernel(
         double vs_next = __shfl_down_sync(0xffffffffu, vs, 1);
         if (lane == 31) vs_next = carry_vs;
         if (ok) {
-            vs_out[row] = (float)vs;
-            pg_adv[row] = (float)(rhob * (r + gamma * vs_next - v));
+            if constexpr (kIndexed) {
+                if (t >= 0) {
+                    vs_out[t] = (float)vs;
+                    pg_adv[t] = (float)(rhob * (r + gamma * vs_next - v));
+                }
+            } else {
+                vs_out[row] = (float)vs;
+                pg_adv[row] = (float)(rhob * (r + gamma * vs_next - v));
+            }
             if (row < valid_end) {
                 st_n += 1.0;
                 st_logrho += logrho;
@@ -127,9 +152,30 @@ extern "C" int dc_vtrace_scan(const float *rewards, int n_sub, const float *valu
     if (n_seg == 0) return DC_OK;
     DC_REQUIRE(rewards && values && logp_target && logp_behaviour && seg_off && pg_adv && vs, DC_EINVAL,
                "dc_vtrace_scan: null pointer");
-    vtrace_scan_kernel<<<(n_seg + kWarps - 1) / kWarps, kWarps * 32, 0, dc_cu_stream(stream)>>>(
+    vtrace_scan_kernel<false><<<(n_seg + kWarps - 1) / kWarps, kWarps * 32, 0, dc_cu_stream(stream)>>>(
         rewards, n_sub, values, logp_target, logp_behaviour, seg_off, n_seg, valid_len, boot_value, gamma, lam, rho_clip,
-        c_clip, pg_adv, vs, seg_stats);
+        c_clip, pg_adv, vs, seg_stats, nullptr, 1);
+    DC_LAUNCH_OK();
+    return DC_OK;
+}
+
+extern "C" int dc_vtrace_scan_indexed(const float *rewards, int n_sub, const float *values, int64_t ld_values,
+                                      const float *logp_target, const float *logp_behaviour, const int64_t *tok,
+                                      const int64_t *seg_off, int n_seg, const int64_t *valid_len,
+                                      const float *boot_value, double gamma, double lam, double rho_clip,
+                                      double c_clip, float *pg_adv, float *vs, double *seg_stats,
+                                      dc_stream_t stream) {
+    DC_REQUIRE(n_seg >= 0 && n_sub >= 1 && n_sub < 128, DC_EINVAL, "dc_vtrace_scan_indexed: n_seg=%d n_sub=%d", n_seg,
+               n_sub);
+    DC_REQUIRE(ld_values >= 1, DC_EINVAL, "dc_vtrace_scan_indexed: ld_values=%lld must be >= 1", (long long)ld_values);
+    DC_REQUIRE(rho_clip > 0.0 && c_clip > 0.0, DC_EINVAL, "dc_vtrace_scan_indexed: rho_clip=%g c_clip=%g must be > 0",
+               rho_clip, c_clip);
+    if (n_seg == 0) return DC_OK;
+    DC_REQUIRE(rewards && values && logp_target && logp_behaviour && tok && seg_off && pg_adv && vs, DC_EINVAL,
+               "dc_vtrace_scan_indexed: null pointer");
+    vtrace_scan_kernel<true><<<(n_seg + kWarps - 1) / kWarps, kWarps * 32, 0, dc_cu_stream(stream)>>>(
+        rewards, n_sub, values, logp_target, logp_behaviour, seg_off, n_seg, valid_len, boot_value, gamma, lam, rho_clip,
+        c_clip, pg_adv, vs, seg_stats, tok, ld_values);
     DC_LAUNCH_OK();
     return DC_OK;
 }

@@ -157,6 +157,72 @@ def vtrace_scan(rewards, values, logp_target, logp_behaviour, seg_off, gamma, la
     return (pg_adv, vs, seg_stats) if stats else (pg_adv, vs)
 
 
+def _indexed_args(rewards, values, tok, seg_off, out_a, out_b, boot_value):
+    """Checks and normalises the operands of the indexed scans: ``values`` (any shape) as a flat strided view and its
+    stride, the rollout-major ``rewards`` [n_rows(, n_sub)], ``tok`` [n_rows] int64, and the two contiguous fp32 outputs
+    of the token layout, written in place."""
+    _need_cuda(rewards, values, tok, seg_off, out_a, out_b, boot_value)
+    rewards = _f32c(rewards)
+    flat = values.detach().reshape(-1)
+    if flat.dtype != torch.float32:
+        raise ValueError("values must be fp32, got %s" % flat.dtype)
+    ld = flat.stride(0) if flat.numel() > 1 else 1
+    if tok.dtype != torch.int64 or tok.dim() != 1 or not tok.is_contiguous():
+        raise ValueError("tok must be a contiguous 1-D int64 tensor")
+    n_rows = tok.numel()
+    n_sub = 1 if rewards.dim() == 1 else rewards.shape[1]
+    if rewards.numel() != n_rows * n_sub:
+        raise ValueError("rewards have %d elements for %d rows of %d sub-rewards" % (rewards.numel(), n_rows, n_sub))
+    for o in (out_a, out_b):
+        if o.dtype != torch.float32 or not o.is_contiguous() or o.numel() != flat.numel():
+            raise ValueError("the outputs must be contiguous fp32 tensors of one element per value")
+    seg_off = seg_off.to(torch.int64).contiguous()
+    if boot_value is not None:
+        boot_value = _f32c(boot_value)
+        assert boot_value.numel() == seg_off.numel() - 1
+    return rewards, n_sub, flat, ld, seg_off, boot_value
+
+
+def gae_scan_indexed(rewards, values, tok, seg_off, adv, ret, gamma, lam, boot_value=None, boot_reward=None):
+    """``gae_scan`` over rollout-major rows whose values and outputs live in a token layout of their own
+    (``dc_gae_scan_indexed``): row r reads ``values.reshape(-1)[tok[r]]`` -- ``values`` may be a strided view whose
+    elements lie at one stride, such as the value column of the packed head output -- and writes ``adv`` / ``ret``
+    (contiguous fp32, one element per value) at ``tok[r]``, in place; rows with ``tok[r] < 0`` read a value of 0 and write
+    nothing.  ``rewards`` [n_rows(, n_sub)], ``seg_off``, ``boot_value`` and ``boot_reward`` are as ``gae_scan``'s.
+    ``tok`` (int64 [n_rows], device) must index ``values`` and name no token twice: the kernel cannot check it."""
+    rewards, n_sub, flat, ld, seg_off, boot_value = _indexed_args(rewards, values, tok, seg_off, adv, ret, boot_value)
+    if boot_reward is not None:
+        boot_reward = _f32c(boot_reward)
+    with PROFILE.span("gae_scan_indexed", 1):
+        _lib.check(_lib.load().dc_gae_scan_indexed(rewards.data_ptr(), n_sub, flat.data_ptr(), ld, tok.data_ptr(),
+                                                   seg_off.data_ptr(), seg_off.numel() - 1, _lib.ptr(boot_value),
+                                                   _lib.ptr(boot_reward), float(gamma), float(lam), adv.data_ptr(),
+                                                   ret.data_ptr(), _lib.stream_ptr()), "dc_gae_scan_indexed")
+    return adv, ret
+
+
+def vtrace_scan_indexed(rewards, values, logp_target, logp_behaviour, tok, seg_off, pg_adv, vs, gamma, lam, rho_clip,
+                        c_clip, boot_value=None, valid_len=None):
+    """``vtrace_scan`` with ``gae_scan_indexed``'s token layout (``dc_vtrace_scan_indexed``): row r reads its value and its
+    target log-probs ``logp_target`` [n_tokens, 5] at token ``tok[r]`` and writes ``pg_adv`` / ``vs`` there, in place;
+    ``logp_behaviour`` [n_rows, 5], ``valid_len`` and the rest stay rollout-major.  The per-segment statistics are not
+    computed."""
+    rewards, n_sub, flat, ld, seg_off, boot_value = _indexed_args(rewards, values, tok, seg_off, pg_adv, vs, boot_value)
+    _need_cuda(logp_target, logp_behaviour, valid_len)
+    logp_target, logp_behaviour = _f32c(logp_target), _f32c(logp_behaviour)
+    if logp_target.numel() != flat.numel() * 5 or logp_behaviour.numel() != tok.numel() * 5:
+        raise ValueError("logp_target must be [n_tokens, 5] and logp_behaviour [n_rows, 5]")
+    if valid_len is not None:
+        valid_len = valid_len.to(torch.int64).contiguous()
+    with PROFILE.span("vtrace_scan_indexed", 1):
+        _lib.check(_lib.load().dc_vtrace_scan_indexed(
+            rewards.data_ptr(), n_sub, flat.data_ptr(), ld, logp_target.data_ptr(), logp_behaviour.data_ptr(),
+            tok.data_ptr(), seg_off.data_ptr(), seg_off.numel() - 1, _lib.ptr(valid_len), _lib.ptr(boot_value),
+            float(gamma), float(lam), float(rho_clip), float(c_clip), pg_adv.data_ptr(), vs.data_ptr(), None,
+            _lib.stream_ptr()), "dc_vtrace_scan_indexed")
+    return pg_adv, vs
+
+
 # --------------------------------------------------------------------------------------------- minibatch gather
 _index_staging = {}     # device -> (pinned int64 buffer, event recorded after the last upload from it)
 

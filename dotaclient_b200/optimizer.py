@@ -237,6 +237,7 @@ class ExperienceBatch:
         self.reset_slot, self.reset_h, self.reset_c = reset_slot, reset_h, reset_c
         self._ready = {}        # data_ptr -> event of an upload still to be waited for (``to`` from pinned memory)
         self._slot = None       # the DotaOptimizer input slot whose static buffers these tensors are (``prefetch``)
+        self.refresh = None     # AdvantageRefresh of batch_from_rollouts under recompute_advantages; not copied by map
 
     def map(self, fn):
         """A batch of the same structure with ``fn(tensor)`` in every slot; absent optional fields stay None."""
@@ -363,6 +364,21 @@ class ExperienceBatch:
                                old_values=old_values, valid=valid, old_log_probs=old_log_probs)
 
 
+class AdvantageRefresh(typing.NamedTuple):
+    """What the advantage refresh between PPO epochs (``DotaOptimizer(recompute_advantages=True)``) needs beyond the batch,
+    as experience prep had it (device tensors, rows rollout-major): ``rewards [n_rows, 10]``, the scan segments
+    ``seg_off [n_seg + 1]`` (``rollout_segments``), the per-segment bootstraps ``boot [n_seg]`` (None: all 0), ``tok
+    [n_rows]`` (``refresh_token_map``) and, for V-trace, the behaviour log-probs ``behaviour_logp [n_rows, 5]`` and
+    ``valid_len [n_seg]``.  ``batch_from_rollouts`` sets it as ``ExperienceBatch.refresh``, a plain attribute outside
+    ``FIELDS``: ``map``, ``gather``, ``to`` and the graph input slots do not carry it."""
+    rewards: torch.Tensor
+    seg_off: torch.Tensor
+    boot: typing.Optional[torch.Tensor]
+    tok: typing.Optional[torch.Tensor]
+    behaviour_logp: typing.Optional[torch.Tensor]
+    valid_len: typing.Optional[torch.Tensor]
+
+
 class _CapturedStep(typing.NamedTuple):
     """A CUDA graph of the whole step, its static input batch and its device result vector (loss slots)."""
     static: ExperienceBatch
@@ -396,13 +412,15 @@ POLICY_RATIOS = ('per_head', 'joint')
 def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
                        vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False, pack_sequences=False,
                        policy_ratio='per_head', value_norm=False, value_norm_decay=0.99, kl_coef=0.0, kl_target=None,
-                       kl_stop=None):
+                       kl_stop=None, recompute_advantages=False):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
     vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool,
     pack_sequences a bool that is True only with mask_padding, policy_ratio one of ``POLICY_RATIOS``, value_norm a bool
     and 0 <= value_norm_decay < 1, finite kl_coef >= 0, kl_target None or finite > 0 (and then kl_coef > 0), kl_stop None
-    or finite > 0.  NaN fails every check."""
+    or finite > 0, recompute_advantages a bool.  NaN fails every check."""
+    if not isinstance(recompute_advantages, bool):
+        raise ValueError("recompute_advantages=%r: must be True or False" % (recompute_advantages,))
     if not isinstance(value_norm, bool):
         raise ValueError("value_norm=%r: must be True or False" % (value_norm,))
     if isinstance(value_norm_decay, bool) or not isinstance(value_norm_decay, numbers.Real) \
@@ -615,6 +633,53 @@ def pack_layout(lengths, seq_len):
     return PackLayout(B, K, n_full, rollout, step, reset_slot, h0_rollout, h0_step)
 
 
+def chunk_columns(t, Lps, seq_len, whole=False):
+    """The unpacked batch layout: a time-major ``[L_max, R, ...]`` tensor -> ``[seq_len, sum(Lp_i / seq_len), ...]``, rollout
+    i's ``Lps[i]`` padded rows cut into ``seq_len`` chunks of one column each, rollout by rollout, chunk by chunk.
+    ``whole``: every rollout is exactly one chunk, and ``t`` is returned as it is."""
+    if whole:
+        return t
+    S = int(seq_len)
+    parts = [t[:Lps[i], i].reshape((Lps[i] // S, S) + tuple(t.shape[2:])).transpose(0, 1) for i in range(len(Lps))]
+    return torch.cat(parts, dim=1)
+
+
+def packed_rows(lay, Lps):
+    """The rollout-major row of experience prep (rollout i's padded rows follow rollouts 0 .. i-1's) that every token of
+    the packed layout ``lay`` holds: int64 ``[S, B]``, -1 at padding tokens."""
+    base = np.concatenate([[0], np.cumsum(Lps)[:-1]]).astype(np.int64)
+    return np.where(lay.rollout >= 0, base[np.maximum(lay.rollout, 0)] + lay.step, -1)
+
+
+def refresh_token_map(lengths, seq_len, pack, mask_padding, layout=None):
+    """For the rollout-major rows of experience prep (rollout i's ``Lp_i`` padded rows in turn), the token ``t * B + c``
+    of the ``[S, B]`` training batch that ``batch_from_rollouts`` builds from rollouts of ``lengths`` real steps, or -1
+    where the batch holds no such row or prep zeroes it (under ``mask_padding``: the rows after a rollout's real steps).
+    Derived from the batch's own layout: ``chunk_columns`` applied to the row numbers, or with ``pack`` the inverse of
+    ``packed_rows``.  Returns int64 ``[sum(Lp_i)]``.  The advantage refresh (``recompute_advantages``) scans the rows and
+    reads values from, and writes advantages to, these tokens (``ops.gae_scan_indexed``).  ``layout``: with ``pack``, the
+    ``pack_layout`` of ``lengths`` when the caller has it already."""
+    S = int(seq_len)
+    Ls = [int(L) for L in lengths]
+    Lps = [(L + S - 1) // S * S for L in Ls]
+    n_rows = int(sum(Lps))
+    base = np.concatenate([[0], np.cumsum(Lps)[:-1]]).astype(np.int64)
+    if pack:
+        rows = packed_rows(pack_layout(Ls, S) if layout is None else layout, Lps)
+    else:
+        Lmax = max(Lps, default=0)
+        t = np.arange(Lmax, dtype=np.int64)[:, None]
+        grid = torch.from_numpy(np.where(t < np.asarray(Lps)[None, :], base[None, :] + t, -1))
+        rows = chunk_columns(grid, Lps, S).numpy().reshape(S, -1) if Lps else np.zeros((S, 0), dtype=np.int64)
+    tok = np.full(n_rows, -1, dtype=np.int64)
+    held = rows >= 0
+    tok[rows[held]] = np.flatnonzero(held.reshape(-1))
+    if mask_padding:                           # prep zeroes the advantages and returns of padded rows
+        step = np.arange(n_rows, dtype=np.int64) - np.repeat(base, Lps)
+        tok[step >= np.repeat(np.asarray(Ls, dtype=np.int64), Lps)] = -1
+    return tok
+
+
 def sequence_count(lengths, seq_len, pack=False):
     """The number of training sequences that rollouts of ``lengths`` steps make: ``ceil(L / seq_len)`` each, or with
     ``pack`` the columns of their ``pack_layout``."""
@@ -712,6 +777,8 @@ class DotaOptimizer:
     BUCKET_NAME = 'dotaservice'
     MODEL_HISTOGRAM_FREQ = 128
     MAX_GRAD_NORM = 0.5
+    # the advantage refresh (recompute_advantages) runs its forward over blocks of time steps of about this many tokens
+    REFRESH_CHUNK_TOKENS = 32768
     SPEED_KEY = 'steps per s'
     ADAM_BETAS = (0.9, 0.999)       # torch.optim.Adam defaults (:275)
     ADAM_EPS = 1e-8
@@ -725,7 +792,7 @@ class DotaOptimizer:
                  iterations=100000, rollout_prefetch=0, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1,
                  max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0,
                  num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False,
-                 value_norm_decay=0.99, kl_coef=0.0, kl_target=None, kl_stop=None):
+                 value_norm_decay=0.99, kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
@@ -734,8 +801,12 @@ class DotaOptimizer:
                            vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                            mask_padding=mask_padding, pack_sequences=pack_sequences, policy_ratio=policy_ratio,
                            value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
-                           kl_stop=kl_stop)
+                           kl_stop=kl_stop, recompute_advantages=recompute_advantages)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # True: before every epoch after the first, train_epochs recomputes the batch's advantages and returns with the
+        # current critic (and, for V-trace, the current policy as the target), from prep's rewards, segments and bootstraps
+        # (_refresh_advantages); batch_from_rollouts then attaches what that needs (ExperienceBatch.refresh)
+        self.recompute_advantages = recompute_advantages
         # KL control: the loss adds kl_coef * KL(pi_prep || pi), the exact KL over the legal actions of every sampled head,
         # and a step whose all-ranks KL exceeds kl_stop is skipped and ends the iteration's updates.  kl_target adapts
         # kl_coef once per iteration.  kl_control fixes at construction whether prep stores the old distribution and the
@@ -1156,13 +1227,15 @@ class DotaOptimizer:
                 rew_c = torch.from_numpy(np.concatenate([rewards_np[i, :Lps[i]] for i in range(R)])).to(dev)
             # [real | padding] per rollout under mask_padding or when cut: the bootstrap follows step L_i
             seg = torch.tensor(seg_np, dtype=torch.int64, device=dev)
+            blp_c = valid_len = None
             if vtrace:
                 # heads that took no action carry no behaviour log-prob (old_logp is 0 there too); padding rows are 0 already
                 acted = torch.stack([actions[k].any(dim=-1) for k in keys], dim=-1)
                 behaviour_logp = torch.where(acted, behaviour_logp, 0.0)
                 valid_len = torch.from_numpy(seg_valid).pin_memory().to(dev, non_blocking=True)  # padding: no real steps
+                blp_c = rollout_major(behaviour_logp)
                 adv_c, ret_c, self._vtrace_seg_stats = ops.vtrace_scan(
-                    rew_c, vals_c, rollout_major(old_logp), rollout_major(behaviour_logp), seg, gamma=self.gamma,
+                    rew_c, vals_c, rollout_major(old_logp), blp_c, seg, gamma=self.gamma,
                     lam=self.gae_lambda, rho_clip=self.vtrace_rho_clip, c_clip=self.vtrace_c_clip, boot_value=boot,
                     valid_len=valid_len, stats=True)
             else:
@@ -1180,7 +1253,8 @@ class DotaOptimizer:
                 self._update_value_norm(ret_c, real if self.mask_padding else None)
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
                     adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same, valid=valid,
-                    bootstrap=bootstrap, old_log_probs=old_log_probs)
+                    bootstrap=bootstrap, old_log_probs=old_log_probs,
+                    refresh=dict(rewards=rew_c, seg_off=seg, boot=boot, behaviour_logp=blp_c, valid_len=valid_len))
 
     def experiences_from_rollouts(self, datas):
         """``experiences_from_rollout`` (:328-430) for all rollouts of an iteration at once: per rollout the result equals a
@@ -1222,16 +1296,23 @@ class DotaOptimizer:
         Python objects, no per-sequence re-stacking (an iteration of the stream has ~1000 sequences of 16 steps)."""
         S, pol = self.seq_len, self.policy_base
         p = self._prepare_rollouts(datas)
-        if self.pack_sequences:
-            return self._packed_batch(p)
-        R, Lps = len(datas), p['Lps']
+        lay = pack_layout(p['Ls'], S) if self.pack_sequences else None
+        batch = self._packed_batch(p, lay) if self.pack_sequences else self._unpacked_batch(p)
+        if self.recompute_advantages:          # the scan inputs of prep and where each of its rows sits in the batch
+            tok = refresh_token_map(p['Ls'], S, self.pack_sequences, self.mask_padding, layout=lay)
+            tok = torch.from_numpy(tok).pin_memory().to(self.device, non_blocking=True)
+            batch.refresh = AdvantageRefresh(tok=tok, **p['refresh'])
+        return batch
+
+    def _unpacked_batch(self, p):
+        """The ``ExperienceBatch`` of ``batch_from_rollouts`` without packing: every rollout's chunks in turn
+        (``chunk_columns``)."""
+        S, pol = self.seq_len, self.policy_base
+        R, Lps = len(p['Ls']), p['Lps']
         n_chunks = [lp // S for lp in Lps]
 
         def chunked(t):                       # [Lmax, R, ...] -> [S, sum(n_chunks), ...]
-            if p['same'] and p['Lmax'] == S:
-                return t
-            parts = [t[:Lps[i], i].reshape((n_chunks[i], S) + tuple(t.shape[2:])).transpose(0, 1) for i in range(R)]
-            return torch.cat(parts, dim=1)
+            return chunk_columns(t, Lps, S, whole=p['same'] and p['Lmax'] == S)
         obs = {k: chunked(v) for k, v in p['obs'].items()}
         masks = {k: chunked(v) for k, v in p['masks'].items()}
         actions = {k: chunked(v) for k, v in p['actions'].items()}
@@ -1250,7 +1331,7 @@ class DotaOptimizer:
         return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values, valid=p['valid'],
                                old_log_probs=old_log_probs)
 
-    def _packed_batch(self, p):
+    def _packed_batch(self, p, lay):
         """The packed ``ExperienceBatch`` of ``pack_layout`` from the prepared ``[L_max, R, ...]`` tensors: every field is
         one token gather per index (``dc_gather_columns`` over ``[1, L_max * R, ...]`` views, and over the rollout-major
         advantages and returns), so the assembly is a handful of launches whatever the number of sequences.  A padding token
@@ -1259,7 +1340,6 @@ class DotaOptimizer:
         S, pol, dev = self.seq_len, self.policy_base, self.device
         Ls, Lps, Lmax = p['Ls'], p['Lps'], p['Lmax']
         R = len(Ls)
-        lay = pack_layout(Ls, S)
         check_reset_slots(lay.reset_slot, lay.K)
         B = lay.B
         real = lay.rollout >= 0
@@ -1268,7 +1348,8 @@ class DotaOptimizer:
         src_t = np.where(real, lay.step, Ls[pad_r])
         base = np.concatenate([[0], np.cumsum(Lps)[:-1]]).astype(np.int64)
         idx_tm = (src_t * R + src_r).reshape(-1)                          # rows of the time-major [L_max, R] tensors
-        idx_rm = (base[src_r] + src_t).reshape(-1)                        # rows of the rollout-major scan outputs
+        # rows of the rollout-major scan outputs
+        idx_rm = np.where(real, packed_rows(lay, Lps), base[pad_r] + Ls[pad_r]).reshape(-1)
 
         def gather(tensors, index, n_src):
             outs = [torch.empty((S, B) + tuple(t.shape[2:]) if t.dim() >= 2 else (S, B), dtype=t.dtype, device=dev)
@@ -1598,16 +1679,26 @@ class DotaOptimizer:
         ``(losses, entropies, grad_norms, ppo_stats)``.  Raises ``ValueError`` when the batch has fewer sequences than
         minibatches.  Under ``kl_stop`` the first step whose all-ranks KL exceeds the limit is skipped and ends the
         iteration's updates (the shuffles of the epochs not run are not drawn); its results are the last in the lists, and
-        ``last_kl_updates`` holds (updates run, updates skipped)."""
+        ``last_kl_updates`` holds (updates run, updates skipped).
+
+        With ``recompute_advantages`` every epoch after the first starts with ``_refresh_advantages``, which rewrites
+        ``batch.advantages`` and ``batch.returns`` in place; no refresh follows a step that ``kl_stop`` skipped.  The batch
+        must then come from ``batch_from_rollouts`` (``ExperienceBatch.refresh``), else ``ValueError`` before any launch."""
         M = self.num_minibatches
         if batch.batch_size < M:
             raise ValueError("the batch has %d sequences, fewer than num_minibatches=%d" % (batch.batch_size, M))
+        refresh = self.recompute_advantages and self.epochs > 1
+        if refresh and batch.refresh is None:
+            raise ValueError("recompute_advantages=True needs the scan inputs of experience prep, and this batch has none "
+                             "(ExperienceBatch.refresh): train on a batch from batch_from_rollouts")
         if M > 1 and not batch.advantages.is_cuda:
             batch = batch.to(self.device)                  # uploaded once; the minibatches are gathered on the device
         losses, entropies, grad_norms, ppo_stats = [], [], [], []
         stopped = False
         for ep in range(self.epochs):                                      # :469
             self.mq.process_data_events()
+            if refresh and ep > 0:
+                self._refresh_advantages(batch)
             for idx in minibatch_indices(batch.batch_size, M, self.minibatch_rng):
                 loss_d, entropy_d, grad_norm_d = self.train(experiences=batch if M == 1 else batch.gather(idx))
                 losses.append(loss_d)
@@ -1623,6 +1714,54 @@ class DotaOptimizer:
             run = len(losses) - (1 if stopped else 0)
             self.last_kl_updates = (run, self.epochs * M - run)
         return losses, entropies, grad_norms, ppo_stats
+
+    def _refresh_advantages(self, batch):
+        """Recomputes ``batch.advantages`` and ``batch.returns`` in place with the current weights (``recompute_advantages``;
+        Andrychowicz et al. 2021, section 3.5): a no-grad training forward over the whole batch gives V for every token
+        (denormalised with the current statistics under ``value_norm``) and, for V-trace, the current policy's log-probs of
+        the taken actions, the new target; then prep's segmented scan runs again over prep's rollout-major rewards,
+        segments and bootstraps, reading and writing the batch's tokens (``ops.gae_scan_indexed`` /
+        ``vtrace_scan_indexed``, ``refresh_token_map``).  Rows that prep zeroed are not written.  Everything else in the
+        batch -- the old log-probs, the old values, the initial and reset states -- stays as prep made it.
+
+        The forward is the training step's (``Policy._train_forward``: encoder, recurrence with the batch's resets, heads),
+        run over blocks of ``max(1, REFRESH_CHUNK_TOKENS // B)`` time steps with the recurrent
+        state carried from block to block, so its transient memory is bounded by the block, not by the batch."""
+        r, pol, keys = batch.refresh, self.policy_base, ops.HEAD_KEYS
+        S, B = batch.seq_len, batch.batch_size
+        vtrace = self.advantage_estimator == 'vtrace'
+        hidden = (batch.h0, batch.c0) if pol.cell == "lstm" else batch.h0
+        reset = batch.reset()
+        T = max(1, self.REFRESH_CHUNK_TOKENS // B)
+        col = ops.PACK_COLS["value"][0]
+        values = None if T >= S else torch.empty((S, B), dtype=torch.float32, device=self.device)
+        target = torch.empty((S * B, 5), dtype=torch.float32, device=self.device) if vtrace else None
+        with torch.no_grad():
+            for t0 in range(0, S, T):
+                t1 = min(S, t0 + T)
+                x, unit_embedding = pol._encode(batch.observations['env'][t0:t1],
+                                                [batch.observations[k][t0:t1] for k in Policy.INPUT_KEYS[1:]])
+                y, hidden = pol._recur(x.contiguous(), hidden, None if reset is None else (reset[0][t0:t1],) + reset[1:])
+                packed, target_unit = pol._head_outputs(y, unit_embedding)
+                if values is None:                  # one block: the scan reads the value column where the GEMM wrote it
+                    values = packed[..., col]
+                else:
+                    values[t0:t1] = packed[..., col]
+                if vtrace:
+                    logits = [target_unit if k == "target_unit" else packed[..., ops.PACK_COLS[k][0]:ops.PACK_COLS[k][1]]
+                              for k in keys]
+                    target[t0 * B:t1 * B] = ops.selected_logp(logits, [batch.masks[k][t0:t1] for k in keys],
+                                                              [batch.actions[k][t0:t1] for k in keys])
+                del x, unit_embedding, y, packed, target_unit
+            if self.value_norm:
+                values = ops.value_denorm(values, *self._value_norm_moments())
+            if vtrace:
+                ops.vtrace_scan_indexed(r.rewards, values, target, r.behaviour_logp, r.tok, r.seg_off, batch.advantages,
+                                        batch.returns, self.gamma, self.gae_lambda, self.vtrace_rho_clip,
+                                        self.vtrace_c_clip, boot_value=r.boot, valid_len=r.valid_len)
+            else:
+                ops.gae_scan_indexed(r.rewards, values, r.tok, r.seg_off, batch.advantages, batch.returns, self.gamma,
+                                     self.gae_lambda, boot_value=r.boot, boot_reward=r.boot)
 
     # -- iteration driver (:436-579) ----------------------------------------------------------------
     def run(self):
@@ -1853,13 +1992,13 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
          value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
          mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False, value_norm_decay=0.99,
-         kl_coef=0.0, kl_target=None, kl_stop=None):
+         kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                        mask_padding=mask_padding, pack_sequences=pack_sequences,
                        policy_ratio=policy_ratio, value_norm=value_norm,
                        value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
-                       kl_stop=kl_stop)                                                   # before any process-group setup
+                       kl_stop=kl_stop, recompute_advantages=recompute_advantages)        # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -1872,7 +2011,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         advantage_estimator=advantage_estimator, vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip,
         num_minibatches=num_minibatches, mask_padding=mask_padding, pack_sequences=pack_sequences,
         policy_ratio=policy_ratio, value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef,
-        kl_target=kl_target, kl_stop=kl_stop)
+        kl_target=kl_target, kl_stop=kl_stop, recompute_advantages=recompute_advantages)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -1940,6 +2079,9 @@ def build_arg_parser():
                    help="adapt --kl-coef once per iteration: doubled above 1.5x this KL, halved below it / 1.5")
     p.add_argument("--kl-stop", type=float, default=None,
                    help="skip a step whose KL to the prep-time policy exceeds this, and the rest of the iteration's steps")
+    p.add_argument("--recompute-advantages", action="store_true",
+                   help="recompute the batch's advantages and returns with the current critic before every epoch after "
+                        "the first")
     return p
 
 
@@ -1956,6 +2098,6 @@ if __name__ == '__main__':
              vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip, num_minibatches=args.num_minibatches,
              mask_padding=args.mask_padding, pack_sequences=args.pack_sequences, policy_ratio=args.policy_ratio,
              value_norm=args.value_norm, value_norm_decay=args.value_norm_decay, kl_coef=args.kl_coef,
-             kl_target=args.kl_target, kl_stop=args.kl_stop)
+             kl_target=args.kl_target, kl_stop=args.kl_stop, recompute_advantages=args.recompute_advantages)
     except KeyboardInterrupt:
         pass

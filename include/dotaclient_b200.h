@@ -84,6 +84,29 @@ int dc_vtrace_scan(const float *rewards, int n_sub, const float *values, const f
                    const float *boot_value, double gamma, double lam, double rho_clip, double c_clip, float *pg_adv,
                    float *vs, double *seg_stats, dc_stream_t stream);
 
+/* ---- GAE / V-trace over a token layout of their own -----------------------------------------
+ * The advantage refresh between PPO epochs (DotaOptimizer(recompute_advantages=True)): the same scans, with the same
+ * arithmetic, where the rows -- rewards, seg_off, boot_value, boot_reward, logp_behaviour and valid_len, all as above
+ * -- stay rollout-major, while each row's value and outputs live at a token of a [S, B] training batch:
+ *   tok       [n_rows] int64   the token of row r; tok[r] < 0: the row's value (and target log-probs) read as 0, and
+ *                              nothing is written for it
+ *   values    value of row r at values[tok[r] * ld_values]; ld_values >= 1 (the packed head output's value column:
+ *             ld_values = its row width)
+ *   logp_target  [n_tokens, 5] (V-trace) the target log-probs of row r at logp_target[tok[r] * 5 + h]
+ *   adv / pg_adv, ret / vs   written at [tok[r]] only; every other element keeps its contents
+ * Preconditions the library cannot check (tok is on the device): every tok[r] >= 0 indexes the token arrays, and no
+ * two rows share a token.  The caller builds tok on the host and checks it there.
+ * Checked: as dc_gae_scan / dc_vtrace_scan, ld_values >= 1 and tok non-null -> DC_EINVAL before any CUDA call.
+ */
+int dc_gae_scan_indexed(const float *rewards, int n_sub, const float *values, int64_t ld_values, const int64_t *tok,
+                        const int64_t *seg_off, int n_seg, const float *boot_value, const float *boot_reward,
+                        double gamma, double lam, float *adv, float *ret, dc_stream_t stream);
+int dc_vtrace_scan_indexed(const float *rewards, int n_sub, const float *values, int64_t ld_values,
+                           const float *logp_target, const float *logp_behaviour, const int64_t *tok,
+                           const int64_t *seg_off, int n_seg, const int64_t *valid_len, const float *boot_value,
+                           double gamma, double lam, double rho_clip, double c_clip, float *pg_adv, float *vs,
+                           double *seg_stats, dc_stream_t stream);
+
 /* ---- minibatch assembly: column gather ----------------------------------------------------
  * Picks the sequence columns `index` out of many time-major tensors in ONE launch (the minibatches of PPO epochs,
  * DotaOptimizer.train_epochs; the reference trains on the whole batch and has no counterpart).  Descriptor d describes a
