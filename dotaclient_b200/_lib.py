@@ -29,6 +29,9 @@ SIGNATURES = {
     "dc_vtrace_scan_indexed": (_i32, [_vp, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _f64, _f64, _vp,
                                       _vp, _vp, _vp]),
     "dc_gather_columns": (_i32, [_c.POINTER(GatherDesc), _i32, _vp, _i64, _vp]),
+    "dc_gather_columns_fill": (_i32, [_c.POINTER(GatherDesc), _i32, _vp, _i64, _vp]),
+    "dc_refresh_states": (_i32, [_i32, _i32, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp,
+                                 _vp, _vp]),
     "dc_rnn_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "dc_rnn_seq_fwd": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "dc_rnn_seq_bwd": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
@@ -96,6 +99,7 @@ KL_ROW_FLOATS = 65          # entries of one token's masked log-prob row over th
 FINISH_KL_METRICS = 6       # metrics of dc_grad_finish_kl: the four of dc_grad_finish, the all-ranks KL, the skip flag
 VTRACE_STATS_SLOTS = 8      # per-segment fp64 sums written by dc_vtrace_scan (DC_VTRACE_STATS_SLOTS)
 GATHER_MAX_TENSORS = 32     # descriptors per dc_gather_columns call (DC_GATHER_MAX_TENSORS)
+REFRESH_MAX_LAYERS = 16     # recurrent layers dc_refresh_states handles (DC_REFRESH_MAX_LAYERS)
 MAX_PARAM_TENSORS = 96      # kMaxSeg of csrc/grad_finish.cu: parameter tensors dc_grad_flags / dc_grad_finish can handle
 
 _lib = None

@@ -13,6 +13,11 @@
 // the reads are contiguous within a source row.  Each thread issues its kUnroll loads before its stores.
 //
 // HBM traffic: outer*n_index*row_bytes read and the same written per descriptor, plus the index (L1/L2 resident).
+//
+// kFill (dc_gather_columns_fill): an index value < 0 writes a row of zeros and reads nothing.  The state refresh between
+// PPO epochs uses it to build the rollout-major [T, R, ...] inputs of each time block from a training batch (rows the
+// batch does not hold are zeros, as in experience prep) and to bring rollout-major values back into the batch layout.
+// Bytes as above, less the rows a negative index skips on the read side.
 #include <climits>
 #include "dc_common.cuh"
 
@@ -32,7 +37,7 @@ struct GatherParams {
 
 // Copies units [u0, u0 + kUnitsPerBlock) of the destination, clipped to `total`.  I is the index type of the unit
 // arithmetic: 32-bit division is several times cheaper than 64-bit, and the byte path is division-bound.
-template <typename V, typename I>
+template <bool kFill, typename V, typename I>
 __device__ __forceinline__ void gather_units(const V *__restrict__ src, V *__restrict__ dst, const int64_t *__restrict__ index,
                                              I row_units, I n_index, I src_cols, I total, I u0) {
     V v[kUnroll];
@@ -44,7 +49,12 @@ __device__ __forceinline__ void gather_units(const V *__restrict__ src, V *__res
         if (u < total) {
             const I row = u / row_units, b = u - row * row_units;
             const I o = row / n_index, j = row - o * n_index;
-            v[k] = src[(o * src_cols + (I)index[j]) * row_units + b];
+            if constexpr (kFill) {
+                const int64_t s = index[j];
+                v[k] = s < 0 ? V{} : src[(o * src_cols + (I)s) * row_units + b];
+            } else {
+                v[k] = src[(o * src_cols + (I)index[j]) * row_units + b];
+            }
         }
     }
 #pragma unroll
@@ -52,7 +62,7 @@ __device__ __forceinline__ void gather_units(const V *__restrict__ src, V *__res
         if (at[k] < total) dst[at[k]] = v[k];
 }
 
-template <typename V>
+template <bool kFill, typename V>
 __device__ __forceinline__ void gather_desc(const dc_gather_desc &d, int narrow, const int64_t *__restrict__ index,
                                             int64_t n_index, long long block) {
     const int64_t row_units = d.row_bytes / (int64_t)sizeof(V);
@@ -61,12 +71,13 @@ __device__ __forceinline__ void gather_desc(const dc_gather_desc &d, int narrow,
     const V *src = static_cast<const V *>(d.src);
     V *dst = static_cast<V *>(d.dst);
     if (narrow)
-        gather_units<V, uint32_t>(src, dst, index, (uint32_t)row_units, (uint32_t)n_index, (uint32_t)d.src_cols,
+        gather_units<kFill, V, uint32_t>(src, dst, index, (uint32_t)row_units, (uint32_t)n_index, (uint32_t)d.src_cols,
                                   (uint32_t)total, (uint32_t)u0);
     else
-        gather_units<V, int64_t>(src, dst, index, row_units, n_index, d.src_cols, total, u0);
+        gather_units<kFill, V, int64_t>(src, dst, index, row_units, n_index, d.src_cols, total, u0);
 }
 
+template <bool kFill>
 __global__ void __launch_bounds__(kThreads) gather_columns_kernel(const __grid_constant__ GatherParams p,
                                                                   const int64_t *__restrict__ index, int64_t n_index) {
     const long long b = blockIdx.x;
@@ -74,31 +85,30 @@ __global__ void __launch_bounds__(kThreads) gather_columns_kernel(const __grid_c
     while (k + 1 < p.n_desc && b >= p.block_start[k + 1]) ++k;      // block-uniform, at most 31 steps
     const long long block = b - p.block_start[k];
     switch (p.unit[k]) {
-        case 16: gather_desc<uint4>(p.d[k], p.narrow[k], index, n_index, block); break;
-        case 4: gather_desc<uint32_t>(p.d[k], p.narrow[k], index, n_index, block); break;
-        default: gather_desc<uint8_t>(p.d[k], p.narrow[k], index, n_index, block); break;
+        case 16: gather_desc<kFill, uint4>(p.d[k], p.narrow[k], index, n_index, block); break;
+        case 4: gather_desc<kFill, uint32_t>(p.d[k], p.narrow[k], index, n_index, block); break;
+        default: gather_desc<kFill, uint8_t>(p.d[k], p.narrow[k], index, n_index, block); break;
     }
 }
 
 bool aligned(const void *p, int64_t a) { return reinterpret_cast<uintptr_t>(p) % (uintptr_t)a == 0; }
 
-}  // namespace
-
-extern "C" int dc_gather_columns(const dc_gather_desc *descs, int n_desc, const int64_t *index, int64_t n_index,
-                                 dc_stream_t stream) {
-    DC_REQUIRE(n_desc >= 0 && n_desc <= DC_GATHER_MAX_TENSORS, DC_EINVAL, "dc_gather_columns: n_desc=%d outside [0, %d]",
+template <bool kFill>
+int gather_launch(const char *name, const dc_gather_desc *descs, int n_desc, const int64_t *index, int64_t n_index,
+                  dc_stream_t stream) {
+    DC_REQUIRE(n_desc >= 0 && n_desc <= DC_GATHER_MAX_TENSORS, DC_EINVAL, "%s: n_desc=%d outside [0, %d]", name,
                n_desc, DC_GATHER_MAX_TENSORS);
-    DC_REQUIRE(n_index >= 0, DC_EINVAL, "dc_gather_columns: n_index=%lld < 0", (long long)n_index);
+    DC_REQUIRE(n_index >= 0, DC_EINVAL, "%s: n_index=%lld < 0", name, (long long)n_index);
     if (n_desc == 0) return DC_OK;
-    DC_REQUIRE(descs, DC_EINVAL, "dc_gather_columns: null descriptor array");
+    DC_REQUIRE(descs, DC_EINVAL, "%s: null descriptor array", name);
     for (int k = 0; k < n_desc; ++k) {
         const dc_gather_desc &d = descs[k];
         DC_REQUIRE(d.row_bytes > 0 && d.outer >= 0 && d.src_cols >= 0, DC_EINVAL,
-                   "dc_gather_columns: descriptor %d has outer=%lld src_cols=%lld row_bytes=%lld (need outer >= 0, "
-                   "src_cols >= 0, row_bytes > 0)", k, (long long)d.outer, (long long)d.src_cols, (long long)d.row_bytes);
+                   "%s: descriptor %d has outer=%lld src_cols=%lld row_bytes=%lld (need outer >= 0, "
+                   "src_cols >= 0, row_bytes > 0)", name, k, (long long)d.outer, (long long)d.src_cols, (long long)d.row_bytes);
     }
     if (n_index == 0) return DC_OK;
-    DC_REQUIRE(index, DC_EINVAL, "dc_gather_columns: null index");
+    DC_REQUIRE(index, DC_EINVAL, "%s: null index", name);
     GatherParams p;
     p.n_desc = n_desc;
     long long blocks = 0;
@@ -109,16 +119,16 @@ extern "C" int dc_gather_columns(const dc_gather_desc *descs, int n_desc, const 
         p.unit[k] = 1;
         p.narrow[k] = 1;
         if (d.outer == 0) continue;
-        DC_REQUIRE(d.src && d.dst, DC_EINVAL, "dc_gather_columns: descriptor %d has a null pointer", k);
-        DC_REQUIRE(d.src_cols > 0, DC_EINVAL, "dc_gather_columns: descriptor %d has src_cols=0 and %lld indices", k,
+        DC_REQUIRE(d.src && d.dst, DC_EINVAL, "%s: descriptor %d has a null pointer", name, k);
+        DC_REQUIRE(d.src_cols > 0, DC_EINVAL, "%s: descriptor %d has src_cols=0 and %lld indices", name, k,
                    (long long)n_index);
         DC_REQUIRE(n_index <= INT64_MAX / d.outer && d.outer * n_index <= INT64_MAX / d.row_bytes &&
                        d.src_cols <= INT64_MAX / d.outer && d.outer * d.src_cols <= INT64_MAX / d.row_bytes,
-                   DC_EINVAL, "dc_gather_columns: descriptor %d is too large", k);
+                   DC_EINVAL, "%s: descriptor %d is too large", name, k);
         const int64_t dst_bytes = d.outer * n_index * d.row_bytes, src_bytes = d.outer * d.src_cols * d.row_bytes;
         const uintptr_t s = reinterpret_cast<uintptr_t>(d.src), t = reinterpret_cast<uintptr_t>(d.dst);
         DC_REQUIRE(t + (uintptr_t)dst_bytes <= s || s + (uintptr_t)src_bytes <= t, DC_EINVAL,
-                   "dc_gather_columns: descriptor %d: dst overlaps src", k);
+                   "%s: descriptor %d: dst overlaps src", name, k);
         if (d.row_bytes % 16 == 0 && aligned(d.src, 16) && aligned(d.dst, 16))
             p.unit[k] = 16;
         else if (d.row_bytes % 4 == 0 && aligned(d.src, 4) && aligned(d.dst, 4))
@@ -130,9 +140,21 @@ extern "C" int dc_gather_columns(const dc_gather_desc *descs, int n_desc, const 
         blocks += nb;
     }
     p.block_start[n_desc] = blocks;
-    DC_REQUIRE(blocks <= INT_MAX, DC_EUNSUPPORTED, "dc_gather_columns: %lld blocks exceed the grid limit", blocks);
+    DC_REQUIRE(blocks <= INT_MAX, DC_EUNSUPPORTED, "%s: %lld blocks exceed the grid limit", name, blocks);
     if (blocks == 0) return DC_OK;
-    gather_columns_kernel<<<(unsigned)blocks, kThreads, 0, dc_cu_stream(stream)>>>(p, index, n_index);
+    gather_columns_kernel<kFill><<<(unsigned)blocks, kThreads, 0, dc_cu_stream(stream)>>>(p, index, n_index);
     DC_LAUNCH_OK();
     return DC_OK;
+}
+
+}  // namespace
+
+extern "C" int dc_gather_columns(const dc_gather_desc *descs, int n_desc, const int64_t *index, int64_t n_index,
+                                 dc_stream_t stream) {
+    return gather_launch<false>("dc_gather_columns", descs, n_desc, index, n_index, stream);
+}
+
+extern "C" int dc_gather_columns_fill(const dc_gather_desc *descs, int n_desc, const int64_t *index, int64_t n_index,
+                                      dc_stream_t stream) {
+    return gather_launch<true>("dc_gather_columns_fill", descs, n_desc, index, n_index, stream);
 }

@@ -287,6 +287,104 @@ def gather_columns(pairs, index):
                                              idx.size, _lib.stream_ptr()), "dc_gather_columns")
 
 
+def gather_columns_fill(pairs, index):
+    """``gather_columns`` with a DEVICE index in which -1 writes zeros (``dc_gather_columns_fill``): column j of every
+    ``dst`` is column ``index[j]`` of its ``src``, or zeros where ``index[j] < 0``.  ``src`` / ``dst`` are as
+    ``gather_columns``'; ``index`` is a contiguous 1-D int64 CUDA tensor.  The caller guarantees ``-1 <= index <
+    src.shape[1]``: the kernel cannot check a device index, so it is built and checked on the host where it is made
+    (``state_refresh_layout``).  Raises ``ValueError`` for malformed operands before any launch."""
+    if not isinstance(index, torch.Tensor) or index.dtype != torch.int64 or index.dim() != 1 \
+            or not index.is_contiguous():
+        raise ValueError("gather_columns_fill: index must be a contiguous 1-D int64 tensor")
+    _need_cuda(index)
+    n = index.numel()
+    descs = []
+    for src, dst in pairs:
+        if src.dim() < 2 or not src.is_contiguous() or not dst.is_contiguous():
+            raise ValueError("gather_columns_fill: tensors must be contiguous with at least 2 dims, got %s"
+                             % (tuple(src.shape),))
+        _need_cuda(src, dst)
+        shape = src.shape
+        if dst.shape != (shape[0], n) + shape[2:] or dst.dtype != src.dtype or dst.device != index.device \
+                or src.device != index.device:
+            raise ValueError("gather_columns_fill: dst %s %s does not match src %s %s gathered at %d columns"
+                             % (dst.dtype, tuple(dst.shape), src.dtype, tuple(shape), n))
+        row_bytes = math.prod(shape[2:]) * src.element_size()
+        if row_bytes and shape[0]:
+            descs.append(_lib.GatherDesc(src.data_ptr(), dst.data_ptr(), shape[0], shape[1], row_bytes))
+    if not descs or n == 0:
+        return
+    lib = _lib.load()
+    n_max = _lib.GATHER_MAX_TENSORS
+    for k in range(0, len(descs), n_max):
+        chunk = descs[k:k + n_max]
+        with PROFILE.span("gather_columns_fill", 1):
+            _lib.check(lib.dc_gather_columns_fill((_lib.GatherDesc * len(chunk))(*chunk), len(chunk), index.data_ptr(), n,
+                                                  _lib.stream_ptr()), "dc_gather_columns_fill")
+
+
+def gather_rows_fill(srcs, index):
+    """``src[index]`` (zeros where ``index < 0``) for every contiguous ``src`` ``[N, ...]`` with a device ``index`` (one
+    ``dc_gather_columns_fill`` launch on ``[1, N, ...]`` views).  Returns the new ``[len(index), ...]`` tensors."""
+    n = index.numel()
+    outs = [torch.empty((n,) + tuple(s.shape[1:]), dtype=s.dtype, device=s.device) for s in srcs]
+    gather_columns_fill([(s.view((1,) + tuple(s.shape)), o.view((1,) + tuple(o.shape))) for s, o in zip(srcs, outs)],
+                        index)
+    return outs
+
+
+def refresh_states(ybufs, cbufs, t0, step, rollout, slot, h0, c0, reset_h, reset_c, acc):
+    """Writes the recomputed recurrent states of one time block into a training batch, in place, and adds the drift sums
+    to ``acc`` (``dc_refresh_states``): for every destination d, every layer l's state ``ybufs[l][step[d] - t0,
+    rollout[d]]`` (``[T + 1, R, H]`` state buffers of ``rnn_stack_forward_states``; ``cbufs`` too for the LSTM) goes to
+    ``h0[l, slot[d]]`` (``[L, B, H]``) for ``slot[d] < B``, else to the H-wide slice l of row ``slot[d] - B`` of the
+    ``[K, B, L*H]`` reset tables; ``acc`` (float64 [2], device) += (sum (new - old)^2, sum old^2).  ``step``, ``rollout``
+    and ``slot`` are int64 device tensors of one length that the caller built and checked on the host.  ``c0``,
+    ``reset_c`` and ``cbufs``: None for the GRU; ``reset_h`` / ``reset_c`` None without resets."""
+    n_layers = len(ybufs)
+    lstm = c0 is not None
+    _need_cuda(h0, c0, reset_h, reset_c, acc, step, rollout, slot, *ybufs)
+    L, B, H = h0.shape
+    T1, R = ybufs[0].shape[:2]
+    if L != n_layers or not 1 <= n_layers <= _lib.REFRESH_MAX_LAYERS:
+        raise ValueError("refresh_states: %d state buffers for h0 of %d layers (1 to %d)"
+                         % (n_layers, L, _lib.REFRESH_MAX_LAYERS))
+    if acc.dtype != torch.float64 or acc.numel() != 2:
+        raise ValueError("refresh_states: acc must be float64 [2]")
+    bufs = list(ybufs) + (list(cbufs) if lstm else [])
+    if lstm and len(cbufs) != n_layers:
+        raise ValueError("refresh_states: the LSTM needs one c buffer per layer")
+    for b in bufs:
+        if b.dtype != torch.float32 or b.shape != (T1, R, H) or not b.is_contiguous():
+            raise ValueError("refresh_states: state buffers must be contiguous fp32 [%d, %d, %d]" % (T1, R, H))
+    tabs = [h0] + ([c0] if lstm else [])
+    K = 0
+    if reset_h is not None:
+        K = reset_h.shape[0]
+        tabs += [reset_h] + ([reset_c] if lstm else [])
+        for t in tabs[2 if lstm else 1:]:
+            if t.shape != (K, B, L * H):
+                raise ValueError("refresh_states: reset tables must be [K, %d, %d]" % (B, L * H))
+    if lstm and (c0.shape != h0.shape):
+        raise ValueError("refresh_states: c0 must match h0")
+    for t in tabs:
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise ValueError("refresh_states: the batch's states must be contiguous fp32")
+    n = step.numel()
+    for t in (step, rollout, slot):
+        if t.dtype != torch.int64 or t.dim() != 1 or t.numel() != n or not t.is_contiguous():
+            raise ValueError("refresh_states: step, rollout and slot must be contiguous int64 [n]")
+    partial = torch.empty((max(n, 1) * n_layers, 2), dtype=torch.float64, device=h0.device)
+    ptrs = ctypes.c_void_p * n_layers
+    hp = ptrs(*[b.data_ptr() for b in ybufs])
+    cp = ptrs(*[b.data_ptr() for b in cbufs]) if lstm else None
+    with PROFILE.span("refresh_states", 2, 12 * n * n_layers * H * (2 if lstm else 1)):
+        _lib.check(_lib.load().dc_refresh_states(n_layers, H, hp, cp, R, int(t0), step.data_ptr(), rollout.data_ptr(),
+                                                 slot.data_ptr(), n, B, K, h0.data_ptr(), _lib.ptr(c0), _lib.ptr(reset_h),
+                                                 _lib.ptr(reset_c), partial.data_ptr(), acc.data_ptr(),
+                                                 _lib.stream_ptr()), "dc_refresh_states")
+
+
 # --------------------------------------------------------------------------------------------- RNN
 _workspaces = {}
 

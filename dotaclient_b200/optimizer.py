@@ -238,6 +238,7 @@ class ExperienceBatch:
         self._ready = {}        # data_ptr -> event of an upload still to be waited for (``to`` from pinned memory)
         self._slot = None       # the DotaOptimizer input slot whose static buffers these tensors are (``prefetch``)
         self.refresh = None     # AdvantageRefresh of batch_from_rollouts under recompute_advantages; not copied by map
+        self.state_refresh = None   # StateRefresh of batch_from_rollouts under recompute_states; not copied by map
 
     def map(self, fn):
         """A batch of the same structure with ``fn(tensor)`` in every slot; absent optional fields stay None."""
@@ -379,6 +380,45 @@ class AdvantageRefresh(typing.NamedTuple):
     valid_len: typing.Optional[torch.Tensor]
 
 
+class StateRefreshLayout(typing.NamedTuple):
+    """Where the state refresh (``DotaOptimizer(recompute_states=True)``) finds its inputs and puts its states, for rollouts
+    whose forward runs time-major over ``[L_max, R]`` (row ``t * R + i``: step t of rollout i) and a ``[S, B]`` training
+    batch (token ``t * B + c``), from ``state_refresh_layout`` (host int64 arrays):
+    ``obs_token [L_max * R]`` the batch token holding row r's observation, or -1 where the batch holds none (the row is fed
+    zeros, as experience prep pads); ``token_row [S * B]`` the row each token holds, or -1 (padding of a packed column);
+    ``step``, ``rollout``, ``slot`` ``[n]``, sorted by step: the state entering ``step`` (a multiple of ``seq_len``, >= 1) of
+    ``rollout`` is written to ``h0[:, slot]`` for ``slot < B`` or to row ``slot - B = k * B + c`` of the reset tables."""
+    R: int
+    L_max: int
+    obs_token: np.ndarray
+    token_row: np.ndarray
+    step: np.ndarray
+    rollout: np.ndarray
+    slot: np.ndarray
+
+
+class StateRefresh(typing.NamedTuple):
+    """What the state refresh between PPO epochs (``DotaOptimizer(recompute_states=True)``) needs beyond the batch: the
+    ``layout`` (host ``StateRefreshLayout``) and its index arrays on the device (``obs_token``, ``token_row``, ``step``,
+    ``rollout``, ``slot``); prep's start states ``h0`` / ``c0 [L, R, H]`` (None: all zero); and, with
+    ``recompute_advantages``, the cut rollouts' extra observation rows ``obs_next`` (``[1, R', ...]`` per input key), their
+    lengths ``cut_len`` and columns ``cut_rollout`` (host int64 ``[R']``) and prep's bootstrap slot map ``boot_slot [n_seg]``
+    (None when no rollout is cut).  ``batch_from_rollouts`` sets it as ``ExperienceBatch.state_refresh``, a plain attribute
+    outside ``FIELDS``: ``map``, ``gather``, ``to`` and the graph input slots do not carry it."""
+    layout: StateRefreshLayout
+    obs_token: torch.Tensor
+    token_row: torch.Tensor
+    step: torch.Tensor
+    rollout: torch.Tensor
+    slot: torch.Tensor
+    h0: typing.Optional[torch.Tensor]
+    c0: typing.Optional[torch.Tensor]
+    obs_next: typing.Optional[dict]
+    cut_len: typing.Optional[np.ndarray]
+    cut_rollout: typing.Optional[np.ndarray]
+    boot_slot: typing.Optional[torch.Tensor]
+
+
 class _CapturedStep(typing.NamedTuple):
     """A CUDA graph of the whole step, its static input batch and its device result vector (loss slots)."""
     static: ExperienceBatch
@@ -412,13 +452,15 @@ POLICY_RATIOS = ('per_head', 'joint')
 def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
                        vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False, pack_sequences=False,
                        policy_ratio='per_head', value_norm=False, value_norm_decay=0.99, kl_coef=0.0, kl_target=None,
-                       kl_stop=None, recompute_advantages=False):
+                       kl_stop=None, recompute_advantages=False, recompute_states=False):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
     vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool,
     pack_sequences a bool that is True only with mask_padding, policy_ratio one of ``POLICY_RATIOS``, value_norm a bool
     and 0 <= value_norm_decay < 1, finite kl_coef >= 0, kl_target None or finite > 0 (and then kl_coef > 0), kl_stop None
-    or finite > 0, recompute_advantages a bool.  NaN fails every check."""
+    or finite > 0, recompute_advantages and recompute_states bools.  NaN fails every check."""
+    if not isinstance(recompute_states, bool):
+        raise ValueError("recompute_states=%r: must be True or False" % (recompute_states,))
     if not isinstance(recompute_advantages, bool):
         raise ValueError("recompute_advantages=%r: must be True or False" % (recompute_advantages,))
     if not isinstance(value_norm, bool):
@@ -467,6 +509,13 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
                              "doubles or halves it" % (kl_target,))
     if kl_stop is not None and not 0.0 < number('kl_stop', kl_stop) < math.inf:
         raise ValueError("kl_stop=%r: the KL limit must be finite and > 0 (or None: no early stop)" % (kl_stop,))
+
+
+def _drift(sq_change, sq_old):
+    """sqrt(sum (new - old)^2 / sum old^2) from the two sums of ``dc_refresh_states``; 0 when nothing moved."""
+    if sq_old > 0:
+        return math.sqrt(sq_change / sq_old)
+    return 0.0 if sq_change == 0 else math.inf
 
 
 def kl_coef_update(kl_coef, kl, kl_target):
@@ -651,6 +700,82 @@ def packed_rows(lay, Lps):
     return np.where(lay.rollout >= 0, base[np.maximum(lay.rollout, 0)] + lay.step, -1)
 
 
+def _batch_rows(Ls, S, pack, layout=None):
+    """The rollout-major row of experience prep (rollout i's ``Lp_i`` padded rows follow rollouts 0 .. i-1's) that every
+    token of the ``[S, B]`` batch of ``batch_from_rollouts`` holds, -1 at padding tokens of a packed batch: ``packed_rows``
+    of the pack layout, or ``chunk_columns`` applied to the row numbers."""
+    Lps = [(L + S - 1) // S * S for L in Ls]
+    if pack:
+        return packed_rows(pack_layout(Ls, S) if layout is None else layout, Lps)
+    base = np.concatenate([[0], np.cumsum(Lps)[:-1]]).astype(np.int64)
+    Lmax = max(Lps, default=0)
+    t = np.arange(Lmax, dtype=np.int64)[:, None]
+    grid = torch.from_numpy(np.where(t < np.asarray(Lps)[None, :], base[None, :] + t, -1))
+    return chunk_columns(grid, Lps, S).numpy().reshape(S, -1) if Lps else np.zeros((S, 0), dtype=np.int64)
+
+
+def state_refresh_layout(lengths, seq_len, pack, layout=None):
+    """The ``StateRefreshLayout`` of the batch that ``batch_from_rollouts`` builds from rollouts of ``lengths`` real steps
+    (``pack``: the packed batch; ``layout`` its ``pack_layout`` when the caller has it), derived from the batch's own layout
+    (``chunk_columns`` / ``packed_rows``).  A batch column starts at the row its first token holds, and a packed reset at
+    the row of its token; a start at step 0 keeps prep's state (it is data, not a product of the network) and is not a
+    destination.  Checked with ``check_state_refresh_layout``."""
+    S = int(seq_len)
+    Ls = [int(L) for L in lengths]
+    Lps = [(L + S - 1) // S * S for L in Ls]
+    R, Lmax = len(Ls), max(Lps, default=0)
+    if pack and layout is None:
+        layout = pack_layout(Ls, S)
+    rows = _batch_rows(Ls, S, pack, layout)                              # [S, B] rollout-major rows
+    B = rows.shape[1]
+    base = np.concatenate([[0], np.cumsum(Lps)[:-1]]).astype(np.int64)
+    row_rollout = np.repeat(np.arange(R, dtype=np.int64), Lps)
+    row_step = np.arange(int(sum(Lps)), dtype=np.int64) - np.repeat(base, Lps)
+    held = rows >= 0
+    r = np.where(held, rows, 0)
+    tm = np.where(held, row_step[r] * R + row_rollout[r], -1)            # [S, B] rows of the [L_max, R] forward
+    token_row = tm.reshape(-1).astype(np.int64)
+    obs_token = np.full(Lmax * R, -1, dtype=np.int64)
+    obs_token[token_row[token_row >= 0]] = np.flatnonzero(token_row >= 0)
+    dst_rows, dst_slot = [rows[0]], [np.arange(B, dtype=np.int64)]      # every column's initial state
+    if pack:                                                             # every reset inside a column
+        t_rs, c_rs = np.nonzero(layout.reset_slot >= 0)
+        dst_rows.append(rows[t_rs, c_rs])
+        dst_slot.append(B + layout.reset_slot[t_rs, c_rs].astype(np.int64) * B + c_rs)
+    dst_rows, dst_slot = np.concatenate(dst_rows), np.concatenate(dst_slot)
+    step, rollout = row_step[dst_rows], row_rollout[dst_rows]
+    keep = step > 0
+    order = np.argsort(step[keep], kind="stable")
+    return StateRefreshLayout(R, Lmax, obs_token, token_row, step[keep][order], rollout[keep][order],
+                              dst_slot[keep][order])
+
+
+def check_state_refresh_layout(lay, B, K):
+    """Raises ``ValueError`` unless the host ``StateRefreshLayout`` ``lay`` indexes a ``[S, B]`` batch with ``K`` reset rows
+    per column: tokens and rows in range or -1, destinations at steps in [1, L_max) of rollouts in [0, R), sorted by step,
+    and slots in [0, B + K*B), none twice.  ``dc_gather_columns_fill`` and ``dc_refresh_states`` index with them on the
+    device, where they cannot be checked."""
+    n_tok = lay.token_row.size
+    if n_tok % max(B, 1) or lay.obs_token.size != lay.L_max * lay.R:
+        raise ValueError("state refresh layout: %d tokens for %d columns, %d rows for L_max=%d, R=%d"
+                         % (n_tok, B, lay.obs_token.size, lay.L_max, lay.R))
+    for name, a, hi in (("obs_token", lay.obs_token, n_tok), ("token_row", lay.token_row, lay.obs_token.size)):
+        if a.size and (a.min() < -1 or a.max() >= hi):
+            raise ValueError("state refresh layout: %s values %d..%d outside [-1, %d)" % (name, a.min(), a.max(), hi))
+    n = lay.step.size
+    if lay.rollout.size != n or lay.slot.size != n:
+        raise ValueError("state refresh layout: step, rollout and slot differ in length")
+    if n and (lay.step.min() < 1 or lay.step.max() >= lay.L_max or np.any(np.diff(lay.step) < 0)):
+        raise ValueError("state refresh layout: destination steps must be sorted and in [1, %d)" % lay.L_max)
+    if n and (lay.rollout.min() < 0 or lay.rollout.max() >= lay.R):
+        raise ValueError("state refresh layout: destination rollouts outside [0, %d)" % lay.R)
+    if n and (lay.slot.min() < 0 or lay.slot.max() >= B + K * B):
+        raise ValueError("state refresh layout: destination slots %d..%d outside [0, %d)"
+                         % (lay.slot.min(), lay.slot.max(), B + K * B))
+    if np.unique(lay.slot).size != n:
+        raise ValueError("state refresh layout: a destination slot is written twice")
+
+
 def refresh_token_map(lengths, seq_len, pack, mask_padding, layout=None):
     """For the rollout-major rows of experience prep (rollout i's ``Lp_i`` padded rows in turn), the token ``t * B + c``
     of the ``[S, B]`` training batch that ``batch_from_rollouts`` builds from rollouts of ``lengths`` real steps, or -1
@@ -664,13 +789,7 @@ def refresh_token_map(lengths, seq_len, pack, mask_padding, layout=None):
     Lps = [(L + S - 1) // S * S for L in Ls]
     n_rows = int(sum(Lps))
     base = np.concatenate([[0], np.cumsum(Lps)[:-1]]).astype(np.int64)
-    if pack:
-        rows = packed_rows(pack_layout(Ls, S) if layout is None else layout, Lps)
-    else:
-        Lmax = max(Lps, default=0)
-        t = np.arange(Lmax, dtype=np.int64)[:, None]
-        grid = torch.from_numpy(np.where(t < np.asarray(Lps)[None, :], base[None, :] + t, -1))
-        rows = chunk_columns(grid, Lps, S).numpy().reshape(S, -1) if Lps else np.zeros((S, 0), dtype=np.int64)
+    rows = _batch_rows(Ls, S, pack, layout)
     tok = np.full(n_rows, -1, dtype=np.int64)
     held = rows >= 0
     tok[rows[held]] = np.flatnonzero(held.reshape(-1))
@@ -777,7 +896,8 @@ class DotaOptimizer:
     BUCKET_NAME = 'dotaservice'
     MODEL_HISTOGRAM_FREQ = 128
     MAX_GRAD_NORM = 0.5
-    # the advantage refresh (recompute_advantages) runs its forward over blocks of time steps of about this many tokens
+    # the advantage and state refreshes (recompute_advantages, recompute_states) run their forwards over blocks of time
+    # steps of about this many tokens
     REFRESH_CHUNK_TOKENS = 32768
     SPEED_KEY = 'steps per s'
     ADAM_BETAS = (0.9, 0.999)       # torch.optim.Adam defaults (:275)
@@ -792,7 +912,8 @@ class DotaOptimizer:
                  iterations=100000, rollout_prefetch=0, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1,
                  max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0,
                  num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False,
-                 value_norm_decay=0.99, kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False):
+                 value_norm_decay=0.99, kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False,
+                 recompute_states=False):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
@@ -801,8 +922,13 @@ class DotaOptimizer:
                            vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                            mask_padding=mask_padding, pack_sequences=pack_sequences, policy_ratio=policy_ratio,
                            value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
-                           kl_stop=kl_stop, recompute_advantages=recompute_advantages)
+                           kl_stop=kl_stop, recompute_advantages=recompute_advantages, recompute_states=recompute_states)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # True: before every epoch after the first, train_epochs reruns every rollout of the batch whole with the current
+        # weights and writes the recurrent states entering its chunks (after the first) over the batch's h0 / c0 and reset
+        # tables (_refresh_states); batch_from_rollouts then attaches what that needs (ExperienceBatch.state_refresh)
+        self.recompute_states = recompute_states
+        self._state_refresh_sums = []       # (device float64 [2] drift sums, states replaced) of this iteration's refreshes
         # True: before every epoch after the first, train_epochs recomputes the batch's advantages and returns with the
         # current critic (and, for V-trace, the current policy as the target), from prep's rewards, segments and bootstraps
         # (_refresh_advantages); batch_from_rollouts then attaches what that needs (ExperienceBatch.refresh)
@@ -1181,26 +1307,21 @@ class DotaOptimizer:
         for i, d in enumerate(datas):
             rewards_np[i, :Ls[i]] = np.asarray(d['rewards'], dtype=np.float32)
         with torch.no_grad():
-            x, unit_embedding = pol._encode(obs['env'], [obs[k] for k in Policy.INPUT_KEYS[1:]])
             if carried:
                 h0, c0 = state0[0], (state0[1] if lstm else None)
             else:
                 h0 = torch.zeros((n_layers, R, H), dtype=torch.float32, device=dev)
                 c0 = torch.zeros_like(h0) if lstm else None
             # every layer's state buffers are kept: the state entering chunk j of rollout i is ybufs[k][j*S, i] per layer k
-            layers = [pol.rnn.layer(k) for k in range(n_layers)]
-            ybufs, cbufs = ops.rnn_stack_forward_states(x.contiguous(), layers, h0, c0, pol.cell)
-            logits, values = pol._heads(ybufs[-1][1:], unit_embedding)
+            ybufs, cbufs, logits, values = self._rollout_forward(obs, h0, c0)
             # value_norm: the head is normalised; everything prep makes from it is in raw units, V = mu + sigma v with the
             # statistics this forward ran under (denormalised from the packed column into a contiguous [Lmax, R] tensor)
             vn = self._value_norm_moments() if self.value_norm else None
             bootstrap = boot = None
             if cut:                                    # V(s_L) of every cut rollout: one step of batch R' from slot L_i
-                xb, ue = pol._encode(obs_next['env'], [obs_next[k] for k in Policy.INPUT_KEYS[1:]])
                 hb = ops.stack_layers([yb[slot_last, col_last] for yb in ybufs])
                 cb = ops.stack_layers([c[slot_last, col_last] for c in cbufs]) if lstm else None
-                yb_next, _ = ops.rnn_stack_forward_states(xb.contiguous(), layers, hb, cb, pol.cell)
-                bootstrap = pol._heads(yb_next[-1][1:], ue)[1].reshape(len(cut))
+                bootstrap = self._rollout_forward(obs_next, hb, cb)[3].reshape(len(cut))
                 if vn is not None:
                     bootstrap = ops.value_denorm(bootstrap, *vn)
                 boot = torch.cat([bootstrap.new_zeros(1), bootstrap])[boot_slot]          # per segment
@@ -1254,7 +1375,25 @@ class DotaOptimizer:
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
                     adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same, valid=valid,
                     bootstrap=bootstrap, old_log_probs=old_log_probs,
-                    refresh=dict(rewards=rew_c, seg_off=seg, boot=boot, behaviour_logp=blp_c, valid_len=valid_len))
+                    refresh=dict(rewards=rew_c, seg_off=seg, boot=boot, behaviour_logp=blp_c, valid_len=valid_len),
+                    state_refresh=dict(h0=h0, c0=c0,
+                                       obs_next=obs_next if cut else None,
+                                       cut_len=np.array([Ls[i] for i in cut], dtype=np.int64) if cut else None,
+                                       cut_rollout=np.array(cut, dtype=np.int64) if cut else None,
+                                       boot_slot=boot_slot if cut else None))
+
+    def _rollout_forward(self, obs, h0, c0):
+        """The no-grad rollout-major forward of experience prep and of the state refresh: the encoder over time-major
+        ``[T, R, ...]`` observations (``Policy.INPUT_KEYS``), every recurrent layer from ``h0`` / ``c0 [L, R, H]`` (c0 None
+        for the GRU) keeping its state buffers, and the heads.  Returns ``(ybufs, cbufs, logits, values)``: per layer the
+        ``[T + 1, R, H]`` state buffers of ``ops.rnn_stack_forward_states`` (slot t: the state entering step t), the head
+        logits and the value column ``[T, R, 1]`` of the packed head output (normalised under ``value_norm``)."""
+        pol = self.policy_base
+        x, unit_embedding = pol._encode(obs['env'], [obs[k] for k in Policy.INPUT_KEYS[1:]])
+        layers = [pol.rnn.layer(k) for k in range(pol.num_layers)]
+        ybufs, cbufs = ops.rnn_stack_forward_states(x.contiguous(), layers, h0, c0, pol.cell)
+        logits, values = pol._heads(ybufs[-1][1:], unit_embedding)
+        return ybufs, cbufs, logits, values
 
     def experiences_from_rollouts(self, datas):
         """``experiences_from_rollout`` (:328-430) for all rollouts of an iteration at once: per rollout the result equals a
@@ -1302,6 +1441,20 @@ class DotaOptimizer:
             tok = refresh_token_map(p['Ls'], S, self.pack_sequences, self.mask_padding, layout=lay)
             tok = torch.from_numpy(tok).pin_memory().to(self.device, non_blocking=True)
             batch.refresh = AdvantageRefresh(tok=tok, **p['refresh'])
+        if self.recompute_states:              # where the rollouts' rows and chunk starts sit in the batch, checked here
+            sl = state_refresh_layout(p['Ls'], S, self.pack_sequences, layout=lay)
+            check_state_refresh_layout(sl, batch.batch_size, 0 if batch.reset_h is None else batch.reset_h.shape[0])
+            idx = np.concatenate([sl.obs_token, sl.token_row, sl.step, sl.rollout, sl.slot])
+            idx = torch.from_numpy(idx).pin_memory().to(self.device, non_blocking=True)
+            n_o, n_t, n = sl.obs_token.size, sl.token_row.size, sl.step.size
+            o = n_o + n_t
+            rec = dict(p['state_refresh'])
+            if not any('initial_hidden' in d for d in datas):       # every rollout starts from zeros
+                rec.update(h0=None, c0=None)
+            if not self.recompute_advantages:     # the bootstrap inputs serve only the advantages
+                rec.update(obs_next=None, cut_len=None, cut_rollout=None, boot_slot=None)
+            batch.state_refresh = StateRefresh(sl, idx[:n_o], idx[n_o:o], idx[o:o + n], idx[o + n:o + 2 * n],
+                                               idx[o + 2 * n:], **rec)
         return batch
 
     def _unpacked_batch(self, p):
@@ -1683,14 +1836,21 @@ class DotaOptimizer:
 
         With ``recompute_advantages`` every epoch after the first starts with ``_refresh_advantages``, which rewrites
         ``batch.advantages`` and ``batch.returns`` in place; no refresh follows a step that ``kl_stop`` skipped.  The batch
-        must then come from ``batch_from_rollouts`` (``ExperienceBatch.refresh``), else ``ValueError`` before any launch."""
+        must then come from ``batch_from_rollouts`` (``ExperienceBatch.refresh``), else ``ValueError`` before any launch.
+        With ``recompute_states`` the same epochs start with ``_refresh_states`` instead, which rewrites the batch's
+        recurrent start states (and, with ``recompute_advantages``, its advantages and returns from the same forward); the
+        batch must carry ``ExperienceBatch.state_refresh``."""
         M = self.num_minibatches
         if batch.batch_size < M:
             raise ValueError("the batch has %d sequences, fewer than num_minibatches=%d" % (batch.batch_size, M))
-        refresh = self.recompute_advantages and self.epochs > 1
-        if refresh and batch.refresh is None:
+        refresh = (self.recompute_advantages or self.recompute_states) and self.epochs > 1
+        if refresh and self.recompute_advantages and batch.refresh is None:
             raise ValueError("recompute_advantages=True needs the scan inputs of experience prep, and this batch has none "
                              "(ExperienceBatch.refresh): train on a batch from batch_from_rollouts")
+        if refresh and self.recompute_states and batch.state_refresh is None:
+            raise ValueError("recompute_states=True needs the rollout layout of experience prep, and this batch has none "
+                             "(ExperienceBatch.state_refresh): train on a batch from batch_from_rollouts")
+        self._state_refresh_sums = []
         if M > 1 and not batch.advantages.is_cuda:
             batch = batch.to(self.device)                  # uploaded once; the minibatches are gathered on the device
         losses, entropies, grad_norms, ppo_stats = [], [], [], []
@@ -1698,7 +1858,10 @@ class DotaOptimizer:
         for ep in range(self.epochs):                                      # :469
             self.mq.process_data_events()
             if refresh and ep > 0:
-                self._refresh_advantages(batch)
+                if self.recompute_states:
+                    self._refresh_states(batch)
+                else:
+                    self._refresh_advantages(batch)
             for idx in minibatch_indices(batch.batch_size, M, self.minibatch_rng):
                 loss_d, entropy_d, grad_norm_d = self.train(experiences=batch if M == 1 else batch.gather(idx))
                 losses.append(loss_d)
@@ -1755,13 +1918,114 @@ class DotaOptimizer:
                 del x, unit_embedding, y, packed, target_unit
             if self.value_norm:
                 values = ops.value_denorm(values, *self._value_norm_moments())
-            if vtrace:
-                ops.vtrace_scan_indexed(r.rewards, values, target, r.behaviour_logp, r.tok, r.seg_off, batch.advantages,
-                                        batch.returns, self.gamma, self.gae_lambda, self.vtrace_rho_clip,
-                                        self.vtrace_c_clip, boot_value=r.boot, valid_len=r.valid_len)
-            else:
-                ops.gae_scan_indexed(r.rewards, values, r.tok, r.seg_off, batch.advantages, batch.returns, self.gamma,
-                                     self.gae_lambda, boot_value=r.boot, boot_reward=r.boot)
+            self._rescan(batch, values, target, r.boot)
+
+    def _rescan(self, batch, values, target, boot):
+        """Prep's segmented GAE or V-trace scan over prep's rollout-major rewards and segments, reading the raw values
+        (and for V-trace the target log-probs ``[S * B, 5]``) at the batch's tokens and writing ``batch.advantages`` /
+        ``batch.returns`` there (``ops.gae_scan_indexed`` / ``vtrace_scan_indexed``), ending the segments on ``boot``."""
+        r = batch.refresh
+        if self.advantage_estimator == 'vtrace':
+            ops.vtrace_scan_indexed(r.rewards, values, target, r.behaviour_logp, r.tok, r.seg_off, batch.advantages,
+                                    batch.returns, self.gamma, self.gae_lambda, self.vtrace_rho_clip, self.vtrace_c_clip,
+                                    boot_value=boot, valid_len=r.valid_len)
+        else:
+            ops.gae_scan_indexed(r.rewards, values, r.tok, r.seg_off, batch.advantages, batch.returns, self.gamma,
+                                 self.gae_lambda, boot_value=boot, boot_reward=boot)
+
+    def _refresh_states(self, batch):
+        """Recomputes the recurrent states entering the batch's chunks with the current weights (``recompute_states``;
+        Kapturowski et al. 2019, section 3): every rollout runs again whole, in sequence, over its padded length, from the
+        state prep started it from (zeros or its ``'initial_hidden'``), as experience prep runs it (``_rollout_forward``),
+        with the observations gathered from the batch (``ExperienceBatch.state_refresh``, ``state_refresh_layout``; rows the
+        batch does not hold are zeros, as in prep).  Every layer's state at each chunk start after a rollout's first is
+        written over ``batch.h0`` / ``c0`` or the reset tables, in place (``ops.refresh_states``), and the drift sums go to
+        ``last_state_refresh_stats``.  A rollout's first chunk keeps prep's start state.
+
+        With ``recompute_advantages`` the same forward gives the values of every row (denormalised with the current
+        statistics under ``value_norm``) and, for V-trace, the current policy's log-probs of the taken actions; a cut
+        rollout's V(s_L) is recomputed from the refreshed state after its last step and its extra observation row; then
+        prep's scan runs again (``_rescan``).  Everything else in the batch stays as prep made it.
+
+        The forward runs over blocks of ``max(1, REFRESH_CHUNK_TOKENS // R)`` time steps of the ``R`` rollouts, with the
+        state carried from block to block, so its transient memory is bounded by the block, not by the batch."""
+        st, pol, keys = batch.state_refresh, self.policy_base, ops.HEAD_KEYS
+        lay, dev = st.layout, self.device
+        R, Lmax = lay.R, lay.L_max
+        lstm = pol.cell == "lstm"
+        adv = self.recompute_advantages
+        vtrace = adv and self.advantage_estimator == 'vtrace'
+        cut = adv and st.cut_len is not None
+        T = max(1, self.REFRESH_CHUNK_TOKENS // R)
+        if st.h0 is not None:
+            h, c = st.h0, st.c0
+        else:
+            h = torch.zeros((pol.num_layers, R, pol.hidden_size), dtype=torch.float32, device=dev)
+            c = torch.zeros_like(h) if lstm else None
+        acc = torch.zeros(2, dtype=torch.float64, device=dev)
+        values = torch.empty((Lmax, R), dtype=torch.float32, device=dev) if adv else None
+        target = torch.empty((Lmax * R, 5), dtype=torch.float32, device=dev) if vtrace else None
+        if cut:                                # the state after each cut rollout's last step, taken from its block
+            hb = torch.empty((pol.num_layers, st.cut_len.size, pol.hidden_size), dtype=torch.float32, device=dev)
+            cb = torch.empty_like(hb) if lstm else None
+            cut_block = (st.cut_len - 1) // T
+        srcs = dict(batch.observations)
+        if vtrace:
+            srcs.update({('m', k): batch.masks[k] for k in keys})
+            srcs.update({('a', k): batch.actions[k] for k in keys})
+        with torch.no_grad():
+            for blk, t0 in enumerate(range(0, Lmax, T)):
+                t1 = min(Lmax, t0 + T)
+                n = t1 - t0
+                ins = {k: torch.empty((n, R) + tuple(v.shape[2:]), dtype=v.dtype, device=dev) for k, v in srcs.items()}
+                ops.gather_columns_fill([(v.view((1, -1) + tuple(v.shape[2:])), ins[k].view((1, n * R) + tuple(v.shape[2:])))
+                                         for k, v in srcs.items()], st.obs_token[t0 * R:t1 * R])
+                ybufs, cbufs, logits, v = self._rollout_forward(ins, h, c)
+                lo, hi = np.searchsorted(lay.step, [t0, t1])
+                if hi > lo:
+                    ops.refresh_states(ybufs, cbufs if lstm else None, t0, st.step[lo:hi], st.rollout[lo:hi],
+                                       st.slot[lo:hi], batch.h0, batch.c0, batch.reset_h, batch.reset_c, acc)
+                if adv:
+                    values[t0:t1] = v.reshape(n, R)
+                if vtrace:
+                    target[t0 * R:t1 * R] = ops.selected_logp([logits[k] for k in keys], [ins[('m', k)] for k in keys],
+                                                              [ins[('a', k)] for k in keys])
+                if cut and (cut_block == blk).any():
+                    sel = np.flatnonzero(cut_block == blk)
+                    ij = torch.from_numpy(np.stack([st.cut_len[sel] - t0, st.cut_rollout[sel], sel])).to(dev)
+                    for k in range(pol.num_layers):
+                        hb[k, ij[2]] = ybufs[k][ij[0], ij[1]]
+                        if lstm:
+                            cb[k, ij[2]] = cbufs[k][ij[0], ij[1]]
+                h = ops.stack_layers([yb[n] for yb in ybufs])
+                c = ops.stack_layers([cf[n] for cf in cbufs]) if lstm else None
+                del ins, ybufs, cbufs, logits, v
+            self._state_refresh_sums.append((acc, int(lay.step.size)))
+            if not adv:
+                return
+            vn = self._value_norm_moments() if self.value_norm else None
+            boot = batch.refresh.boot
+            if cut:                            # V(s_L) from the refreshed state after the last step
+                bootstrap = self._rollout_forward(st.obs_next, hb, cb)[3].reshape(-1)
+                if vn is not None:
+                    bootstrap = ops.value_denorm(bootstrap, *vn)
+                boot = torch.cat([bootstrap.new_zeros(1), bootstrap])[st.boot_slot]
+            if vn is not None:
+                values = ops.value_denorm(values, *vn)
+            vals_b = ops.gather_rows_fill([values.reshape(-1)], st.token_row)[0]
+            target_b = ops.gather_rows_fill([target], st.token_row)[0] if vtrace else None
+            self._rescan(batch, vals_b, target_b, boot)
+
+    @property
+    def last_state_refresh_stats(self):
+        """The last state refresh of ``train_epochs`` (``recompute_states``): ``{'drift': sqrt(sum (new - old)^2 /
+        sum old^2), 'states': n}`` over the ``n`` (rollout, chunk start) states it replaced, every layer's h and, for the
+        LSTM, c, summed in float64 in a fixed order (bitwise reproducible; 0 when nothing was replaced).  None before the
+        first.  Reading it waits for the device."""
+        if not self._state_refresh_sums:
+            return None
+        acc, n = self._state_refresh_sums[-1]
+        return {'drift': _drift(*acc.tolist()), 'states': n}
 
     # -- iteration driver (:436-579) ----------------------------------------------------------------
     def run(self):
@@ -1868,6 +2132,9 @@ class DotaOptimizer:
         if self.value_norm:                                                # the statistics this iteration trained under
             st = self.value_norm_stats
             metrics['value_norm/mean'], metrics['value_norm/std'] = st['mean'], st['std']
+        if self.recompute_states:                                          # how far the refreshes moved the start states
+            drifts = [_drift(*acc.tolist()) for acc, _ in self._state_refresh_sums]
+            metrics['refresh/state_drift'] = float(np.mean(drifts)) if drifts else 0.0
         logger.info('steps_per_s={:.2f}, avg_weight_age={:.1f}, loss={:.4f}, entropy={:.3f}'.format(
             metrics[self.SPEED_KEY], float(metrics['avg_weight_age']), float(metrics['loss/sum']), float(metrics['entropy'])))
         if self.checkpoint:
@@ -1992,13 +2259,14 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
          value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
          mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False, value_norm_decay=0.99,
-         kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False):
+         kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False, recompute_states=False):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                        mask_padding=mask_padding, pack_sequences=pack_sequences,
                        policy_ratio=policy_ratio, value_norm=value_norm,
                        value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
-                       kl_stop=kl_stop, recompute_advantages=recompute_advantages)        # before any process-group setup
+                       kl_stop=kl_stop, recompute_advantages=recompute_advantages,
+                       recompute_states=recompute_states)                                 # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -2011,7 +2279,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         advantage_estimator=advantage_estimator, vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip,
         num_minibatches=num_minibatches, mask_padding=mask_padding, pack_sequences=pack_sequences,
         policy_ratio=policy_ratio, value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef,
-        kl_target=kl_target, kl_stop=kl_stop, recompute_advantages=recompute_advantages)
+        kl_target=kl_target, kl_stop=kl_stop, recompute_advantages=recompute_advantages,
+        recompute_states=recompute_states)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -2082,6 +2351,9 @@ def build_arg_parser():
     p.add_argument("--recompute-advantages", action="store_true",
                    help="recompute the batch's advantages and returns with the current critic before every epoch after "
                         "the first")
+    p.add_argument("--recompute-states", action="store_true",
+                   help="rerun every rollout with the current network before every epoch after the first and replace the "
+                        "recurrent states its training sequences start from")
     return p
 
 
@@ -2098,6 +2370,7 @@ if __name__ == '__main__':
              vtrace_rho_clip=args.vtrace_rho_clip, vtrace_c_clip=args.vtrace_c_clip, num_minibatches=args.num_minibatches,
              mask_padding=args.mask_padding, pack_sequences=args.pack_sequences, policy_ratio=args.policy_ratio,
              value_norm=args.value_norm, value_norm_decay=args.value_norm_decay, kl_coef=args.kl_coef,
-             kl_target=args.kl_target, kl_stop=args.kl_stop, recompute_advantages=args.recompute_advantages)
+             kl_target=args.kl_target, kl_stop=args.kl_stop, recompute_advantages=args.recompute_advantages,
+             recompute_states=args.recompute_states)
     except KeyboardInterrupt:
         pass

@@ -133,6 +133,30 @@ typedef struct {
 #define DC_GATHER_MAX_TENSORS 32
 int dc_gather_columns(const dc_gather_desc *descs, int n_desc, const int64_t *index, int64_t n_index,
                       dc_stream_t stream);
+/* dc_gather_columns_fill: dc_gather_columns, except that index[j] < 0 writes zeros to column j (and reads nothing).
+ * Preconditions the library cannot check: -1 <= index[j] < src_cols.  Checked as dc_gather_columns. */
+int dc_gather_columns_fill(const dc_gather_desc *descs, int n_desc, const int64_t *index, int64_t n_index,
+                           dc_stream_t stream);
+
+/* ---- state refresh between PPO epochs (DotaOptimizer(recompute_states=True)) -------------------------------------
+ * After a no-grad forward over time steps [t0, t0 + T) of R rollouts (every layer l's state buffers h_bufs[l] /
+ * c_bufs[l], [T + 1, R, H]: slot s holds the state entering step t0 + s), for each destination d < n:
+ *   new = h_bufs[l][(step[d] - t0) * R + rollout[d]]  (every layer l; and the c buffer for the LSTM)
+ *   slot[d] <  B: written over h0[l, slot[d], :] (and c0), h0 [L, B, H]
+ *   slot[d] >= B: written over reset_h[slot[d] - B, l*H : (l+1)*H] (and reset_c), the [K, B, L*H] reset tables
+ * and acc[0] += sum (new - old)^2, acc[1] += sum old^2 over every float written, in float64, in a fixed order (no atomics;
+ * two calls on the same data give the same bits).  partial: device workspace of 2 * n * n_layers doubles.
+ * c_bufs / c0 / reset_c: NULL for the GRU.  All state pointers 16-byte aligned.
+ * Preconditions the library cannot check (the tables are on the device): t0 <= step[d] <= t0 + T, 0 <= rollout[d] < R,
+ * 0 <= slot[d] < B + K*B, and no slot twice.  The caller builds and checks them on the host.
+ * Checked: 1 <= n_layers <= DC_REFRESH_MAX_LAYERS, H a positive multiple of 32, R, B >= 1, K, n, t0 >= 0, non-null and
+ * aligned pointers where there is work -> DC_EINVAL before any CUDA call.  n = 0 does nothing.
+ */
+#define DC_REFRESH_MAX_LAYERS 16
+int dc_refresh_states(int n_layers, int H, const float *const *h_bufs, const float *const *c_bufs, int64_t R, int64_t t0,
+                      const int64_t *step, const int64_t *rollout, const int64_t *slot, int64_t n, int64_t B, int64_t K,
+                      float *h0, float *c0, float *reset_h, float *reset_c, double *partial, double *acc,
+                      dc_stream_t stream);
 
 /* ---- recurrent core --------------------------------------------------------------------
  * Replaces the time recurrence inside nn.GRU / nn.LSTM (policy.py:66,141) -- forward and
