@@ -28,6 +28,10 @@ SIGNATURES = {
     "dc_gae_scan_indexed": (_i32, [_vp, _i32, _vp, _i64, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _vp, _vp, _vp]),
     "dc_vtrace_scan_indexed": (_i32, [_vp, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _f64, _f64, _vp,
                                       _vp, _vp, _vp]),
+    "dc_gae_scan_heads": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _f64, _vp, _vp, _vp]),
+    "dc_gae_scan_heads_indexed": (_i32, [_vp, _i32, _vp, _i32, _vp, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _f64, _vp, _vp,
+                                         _vp]),
+    "dc_value_heads_loss": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "dc_gather_columns": (_i32, [_c.POINTER(GatherDesc), _i32, _vp, _i64, _vp]),
     "dc_gather_columns_fill": (_i32, [_c.POINTER(GatherDesc), _i32, _vp, _i64, _vp]),
     "dc_refresh_states": (_i32, [_i32, _i32, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp,
@@ -98,6 +102,9 @@ STAT_KL, STAT_KL_PENALTY = 16, 22                           # dc_ppo_loss_fwd_bw
 KL_ROW_FLOATS = 65          # entries of one token's masked log-prob row over the five heads (DC_KL_ROW_FLOATS)
 FINISH_KL_METRICS = 6       # metrics of dc_grad_finish_kl: the four of dc_grad_finish, the all-ranks KL, the skip flag
 VTRACE_STATS_SLOTS = 8      # per-segment fp64 sums written by dc_vtrace_scan (DC_VTRACE_STATS_SLOTS)
+VALUE_HEADS_MAX = 10        # value heads of dc_gae_scan_heads / dc_value_heads_loss (DC_VALUE_HEADS_MAX)
+VALUE_HEADS_STATS_SLOTS = 20    # dc_value_heads_loss: [k] value loss, [VALUE_HEADS_MAX + k] explained variance of head k
+VALUE_HEADS_WORKSPACE_BYTES = 131072
 GATHER_MAX_TENSORS = 32     # descriptors per dc_gather_columns call (DC_GATHER_MAX_TENSORS)
 REFRESH_MAX_LAYERS = 16     # recurrent layers dc_refresh_states handles (DC_REFRESH_MAX_LAYERS)
 MAX_PARAM_TENSORS = 96      # kMaxSeg of csrc/grad_finish.cu: parameter tensors dc_grad_flags / dc_grad_finish can handle

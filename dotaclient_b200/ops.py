@@ -119,6 +119,80 @@ def gae_scan(rewards, values, seg_off, gamma=0.98, lam=0.97, boot_value=None, bo
     return adv, ret
 
 
+def _heads_args(group, gammas, K):
+    """The host group map (int32 [n_sub]) and discounts (float64 [K]) of the multi-head scans, as ctypes arrays."""
+    group = np.ascontiguousarray(group, dtype=np.int32)
+    gammas = np.ascontiguousarray(gammas, dtype=np.float64)
+    if gammas.shape != (K,):
+        raise ValueError("gammas must hold one discount per value head (%d), got %s" % (K, gammas.shape))
+    return (ctypes.c_int32 * group.size)(*group.tolist()), (ctypes.c_double * K)(*gammas.tolist()), group.size
+
+
+def _heads_boot(boot, n_seg, K):
+    if boot is None:
+        return None
+    boot = _f32c(boot)
+    if boot.numel() != n_seg * K:
+        raise ValueError("bootstraps must be [n_seg=%d, K=%d], got %s" % (n_seg, K, tuple(boot.shape)))
+    return boot
+
+
+def gae_scan_heads(rewards, values, seg_off, group, gammas, lam, boot_value=None, boot_reward=None):
+    """GAE with one value head per reward group (``dc_gae_scan_heads``): ``rewards`` [n_rows, n_sub] fp32, ``values``
+    [n_rows, K], ``seg_off`` int64 [n_seg + 1] (device); ``group`` the host int32 [n_sub] group of every reward column,
+    ``gammas`` the K discounts; ``boot_value`` / ``boot_reward`` [n_seg, K] or None (0).  Returns ``(adv [n_rows], ret
+    [n_rows, K])``: the advantage summed over the heads, and every head's return."""
+    _need_cuda(rewards, values, seg_off, boot_value, boot_reward)
+    rewards, values = _f32c(rewards), _f32c(values)
+    n_rows, K = values.shape
+    g, gm, n_sub = _heads_args(group, gammas, K)
+    if rewards.numel() != n_rows * n_sub:
+        raise ValueError("rewards have %d elements for %d rows of %d sub-rewards" % (rewards.numel(), n_rows, n_sub))
+    seg_off = seg_off.to(torch.int64).contiguous()
+    n_seg = seg_off.numel() - 1
+    boot_value, boot_reward = _heads_boot(boot_value, n_seg, K), _heads_boot(boot_reward, n_seg, K)
+    adv = torch.empty(n_rows, dtype=torch.float32, device=values.device)
+    ret = torch.empty((n_rows, K), dtype=torch.float32, device=values.device)
+    with PROFILE.span("gae_scan_heads", 1):
+        _lib.check(_lib.load().dc_gae_scan_heads(rewards.data_ptr(), n_sub, g, K, values.data_ptr(), seg_off.data_ptr(),
+                                                 n_seg, _lib.ptr(boot_value), _lib.ptr(boot_reward), gm, float(lam),
+                                                 adv.data_ptr(), ret.data_ptr(), _lib.stream_ptr()), "dc_gae_scan_heads")
+    return adv, ret
+
+
+def gae_scan_heads_indexed(rewards, values, tok, seg_off, adv, ret, group, gammas, lam, boot_value=None,
+                           boot_reward=None):
+    """``gae_scan_heads`` in ``gae_scan_indexed``'s token layout (``dc_gae_scan_heads_indexed``): ``values`` [..., K] may be
+    a view whose rows of K lie at one stride (the packed head output's value columns); row r reads the K values of token
+    ``tok[r]`` and writes ``adv`` [n_tokens] and ``ret`` [n_tokens, K] (contiguous fp32) there, in place; rows with
+    ``tok[r] < 0`` read 0 and write nothing."""
+    _need_cuda(rewards, values, tok, seg_off, adv, ret, boot_value, boot_reward)
+    rewards = _f32c(rewards)
+    K = values.shape[-1]
+    rows = values.detach().reshape(-1, K)
+    if rows.dtype != torch.float32 or rows.stride(1) != 1:
+        raise ValueError("values must be fp32 rows of K contiguous elements")
+    ld = rows.stride(0) if rows.shape[0] > 1 else K
+    if tok.dtype != torch.int64 or tok.dim() != 1 or not tok.is_contiguous():
+        raise ValueError("tok must be a contiguous 1-D int64 tensor")
+    g, gm, n_sub = _heads_args(group, gammas, K)
+    if rewards.numel() != tok.numel() * n_sub:
+        raise ValueError("rewards have %d elements for %d rows of %d sub-rewards" % (rewards.numel(), tok.numel(), n_sub))
+    n_tok = rows.shape[0]
+    for o, n in ((adv, n_tok), (ret, n_tok * K)):
+        if o.dtype != torch.float32 or not o.is_contiguous() or o.numel() != n:
+            raise ValueError("adv / ret must be contiguous fp32 tensors of %d / %d elements" % (n_tok, n_tok * K))
+    seg_off = seg_off.to(torch.int64).contiguous()
+    n_seg = seg_off.numel() - 1
+    boot_value, boot_reward = _heads_boot(boot_value, n_seg, K), _heads_boot(boot_reward, n_seg, K)
+    with PROFILE.span("gae_scan_heads_indexed", 1):
+        _lib.check(_lib.load().dc_gae_scan_heads_indexed(
+            rewards.data_ptr(), n_sub, g, K, rows.data_ptr(), ld, tok.data_ptr(), seg_off.data_ptr(), n_seg,
+            _lib.ptr(boot_value), _lib.ptr(boot_reward), gm, float(lam), adv.data_ptr(), ret.data_ptr(),
+            _lib.stream_ptr()), "dc_gae_scan_heads_indexed")
+    return adv, ret
+
+
 def vtrace_scan(rewards, values, logp_target, logp_behaviour, seg_off, gamma, lam, rho_clip, c_clip, boot_value=None,
                 valid_len=None, stats=False):
     """V-trace value targets and policy-gradient advantages for many rollouts (``dc_vtrace_scan``).
@@ -987,6 +1061,47 @@ def select_actions(logits, masks, u):
 # --------------------------------------------------------------------------------------------- packed small heads
 PACK_COLS = {"enum": (0, 4), "x": (4, 13), "y": (13, 22), "ability": (22, 25), "value": (25, 26)}   # columns of the packed GEMM
 PACK_WIDTH = 128
+
+
+def pack_cols(K=1):
+    """The columns of the packed GEMM for a policy with ``K`` value heads: ``PACK_COLS`` with ``value`` = (25, 25 + K)."""
+    return dict(PACK_COLS, value=(25, 25 + int(K)))
+
+
+_value_heads_ws = {}
+
+
+def value_heads_loss(packed, d_packed, ret, hparams, out, head_stats, old_value=None, valid=None, stats=None):
+    """The value term of ``K`` value heads (``dc_value_heads_loss``), run after ``ppo_loss_packed`` with a hparams block
+    whose value term is off: reads the K value columns of ``packed`` [..., PACK_WIDTH] and ``ret`` [N, K] (``old_value``
+    [N, K] for the clipped loss, ``valid`` [N]), writes the K value columns of ``d_packed``, ``out[3]`` (and adds it to
+    ``out[0]``), ``head_stats`` [``_lib.VALUE_HEADS_STATS_SLOTS``] and the total's explained variance into ``stats``."""
+    _need_cuda(packed, d_packed, ret, hparams, out, head_stats, old_value, valid, stats)
+    p2 = packed.detach().reshape(-1, PACK_WIDTH)
+    d2 = d_packed.reshape(-1, PACK_WIDTH)
+    N = p2.shape[0]
+    ret = _f32c(ret)
+    K = ret.numel() // max(N, 1)
+    if ret.numel() != N * K or not 1 <= K <= _lib.VALUE_HEADS_MAX:
+        raise ValueError("ret has %d elements for %d tokens" % (ret.numel(), N))
+    assert p2.is_contiguous() and d2.is_contiguous() and p2.dtype == torch.float32 and d2.dtype == torch.float32
+    assert hparams.dtype == torch.float64 and hparams.numel() == _lib.HPARAM_SLOTS
+    assert head_stats.dtype == torch.float32 and head_stats.numel() == _lib.VALUE_HEADS_STATS_SLOTS
+    if old_value is not None:
+        old_value = _f32c(old_value)
+        assert old_value.numel() == N * K
+    if valid is not None:
+        valid = _u8(valid)
+        assert valid.numel() == N
+    ws = _value_heads_ws.get(p2.device)
+    if ws is None:
+        ws = _value_heads_ws[p2.device] = torch.empty(_lib.VALUE_HEADS_WORKSPACE_BYTES, dtype=torch.uint8, device=p2.device)
+    col = 4 * PACK_COLS["value"][0]
+    with PROFILE.span("value_heads_loss", 3, N * (12 * K + (0 if valid is None else 1) + (0 if old_value is None else 4 * K))):
+        _lib.check(_lib.load().dc_value_heads_loss(p2.data_ptr() + col, PACK_WIDTH, ret.data_ptr(), _lib.ptr(old_value),
+                                                   _lib.ptr(valid), N, K, hparams.data_ptr(), d2.data_ptr() + col,
+                                                   PACK_WIDTH, out.data_ptr(), _lib.ptr(stats), head_stats.data_ptr(),
+                                                   ws.data_ptr(), _lib.stream_ptr()), "dc_value_heads_loss")
 
 
 def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e_clip, entropy_coef, vf_coef, hparams=None,

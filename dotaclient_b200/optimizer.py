@@ -33,7 +33,7 @@ import torch.distributed as dist
 from . import _lib, ops
 from .distributed import DistributedDataParallelSparseParamCPU
 from .flat import FlatParameterSpace, VALUE_SLOT
-from .policy import Policy, REWARD_KEYS
+from .policy import Policy, REWARD_KEYS, fold_value_heads, split_value_head
 
 logging.basicConfig(format='%(asctime)s %(levelname)-8s %(message)s')
 logger = logging.getLogger(__name__)
@@ -223,6 +223,8 @@ class ExperienceBatch:
     ``old_log_probs [S, B, 65]`` (optional) are every head's full masked log-prob rows at experience prep, in head order
     with 0 at illegal entries, which the KL penalty and the KL early stop (``DotaOptimizer(kl_coef=..., kl_stop=...)``)
     compare against; absent from ``tensors()`` when None.
+    With ``K > 1`` value heads (``DotaOptimizer(value_heads=...)``) ``returns`` and ``old_values`` are ``[S, B, K]``, one
+    column per head; ``advantages`` stay ``[S, B]``, the heads' sum.
     """
     FIELDS = ("advantages", "returns", "old_logp", "h0", "c0", "old_values", "valid", "reset_slot", "reset_h", "reset_c",
               "old_log_probs")
@@ -354,7 +356,10 @@ class ExperienceBatch:
             h0, c0 = torch.cat([e.hidden.to(device) for e in experiences], dim=1), None      # :591
         old_values = None
         if all(e.values is not None for e in experiences):
-            old_values = stack([torch.as_tensor(e.values).detach().reshape(-1).float() for e in experiences])
+            def rows(v):                        # [1, S, 1] -> [S]; [1, S, K] (value heads) -> [S, K]
+                v = torch.as_tensor(v).detach().float()
+                return v.reshape(-1) if v.dim() == 1 or v.shape[-1] == 1 else v.reshape(-1, v.shape[-1])
+            old_values = stack([rows(e.values) for e in experiences])
         valid = None
         if all(getattr(e, 'valid', None) is not None for e in experiences):
             valid = stack([torch.as_tensor(e.valid).reshape(-1).bool() for e in experiences])
@@ -452,13 +457,15 @@ POLICY_RATIOS = ('per_head', 'joint')
 def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
                        vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False, pack_sequences=False,
                        policy_ratio='per_head', value_norm=False, value_norm_decay=0.99, kl_coef=0.0, kl_target=None,
-                       kl_stop=None, recompute_advantages=False, recompute_states=False):
+                       kl_stop=None, recompute_advantages=False, recompute_states=False, value_heads=None,
+                       value_gammas=None):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
     vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool,
     pack_sequences a bool that is True only with mask_padding, policy_ratio one of ``POLICY_RATIOS``, value_norm a bool
     and 0 <= value_norm_decay < 1, finite kl_coef >= 0, kl_target None or finite > 0 (and then kl_coef > 0), kl_stop None
-    or finite > 0, recompute_advantages and recompute_states bools.  NaN fails every check."""
+    or finite > 0, recompute_advantages and recompute_states bools, value_heads / value_gammas as ``value_head_groups``
+    checks them (value heads refuse V-trace and value_norm).  NaN fails every check."""
     if not isinstance(recompute_states, bool):
         raise ValueError("recompute_states=%r: must be True or False" % (recompute_states,))
     if not isinstance(recompute_advantages, bool):
@@ -509,6 +516,92 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
                              "doubles or halves it" % (kl_target,))
     if kl_stop is not None and not 0.0 < number('kl_stop', kl_stop) < math.inf:
         raise ValueError("kl_stop=%r: the KL limit must be finite and > 0 (or None: no early stop)" % (kl_stop,))
+    value_head_groups(value_heads, value_gammas, gamma)
+    if value_heads is not None and advantage_estimator == 'vtrace':
+        raise ValueError("value_heads with advantage_estimator='vtrace': per-head V-trace targets are not defined yet "
+                         "(the importance weights would need a per-head definition); use 'gae'")
+    if value_heads is not None and value_norm:
+        raise ValueError("value_heads with value_norm=True: PopArt would need one set of statistics per head and a "
+                         "per-row rescale of the value head, which is not implemented")
+
+
+class ValueHeads(typing.NamedTuple):
+    """The value heads of ``DotaOptimizer(value_heads=...)``: ``names`` in head order, ``keys`` the ``REWARD_KEYS`` of each,
+    ``group`` (int32 [10]) the head of every reward column, ``gammas`` (float64 [K]) their discounts."""
+    names: tuple
+    keys: tuple
+    group: np.ndarray
+    gammas: np.ndarray
+
+
+def value_head_groups(value_heads, value_gammas, gamma):
+    """Checks ``value_heads`` (None, or an ordered mapping ``{name: [reward keys]}`` of K >= 1 groups that together hold
+    every key of ``REWARD_KEYS`` exactly once, names matching ``[A-Za-z0-9_]+``) and ``value_gammas`` (None, or a mapping
+    of some of the names to a discount in (0, 1]; the others take ``gamma``).  Returns None for None, else ``ValueHeads``.
+    Raises ``ValueError``."""
+    if value_heads is None:
+        if value_gammas is not None:
+            raise ValueError("value_gammas=%r needs value_heads" % (value_gammas,))
+        return None
+    if not isinstance(value_heads, collections.abc.Mapping) or not value_heads:
+        raise ValueError("value_heads=%r: must be a non-empty mapping {name: [reward keys]}" % (value_heads,))
+    names, keys, group = [], [], np.full(len(REWARD_KEYS), -1, dtype=np.int32)
+    for name, ks in value_heads.items():
+        if not isinstance(name, str) or not re.fullmatch(r'[A-Za-z0-9_]+', name):
+            raise ValueError("value head name %r: names must be non-empty and match [A-Za-z0-9_]+" % (name,))
+        if isinstance(ks, str) or not isinstance(ks, collections.abc.Iterable):
+            raise ValueError("value head %r: its reward keys must be a list, got %r" % (name, ks))
+        ks = list(ks)
+        if not ks:
+            raise ValueError("value head %r has no reward keys" % name)
+        for k in ks:
+            if k not in REWARD_KEYS:
+                raise ValueError("value head %r: %r is not a reward key (%s)" % (name, k, ", ".join(REWARD_KEYS)))
+            i = REWARD_KEYS.index(k)
+            if group[i] >= 0:
+                raise ValueError("reward key %r is in more than one value head group" % k)
+            group[i] = len(names)
+        names.append(name)
+        keys.append(tuple(ks))
+    missing = [REWARD_KEYS[i] for i in np.flatnonzero(group < 0)]
+    if missing:
+        raise ValueError("value_heads leaves the reward keys %s out: every key must be in exactly one group, so that the "
+                         "summed reward does not change" % ", ".join(missing))
+    gammas = np.full(len(names), float(gamma), dtype=np.float64)
+    if value_gammas is not None:
+        if not isinstance(value_gammas, collections.abc.Mapping):
+            raise ValueError("value_gammas=%r: must be a mapping {head name: discount}" % (value_gammas,))
+        for name, g in value_gammas.items():
+            if name not in names:
+                raise ValueError("value_gammas names %r, which is not a value head (%s)" % (name, ", ".join(names)))
+            if isinstance(g, bool) or not isinstance(g, numbers.Real) or not 0.0 < float(g) <= 1.0:
+                raise ValueError("value_gammas[%r]=%r: the discount must be in (0, 1]" % (name, g))
+            gammas[names.index(name)] = float(g)
+    return ValueHeads(tuple(names), tuple(keys), group, gammas)
+
+
+def parse_value_heads(text):
+    """``--value-heads``: ``'name=key,key;name=key,...'`` -> ``{name: [keys]}`` in the order given (checked later by
+    ``value_head_groups``)."""
+    out = {}
+    for part in text.split(';'):
+        name, sep, keys = part.partition('=')
+        name = name.strip()
+        if not sep or name in out:
+            raise ValueError("--value-heads %r: expected 'name=key,key;name=key', each name once" % text)
+        out[name] = [k.strip() for k in keys.split(',') if k.strip()]
+    return out
+
+
+def parse_value_gammas(text):
+    """``--value-gammas``: ``'name=0.999;name=0.9'`` -> ``{name: float}``."""
+    out = {}
+    for part in text.split(';'):
+        name, sep, g = part.partition('=')
+        if not sep or name.strip() in out:
+            raise ValueError("--value-gammas %r: expected 'name=discount;name=discount', each name once" % text)
+        out[name.strip()] = float(g)
+    return out
 
 
 def _drift(sq_change, sq_old):
@@ -892,6 +985,8 @@ class DotaOptimizer:
     # extension: the value statistics and the normalised value head of the same iteration (value_norm=True)
     VALUE_NORM_FILENAME_FMT = "value_norm_%09d.state"
     KL_COEF_FILENAME_FMT = "kl_coef_%09d.state"     # the adaptive KL coefficient of the same iteration (kl_target)
+    # the K-row value head and its groups of the same iteration (value_heads); the published model holds it folded
+    VALUE_HEADS_FILENAME_FMT = "value_heads_%09d.state"
     VALUE_NORM_MIN_STD = 1e-2       # floor of the value statistics' sigma: bounds the value head's rescale factor
     BUCKET_NAME = 'dotaservice'
     MODEL_HISTOGRAM_FREQ = 128
@@ -899,6 +994,7 @@ class DotaOptimizer:
     # the advantage and state refreshes (recompute_advantages, recompute_states) run their forwards over blocks of time
     # steps of about this many tokens
     REFRESH_CHUNK_TOKENS = 32768
+    value_heads, n_value_heads, _vh_shape = None, 1, ()     # set by __init__ (value_heads)
     SPEED_KEY = 'steps per s'
     ADAM_BETAS = (0.9, 0.999)       # torch.optim.Adam defaults (:275)
     ADAM_EPS = 1e-8
@@ -913,7 +1009,7 @@ class DotaOptimizer:
                  max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0,
                  num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False,
                  value_norm_decay=0.99, kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False,
-                 recompute_states=False):
+                 recompute_states=False, value_heads=None, value_gammas=None):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
@@ -922,8 +1018,15 @@ class DotaOptimizer:
                            vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                            mask_padding=mask_padding, pack_sequences=pack_sequences, policy_ratio=policy_ratio,
                            value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
-                           kl_stop=kl_stop, recompute_advantages=recompute_advantages, recompute_states=recompute_states)
+                           kl_stop=kl_stop, recompute_advantages=recompute_advantages, recompute_states=recompute_states,
+                           value_heads=value_heads, value_gammas=value_gammas)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # value heads: one critic column per reward group, each with its own discount.  Prep scans every group
+        # (gae_scan_heads), the policy trains on the summed advantage, the value loss is dc_value_heads_loss's and the
+        # published model holds the heads folded into one row.  None: the reference's single critic, and none of this runs
+        self.value_heads = value_head_groups(value_heads, value_gammas, gamma)
+        self.n_value_heads = 1 if self.value_heads is None else len(self.value_heads.names)
+        self._vh_shape = () if self.n_value_heads == 1 else (self.n_value_heads,)   # trailing dim of values / returns
         # True: before every epoch after the first, train_epochs reruns every rollout of the batch whole with the current
         # weights and writes the recurrent states entering its chunks (after the first) over the batch's h0 / c0 and reset
         # tables (_refresh_states); batch_from_rollouts then attaches what that needs (ExperienceBatch.state_refresh)
@@ -989,7 +1092,8 @@ class DotaOptimizer:
 
         with torch.random.fork_rng(devices=[]):     # :34 seeds torch with 7 at import and Policy() init depends on it;
             torch.manual_seed(7)                    # forked so that constructing an optimizer leaves the caller's RNG alone
-            self.policy_base = Policy(hidden_size=hidden_size, cell=cell, num_layers=num_layers)
+            self.policy_base = Policy(hidden_size=hidden_size, cell=cell, num_layers=num_layers,
+                                      value_heads=self.n_value_heads)
 
         if self.checkpoint:
             logger.info('Checkpointing to: {}'.format(self.log_dir))
@@ -1008,7 +1112,10 @@ class DotaOptimizer:
             # strict=False as the reference (:263-266): a checkpoint with fewer recurrent layers (e.g. a 1-layer model
             # loaded into num_layers=2) sets the layers it has and leaves rnn.*_l1 ... at their seeded initial values; its
             # Adam moments (keyed by parameter index) do not fit the new layout and are not restored (below)
-            self.policy_base.load_state_dict(torch.load(pretrained_model, map_location='cpu'), strict=False)
+            state = torch.load(pretrained_model, map_location='cpu')
+            if self.value_heads is not None:        # the published head is one row: the K rows come from the side file
+                state = self._value_heads_state(state, pretrained_model)
+            self.policy_base.load_state_dict(state, strict=False)
             if self.checkpoint:
                 # before the data-parallel wrapper broadcasts the weights: the normalised head must be in place
                 self._restore_value_norm(os.path.join(os.path.dirname(pretrained_model),
@@ -1041,18 +1148,27 @@ class DotaOptimizer:
         # grad-norm metrics and PPO diagnostics side by side: the step reads both back with one copy.  KL control: two more
         # metrics, the all-ranks KL and the skip flag of dc_grad_finish_kl
         self._n_metrics = _lib.FINISH_KL_METRICS if self.kl_control else 4
-        self._result_dev = torch.zeros(self._n_metrics + _lib.PPO_STATS_SLOTS, dtype=torch.float32, device=self.device)
-        self._metrics, self._ppo_stats = self._result_dev[:self._n_metrics], self._result_dev[self._n_metrics:]
+        # value heads: their statistics (dc_value_heads_loss) follow the PPO diagnostics, read back by the same copy
+        n_vh = 0 if self.value_heads is None else _lib.VALUE_HEADS_STATS_SLOTS
+        self._result_dev = torch.zeros(self._n_metrics + _lib.PPO_STATS_SLOTS + n_vh, dtype=torch.float32,
+                                       device=self.device)
+        self._metrics = self._result_dev[:self._n_metrics]
+        self._ppo_stats = self._result_dev[self._n_metrics:self._n_metrics + _lib.PPO_STATS_SLOTS]
+        self._value_head_stats = self._result_dev[self._n_metrics + _lib.PPO_STATS_SLOTS:] if n_vh else None
         self._finish_ws = torch.zeros(_lib.FINISH_WORKSPACE_BYTES, dtype=torch.uint8, device=self.device)
         # learning_rate, e_clip, entropy_coef, vf_coef, MAX_GRAD_NORM and value_clip are read by the step's kernels from this
         # device block, rewritten from the pinned host copy before every step: a captured graph of the step holds the
         # block's address, not the values, so assignments between steps reach replayed steps too
-        self._hparams_host = torch.zeros(_lib.HPARAM_SLOTS, dtype=torch.float64).pin_memory()
-        self._hparams_dev = torch.zeros(_lib.HPARAM_SLOTS, dtype=torch.float64, device=self.device)
+        # Value heads: a second block, the first with vf_coef = 0 and no value clip, for the PPO loss, whose value term
+        # dc_value_heads_loss replaces; both blocks go up in the one copy
+        n_blocks = 1 if self.value_heads is None else 2
+        self._hparams_host_all = torch.zeros((n_blocks, _lib.HPARAM_SLOTS), dtype=torch.float64).pin_memory()
+        self._hparams_dev_all = torch.zeros((n_blocks, _lib.HPARAM_SLOTS), dtype=torch.float64, device=self.device)
+        self._hparams_host, self._hparams_dev = self._hparams_host_all[0], self._hparams_dev_all[0]
+        self._hparams_dev_ppo = self._hparams_dev_all[n_blocks - 1]
         self._hparams_uploaded = None       # the values the device block holds
         self.last_ppo_stats = None          # approx_kl, clip_fraction (and per head), explained_variance of the last step
-        self._host_result = torch.zeros(_lib.LOSS_SLOTS + self._n_metrics + _lib.PPO_STATS_SLOTS,
-                                        dtype=torch.float32).pin_memory()
+        self._host_result = torch.zeros(_lib.LOSS_SLOTS + self._result_dev.numel(), dtype=torch.float32).pin_memory()
         self.last_step_launch_estimate = 0
         self._staging, self._staging_event = {}, None    # pinned host staging of the batched experience prep
         # rollout_prefetch > 0: a background thread pulls and unpickles up to that many rollouts ahead (same order, same
@@ -1114,6 +1230,28 @@ class DotaOptimizer:
         logger.info('Restoring the adaptive KL coefficient from {}'.format(path))
         self.kl_coef = float(torch.load(path, map_location='cpu')['kl_coef'])
 
+    def _value_heads_state(self, state, model_path):
+        """Resume with ``value_heads``: ``state`` (the published model at ``model_path``, whose value head is one row) with
+        the K-row head from the ``VALUE_HEADS_FILENAME_FMT`` file of the same iteration next to it (``upload_model``).  Raises ``ValueError`` when the file's groups are not this run's: its rows
+        cannot be reinterpreted.  Without the file -- a model of the reference or of a run without heads -- every head
+        starts from ``split_value_head``: W / K and b / K, so the summed value starts where the one-row head's was."""
+        vh = self.value_heads
+        it = re.search(r'(\d+)(?=\.pt$)', os.path.basename(model_path))
+        path = os.path.join(os.path.dirname(model_path), self.VALUE_HEADS_FILENAME_FMT % int(it.group(0))) if it else ''
+        if os.path.isfile(path):
+            st = torch.load(path, map_location='cpu')
+            saved = (tuple(st['names']), tuple(tuple(k) for k in st['keys']))
+            if saved != (vh.names, vh.keys):
+                raise ValueError("%s holds value heads %s; this run's are %s: the heads cannot be reinterpreted"
+                                 % (path, dict(zip(*saved)), dict(zip(vh.names, vh.keys))))
+            logger.info('Restoring the %d value heads from %s', len(vh.names), path)
+            return dict(state, **{'affine_value.weight': st['weight'], 'affine_value.bias': st['bias']})
+        if 'affine_value.weight' in state and state['affine_value.weight'].shape[0] == 1:
+            logger.info('No value heads next to %s: every one of the %d heads starts from 1/%d of its one-row value head',
+                        model_path, self.n_value_heads, self.n_value_heads)
+            return split_value_head(state, self.n_value_heads)
+        return state
+
     def _restore_value_norm(self, path):
         """Resume with ``value_norm``: the statistics and the exact normalised value head from ``path`` (written by
         ``upload_model`` next to the weights).  Without the file -- e.g. a model trained without the feature -- the
@@ -1157,6 +1295,11 @@ class DotaOptimizer:
             w_n, b_n = state_dict['affine_value.weight'], state_dict['affine_value.bias']
             state_dict['affine_value.weight'] = (sigma * w_n.double()).float()
             state_dict['affine_value.bias'] = (sigma * b_n.double() + mu).float()
+        if self.value_heads is not None:
+            # the published model is the reference's network: the K rows folded into one, V = sum_k V_k (strict-loadable
+            # by unmodified agents); the rows themselves go to the side file below
+            w_h, b_h = state_dict['affine_value.weight'], state_dict['affine_value.bias']
+            state_dict = fold_value_heads(state_dict)
         torch.save(obj=state_dict, f=buffer)                              # same bytes-format as :705-709
         state_dict_b = buffer.getvalue()
         if self.checkpoint:
@@ -1171,6 +1314,11 @@ class DotaOptimizer:
                 torch.save({'m': m, 'q': q, 'w': w, 'weight': w_n, 'bias': b_n},
                            os.path.join(self.log_dir, self.VALUE_NORM_FILENAME_FMT % version))
                 side.append(r'value_norm_\d{9}\.state')
+            if self.value_heads is not None:    # the K rows and what they mean, for resume
+                vh = self.value_heads
+                torch.save({'names': list(vh.names), 'keys': [list(k) for k in vh.keys], 'gammas': vh.gammas.tolist(),
+                            'weight': w_h, 'bias': b_h}, os.path.join(self.log_dir, self.VALUE_HEADS_FILENAME_FMT % version))
+                side.append(r'value_heads_\d{9}\.state')
             if self.kl_target is not None:  # the adaptive KL coefficient the next iteration trains with, for resume
                 torch.save({'kl_coef': self.kl_coef}, os.path.join(self.log_dir, self.KL_COEF_FILENAME_FMT % version))
                 side.append(r'kl_coef_\d{9}\.state')
@@ -1321,10 +1469,10 @@ class DotaOptimizer:
             if cut:                                    # V(s_L) of every cut rollout: one step of batch R' from slot L_i
                 hb = ops.stack_layers([yb[slot_last, col_last] for yb in ybufs])
                 cb = ops.stack_layers([c[slot_last, col_last] for c in cbufs]) if lstm else None
-                bootstrap = self._rollout_forward(obs_next, hb, cb)[3].reshape(len(cut))
+                bootstrap = self._rollout_forward(obs_next, hb, cb)[3].reshape((len(cut),) + self._vh_shape)
                 if vn is not None:
                     bootstrap = ops.value_denorm(bootstrap, *vn)
-                boot = torch.cat([bootstrap.new_zeros(1), bootstrap])[boot_slot]          # per segment
+                boot = torch.cat([bootstrap.new_zeros((1,) + self._vh_shape), bootstrap])[boot_slot]   # per segment
             keys = ops.HEAD_KEYS
             old_log_probs = None
             if self.kl_control:                        # and every head's full masked log-prob row, for the KL terms
@@ -1335,7 +1483,8 @@ class DotaOptimizer:
                 old_logp = ops.selected_logp([logits[k] for k in keys], [masks[k] for k in keys],
                                              [actions[k] for k in keys]).view(Lmax, R, 5)        # :387-390
             # GAE per rollout over ITS padded length: back-to-back segments, rollout-major
-            values_lr = values.reshape(Lmax, R) if vn is None else ops.value_denorm(values, *vn).view(Lmax, R)
+            values_lr = values.reshape((Lmax, R) + self._vh_shape) if vn is None else \
+                ops.value_denorm(values, *vn).view(Lmax, R)
 
             def rollout_major(t):                    # [Lmax, R, ...] -> the rows of every rollout's padded length in turn
                 if same:
@@ -1359,6 +1508,12 @@ class DotaOptimizer:
                     rew_c, vals_c, rollout_major(old_logp), blp_c, seg, gamma=self.gamma,
                     lam=self.gae_lambda, rho_clip=self.vtrace_rho_clip, c_clip=self.vtrace_c_clip, boot_value=boot,
                     valid_len=valid_len, stats=True)
+            elif self.value_heads is not None:
+                # every group's GAE with its own discount and head, the advantages summed; ret_c [rows(, K)]
+                vh = self.value_heads
+                adv_c, ret_c = ops.gae_scan_heads(rew_c, vals_c.reshape(-1, self.n_value_heads), seg, vh.group,
+                                                  vh.gammas, self.gae_lambda, boot_value=boot, boot_reward=boot)
+                ret_c = ret_c.view((-1,) + self._vh_shape)
             else:
                 # :417-421; a cut rollout's returns go on past the cut as gamma^(L-t) V(s_L), its advantages from V(s_L)
                 adv_c, ret_c = ops.gae_scan(rew_c, vals_c, seg, gamma=self.gamma, lam=self.gae_lambda, boot_value=boot,
@@ -1369,7 +1524,7 @@ class DotaOptimizer:
                 valid = torch.arange(S, device=dev).unsqueeze(1) < lens.unsqueeze(0)             # [S, B]
                 real = valid.t().reshape(-1)                                                      # rollout-major rows
                 adv_c.masked_fill_(~real, 0.0)
-                ret_c.masked_fill_(~real, 0.0)
+                ret_c.masked_fill_(~real.view((-1,) + (1,) * len(self._vh_shape)), 0.0)
             if self.value_norm:                        # the statistics of this batch's raw targets, then the POP rescale
                 self._update_value_norm(ret_c, real if self.mask_padding else None)
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
@@ -1387,7 +1542,8 @@ class DotaOptimizer:
         ``[T, R, ...]`` observations (``Policy.INPUT_KEYS``), every recurrent layer from ``h0`` / ``c0 [L, R, H]`` (c0 None
         for the GRU) keeping its state buffers, and the heads.  Returns ``(ybufs, cbufs, logits, values)``: per layer the
         ``[T + 1, R, H]`` state buffers of ``ops.rnn_stack_forward_states`` (slot t: the state entering step t), the head
-        logits and the value column ``[T, R, 1]`` of the packed head output (normalised under ``value_norm``)."""
+        logits and the value columns ``[T, R, K]`` of the packed head output (K = the value heads, 1 without them;
+        normalised under ``value_norm``)."""
         pol = self.policy_base
         x, unit_embedding = pol._encode(obs['env'], [obs[k] for k in Policy.INPUT_KEYS[1:]])
         layers = [pol.rnn.layer(k) for k in range(pol.num_layers)]
@@ -1418,7 +1574,8 @@ class DotaOptimizer:
                                observations={k: v[sl, i] for k, v in obs.items()},
                                actions={k: v[sl, i] for k, v in actions.items()},
                                masks={k: v[sl, i] for k, v in masks.items()},
-                               values=p['values_lr'][sl, i].reshape(1, S, 1), rewards=p['rewards_np'][i, sl], hidden=hid,
+                               values=p['values_lr'][sl, i].reshape(1, S, self.n_value_heads), rewards=p['rewards_np'][i, sl],
+                               hidden=hid,
                                old_logp=p['old_logp'][sl, i],
                                valid=None if p['valid'] is None else p['valid'][:, col + j],
                                old_log_probs=None if p['old_log_probs'] is None else p['old_log_probs'][sl, i])
@@ -1472,7 +1629,7 @@ class DotaOptimizer:
         old_logp = chunked(p['old_logp'])
         B = sum(n_chunks)
         adv = p['adv_c'].view(B, S).t().contiguous()                  # the GAE outputs are rollout-major back-to-back segments
-        ret = p['ret_c'].view(B, S).t().contiguous()
+        ret = p['ret_c'].view((B, S) + tuple(p['ret_c'].shape[1:])).transpose(0, 1).contiguous()   # [S, B(, K)]
         # hidden state entering chunk j of rollout i = state buffer slot j*S of every layer (:340,384-385: carried, not
         # re-zeroed), stacked [L, B, H]
         t_idx = torch.tensor([j * S for i in range(R) for j in range(n_chunks[i])], dtype=torch.int64, device=self.device)
@@ -1521,7 +1678,9 @@ class DotaOptimizer:
         n_tm = len(keys_o) + 2 * len(keys_h)
         old_logp, old_values = g[n_tm], g[n_tm + 1]
         old_log_probs = g[n_tm + 2] if kl_rows else None
-        adv, ret = gather([p['adv_c'], p['ret_c']], idx_rm, int(sum(Lps)))
+        # the K returns of a row gathered as one [rows, 1, K] row of K elements
+        ret_c = p['ret_c'] if p['ret_c'].dim() == 1 else p['ret_c'].unsqueeze(1)
+        adv, ret = gather([p['adv_c'], ret_c], idx_rm, int(sum(Lps)))
         # the host layout goes up in one pinned copy: valid, the reset slots and the state-buffer coordinates
         t_rs, c_rs = np.nonzero(lay.reset_slot >= 0)
         meta = np.concatenate([real.reshape(-1), lay.reset_slot.reshape(-1), lay.h0_step, lay.h0_rollout,
@@ -1604,6 +1763,11 @@ class DotaOptimizer:
         keys = ops.HEAD_KEYS
         self.last_ppo_stats = self._ppo_stats_dict(res[_lib.LOSS_SLOTS + self._n_metrics:].tolist(),
                                                    joint=self.policy_ratio == 'joint', kl=self.kl_control)
+        if self.value_heads is not None:    # per head: its share of the value loss and its explained variance
+            hs = res[_lib.LOSS_SLOTS + self._n_metrics + _lib.PPO_STATS_SLOTS:].tolist()
+            for k, name in enumerate(self.value_heads.names):
+                self.last_ppo_stats['loss/value/' + name] = hs[k]
+                self.last_ppo_stats['explained_variance/' + name] = hs[_lib.VALUE_HEADS_MAX + k]
         if self.kl_control:             # the all-ranks KL of the finish, and whether it skipped the update
             self.last_ppo_stats['kl_all_ranks'] = float(res[_lib.LOSS_SLOTS + 4])
             self.last_ppo_stats['kl_skipped'] = float(res[_lib.LOSS_SLOTS + 5])
@@ -1691,7 +1855,11 @@ class DotaOptimizer:
                             _lib.HP_VALUE_CLIP, _lib.HP_VALUE_NORM_MEAN, _lib.HP_VALUE_NORM_STD, _lib.HP_KL_COEF,
                             _lib.HP_KL_STOP), vals):
             h[slot] = v
-        self._hparams_dev.copy_(self._hparams_host, non_blocking=True)
+        if self.value_heads is not None:    # the PPO loss's block: the same, its value term off
+            self._hparams_host_all[1].copy_(self._hparams_host_all[0])
+            hp = self._hparams_host_all[1].numpy()
+            hp[_lib.HP_VF_COEF] = hp[_lib.HP_VALUE_CLIP] = 0.0
+        self._hparams_dev_all.copy_(self._hparams_host_all, non_blocking=True)
         # the value head has a gradient only while the value loss is on (optimizer.py:660-662): with vf_coef = 0 the
         # gradient finish skips its tensors (no Adam step, no share of the mean grad norm), like the reference's .grad = None
         self._n_actions[VALUE_SLOT:VALUE_SLOT + 1].fill_(1 if self.vf_coef > 0 else 0)
@@ -1712,11 +1880,18 @@ class DotaOptimizer:
         # e_clip / entropy_coef / vf_coef / value_clip are read from the device block (_upload_hparams); padded tokens
         # (valid = False) count for nothing under mask_padding; the policy ratio is fixed per optimizer, so a captured
         # graph of the step keeps it
+        heads = self.value_heads is not None
+        # value heads: the PPO loss runs with its value term off (_hparams_dev_ppo); the value target it is handed then
+        # feeds only an explained variance that dc_value_heads_loss overwrites, so the advantages stand in for it
         out, n_actions, d_packed, d_tu, _ = ops.ppo_loss_packed(
             packed, target_unit, [batch.masks[k] for k in keys], [batch.actions[k] for k in keys],
-            batch.old_logp, batch.advantages, batch.returns, self.e_clip, self.entropy_coef, self.vf_coef,
-            hparams=self._hparams_dev, old_value=batch.old_values, stats=self._ppo_stats, valid=valid,
-            joint=self.policy_ratio == 'joint', old_log_probs=old_log_probs, kl_out=self.flat.kl_tail)
+            batch.old_logp, batch.advantages, batch.advantages if heads else batch.returns, self.e_clip,
+            self.entropy_coef, self.vf_coef, hparams=self._hparams_dev_ppo, old_value=None if heads else batch.old_values,
+            stats=self._ppo_stats, valid=valid, joint=self.policy_ratio == 'joint', old_log_probs=old_log_probs,
+            kl_out=self.flat.kl_tail)
+        if heads:
+            ops.value_heads_loss(packed, d_packed, batch.returns, self._hparams_dev, out, self._value_head_stats,
+                                 old_value=batch.old_values, valid=valid, stats=self._ppo_stats)
         self._n_actions[:5].copy_(n_actions)
         torch.autograd.backward([packed, target_unit], [d_packed, d_tu])                                # :672
         # drop every reference into this step's autograd graph before the gradient finish: it holds the saved activations
@@ -1897,7 +2072,10 @@ class DotaOptimizer:
         reset = batch.reset()
         T = max(1, self.REFRESH_CHUNK_TOKENS // B)
         col = ops.PACK_COLS["value"][0]
-        values = None if T >= S else torch.empty((S, B), dtype=torch.float32, device=self.device)
+        c0, c1 = ops.pack_cols(self.n_value_heads)["value"]
+        heads = self.value_heads is not None          # then every head's value, [S, B, K] (K = 1 included)
+        values = None if T >= S else torch.empty((S, B) + ((c1 - c0,) if heads else ()), dtype=torch.float32,
+                                                  device=self.device)
         target = torch.empty((S * B, 5), dtype=torch.float32, device=self.device) if vtrace else None
         with torch.no_grad():
             for t0 in range(0, S, T):
@@ -1906,10 +2084,11 @@ class DotaOptimizer:
                                                 [batch.observations[k][t0:t1] for k in Policy.INPUT_KEYS[1:]])
                 y, hidden = pol._recur(x.contiguous(), hidden, None if reset is None else (reset[0][t0:t1],) + reset[1:])
                 packed, target_unit = pol._head_outputs(y, unit_embedding)
+                v = packed[..., c0:c1] if heads else packed[..., col]
                 if values is None:                  # one block: the scan reads the value column where the GEMM wrote it
-                    values = packed[..., col]
+                    values = v
                 else:
-                    values[t0:t1] = packed[..., col]
+                    values[t0:t1] = v
                 if vtrace:
                     logits = [target_unit if k == "target_unit" else packed[..., ops.PACK_COLS[k][0]:ops.PACK_COLS[k][1]]
                               for k in keys]
@@ -1925,7 +2104,12 @@ class DotaOptimizer:
         (and for V-trace the target log-probs ``[S * B, 5]``) at the batch's tokens and writing ``batch.advantages`` /
         ``batch.returns`` there (``ops.gae_scan_indexed`` / ``vtrace_scan_indexed``), ending the segments on ``boot``."""
         r = batch.refresh
-        if self.advantage_estimator == 'vtrace':
+        if self.value_heads is not None:
+            vh = self.value_heads
+            ops.gae_scan_heads_indexed(r.rewards, values.reshape(-1, self.n_value_heads), r.tok, r.seg_off,
+                                       batch.advantages, batch.returns, vh.group, vh.gammas, self.gae_lambda,
+                                       boot_value=boot, boot_reward=boot)
+        elif self.advantage_estimator == 'vtrace':
             ops.vtrace_scan_indexed(r.rewards, values, target, r.behaviour_logp, r.tok, r.seg_off, batch.advantages,
                                     batch.returns, self.gamma, self.gae_lambda, self.vtrace_rho_clip, self.vtrace_c_clip,
                                     boot_value=boot, valid_len=r.valid_len)
@@ -1963,7 +2147,7 @@ class DotaOptimizer:
             h = torch.zeros((pol.num_layers, R, pol.hidden_size), dtype=torch.float32, device=dev)
             c = torch.zeros_like(h) if lstm else None
         acc = torch.zeros(2, dtype=torch.float64, device=dev)
-        values = torch.empty((Lmax, R), dtype=torch.float32, device=dev) if adv else None
+        values = torch.empty((Lmax, R) + self._vh_shape, dtype=torch.float32, device=dev) if adv else None
         target = torch.empty((Lmax * R, 5), dtype=torch.float32, device=dev) if vtrace else None
         if cut:                                # the state after each cut rollout's last step, taken from its block
             hb = torch.empty((pol.num_layers, st.cut_len.size, pol.hidden_size), dtype=torch.float32, device=dev)
@@ -1986,7 +2170,7 @@ class DotaOptimizer:
                     ops.refresh_states(ybufs, cbufs if lstm else None, t0, st.step[lo:hi], st.rollout[lo:hi],
                                        st.slot[lo:hi], batch.h0, batch.c0, batch.reset_h, batch.reset_c, acc)
                 if adv:
-                    values[t0:t1] = v.reshape(n, R)
+                    values[t0:t1] = v.reshape((n, R) + self._vh_shape)
                 if vtrace:
                     target[t0 * R:t1 * R] = ops.selected_logp([logits[k] for k in keys], [ins[('m', k)] for k in keys],
                                                               [ins[('a', k)] for k in keys])
@@ -2006,13 +2190,13 @@ class DotaOptimizer:
             vn = self._value_norm_moments() if self.value_norm else None
             boot = batch.refresh.boot
             if cut:                            # V(s_L) from the refreshed state after the last step
-                bootstrap = self._rollout_forward(st.obs_next, hb, cb)[3].reshape(-1)
+                bootstrap = self._rollout_forward(st.obs_next, hb, cb)[3].reshape((-1,) + self._vh_shape)
                 if vn is not None:
                     bootstrap = ops.value_denorm(bootstrap, *vn)
-                boot = torch.cat([bootstrap.new_zeros(1), bootstrap])[st.boot_slot]
+                boot = torch.cat([bootstrap.new_zeros((1,) + self._vh_shape), bootstrap])[st.boot_slot]
             if vn is not None:
                 values = ops.value_denorm(values, *vn)
-            vals_b = ops.gather_rows_fill([values.reshape(-1)], st.token_row)[0]
+            vals_b = ops.gather_rows_fill([values.reshape((-1,) + self._vh_shape)], st.token_row)[0]
             target_b = ops.gather_rows_fill([target], st.token_row)[0] if vtrace else None
             self._rescan(batch, vals_b, target_b, boot)
 
@@ -2108,8 +2292,8 @@ class DotaOptimizer:
         # means over the steps.  Under kl_stop they include the step that was skipped: its losses, grad norms and statistics were
         # measured at the parameters it left unchanged, and its KL is the measurement that stopped the iteration
         for k in ppo_stats[0]:
-            if k not in ('kl_all_ranks', 'kl_skipped'):
-                metrics['ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
+            if k not in ('kl_all_ranks', 'kl_skipped'):     # value heads: 'loss/value/<name>' next to 'loss/value'
+                metrics[k if k.startswith('loss/') else 'ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
         if self.kl_control:
             # d: the mean over the steps (a skipped one included) of the all-ranks KL, the same number on every rank, so
             # the adaptive coefficient stays identical across ranks
@@ -2259,14 +2443,16 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          hidden_size=256, cell="gru", num_layers=1, gamma=GAMMA, gae_lambda=LAMBDA, clip_range=0.1, max_grad_norm=0.5,
          value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
          mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False, value_norm_decay=0.99,
-         kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False, recompute_states=False):
+         kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False, recompute_states=False, value_heads=None,
+         value_gammas=None):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                        mask_padding=mask_padding, pack_sequences=pack_sequences,
                        policy_ratio=policy_ratio, value_norm=value_norm,
                        value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
                        kl_stop=kl_stop, recompute_advantages=recompute_advantages,
-                       recompute_states=recompute_states)                                 # before any process-group setup
+                       recompute_states=recompute_states, value_heads=value_heads,
+                       value_gammas=value_gammas)                                         # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -2280,7 +2466,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         num_minibatches=num_minibatches, mask_padding=mask_padding, pack_sequences=pack_sequences,
         policy_ratio=policy_ratio, value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef,
         kl_target=kl_target, kl_stop=kl_stop, recompute_advantages=recompute_advantages,
-        recompute_states=recompute_states)
+        recompute_states=recompute_states, value_heads=value_heads, value_gammas=value_gammas)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -2296,8 +2482,8 @@ def build_arg_parser():
     """The reference's flags and defaults (:777-794) plus ``--hidden-size``, ``--cell``, ``--num-layers`` and the PPO
     settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm``, ``--value-clip``,
     ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches``, ``--mask-padding``,
-    ``--pack-sequences``, ``--policy-ratio``, ``--value-norm``, ``--value-norm-decay``, ``--kl-coef``, ``--kl-target`` and
-    ``--kl-stop``."""
+    ``--pack-sequences``, ``--policy-ratio``, ``--value-norm``, ``--value-norm-decay``, ``--kl-coef``, ``--kl-target``,
+    ``--kl-stop``, ``--value-heads`` and ``--value-gammas``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -2354,6 +2540,11 @@ def build_arg_parser():
     p.add_argument("--recompute-states", action="store_true",
                    help="rerun every rollout with the current network before every epoch after the first and replace the "
                         "recurrent states its training sequences start from")
+    p.add_argument("--value-heads", type=parse_value_heads, default=None,
+                   help="one value head per reward group, 'name=key,key;name=key,...' holding every reward key once "
+                        "(default: one critic of the summed reward)")
+    p.add_argument("--value-gammas", type=parse_value_gammas, default=None,
+                   help="discounts of some value heads, 'name=0.999;...' (the others take --gamma)")
     return p
 
 
@@ -2371,6 +2562,6 @@ if __name__ == '__main__':
              mask_padding=args.mask_padding, pack_sequences=args.pack_sequences, policy_ratio=args.policy_ratio,
              value_norm=args.value_norm, value_norm_decay=args.value_norm_decay, kl_coef=args.kl_coef,
              kl_target=args.kl_target, kl_stop=args.kl_stop, recompute_advantages=args.recompute_advantages,
-             recompute_states=args.recompute_states)
+             recompute_states=args.recompute_states, value_heads=args.value_heads, value_gammas=args.value_gammas)
     except KeyboardInterrupt:
         pass

@@ -30,6 +30,7 @@ logger = logging.getLogger(__name__)
 eps = np.finfo(np.float32).eps.item()          # policy.py:15
 TICKS_PER_OBSERVATION = 15                      # policy.py:17
 REWARD_KEYS = ['enemy', 'win', 'xp', 'hp', 'kills', 'death', 'lh', 'denies', 'tower_hp', 'mana']  # policy.py:20
+MAX_VALUE_HEADS = len(REWARD_KEYS)             # one value head per reward group (DotaOptimizer(value_heads=...))
 
 # (parameter suffix, observation key, units per step) in concatenation order (policy.py:99-131)
 UNIT_GROUPS = (("ah", "allied_heroes", 1), ("eh", "enemy_heroes", 5), ("anh", "allied_nonheroes", 16),
@@ -78,12 +79,15 @@ class Policy(nn.Module):
     INPUT_KEYS = ['env', 'allied_heroes', 'enemy_heroes', 'allied_nonheroes', 'enemy_nonheroes',
                   'allied_towers', 'enemy_towers']
 
-    def __init__(self, *, hidden_size=256, cell="gru", num_layers=1):
+    def __init__(self, *, hidden_size=256, cell="gru", num_layers=1, value_heads=1):
         super().__init__()
         if cell not in ("gru", "lstm"):
             raise ValueError("cell must be 'gru' or 'lstm'")
         if int(num_layers) != num_layers or num_layers < 1:
             raise ValueError("num_layers must be an integer >= 1, got %r" % (num_layers,))
+        if isinstance(value_heads, bool) or int(value_heads) != value_heads or not 1 <= value_heads <= MAX_VALUE_HEADS:
+            raise ValueError("value_heads must be an integer in [1, %d], got %r" % (MAX_VALUE_HEADS, value_heads))
+        self.value_heads = int(value_heads)
         self.hidden_size = H = int(hidden_size)
         self.cell = cell
         self.num_layers = int(num_layers)
@@ -101,7 +105,7 @@ class Policy(nn.Module):
         self.affine_move_y = nn.Linear(H, self.N_MOVE_ENUMS)
         self.affine_unit_attention = nn.Linear(H, 128)
         self.affine_head_ability = nn.Linear(H, 3)
-        self.affine_value = nn.Linear(H, 1)
+        self.affine_value = nn.Linear(H, self.value_heads)      # created last: value_heads leaves every other init as is
 
     # ------------------------------------------------------------------ reference API
     def init_hidden(self):
@@ -123,7 +127,8 @@ class Policy(nn.Module):
 
     def forward(self, env, allied_heroes, enemy_heroes, allied_nonheroes, enemy_nonheroes,
                 allied_towers, enemy_towers, hidden):
-        """Batch-first ``(b, s, ...)`` inputs -> (logits dict ``(b, s, n)``, value ``(b, s, 1)``, hidden).  ``hidden`` is
+        """Batch-first ``(b, s, ...)`` inputs -> (logits dict ``(b, s, n)``, value ``(b, s, K)`` with K = ``value_heads``,
+        hidden).  ``hidden`` is
         ``[L, b, H]`` (an ``(h, c)`` pair for the LSTM) in and out: as in torch, not batch-first."""
         return self._run((env, allied_heroes, enemy_heroes, allied_nonheroes, enemy_nonheroes,
                           allied_towers, enemy_towers), hidden, time_major=False)
@@ -181,11 +186,11 @@ class Policy(nn.Module):
 
     def _head_outputs(self, y, unit_embedding):
         """The attention projection and ONE packed ``[*, 128]`` tensor-core GEMM for the four small heads + the value head
-        (26 real rows, zero padding; their logits are column ranges of its output, ``ops.PACK_COLS``), then the target-unit
+        (25 + value_heads real rows, zero padding; their logits are column ranges of its output, ``ops.pack_cols``), then the target-unit
         dot products -> (packed output, target-unit logits)."""
         attention = ops.linear(y, self.affine_unit_attention.weight, self.affine_unit_attention.bias)
         H = self.hidden_size
-        pad = y.new_zeros(ops.PACK_WIDTH - 26, H)
+        pad = y.new_zeros(ops.PACK_WIDTH - 25 - self.value_heads, H)
         w_pack = torch.cat([self.affine_head_enum.weight, self.affine_move_x.weight, self.affine_move_y.weight,
                             self.affine_head_ability.weight, self.affine_value.weight, pad], dim=0)
         b_pack = torch.cat([self.affine_head_enum.bias, self.affine_move_x.bias, self.affine_move_y.bias,
@@ -196,7 +201,7 @@ class Policy(nn.Module):
     def _heads(self, y, unit_embedding):
         """Action heads + value (``policy.py:144-155``): column ranges of the packed output, and the target-unit logits."""
         packed, target_unit = self._head_outputs(y, unit_embedding)
-        cols = ops.PACK_COLS
+        cols = ops.pack_cols(self.value_heads)
         head_enum, move_x, move_y, ability, value = (packed[..., cols[k][0]:cols[k][1]]
                                                      for k in ("enum", "x", "y", "ability", "value"))
         return {'enum': head_enum, 'x': move_x, 'y': move_y, 'target_unit': target_unit, 'ability': ability}, value
@@ -267,7 +272,7 @@ class Policy(nn.Module):
         ``hidden``: ``[L, A, H]`` (``(h, c)`` for the LSTM; L = ``num_layers``); ``observations``: ``{key: [A, ...]}`` (what ``single`` takes, with
         a leading agent dimension); ``masks``: ``{head: [A, n]}`` legal-action masks (``action_masks``); ``u``: optional
         ``[A, 5]`` uniforms.  Returns ``(chosen {head: int32 [A], -1 = not sampled}, logp [A, 5], logits {head: [A, n]},
-        value [A], new hidden)``.  Index selection is ``oracle.ref_policy.sample_index``'s inverse CDF up to fp32 rounding: the two
+        value [A] ([A, K] with K = value_heads > 1), new hidden)``.  Index selection is ``oracle.ref_policy.sample_index``'s inverse CDF up to fp32 rounding: the two
         agree unless u lies within the rounding band of a cumulative boundary (a few 1e-6 for logits of order 1, up to about
         5e-5 at |logit| 60), where either may take the adjacent legal index.
 
@@ -279,7 +284,7 @@ class Policy(nn.Module):
             logits, value, new_hidden = self.forward_time_major(obs, hidden)
             flat = {k: v[0] for k, v in logits.items()}
             chosen, logp = self.select_actions_batched(flat, masks, u)
-        return chosen, logp, flat, value[0, :, 0], new_hidden
+        return chosen, logp, flat, value[0, :, 0] if self.value_heads == 1 else value[0], new_hidden
 
     @classmethod
     def head_masks(cls, selections):
@@ -312,3 +317,31 @@ class Policy(nn.Module):
             masks['enum'][0, 0, 2] = False
         masks['target_unit'][0, 0] = valid_units
         return masks
+
+
+def fold_value_heads(state_dict):
+    """A copy of ``state_dict`` whose K-row value head is folded into the reference's one-row head: W = sum_k W_k and
+    b = sum_k b_k, summed in fp32 in head order.  Its value is sum_k V_k, which is the value of the total reward only when
+    every head has the same discount.  A one-row head is returned unchanged."""
+    out = dict(state_dict)
+    w, b = out['affine_value.weight'], out['affine_value.bias']
+    if w.shape[0] == 1:
+        return out
+    ws, bs = w[0].clone(), b[0:1].clone()
+    for k in range(1, w.shape[0]):
+        ws = ws + w[k]
+        bs = bs + b[k:k + 1]
+    out['affine_value.weight'], out['affine_value.bias'] = ws.unsqueeze(0), bs
+    return out
+
+
+def split_value_head(state_dict, K):
+    """A copy of ``state_dict`` whose one-row value head is split into ``K`` rows of W / K and b / K, so that the summed
+    value sum_k V_k starts where the one-row head's value was (up to fp32 rounding of the division)."""
+    out = dict(state_dict)
+    w, b = out['affine_value.weight'], out['affine_value.bias']
+    if w.shape[0] != 1:
+        raise ValueError("split_value_head needs a one-row value head, got %s" % (tuple(w.shape),))
+    out['affine_value.weight'] = (w / K).expand(K, -1).clone()
+    out['affine_value.bias'] = (b / K).expand(K).clone()
+    return out

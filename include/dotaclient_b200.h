@@ -107,6 +107,56 @@ int dc_vtrace_scan_indexed(const float *rewards, int n_sub, const float *values,
                            double gamma, double lam, double rho_clip, double c_clip, float *pg_adv, float *vs,
                            double *seg_stats, dc_stream_t stream);
 
+/* ---- GAE with one value head per reward group ------------------------------------------------
+ * DotaOptimizer(value_heads=...): the sub-rewards of a row are split into K groups, each with its own critic column and
+ * discount, all sharing lam.  Per segment, as dc_gae_scan, and per group k:
+ *   r_k,t = the fp32 sum of the row's columns in group k, ascending, in the pairwise order np.sum(rewards, axis=1)
+ *           applies to a row (np.ascontiguousarray(rewards[:, idx_k]).sum(axis=1))
+ *   delta_k,t in fp32 (three roundings), A_k,t = delta_k,t + gamma_k lam A_k,t+1 and R_k,t = r_k,t + gamma_k R_k,t+1
+ *   in float64, from the segment's bootstraps boot_value[seg * K + k] / boot_reward[seg * K + k] (NULL = 0)
+ * outputs: adv[row] = fp32(sum_k A_k,t) (float64 sum in head order, rounded once), ret[row * K + k] = fp32(R_k,t).
+ *   group   [n_sub] int32, HOST: the group 0 .. K-1 of every reward column; every group holds at least one column
+ *   gammas  [K] float64, HOST: the discounts, each in (0, 1]
+ *   values  [n_rows, K]: head k's value of row r at values[r * K + k]
+ * With K = 1 and one group of all columns the results are dc_gae_scan's, bit for bit (the same per-channel step).
+ * The _indexed form has dc_gae_scan_indexed's token layout: row r reads values[tok[r] * ld_values + k] (ld_values >= K;
+ * the packed head output: its row width) and writes adv[tok[r]] and ret[tok[r] * K + k]; tok[r] < 0 reads 0, writes nothing.
+ * Checked before any CUDA call (DC_EINVAL): 1 <= K <= DC_VALUE_HEADS_MAX, 1 <= n_sub < 128, the group map, the gammas,
+ * 0 <= lam <= 1, and null pointers.  One warp per segment, every group's channel in the same pass over the tiles.
+ */
+#define DC_VALUE_HEADS_MAX 10
+int dc_gae_scan_heads(const float *rewards, int n_sub, const int32_t *group, int K, const float *values,
+                      const int64_t *seg_off, int n_seg, const float *boot_value, const float *boot_reward,
+                      const double *gammas, double lam, float *adv, float *ret, dc_stream_t stream);
+int dc_gae_scan_heads_indexed(const float *rewards, int n_sub, const int32_t *group, int K, const float *values,
+                              int64_t ld_values, const int64_t *tok, const int64_t *seg_off, int n_seg,
+                              const float *boot_value, const float *boot_reward, const double *gammas, double lam,
+                              float *adv, float *ret, dc_stream_t stream);
+
+/* ---- value loss of K value heads ----------------------------------------------------------------
+ * Runs after one of the dc_ppo_loss_fwd_bwd_* entry points that was given a hparams block with DC_HP_VF_COEF = 0 and
+ * DC_HP_VALUE_CLIP = 0, on the same stream, and adds the value term of K heads:
+ *   value   head k of token t at value[t * ld_value + k] (ld_value >= K: the packed head output's value columns)
+ *   ret     [N, K] the value targets; old_value [N, K] or NULL: the prep-time values (clipped loss when
+ *           hparams[DC_HP_VALUE_CLIP] > 0); valid [N] or NULL: the tokens that count (NULL: all)
+ *   hparams the step's block: DC_HP_VF_COEF and DC_HP_VALUE_CLIP are read
+ *   dvalue  written at [t * ld_dvalue + k] for every token: vf_coef (v - R) / N_v (or the clipped term's gradient), 0
+ *           on tokens that do not count; N_v = the number of counting tokens (N without a mask)
+ *   out     out[3] = vf_coef * 0.5 * sum_k mean (R_k - V_k)^2 (each head PPO2-clipped as the PPO loss clips one), and
+ *           out[0] += out[3]
+ *   stats   [DC_PPO_STATS_SLOTS] or NULL: DC_STAT_EXPLAINED_VAR = the explained variance of sum_k V_k against sum_k R_k
+ *   head_stats [DC_VALUE_HEADS_STATS_SLOTS]: [k] head k's value loss (vf_coef * 0.5 * mean), [DC_VALUE_HEADS_MAX + k]
+ *           its explained variance; 0 for k >= K
+ *   workspace  DC_VALUE_HEADS_WORKSPACE_BYTES of scratch (zeroed by the call itself)
+ * Float64 reductions in a fixed order (bitwise reproducible).  Checked: N > 0, 1 <= K <= DC_VALUE_HEADS_MAX, pitches,
+ * null pointers -> DC_EINVAL before any CUDA call.
+ */
+#define DC_VALUE_HEADS_STATS_SLOTS 20
+#define DC_VALUE_HEADS_WORKSPACE_BYTES 131072
+int dc_value_heads_loss(const float *value, int64_t ld_value, const float *ret, const float *old_value,
+                        const uint8_t *valid, int64_t N, int K, const double *hparams, float *dvalue, int64_t ld_dvalue,
+                        float *out, float *stats, float *head_stats, void *workspace, dc_stream_t stream);
+
 /* ---- minibatch assembly: column gather ----------------------------------------------------
  * Picks the sequence columns `index` out of many time-major tensors in ONE launch (the minibatches of PPO epochs,
  * DotaOptimizer.train_epochs; the reference trains on the whole batch and has no counterpart).  Descriptor d describes a
