@@ -46,6 +46,8 @@ SIGNATURES = {
     "dc_gemm_tf32x3": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _i64, _i32, _i32, _i32, _vp]),
     "dc_gemm_wgrad_workspace_bytes": (_sz, [_i32, _i32]),
     "dc_gemm_wgrad_tf32x3": (_i32, [_vp, _i32, _vp, _i32, _i64, _i32, _i32, _vp, _i32, _vp, _i32, _vp, _vp]),
+    "dc_gemm_tf32x3_rows": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "dc_gemm_wgrad_tf32x3_rows": (_i32, [_vp, _i32, _vp, _i32, _vp, _i64, _vp, _i32, _i32, _vp, _i32, _vp, _i32, _vp, _vp]),
     "dc_unit_basic_bwd_workspace_bytes": (_sz, []),
     "dc_env_fwd": (_i32, [_vp, _vp, _vp, _vp, _i32, _i64, _vp]),
     "dc_env_bwd_workspace_bytes": (_sz, []),
@@ -59,6 +61,11 @@ SIGNATURES = {
     "dc_unit_embed_fwd_mask": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i64, _i32, _vp]),
     "dc_target_unit_q_fwd": (_i32, [_vp, _i32, _c.c_void_p * 6, _vp, _vp, _vp, _i64, _vp]),
     "dc_target_unit_q_bwd": (_i32, [_vp, _c.c_void_p * 6, _vp, _vp, _vp, _i32, _i64, _vp]),
+    "dc_target_unit_q_fwd_rows": (_i32, [_vp, _i32, _c.c_void_p * 6, _vp, _vp, _vp, _i64, _vp, _vp, _vp]),
+    "dc_target_unit_q_bwd_rows": (_i32, [_vp, _c.c_void_p * 6, _vp, _vp, _vp, _i32, _i64, _vp, _vp, _vp]),
+    "dc_target_rows_workspace_bytes": (_sz, [_i64]),
+    "dc_target_rows": (_i32, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "dc_rows_zero_inactive": (_i32, [_vp, _i64, _vp, _i32, _i32, _vp]),
     "dc_ppo_loss_fwd_bwd": (_i32, [_ptr5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _ptr5, _vp, _vp,
                                    _vp, _vp, _vp]),
     "dc_ppo_loss_fwd_bwd_strided": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _i64, _i64, _f32, _f32, _f32,

@@ -191,16 +191,23 @@ __device__ __forceinline__ float4 basic_row(const float4 *row, const float (&w)[
                        dc_unit_basic(u, w[3], b[3]));
 }
 
+// kRows: the head on a row list -- item i < *count is token rows[i], whose q row is row i of the compact q; the logits go to
+// row rows[i] and other rows are not written.
+template <bool kRows = false>
 __global__ void __launch_bounds__(kThreadsE) target_unit_q_fwd_kernel(const float *__restrict__ q, int ld_q, UnitPtrs units,
                                                                       const float *__restrict__ w_b, const float *__restrict__ b_b,
-                                                                      float *__restrict__ logits, int64_t N) {
+                                                                      float *__restrict__ logits, int64_t N,
+                                                                      const int *__restrict__ rows = nullptr,
+                                                                      const int *__restrict__ count = nullptr) {
     __shared__ float4 s_u[kWarps][kTokenU4];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float w[4][kIn], b[4];
     load_basic_weights(w, b, w_b, b_b, lane);
     float4 *su = s_u[warp];
-    for (int64_t n = (int64_t)blockIdx.x * kWarps + warp; n < N; n += (int64_t)gridDim.x * kWarps) {
-        const float *qrow = q + n * ld_q;
+    if constexpr (kRows) N = min(N, (int64_t)__ldg(count));
+    for (int64_t i = (int64_t)blockIdx.x * kWarps + warp; i < N; i += (int64_t)gridDim.x * kWarps) {
+        const int64_t n = kRows ? (int64_t)__ldg(rows + i) : i;
+        const float *qrow = q + i * ld_q;
         __syncwarp();                                              // the previous token's rows have been read
         stage_token_units(su, units, n, lane);
         __syncwarp();
@@ -225,20 +232,26 @@ __global__ void __launch_bounds__(kThreadsE) target_unit_q_fwd_kernel(const floa
 
 // s[n, g*128 + j] = sum_u dlogits[n, off_g + u] basic_g[n,u,j],  s[n, 768 + g] = sum_u dlogits[n, off_g + u]  (zeros elsewhere):
 // d_att = s [W_0 | ... | W_5 | b_0..b_5]^T is then one GEMM over tokens.  Tokens that did not use the head write zeros, read nothing.
+// kRows: item i < *count is token rows[i]; its s row is row i of the compact s, and no row past the count is written.
+template <bool kRows = false>
 __global__ void __launch_bounds__(kThreadsE) target_unit_q_bwd_kernel(const float *__restrict__ dlogits, UnitPtrs units,
                                                                       const float *__restrict__ w_b, const float *__restrict__ b_b,
-                                                                      float *__restrict__ s, int ld_s, int64_t N) {
+                                                                      float *__restrict__ s, int ld_s, int64_t N,
+                                                                      const int *__restrict__ rows = nullptr,
+                                                                      const int *__restrict__ count = nullptr) {
     __shared__ float4 s_u[kWarps][kTokenU4];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float w[4][kIn], b[4];
     load_basic_weights(w, b, w_b, b_b, lane);
     float4 *su = s_u[warp];
     const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int64_t n = (int64_t)blockIdx.x * kWarps + warp; n < N; n += (int64_t)gridDim.x * kWarps) {
+    if constexpr (kRows) N = min(N, (int64_t)__ldg(count));
+    for (int64_t i = (int64_t)blockIdx.x * kWarps + warp; i < N; i += (int64_t)gridDim.x * kWarps) {
+        const int64_t n = kRows ? (int64_t)__ldg(rows + i) : i;
         const float g_lo = dlogits[n * kMaxUnits + lane];
         const float g_hi = lane < kMaxUnits - 32 ? dlogits[n * kMaxUnits + 32 + lane] : 0.f;
         const bool any = __any_sync(0xffffffffu, g_lo != 0.f || g_hi != 0.f);
-        float4 *srow = reinterpret_cast<float4 *>(s + n * ld_s) + lane;
+        float4 *srow = reinterpret_cast<float4 *>(s + i * ld_s) + lane;
         if (!any) {
 #pragma unroll
             for (int g = 0; g < 7; ++g) srow[g * (kC / 4)] = zero;
@@ -322,31 +335,57 @@ extern "C" int dc_env_bwd(const float *d_out, const float *out, int ld, const fl
     return DC_OK;
 }
 
-extern "C" int dc_target_unit_q_fwd(const float *q, int ld_q, const float *const units[6], const float *w_b, const float *b_b,
-                                    float *logits, int64_t N, dc_stream_t stream) {
-    DC_REQUIRE(q && w_b && b_b && logits && N > 0 && ld_q >= 7 * kC && ld_q % 4 == 0, DC_EINVAL, "dc_target_unit_q_fwd: bad arguments");
+template <bool kRows>
+static int q_fwd(const float *q, int ld_q, const float *const units[6], const float *w_b, const float *b_b, float *logits, int64_t N,
+                 const int32_t *rows, const int32_t *count, dc_stream_t stream, const char *who) {
+    DC_REQUIRE(q && w_b && b_b && logits && N > 0 && ld_q >= 7 * kC && ld_q % 4 == 0 && (!kRows || (rows && count)), DC_EINVAL,
+               "%s: bad arguments", who);
     UnitPtrs up;
-    const int rc = unit_ptrs(units, &up, "dc_target_unit_q_fwd");
+    const int rc = unit_ptrs(units, &up, who);
     if (rc != DC_OK) return rc;
-    DC_REQUIRE(((uintptr_t)q & 15) == 0, DC_EINVAL, "dc_target_unit_q_fwd: alignment");
+    DC_REQUIRE(((uintptr_t)q & 15) == 0, DC_EINVAL, "%s: alignment", who);
     int per_sm = 0;
-    DC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, target_unit_q_fwd_kernel, kThreadsE, 0));
-    target_unit_q_fwd_kernel<<<head_grid(per_sm, N), kThreadsE, 0, dc_cu_stream(stream)>>>(q, ld_q, up, w_b, b_b, logits, N);
+    DC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, target_unit_q_fwd_kernel<kRows>, kThreadsE, 0));
+    target_unit_q_fwd_kernel<kRows><<<head_grid(per_sm, N), kThreadsE, 0, dc_cu_stream(stream)>>>(q, ld_q, up, w_b, b_b, logits, N, rows,
+                                                                                                  count);
     DC_LAUNCH_OK();
     return DC_OK;
 }
 
-extern "C" int dc_target_unit_q_bwd(const float *dlogits, const float *const units[6], const float *w_b, const float *b_b, float *s,
-                                    int ld_s, int64_t N, dc_stream_t stream) {
-    DC_REQUIRE(dlogits && w_b && b_b && s && N > 0 && ld_s >= 7 * kC && ld_s % 4 == 0, DC_EINVAL, "dc_target_unit_q_bwd: bad arguments");
+template <bool kRows>
+static int q_bwd(const float *dlogits, const float *const units[6], const float *w_b, const float *b_b, float *s, int ld_s, int64_t N,
+                 const int32_t *rows, const int32_t *count, dc_stream_t stream, const char *who) {
+    DC_REQUIRE(dlogits && w_b && b_b && s && N > 0 && ld_s >= 7 * kC && ld_s % 4 == 0 && (!kRows || (rows && count)), DC_EINVAL,
+               "%s: bad arguments", who);
     UnitPtrs up;
-    const int rc = unit_ptrs(units, &up, "dc_target_unit_q_bwd");
+    const int rc = unit_ptrs(units, &up, who);
     if (rc != DC_OK) return rc;
-    DC_REQUIRE(((uintptr_t)s & 15) == 0, DC_EINVAL, "dc_target_unit_q_bwd: alignment");
+    DC_REQUIRE(((uintptr_t)s & 15) == 0, DC_EINVAL, "%s: alignment", who);
     int per_sm = 0;
-    DC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, target_unit_q_bwd_kernel, kThreadsE, 0));
-    target_unit_q_bwd_kernel<<<head_grid(per_sm, N), kThreadsE, 0, dc_cu_stream(stream)>>>(dlogits, up, w_b, b_b, s, ld_s, N);
+    DC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, target_unit_q_bwd_kernel<kRows>, kThreadsE, 0));
+    target_unit_q_bwd_kernel<kRows><<<head_grid(per_sm, N), kThreadsE, 0, dc_cu_stream(stream)>>>(dlogits, up, w_b, b_b, s, ld_s, N, rows,
+                                                                                                  count);
     DC_LAUNCH_OK();
     return DC_OK;
+}
+
+extern "C" int dc_target_unit_q_fwd(const float *q, int ld_q, const float *const units[6], const float *w_b, const float *b_b,
+                                    float *logits, int64_t N, dc_stream_t stream) {
+    return q_fwd<false>(q, ld_q, units, w_b, b_b, logits, N, nullptr, nullptr, stream, "dc_target_unit_q_fwd");
+}
+
+extern "C" int dc_target_unit_q_bwd(const float *dlogits, const float *const units[6], const float *w_b, const float *b_b, float *s,
+                                    int ld_s, int64_t N, dc_stream_t stream) {
+    return q_bwd<false>(dlogits, units, w_b, b_b, s, ld_s, N, nullptr, nullptr, stream, "dc_target_unit_q_bwd");
+}
+
+extern "C" int dc_target_unit_q_fwd_rows(const float *q, int ld_q, const float *const units[6], const float *w_b, const float *b_b,
+                                         float *logits, int64_t N, const int32_t *rows, const int32_t *count, dc_stream_t stream) {
+    return q_fwd<true>(q, ld_q, units, w_b, b_b, logits, N, rows, count, stream, "dc_target_unit_q_fwd_rows");
+}
+
+extern "C" int dc_target_unit_q_bwd_rows(const float *dlogits, const float *const units[6], const float *w_b, const float *b_b, float *s,
+                                         int ld_s, int64_t N, const int32_t *rows, const int32_t *count, dc_stream_t stream) {
+    return q_bwd<true>(dlogits, units, w_b, b_b, s, ld_s, N, rows, count, stream, "dc_target_unit_q_bwd_rows");
 }
 

@@ -9,7 +9,7 @@ data-gradient kernels and takes the head's rank-1 share through token-level prod
 import torch
 
 from . import _lib
-from .ops import PROFILE, _f32c, _need_cuda, gemm_tf32x3, gemm_wgrad_supported
+from .ops import PROFILE, _f32c, _need_cuda, _u8, gemm_tf32x3, gemm_wgrad_supported, gemm_wgrad_tf32x3
 
 UNITS = (1, 5, 16, 16, 1, 1)              # allied/enemy heroes, allied/enemy non-heroes, allied/enemy towers
 OFFSETS = (0, 1, 6, 22, 38, 39)
@@ -157,9 +157,9 @@ class UnitEncoder(torch.autograd.Function):
         with PROFILE.span("env_bwd", 2, 4 * N * (2 * C + 3)):
             _lib.check(lib.dc_env_bwd(d_xcat.data_ptr(), xcat.data_ptr(), XCAT, env2.data_ptr(), dw_e.data_ptr(), db_e.data_ptr(),
                                       N, _env_workspace(dev).data_ptr(), st), "dc_env_bwd")
-        dl = att = s_head = None
+        dl = att = s_head = att_head = count = None
         if pending is not None:
-            dl, att, s_head = pending
+            dl, att, s_head, att_head, count = pending     # att_head / s_head: compact rows when count is set (TargetUnitRows)
         dw_b = torch.empty((C, 12), dtype=torch.float32, device=dev)
         db_b = torch.empty(C, dtype=torch.float32, device=dev)
         dw_all = torch.zeros((6, C, C), dtype=torch.float32, device=dev)     # zeros: the enemy-tower layer has no max-pool path
@@ -191,10 +191,7 @@ class UnitEncoder(torch.autograd.Function):
                            "dc_unit_dgrad_fused_mask")
         if dl is not None:
             # the head's share of every dW_g and db_g in ONE token-level product: att^T [s_0 | ... | s_5 | sum_u dlogits]
-            dw_head = torch.empty((C, QW), dtype=torch.float32, device=dev)
-            with PROFILE.span("gemm_wgrad", 2, 4 * (N * C + N * QW + C * QW)):
-                _lib.check(lib.dc_gemm_wgrad_tf32x3(att.data_ptr(), C, s_head.data_ptr(), QW, N, C, QW, dw_head.data_ptr(), QW, None, 0,
-                                                    _wgrad_workspace(C, QW, dev).data_ptr(), st), "dc_gemm_wgrad_tf32x3")
+            dw_head, _ = gemm_wgrad_tf32x3(att_head, s_head, want_bias=False, t_dev=count, t_host=ctx.link.get("n_active"))
             dw_all += dw_head[:, :6 * C].reshape(C, 6, C).permute(1, 0, 2)
             db_all += dw_head[:, 6 * C:6 * C + 6].t()
         dws, dbs = list(dw_all.unbind(0)), list(db_all.unbind(0))
@@ -215,14 +212,11 @@ class TargetUnit(torch.autograd.Function):
     def forward(ctx, att, link):
         _need_cuda(att)
         units, w_b, b_b = link["units"], link["w_b"], link["b_b"]
-        weights, biases = link["weights"], link["biases"]
         lead = att.shape[:-1]
         N = att.numel() // C
         att2 = _f32c(att.detach()).reshape(N, C)
         dev = att2.device
-        bias_block = torch.zeros((C, C), dtype=torch.float32, device=dev)
-        bias_block[:, :6] = torch.stack(biases, dim=1)
-        bm = torch.cat(list(weights) + [bias_block], dim=1)                  # [128, 896]: bm[c, g*128+j] = W_g[c,j], bm[c, 768+g] = b_g[c]
+        bm = _head_matrix(link)
         q = gemm_tf32x3(att2, bm.t().contiguous())                           # [N, 896] = att [W_0 | ... | W_5 | b]
         logits = torch.empty((N, MAX_UNITS), dtype=torch.float32, device=dev)
         with PROFILE.span("target_unit_fwd", 1, 4 * N * (MAX_UNITS * 12 + QW + MAX_UNITS)):
@@ -244,8 +238,131 @@ class TargetUnit(torch.autograd.Function):
             _lib.check(_lib.load().dc_target_unit_q_bwd(dl.data_ptr(), _ptr6(units), w_b.data_ptr(), b_b.data_ptr(), s.data_ptr(),
                                                         QW, N, _lib.stream_ptr()), "dc_target_unit_q_bwd")
         d_att = gemm_tf32x3(s, bm)                                          # [N, 128] = s [W_0 | ... | W_5 | b]^T
-        ctx.link["pending"] = (dl, att2, s)                                  # consumed by UnitEncoder.backward
+        ctx.link["pending"] = (dl, att2, s, att2, None)                      # consumed by UnitEncoder.backward
         return d_att.view(ctx.att_shape), None
+
+
+def _head_matrix(link):
+    """[128, 896]: bm[c, g*128+j] = W_g[c,j], bm[c, 768+g] = b_g[c], zeros in the rest of the bias block."""
+    bias_block = torch.zeros((C, C), dtype=torch.float32, device=link["w_b"].device)
+    bias_block[:, :6] = torch.stack(link["biases"], dim=1)
+    return torch.cat(list(link["weights"]) + [bias_block], dim=1)
+
+
+_rows_ws = {}
+
+
+def target_rows(mask, action):
+    """-> (rows int32 [N], count int32 [1], flags uint8 [N]), all on the device: the tokens, ascending, whose target-unit
+    ``mask`` or ``action`` row (``[..., 40]`` bool) has an entry set -- the rows the PPO loss reads (``dc_target_rows``) --
+    and a 0/1 flag per token.  Entries of ``rows`` past the count are unspecified."""
+    _need_cuda(mask, action)
+    m, a = _u8(mask).reshape(-1, MAX_UNITS), _u8(action).reshape(-1, MAX_UNITS)
+    N = m.shape[0]
+    dev = m.device
+    ws = _rows_ws.get((N, dev))
+    if ws is None:
+        ws = _rows_ws[(N, dev)] = torch.empty(int(_lib.load().dc_target_rows_workspace_bytes(N)), dtype=torch.uint8, device=dev)
+    rows = torch.empty(N, dtype=torch.int32, device=dev)
+    count = torch.empty(1, dtype=torch.int32, device=dev)
+    flags = torch.empty(N, dtype=torch.uint8, device=dev)
+    with PROFILE.span("target_rows", 2, 2 * N * MAX_UNITS + 2 * N + 4 * N):
+        _lib.check(_lib.load().dc_target_rows(m.data_ptr(), a.data_ptr(), N, rows.data_ptr(), count.data_ptr(), flags.data_ptr(),
+                                              ws.data_ptr(), _lib.stream_ptr()), "dc_target_rows")
+    return rows, count, flags
+
+
+def _gemm_rows(a, b, rows, count, n_host, bias=None, gather=False, out=None, out_rows=None):
+    """Rows i < count of ``a' b^T (+ bias)``, a' row i = ``a[rows[i]]`` when ``gather`` else ``a[i]``, into ``out[i]`` and / or
+    ``out_rows[rows[i]]`` (``dc_gemm_tf32x3_rows``).  ``n_host``: the count when known, for the profile's bytes only."""
+    M = rows.numel()
+    K, N = a.shape[1], b.shape[0]
+    ld = (out if out is not None else out_rows).stride(0)
+    n = M if n_host is None else n_host
+    with PROFILE.span("gemm_tf32x3", 1, 4 * (n * K + N * K + n * N * ((out is not None) + (out_rows is not None)))):
+        _lib.check(_lib.load().dc_gemm_tf32x3_rows(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), _lib.ptr(bias), _lib.ptr(out),
+                                                   _lib.ptr(out_rows), ld, M, count.data_ptr(), rows.data_ptr(), 1 if gather else 0,
+                                                   N, K, 0, _lib.stream_ptr()), "dc_gemm_tf32x3_rows")
+
+
+def _zero_inactive(flags, dst, n_host):
+    """Zero rows of ``dst`` at the tokens whose flag is 0 (``dc_rows_zero_inactive``)."""
+    N, width = dst.shape
+    n = 0 if n_host is None else N - n_host
+    with PROFILE.span("rows_zero", 1, N + 4 * n * width):
+        _lib.check(_lib.load().dc_rows_zero_inactive(flags.data_ptr(), N, dst.data_ptr(), dst.stride(0), width, _lib.stream_ptr()),
+                   "dc_rows_zero_inactive")
+
+
+class TargetUnitRows(torch.autograd.Function):
+    """The attention layer and the target-unit head (``TargetUnit``) on the active tokens only: ``rows[:count]`` and the
+    per-token ``flags`` from ``target_rows``, all on the device, so that the training step stays one graph whatever the count.
+    Logits of the active rows are those of ``affine_unit_attention`` + ``TargetUnit`` bit for bit; the other rows are zero,
+    which the loss never reads.  No row is copied: the GEMMs read y through the row list and write their dense outputs at
+    rows[i] themselves; dense outputs get their inactive rows zeroed, which writes nothing when every token is active.
+      forward:  att_c = y[rows] W_att^T + b_att (compact, and dense ``att`` for ``UnitEncoder.backward``), q_c = att_c bm,
+                logits[rows] from q_c;
+      backward: s_c, d_att_c = s_c bm^T, dy[rows] = d_att_c W_att, dW_att = d_att_c^T y[rows], and (dl, att, s_c, att_c) for
+                the encoder's backward (the head's share of dW_g = att_c^T s_c)."""
+
+    @staticmethod
+    def forward(ctx, y, w_att, b_att, link, rows, count, flags):
+        _need_cuda(y, rows, count)
+        units, w_b, b_b = link["units"], link["w_b"], link["b_b"]
+        H = y.shape[-1]
+        lead = y.shape[:-1]
+        N = y.numel() // H
+        dev = y.device
+        n_act = int(count.item()) if PROFILE.enabled else None     # exact bytes for the profile only: a host sync
+        link["n_active"] = n_act
+        y2 = _f32c(y.detach()).reshape(N, H)
+        w_att, b_att = _f32c(w_att.detach()), _f32c(b_att.detach())
+        att_c = torch.empty((N, C), dtype=torch.float32, device=dev)
+        att = torch.empty((N, C), dtype=torch.float32, device=dev)
+        _gemm_rows(y2, w_att, rows, count, n_act, bias=b_att, gather=True, out=att_c, out_rows=att)
+        _zero_inactive(flags, att, n_act)
+        bm = _head_matrix(link)
+        q_c = torch.empty((N, QW), dtype=torch.float32, device=dev)
+        _gemm_rows(att_c, bm.t().contiguous(), rows, count, n_act, out=q_c)
+        logits = torch.empty((N, MAX_UNITS), dtype=torch.float32, device=dev)
+        _zero_inactive(flags, logits, n_act)
+        nb = N if n_act is None else n_act
+        with PROFILE.span("target_unit_fwd", 1, 4 * nb * (MAX_UNITS * 12 + QW + MAX_UNITS)):
+            _lib.check(_lib.load().dc_target_unit_q_fwd_rows(q_c.data_ptr(), QW, _ptr6(units), w_b.data_ptr(), b_b.data_ptr(),
+                                                             logits.data_ptr(), N, rows.data_ptr(), count.data_ptr(),
+                                                             _lib.stream_ptr()), "dc_target_unit_q_fwd_rows")
+        ctx.save_for_backward(y2, att_c, att, w_att, bm, w_b, b_b, rows, count, flags, *units)
+        ctx.link = link
+        ctx.n_act = n_act
+        ctx.y_shape = y.shape
+        return logits.view(*lead, MAX_UNITS)
+
+    @staticmethod
+    def backward(ctx, dlogits):
+        y2, att_c, att, w_att, bm, w_b, b_b, rows, count, flags = ctx.saved_tensors[:10]
+        units = ctx.saved_tensors[10:]
+        N, H = y2.shape
+        n_act = ctx.n_act
+        nb = N if n_act is None else n_act
+        dev = y2.device
+        dl = _f32c(dlogits).reshape(N, MAX_UNITS)
+        s_c = torch.empty((N, QW), dtype=torch.float32, device=dev)
+        with PROFILE.span("target_unit_bwd", 1, 4 * nb * (MAX_UNITS * 12 + MAX_UNITS + QW)):
+            _lib.check(_lib.load().dc_target_unit_q_bwd_rows(dl.data_ptr(), _ptr6(units), w_b.data_ptr(), b_b.data_ptr(),
+                                                             s_c.data_ptr(), QW, N, rows.data_ptr(), count.data_ptr(),
+                                                             _lib.stream_ptr()), "dc_target_unit_q_bwd_rows")
+        d_att_c = torch.empty((N, C), dtype=torch.float32, device=dev)
+        _gemm_rows(s_c, bm, rows, count, n_act, out=d_att_c)                       # [N, 128] = s_c bm^T, rows < count
+        dy = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dy = torch.empty((N, H), dtype=torch.float32, device=dev)
+            _gemm_rows(d_att_c, w_att.t().contiguous(), rows, count, n_act, out_rows=dy)
+            _zero_inactive(flags, dy, n_act)
+            dy = dy.view(ctx.y_shape)
+        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            dw, db = gemm_wgrad_tf32x3(d_att_c, y2, want_bias=True, t_dev=count, t_host=n_act, x_rows=rows)
+        ctx.link["pending"] = (dl, att, s_c, att_c, count)                       # consumed by UnitEncoder.backward
+        return dy, dw, db, None, None, None, None
 
 
 def unit_encoder(env, w_e, b_e, w_b, b_b, units, weights, biases, wait=None):
@@ -263,4 +380,10 @@ def target_unit(att, link):
     return TargetUnit.apply(att, link)
 
 
-__all__ = ["unit_encoder", "target_unit", "gemm_wgrad_supported"]
+def target_unit_rows(y, w_att, b_att, link, rows, count, flags):
+    """Target-unit logits ``[..., 40]`` from the core output ``y`` through the attention layer, on the tokens
+    ``rows[:count]`` of ``target_rows`` only (``TargetUnitRows``); zero rows elsewhere."""
+    return TargetUnitRows.apply(y, w_att, b_att, link, rows, count, flags)
+
+
+__all__ = ["unit_encoder", "target_unit", "target_unit_rows", "target_rows", "gemm_wgrad_supported"]

@@ -1000,12 +1000,15 @@ def gemm_wgrad_supported(T, No, Ni):
     return T > 0 and No % 32 == 0 and Ni % 32 == 0
 
 
-def gemm_wgrad_tf32x3(dy, x, want_bias=True, dw_out=None, db_out=None, accumulate=False):
+def gemm_wgrad_tf32x3(dy, x, want_bias=True, dw_out=None, db_out=None, accumulate=False, t_dev=None, t_host=None, x_rows=None):
     """``dW[No,Ni] = dy[T,No]^T @ x[T,Ni]`` and ``db[No] = dy.sum(0)`` on wgmma (3xTF32, split-K, deterministic).
 
-    ``dy`` / ``x`` are 2-D fp32 CUDA tensors with contiguous rows (column-slice views allowed)."""
+    ``dy`` / ``x`` are 2-D fp32 CUDA tensors with contiguous rows (column-slice views allowed).  ``t_dev`` / ``t_host``:
+    only the rows ``t < min(T, t_dev)`` (an int32 CUDA tensor of one element) are summed; ``t_host``: that count when the
+    caller knows it, for the profile's byte count only.  ``x_rows`` (int32, with ``t_dev``): row t of the product is row
+    ``x_rows[t]`` of ``x``."""
     _need_cuda(dy, x)
-    assert dy.dim() == 2 and x.dim() == 2 and dy.shape[0] == x.shape[0]
+    assert dy.dim() == 2 and x.dim() == 2 and (x_rows is not None or dy.shape[0] == x.shape[0])
     if dy.stride(1) != 1:
         dy = dy.contiguous()
     if x.stride(1) != 1:
@@ -1023,11 +1026,19 @@ def gemm_wgrad_tf32x3(dy, x, want_bias=True, dw_out=None, db_out=None, accumulat
     if ws is None:
         ws = torch.empty(int(lib.dc_gemm_wgrad_workspace_bytes(No, Ni)), dtype=torch.uint8, device=dev)
         _wgrad_ws[key] = ws
-    with PROFILE.span("gemm_wgrad", 2, 4 * (T * No + T * Ni + No * Ni)):
-        _lib.check(lib.dc_gemm_wgrad_tf32x3(dy.data_ptr(), dy.stride(0), x.data_ptr(), x.stride(0), T, No, Ni,
-                                            dw_out.data_ptr(), dw_out.stride(0), _lib.ptr(db_out) if want_bias else None,
-                                            1 if accumulate else 0, ws.data_ptr(), _lib.stream_ptr()),
-                   "dc_gemm_wgrad_tf32x3")
+    Tb = T if t_host is None else t_host
+    with PROFILE.span("gemm_wgrad", 2, 4 * (Tb * No + Tb * Ni + No * Ni)):
+        if t_dev is None:
+            _lib.check(lib.dc_gemm_wgrad_tf32x3(dy.data_ptr(), dy.stride(0), x.data_ptr(), x.stride(0), T, No, Ni,
+                                                dw_out.data_ptr(), dw_out.stride(0), _lib.ptr(db_out) if want_bias else None,
+                                                1 if accumulate else 0, ws.data_ptr(), _lib.stream_ptr()),
+                       "dc_gemm_wgrad_tf32x3")
+        else:
+            _lib.check(lib.dc_gemm_wgrad_tf32x3_rows(dy.data_ptr(), dy.stride(0), x.data_ptr(), x.stride(0), _lib.ptr(x_rows), T,
+                                                     t_dev.data_ptr(),
+                                                     No, Ni, dw_out.data_ptr(), dw_out.stride(0),
+                                                     _lib.ptr(db_out) if want_bias else None, 1 if accumulate else 0,
+                                                     ws.data_ptr(), _lib.stream_ptr()), "dc_gemm_wgrad_tf32x3_rows")
     return dw_out, (db_out if want_bias else None)
 
 

@@ -207,6 +207,10 @@ class Sequence:
         return self.old_logp
 
 
+# Token count of a training batch from which the target-unit head runs on its active tokens only (Policy._head_outputs with
+# `active`).  Smaller batches (C1: 64 tokens) are bound by kernel launches, and the row list adds five of them.
+TARGET_ROWS_MIN_TOKENS = 4096
+
 class ExperienceBatch:
     """A training batch stacked time-major ``[S, B, ...]`` -- the layout the kernels consume.
 
@@ -1872,7 +1876,14 @@ class DotaOptimizer:
         hidden = (batch.h0, batch.c0) if self.policy_base.cell == "lstm" else batch.h0
         batch.wait(batch.observations['env'], batch.h0, batch.c0, batch.reset_slot, batch.reset_h, batch.reset_c)
         # :619 on the module itself: the data-parallel wrapper's hook-driven reduction stays idle, the step reduces below
-        packed, target_unit = self.policy_base._train_forward(batch.observations, hidden, wait=batch.wait, reset=batch.reset())
+        # the attention layer and the target-unit head run only on the tokens whose target-unit row the loss reads (their
+        # mask / action uploads are waited for right before the head), unless the batch is so small that the step is bound by
+        # launches, which the row list adds
+        active = None
+        if batch.seq_len * batch.batch_size >= TARGET_ROWS_MIN_TOKENS:
+            active = (batch.masks['target_unit'], batch.actions['target_unit'])
+        packed, target_unit = self.policy_base._train_forward(batch.observations, hidden, wait=batch.wait, reset=batch.reset(),
+                                                              active=active)
         valid = batch.valid if self.mask_padding else None
         old_log_probs = batch.old_log_probs if self.kl_control else None
         batch.wait(batch.old_logp, batch.advantages, batch.returns, batch.old_values, valid, old_log_probs,

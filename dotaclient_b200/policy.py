@@ -138,14 +138,18 @@ class Policy(nn.Module):
         so ``DotaOptimizer.train`` pays no transposes.  ``observations`` is a dict keyed by INPUT_KEYS."""
         return self._run(tuple(observations[k] for k in self.INPUT_KEYS), hidden, time_major=True)
 
-    def _train_forward(self, observations, hidden, wait=None, reset=None):
+    def _train_forward(self, observations, hidden, wait=None, reset=None, active=None):
         """The training step's forward on time-major inputs -> (the packed ``[S, B, ops.PACK_WIDTH]`` output of the four
         small heads and the value head, target-unit logits ``[S, B, 40]``): the tensors the fused PPO loss reads and
         backward starts from.  ``wait`` (see ``encoder_ops.unit_encoder``) lets the observations arrive while it runs.
-        ``reset``: recurrent-state resets inside the sequences (``_recur``)."""
+        ``reset``: recurrent-state resets inside the sequences (``_recur``).  ``active``: see ``_head_outputs``; ``wait``
+        is also called for its two tensors, right before the head."""
         x, unit_embedding = self._encode(observations['env'], [observations[k] for k in self.INPUT_KEYS[1:]], wait=wait)
         y, _ = self._recur(x.contiguous(), hidden, reset)
-        return self._head_outputs(y, unit_embedding)
+        if active is not None and wait is not None:
+            for t in active:
+                wait(t)
+        return self._head_outputs(y, unit_embedding, active)
 
     # ------------------------------------------------------------------ implementation
     def _encode(self, env, groups, wait=None):
@@ -184,11 +188,16 @@ class Policy(nn.Module):
         h_n = ops.stack_layers(hs)
         return y, ((h_n, ops.stack_layers(cs)) if lstm else h_n)
 
-    def _head_outputs(self, y, unit_embedding):
+    def _head_outputs(self, y, unit_embedding, active=None):
         """The attention projection and ONE packed ``[*, 128]`` tensor-core GEMM for the four small heads + the value head
         (25 + value_heads real rows, zero padding; their logits are column ranges of its output, ``ops.pack_cols``), then the target-unit
-        dot products -> (packed output, target-unit logits)."""
-        attention = ops.linear(y, self.affine_unit_attention.weight, self.affine_unit_attention.bias)
+        dot products -> (packed output, target-unit logits).
+
+        ``active``: None, or the ``(mask, action)`` target-unit rows ``[..., 40]`` of the PPO loss.  The attention layer and the
+        target-unit head then run only on the tokens where either row has an entry set (``encoder_ops.target_unit_rows``):
+        the same logits there, zeros on the other rows, which the loss never reads."""
+        att_w, att_b = self.affine_unit_attention.weight, self.affine_unit_attention.bias
+        attention = ops.linear(y, att_w, att_b) if active is None else None
         H = self.hidden_size
         pad = y.new_zeros(ops.PACK_WIDTH - 25 - self.value_heads, H)
         w_pack = torch.cat([self.affine_head_enum.weight, self.affine_move_x.weight, self.affine_move_y.weight,
@@ -196,7 +205,9 @@ class Policy(nn.Module):
         b_pack = torch.cat([self.affine_head_enum.bias, self.affine_move_x.bias, self.affine_move_y.bias,
                             self.affine_head_ability.bias, self.affine_value.bias, pad[:, 0]], dim=0)
         packed = ops.linear(y, w_pack, b_pack)
-        return packed, encoder_ops.target_unit(attention, unit_embedding)
+        if active is None:
+            return packed, encoder_ops.target_unit(attention, unit_embedding)
+        return packed, encoder_ops.target_unit_rows(y, att_w, att_b, unit_embedding, *encoder_ops.target_rows(*active))
 
     def _heads(self, y, unit_embedding):
         """Action heads + value (``policy.py:144-155``): column ranges of the packed output, and the target-unit logits."""

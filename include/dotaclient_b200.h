@@ -286,6 +286,15 @@ int dc_gemm_tf32x3(const float *A, int lda, const float *B, int ldb, const float
 size_t dc_gemm_wgrad_workspace_bytes(int No, int Ni);
 int dc_gemm_wgrad_tf32x3(const float *dY, int ldy, const float *X, int ldx, int64_t T, int No, int Ni,
                          float *dW, int ldw, float *db, int accumulate, void *workspace, dc_stream_t stream);
+/* The same two GEMMs on a row list held on the device (dc_target_rows; a graph replays them whatever the count):
+ * dc_gemm_tf32x3_rows computes rows i < min(M, *count) of a A'^T B (+ bias) with A' row i = A row (gather_a ? rows[i] : i); row i goes
+ * to C row i (C may be NULL) and to C_rows row rows[i] (C_rows may be NULL; not both NULL), both with pitch ldc.  No other row is
+ * read or written; M sizes the grid.  dc_gemm_wgrad_tf32x3_rows contracts tokens t < min(T, *t_dev) with X row x_rows[t] (x_rows NULL:
+ * row t), split over every split-K range; at count 0, dW = 0, db = 0 (accumulate = 0).  The same requirements and workspace as above. */
+int dc_gemm_tf32x3_rows(const float *A, int lda, const float *B, int ldb, const float *bias, float *C, float *C_rows, int ldc,
+                        int64_t M, const int32_t *count, const int32_t *rows, int gather_a, int N, int K, int relu, dc_stream_t stream);
+int dc_gemm_wgrad_tf32x3_rows(const float *dY, int ldy, const float *X, int ldx, const int32_t *x_rows, int64_t T, const int32_t *t_dev,
+                              int No, int Ni, float *dW, int ldw, float *db, int accumulate, void *workspace, dc_stream_t stream);
 
 /* ---- unit encoder / target-unit head ------------------------------------------------------------
  * (policy.py:99-136,144-153).  The basic layer basic[R,128] = relu(units[R,12] W_b^T + b_b) (policy.py:100,105,...) is
@@ -325,6 +334,22 @@ int dc_target_unit_q_fwd(const float *q, int ld_q, const float *const units[6], 
                          int64_t N, dc_stream_t stream);
 int dc_target_unit_q_bwd(const float *dlogits, const float *const units[6], const float *w_b, const float *b_b, float *s, int ld_s,
                          int64_t N, dc_stream_t stream);
+/* The head on the tokens of a row list (dc_target_rows): item i < min(N, *count) is token rows[i].  _fwd reads row i of q
+ * and writes logits row rows[i] (no other row is written); _bwd reads dlogits row rows[i] and writes row i of s (no row
+ * past the count is written).  N: the capacity of rows, q and s. */
+int dc_target_unit_q_fwd_rows(const float *q, int ld_q, const float *const units[6], const float *w_b, const float *b_b, float *logits,
+                              int64_t N, const int32_t *rows, const int32_t *count, dc_stream_t stream);
+int dc_target_unit_q_bwd_rows(const float *dlogits, const float *const units[6], const float *w_b, const float *b_b, float *s, int ld_s,
+                              int64_t N, const int32_t *rows, const int32_t *count, dc_stream_t stream);
+/* The tokens that use the target-unit head: rows[0 .. *count) = the n < N, ascending, whose target_unit mask row or action
+ * row (mask, action: [N, 40] bool bytes, 8-byte aligned) has a byte set -- the rows the PPO loss reads -- and flags[n] = 1 for
+ * them, 0 for the others ([N] bytes, 4-byte aligned).  All outputs stay on the device.  Workspace:
+ * dc_target_rows_workspace_bytes(N) bytes, 4-byte aligned.
+ * dc_rows_zero_inactive: dst[n, :width] = 0 for every n < N with flags[n] == 0 (width % 4 == 0, 16-byte aligned rows). */
+size_t dc_target_rows_workspace_bytes(int64_t N);
+int dc_target_rows(const uint8_t *mask, const uint8_t *action, int64_t N, int32_t *rows, int32_t *count, uint8_t *flags,
+                   void *workspace, dc_stream_t stream);
+int dc_rows_zero_inactive(const uint8_t *flags, int64_t N, float *dst, int ld, int width, dc_stream_t stream);
 /* Backward of one unit-embedding layer WITHOUT the dense [N*units, 128] gradient of the embedding (what the reference's autograd
  * materialises behind policy.py:100-127,152-153).  R[(n,u), c] = (argmax[n*128 + c] == u) ? d_xmax[n*ld_dx + c] (+ d_xmax2[..]) : 0 is
  * the max-pool routing, generated inside the kernels.
