@@ -78,6 +78,9 @@ SIGNATURES = {
                                          _vp, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "dc_ppo_loss_fwd_bwd_kl": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
                                       _vp, _i32, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dc_ppo_loss_fwd_bwd_teacher": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp,
+                                           _vp, _i64, _vp, _vp, _i32, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp,
+                                           _vp, _vp, _vp, _vp]),
     "dc_selected_logp_rows": (_i32, [_ptr5, _ptr5, _ptr5, _i64, _vp, _vp, _vp]),
     "dc_value_norm_stats": (_i32, [_vp, _vp, _i64, _vp, _vp]),
     "dc_value_denorm": (_i32, [_vp, _i64, _i64, _f64, _f64, _vp, _vp]),
@@ -107,6 +110,8 @@ STAT_APPROX_KL, STAT_CLIP_FRACTION, STAT_EXPLAINED_VAR = 0, 6, 12
 STAT_JOINT_APPROX_KL, STAT_JOINT_CLIP_FRACTION = 13, 14     # dc_ppo_loss_fwd_bwd_joint only
 STAT_KL, STAT_KL_PENALTY = 16, 22                           # dc_ppo_loss_fwd_bwd_kl only (17..21: KL per head)
 KL_ROW_FLOATS = 65          # entries of one token's masked log-prob row over the five heads (DC_KL_ROW_FLOATS)
+# dc_ppo_loss_fwd_bwd_teacher's teacher_stats: 0 the KL to the teacher, 1..5 per head, 6 lambda * KL (DC_TEACHER_STATS_SLOTS)
+TEACHER_STATS_SLOTS = 7
 FINISH_KL_METRICS = 6       # metrics of dc_grad_finish_kl: the four of dc_grad_finish, the all-ranks KL, the skip flag
 VTRACE_STATS_SLOTS = 8      # per-segment fp64 sums written by dc_vtrace_scan (DC_VTRACE_STATS_SLOTS)
 VALUE_HEADS_MAX = 10        # value heads of dc_gae_scan_heads / dc_value_heads_loss (DC_VALUE_HEADS_MAX)

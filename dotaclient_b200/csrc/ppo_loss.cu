@@ -54,6 +54,21 @@
 // the five heads.  Staging takes the CTA from 53.5 KB to 86 KB of dynamic shared memory: ptxas gives the loss kernel
 // about 160 registers, which already limits it to 3 CTAs per SM, and 86 KB + the static rows still allow 2.  The extra
 // HBM traffic is 260 B / token read (686 + 260 = 946 B / token for the loss pass).
+//
+// Kickstarting (`dc_ppo_loss_fwd_bwd_teacher`, kTeacher, with or without kKl): the loss also reads a frozen teacher's
+// rows ([N, 65], as dc_selected_logp_rows writes them) and adds lambda * KL_T with
+//   KL_T = (1 / T_a) sum_t sum_{h in S_t} sum_{a legal} p_T(a) (log p_T(a) - log p(a)),
+// and (lambda / T_a)(p(a) - p_T(a)) to the legal entries of every dlogits row in S_t, in the same loop as the KL term:
+// one more exp per legal entry.  lambda = *teacher_coef (a device double next to the hparams block, not a slot of it);
+// lambda = 0 skips both terms, so the results are those of the instantiation without kTeacher, bit for bit.  The teacher
+// rows are staged like the old rows, one more [128, 65] tile (33,280 bytes) after them.  ptxas (sm_90a, no spills, with
+// __launch_bounds__(128, 2)): teacher alone 214 registers per-head / 196 joint, 86.8 KB dynamic + 8.9 / 9.9 KB static
+// shared memory, 2 CTAs per SM like the KL tile; teacher and KL 194 / 197 registers, 120 KB dynamic + 11.5 / 12.5 KB
+// static, 1 CTA per SM.  Both are staged, for the reason the old rows are: read per thread from global, a warp's rows sit
+// 260 bytes apart and are touched in five head slices.  Measured on an H100 80GB HBM3 (700 W) at 131,072 tokens with a
+// valid mask (tools/teacher_bench.py, medians of 200 calls): _masked 206 us, _kl 320 us, teacher alone 295 us, teacher and
+// KL 441 us, so the 1-CTA combined instantiation costs 121 us more than _kl, about 1 % of the C2 step.  Algorithmic bytes:
+// + 260 / token read for the teacher's rows (946 B / token with one row set, 1,206 B with both, + valid and old value).
 #include "dc_common.cuh"
 
 namespace {
@@ -83,6 +98,9 @@ __host__ __device__ constexpr int row_col(int h) { return byte_off(h) / kTile; }
 static_assert(kRowFloats == byte_off(kHeads) / kTile, "a log-prob row holds every head's entries");
 static_assert(kSmemBytes % 16 == 0, "the old-row tile is 16-byte aligned");
 constexpr size_t kSmemBytesKl = kSmemBytes + (size_t)kTile * kRowFloats * 4;
+// the teacher's rows: one more tile of the same layout, after the old rows when both are staged (teacher alone: kSmemBytesKl)
+constexpr size_t kSmemBytesKlTeacher = kSmemBytesKl + (size_t)kTile * kRowFloats * 4;
+static_assert(DC_TEACHER_STATS_SLOTS >= 2 + DC_NUM_HEADS, "teacher_stats too small");
 
 struct HeadPtrs {
     const float *logits[kHeads];
@@ -102,6 +120,8 @@ constexpr int kTokD = 2 * kHeads, kTokR = kTokD + 1, kTokRows = kTokR + 1;   // 
 constexpr int kTokJoint = kTokRows, kJointStats = 2;
 // KL control only: one staging row and sum per head of the exact KL of that head's row (after the joint rows, if any)
 constexpr int kKlStats = kHeads;
+// teacher only: the same per head for the KL to the teacher's row (after the KL control rows, if any)
+constexpr int kTeachStats = kHeads;
 static_assert(2 * kHeads + 3 < DC_PPO_STATS_SLOTS, "stats output too small");
 static_assert(DC_STAT_KL_PENALTY < DC_PPO_STATS_SLOTS, "stats output too small");
 
@@ -120,6 +140,7 @@ struct Workspace {
     double st_joint[kJointStats];    // joint ratio: sums over the T_a tokens of its k3 KL and of its clip flag
     unsigned long long first_rev;    // N - (index of the first token that counts); 0 when no token counts
     double st_kl[kKlStats];          // KL control: per head, the sum over its action rows of the exact KL of the row
+    double st_teach[kTeachStats];    // teacher: per head, the sum over its action rows of the KL to the teacher's row
 };
 static_assert(sizeof(Workspace) <= DC_PPO_WORKSPACE_BYTES, "workspace too small");
 
@@ -272,11 +293,13 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
 // kKl, loss: `orow` is the token's prep-time log-prob row of head H; the exact KL of the row goes to *kl_row_out (when
 // the head has an action row here) and, with kl_scale = beta / T_a > 0, its gradient joins the dlogits row.
 // kKl, select (logp_out given): the full masked log-prob row overwrites the logits row in the tile, 0 at illegal entries.
-template <int H, bool kGrad, bool kKl = false>
+// kTeach, loss: `trow` is the teacher's log-prob row of head H, used as kKl uses `orow` (t_scale = lambda / T_a).
+template <int H, bool kGrad, bool kKl = false, bool kTeach = false>
 __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, const uint8_t *arow, float old_lp,
                                            float adv_n, int n_h, float e_clip, float entropy_coef, float &pol_acc,
                                            float &ent_acc, float *kl_out, float *clip_out, float *logp_out,
-                                           const float *orow = nullptr, float kl_scale = 0.f, float *kl_row_out = nullptr) {
+                                           const float *orow = nullptr, float kl_scale = 0.f, float *kl_row_out = nullptr,
+                                           const float *trow = nullptr, float t_scale = 0.f, float *t_row_out = nullptr) {
     constexpr int N = head_n(H);
     float l[N], e[N];
     int mask_any = 0, a_idx = -1;
@@ -348,7 +371,7 @@ __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, con
     }
     if (kGrad) {
         const float ce = entropy_coef > 0.f ? entropy_coef / (float)n_h : 0.f;   // optimizer.py:652-656
-        float kl_row = 0.f;
+        float kl_row = 0.f, t_row = 0.f;
 #pragma unroll
         for (int j = 0; j < N; ++j) {
             float g = -g_lp * p[j];                       // through logsumexp (masked entries only: p = 0 outside)
@@ -359,9 +382,15 @@ __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, con
                 kl_row += po * (lo - lp[j]);
                 if (kl_scale > 0.f) g += kl_scale * (p[j] - po);
             }
+            if (kTeach && a_idx >= 0 && mrow[j]) {       // KL(p_T || p), and lambda / T_a (p - p_T)
+                const float lt = trow[j], pt = __expf(lt);
+                t_row += pt * (lt - lp[j]);
+                if (t_scale > 0.f) g += t_scale * (p[j] - pt);
+            }
             lrow[j] = g;
         }
         if (kKl && a_idx >= 0) *kl_row_out = kl_row;
+        if (kTeach && a_idx >= 0) *t_row_out = t_row;
     }
 }
 
@@ -406,11 +435,12 @@ __device__ __forceinline__ void joint_head_fwd(const float *lrow, const uint8_t 
 
 // Joint ratio, sweep 2 over head H: the dlogits row, with g_lp = d loss / d lp[a] of the joint surrogate (the same for
 // every head with an action row) and the head's entropy term, recomputed from the tile exactly as sweep 1 computed it.
-// kKl: the head's exact KL and its gradient, as in head_token.
-template <int H, bool kKl = false>
+// kKl / kTeach: the head's exact KL to the old / teacher row and its gradient, as in head_token.
+template <int H, bool kKl = false, bool kTeach = false>
 __device__ __forceinline__ void joint_head_bwd(float *lrow, const uint8_t *mrow, const uint8_t *arow, int n_h, float g_lp,
                                                float entropy_coef, const float *orow = nullptr, float kl_scale = 0.f,
-                                               float *kl_row_out = nullptr) {
+                                               float *kl_row_out = nullptr, const float *trow = nullptr,
+                                               float t_scale = 0.f, float *t_row_out = nullptr) {
     constexpr int N = head_n(H);
     float l[N], e[N];
     int mask_any = 0, a_idx = -1;
@@ -441,7 +471,7 @@ __device__ __forceinline__ void joint_head_bwd(float *lrow, const uint8_t *mrow,
     }
     if (a_idx < 0) g_lp = 0.f;
     const float ce = entropy_coef > 0.f ? entropy_coef / (float)n_h : 0.f;
-    float kl_row = 0.f;
+    float kl_row = 0.f, t_row = 0.f;
 #pragma unroll
     for (int j = 0; j < N; ++j) {
         float g = -g_lp * p[j];
@@ -452,15 +482,24 @@ __device__ __forceinline__ void joint_head_bwd(float *lrow, const uint8_t *mrow,
             kl_row += po * (lo - lp[j]);
             if (kl_scale > 0.f) g += kl_scale * (p[j] - po);
         }
+        if (kTeach && a_idx >= 0 && mrow[j]) {
+            const float lt = trow[j], pt = __expf(lt);
+            t_row += pt * (lt - lp[j]);
+            if (t_scale > 0.f) g += t_scale * (p[j] - pt);
+        }
         lrow[j] = g;
     }
     if (kKl && a_idx >= 0) *kl_row_out = kl_row;
+    if (kTeach && a_idx >= 0) *t_row_out = t_row;
 }
 
 // kSelectOnly && kKl: the selected log-probs and, written through hp.dlogits (column ranges of the [N, 65] rows), every
-// head's masked log-prob row.  !kSelectOnly && kKl: the loss with the KL penalty (old_rows, kl_out).
-template <bool kSelectOnly, bool kJoint, bool kKl = false>
-__global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const float *__restrict__ old_logp,
+// head's masked log-prob row.  !kSelectOnly && kKl: the loss with the KL penalty (old_rows, kl_out).  kTeacher (a loss):
+// the teacher term (teacher_rows, *teacher_coef, teacher_stats), with or without kKl.
+// kTeacher asks for 2 CTAs per SM, which lets ptxas use more than the ~168 registers it picks otherwise and spill nothing;
+// the other instantiations keep ptxas's default (minBlocks 0 is "not given"), so their code is unchanged.
+template <bool kSelectOnly, bool kJoint, bool kKl = false, bool kTeacher = false>
+__global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadPtrs hp, const float *__restrict__ old_logp,
                                                           const float *__restrict__ adv_raw,
                                                           const float *__restrict__ ret,
                                                           const float *__restrict__ value, int64_t N, float e_clip,
@@ -471,19 +510,26 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
                                                           float *__restrict__ dvalue, float *__restrict__ out,
                                                           float *__restrict__ stats, Workspace *ws,
                                                           float *__restrict__ logp_out,
-                                                          const float *__restrict__ old_rows, float *__restrict__ kl_out) {
+                                                          const float *__restrict__ old_rows, float *__restrict__ kl_out,
+                                                          const float *__restrict__ teacher_rows,
+                                                          const double *__restrict__ teacher_coef,
+                                                          float *__restrict__ teacher_stats) {
     static_assert(!(kSelectOnly && kJoint), "the joint ratio is a loss");
+    static_assert(!(kSelectOnly && kTeacher), "the teacher term is a loss");
     constexpr bool kKlLoss = kKl && !kSelectOnly;
     constexpr int kTokKl = kTokRows + (kJoint ? kJointStats : 0);
-    constexpr int kRows = kTokKl + (kKlLoss ? kKlStats : 0);
+    constexpr int kTokTeach = kTokKl + (kKlLoss ? kKlStats : 0);
+    constexpr int kRows = kTokTeach + (kTeacher ? kTeachStats : 0);
     constexpr int kSumKl = kStats + (kJoint ? kJointStats : 0);
-    constexpr int kSums = kSumKl + (kKlLoss ? kKlStats : 0);
+    constexpr int kSumTeach = kSumKl + (kKlLoss ? kKlStats : 0);
+    constexpr int kSums = kSumTeach + (kTeacher ? kTeachStats : 0);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *s_logits = reinterpret_cast<float *>(smem_raw);
     float *s_old = s_logits + kLogitFloats;
     uint8_t *s_mask = reinterpret_cast<uint8_t *>(s_old + kOldFloats);
     uint8_t *s_act = s_mask + kByteTile;
     float *s_orows = reinterpret_cast<float *>(smem_raw + kSmemBytes);    // kKlLoss: [kTile][65] prep-time log-prob rows
+    float *s_trows = s_orows + (kKlLoss ? kTile * kRowFloats : 0);          // kTeacher: [kTile][65] teacher log-prob rows
     __shared__ float s_red[kTile / 32];
     // per-token diagnostics (rows kStKl.., kStClip.., then ret - v and ret, then the joint ratio's), staged here rather
     // than held in registers across the head loop, and their block sums
@@ -504,6 +550,7 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         vn_sigma = hparams[DC_HP_VALUE_NORM_STD];
         if (kKlLoss) kl_coef = (float)hparams[DC_HP_KL_COEF];
     }
+    const float t_coef = kTeacher ? (float)*teacher_coef : 0.f;     // teacher: lambda
     const bool vnorm = vn_sigma > 0.0;
     const bool clip_value = old_value != nullptr && value_clip > 0.f;
 
@@ -522,6 +569,9 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
     }
     if (kKlLoss)      // contiguous rows: a byte copy of the tile with 16-byte loads
         stage_bytes(reinterpret_cast<uint8_t *>(s_orows), reinterpret_cast<const uint8_t *>(old_rows + t0 * kRowFloats),
+                    count * kRowFloats * 4);
+    if (kTeacher)
+        stage_bytes(reinterpret_cast<uint8_t *>(s_trows), reinterpret_cast<const uint8_t *>(teacher_rows + t0 * kRowFloats),
                     count * kRowFloats * 4);
     __syncthreads();
 
@@ -554,6 +604,13 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
     // KL control: this token's entry in the staging row of head 0's KL (head H's is H rows further).  Without kKl those
     // rows do not exist and nothing is staged there.
     float *const s_kl_tok = kKlLoss ? &s_tok[0][0] + kTokKl * kTile + t : nullptr;
+    // teacher: lambda / T_a (0 when lambda = 0), and this token's entry in the staging row of head 0's teacher KL
+    float t_scale = 0.f;
+    if (kTeacher && t_coef > 0.f) {
+        const unsigned long long n_a = ws->n_joint;
+        if (n_a) t_scale = t_coef / (float)n_a;
+    }
+    float *const s_t_tok = kTeacher ? &s_tok[0][0] + kTokTeach * kTile + t : nullptr;
     if (live) {
         float lp_sel[kHeads];
         if constexpr (kJoint) {
@@ -583,20 +640,26 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             // sweep 2 re-reads the tile: without this the compiler keeps every head's sweep-1 values live instead
             asm volatile("" ::: "memory");
 #define DC_JHEAD(H)                                                                                                 \
-            joint_head_bwd<H, kKlLoss>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H), \
+            joint_head_bwd<H, kKlLoss, kTeacher>(s_logits + logit_off(H) + t * head_pitch(H),                          \
+                                       s_mask + byte_off(H) + t * head_n(H),                                            \
                                        s_act + byte_off(H) + t * head_n(H), use ? cnt[H] : 0, g_lp, entropy_coef,       \
                                        s_orows + t * kRowFloats + row_col(H), kl_scale,                                 \
-                                       kKlLoss ? s_kl_tok + (H) * kTile : nullptr);
+                                       kKlLoss ? s_kl_tok + (H) * kTile : nullptr,                                      \
+                                       s_trows + t * kRowFloats + row_col(H), t_scale,                                  \
+                                       kTeacher ? s_t_tok + (H) * kTile : nullptr);
             DC_JHEAD(0) DC_JHEAD(1) DC_JHEAD(2) DC_JHEAD(3) DC_JHEAD(4)
 #undef DC_JHEAD
         } else {
 #define DC_HEAD(H)                                                                                              \
-        head_token<H, true, kKl>(s_logits + logit_off(H) + t * head_pitch(H), s_mask + byte_off(H) + t * head_n(H), \
+        head_token<H, true, kKl, kTeacher>(s_logits + logit_off(H) + t * head_pitch(H),                          \
+                                 s_mask + byte_off(H) + t * head_n(H),                                               \
                                  s_act + byte_off(H) + t * head_n(H), kSelectOnly ? 0.f : s_old[t * 5 + H], adv_n,   \
                                  use ? cnt[H] : 0, e_clip, entropy_coef, pol[H], ent[H], &s_tok[kStKl + H][t],       \
                                  &s_tok[kStClip + H][t], kSelectOnly ? &lp_sel[H] : nullptr,                         \
                                  s_orows + t * kRowFloats + row_col(H), kl_scale,                                    \
-                                 kKlLoss ? s_kl_tok + (H) * kTile : nullptr);
+                                 kKlLoss ? s_kl_tok + (H) * kTile : nullptr,                                         \
+                                 s_trows + t * kRowFloats + row_col(H), t_scale,                                     \
+                                 kTeacher ? s_t_tok + (H) * kTile : nullptr);
         DC_HEAD(0) DC_HEAD(1) DC_HEAD(2) DC_HEAD(3) DC_HEAD(4)
 #undef DC_HEAD
         }
@@ -656,11 +719,12 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
         }
         sums[2 * kHeads] = block_sum(vl, s_red);
         // the diagnostics (s_tok is complete: block_sum synchronised the block): one warp per sum, in float64.  KL control
-        // needs its sums for kl_out whether or not the diagnostics are asked for.
-        if (stats || kKlLoss) {
+        // and the teacher need their sums for kl_out / teacher_stats whether or not the diagnostics are asked for.
+        if (stats || kKlLoss || kTeacher) {
             const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
             for (int i = warp; i < kSums; i += kTile / 32) {
-                const int row = (kKlLoss && i >= kSumKl) ? kTokKl + (i - kSumKl)
+                const int row = (kTeacher && i >= kSumTeach) ? kTokTeach + (i - kSumTeach)
+                              : (kKlLoss && i >= kSumKl) ? kTokKl + (i - kSumKl)
                               : (kJoint && i >= kStats) ? kTokJoint + (i - kStats) : (i < kStD ? i : (i < kStR ? kTokD : kTokR));
                 const bool square = i == kStD2 || i == kStR2;
                 double s = 0.0;
@@ -691,6 +755,10 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
             if constexpr (kKlLoss) {
                 for (int i = 0; i < kKlStats; ++i)
                     if (s_st[kSumKl + i] != 0.0) atomicAdd(&ws->st_kl[i], s_st[kSumKl + i]);
+            }
+            if constexpr (kTeacher) {
+                for (int i = 0; i < kTeachStats; ++i)
+                    if (s_st[kSumTeach + i] != 0.0) atomicAdd(&ws->st_teach[i], s_st[kSumTeach + i]);
             }
             __threadfence();
             s_last = atomicAdd(&ws->ticket_loss, 1u) == gridDim.x - 1;
@@ -774,6 +842,22 @@ __global__ void __launch_bounds__(kTile) ppo_loss_kernel(HeadPtrs hp, const floa
                     kl_out[1] = (float)n_a;
                 }
             }
+            if constexpr (kTeacher) {
+                // KL_T = (1 / T_a) sum_t sum_{h in S_t} KL(p_T || p) of the row (0 when T_a = 0); lambda KL_T joins the loss
+                // only when lambda > 0, so lambda = 0 leaves out[0] as the instantiation without the teacher computes it
+                const unsigned long long n_a = w->n_joint;
+                double t_sum = 0.0;
+                for (int h = 0; h < kHeads; ++h) t_sum += w->st_teach[h];
+                const float kl_t = n_a ? (float)(t_sum / (double)n_a) : 0.f;
+                const float term = t_coef > 0.f ? t_coef * kl_t : 0.f;
+                if (t_coef > 0.f) out[0] = out[0] + term;
+                teacher_stats[0] = kl_t;
+                for (int h = 0; h < kHeads; ++h) {           // over the head's action rows; 0 for a head without any
+                    const int n = w->cnt[h];
+                    teacher_stats[1 + h] = n ? (float)(w->st_teach[h] / (double)n) : 0.f;
+                }
+                teacher_stats[1 + kHeads] = term;
+            }
         }
     }
 }
@@ -793,7 +877,9 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
                     const float *old_value, const uint8_t *valid, int64_t N, float e_clip, float entropy_coef, float vf_coef,
                     const double *hparams, float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
                     float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions, void *workspace,
-                    dc_stream_t stream, bool joint = false, const float *old_rows = nullptr, float *kl_out = nullptr) {
+                    dc_stream_t stream, bool joint = false, const float *old_rows = nullptr, float *kl_out = nullptr,
+                    const float *teacher_rows = nullptr, const double *teacher_coef = nullptr,
+                    float *teacher_stats = nullptr) {
     DC_REQUIRE(N > 0, DC_EINVAL, "dc_ppo_loss_fwd_bwd: N=%lld", (long long)N);
     DC_REQUIRE(check_heads(logits, masks, actions) && old_logp && adv_raw && ret && value && dvalue && out &&
                    n_actions && workspace && ld_logits && ld_dlogits, DC_EINVAL, "dc_ppo_loss_fwd_bwd: null pointer");
@@ -810,13 +896,27 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
     Workspace *ws = reinterpret_cast<Workspace *>(workspace);
     DC_CUDA(cudaMemsetAsync(ws, 0, sizeof(Workspace), st));
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
+    if (teacher_rows) {         // the teacher term, with or without KL control, either ratio mode; T_a as below
+        ppo_stats_kernel<true><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
+        DC_LAUNCH_OK();
+        auto kern = old_rows ? (joint ? ppo_loss_kernel<false, true, true, true> : ppo_loss_kernel<false, false, true, true>)
+                             : (joint ? ppo_loss_kernel<false, true, false, true> : ppo_loss_kernel<false, false, false, true>);
+        const size_t smem = old_rows ? kSmemBytesKlTeacher : kSmemBytesKl;
+        DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<blocks, kTile, smem, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip, entropy_coef, vf_coef, old_value,
+                                          valid, hparams, dvalue, out, stats, ws, nullptr, old_rows, kl_out, teacher_rows,
+                                          teacher_coef, teacher_stats);
+        DC_LAUNCH_OK();
+        return DC_OK;
+    }
     if (old_rows) {             // KL control, either ratio mode; the statistics pass counts T_a
         ppo_stats_kernel<true><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
         DC_LAUNCH_OK();
         auto kern = joint ? ppo_loss_kernel<false, true, true> : ppo_loss_kernel<false, false, true>;
         DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytesKl));
         kern<<<blocks, kTile, kSmemBytesKl, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip, entropy_coef, vf_coef, old_value,
-                                                  valid, hparams, dvalue, out, stats, ws, nullptr, old_rows, kl_out);
+                                                  valid, hparams, dvalue, out, stats, ws, nullptr, old_rows, kl_out,
+                                                  nullptr, nullptr, nullptr);
         DC_LAUNCH_OK();
         return DC_OK;
     }
@@ -827,7 +927,8 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
                                      (int)kSmemBytes));
         ppo_loss_kernel<false, true><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
                                                                         entropy_coef, vf_coef, old_value, valid, hparams,
-                                                                        dvalue, out, stats, ws, nullptr, nullptr, nullptr);
+                                                                        dvalue, out, stats, ws, nullptr, nullptr, nullptr, nullptr,
+                                                                        nullptr, nullptr);
         DC_LAUNCH_OK();
         return DC_OK;
     }
@@ -838,7 +939,8 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
     DC_CUDA(cudaFuncSetAttribute(ppo_loss_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     ppo_loss_kernel<false, false><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
                                                                      entropy_coef, vf_coef, old_value, valid, hparams,
-                                                                     dvalue, out, stats, ws, nullptr, nullptr, nullptr);
+                                                                     dvalue, out, stats, ws, nullptr, nullptr, nullptr, nullptr,
+                                                                        nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -926,7 +1028,7 @@ extern "C" int dc_selected_logp(const float *const logits[DC_NUM_HEADS], const u
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
     ppo_loss_kernel<true, false><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
         hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-        nullptr, logp_out, nullptr, nullptr);
+        nullptr, logp_out, nullptr, nullptr, nullptr, nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -949,7 +1051,7 @@ extern "C" int dc_selected_logp_rows(const float *const logits[DC_NUM_HEADS], co
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
     ppo_loss_kernel<true, false, true><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
         hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-        nullptr, logp_out, nullptr, nullptr);
+        nullptr, logp_out, nullptr, nullptr, nullptr, nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -967,4 +1069,23 @@ extern "C" int dc_ppo_loss_fwd_bwd_kl(const float *const logits[DC_NUM_HEADS], c
     return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, old_value, valid,
                            N, 0.f, 0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions,
                            workspace, stream, joint != 0, old_log_probs, kl_out);
+}
+
+extern "C" int dc_ppo_loss_fwd_bwd_teacher(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                                           const uint8_t *const masks[DC_NUM_HEADS],
+                                           const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
+                                           const float *old_log_probs, const float *teacher_log_probs,
+                                           const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                                           const float *old_value, const uint8_t *valid, int64_t N, const double *hparams,
+                                           const double *teacher_coef, int joint, float *const dlogits[DC_NUM_HEADS],
+                                           const int64_t ld_dlogits[DC_NUM_HEADS], float *dvalue, int64_t ld_dvalue,
+                                           float *out, float *stats, float *kl_out, float *teacher_stats,
+                                           int32_t *n_actions, void *workspace, dc_stream_t stream) {
+    DC_REQUIRE(hparams, DC_EINVAL, "dc_ppo_loss_fwd_bwd_teacher: null hyper-parameter block");
+    DC_REQUIRE(teacher_log_probs && teacher_coef && teacher_stats, DC_EINVAL,
+               "dc_ppo_loss_fwd_bwd_teacher: null teacher_log_probs, teacher_coef or teacher_stats");
+    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, old_value, valid,
+                           N, 0.f, 0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions,
+                           workspace, stream, joint != 0, old_log_probs, kl_out, teacher_log_probs, teacher_coef,
+                           teacher_stats);
 }

@@ -772,17 +772,45 @@ def _kl_args(old_log_probs, kl_out, N):
     return old_log_probs
 
 
+def _teacher_args(teacher_log_probs, teacher_coef, teacher_stats, N, dev):
+    """Checks the extra operands of ``dc_ppo_loss_fwd_bwd_teacher``: ``teacher_log_probs`` [..., 65] fp32 (contiguous),
+    ``teacher_coef`` (1 fp64 on the device) and ``teacher_stats`` (``_lib.TEACHER_STATS_SLOTS`` fp32, allocated when
+    None)."""
+    if teacher_coef is None:
+        raise ValueError("the teacher term needs its coefficient on the device (teacher_coef=)")
+    _need_cuda(teacher_log_probs, teacher_coef, teacher_stats)
+    teacher_log_probs = _f32c(teacher_log_probs)
+    assert teacher_log_probs.numel() == N * _lib.KL_ROW_FLOATS, "teacher_log_probs has %d elements for %d tokens" % (
+        teacher_log_probs.numel(), N)
+    assert teacher_coef.dtype == torch.float64 and teacher_coef.numel() == 1
+    if teacher_stats is None:
+        teacher_stats = torch.empty(_lib.TEACHER_STATS_SLOTS, dtype=torch.float32, device=dev)
+    assert teacher_stats.dtype == torch.float32 and teacher_stats.numel() == _lib.TEACHER_STATS_SLOTS \
+        and teacher_stats.is_contiguous()
+    return teacher_log_probs, teacher_stats
+
+
 def _ppo_dev_call(lib, lptr, ld_l, masks, actions, old_logp, adv_raw, ret, value_ptr, ld_v, old_value, valid, N, hparams,
-                  dptr, ld_d, dvalue_ptr, ld_dv, out, stats, n_actions, ws, joint=False, old_log_probs=None, kl_out=None):
+                  dptr, ld_d, dvalue_ptr, ld_dv, out, stats, n_actions, ws, joint=False, old_log_probs=None, kl_out=None,
+                  teacher_log_probs=None, teacher_coef=None, teacher_stats=None):
     """``dc_ppo_loss_fwd_bwd_dev``, or ``dc_ppo_loss_fwd_bwd_masked`` when a valid mask is given, or
     ``dc_ppo_loss_fwd_bwd_joint`` (valid or not) when ``joint``; ``dc_ppo_loss_fwd_bwd_kl`` (either ratio mode) when
-    ``old_log_probs`` is given."""
+    ``old_log_probs`` is given; ``dc_ppo_loss_fwd_bwd_teacher`` (either ratio mode, old rows or not) when
+    ``teacher_log_probs`` is given."""
     head = (lptr, ld_l, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(),
             value_ptr, ld_v, _lib.ptr(old_value))
     tail = (N, hparams.data_ptr(), dptr, ld_d, dvalue_ptr, ld_dv, out.data_ptr(), stats.data_ptr(), n_actions.data_ptr(),
             ws.data_ptr(), _lib.stream_ptr())
-    with PROFILE.span("ppo_loss", 2, _lib.KL_ROW_FLOATS * 4 * N if old_log_probs is not None else 0):
-        if old_log_probs is not None:
+    rows = (old_log_probs is not None) + (teacher_log_probs is not None)
+    with PROFILE.span("ppo_loss", 2, _lib.KL_ROW_FLOATS * 4 * N * rows):
+        if teacher_log_probs is not None:
+            _lib.check(lib.dc_ppo_loss_fwd_bwd_teacher(
+                lptr, ld_l, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(), _lib.ptr(old_log_probs),
+                teacher_log_probs.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(), value_ptr, ld_v, _lib.ptr(old_value),
+                _lib.ptr(valid), N, hparams.data_ptr(), teacher_coef.data_ptr(), 1 if joint else 0, dptr, ld_d, dvalue_ptr,
+                ld_dv, out.data_ptr(), stats.data_ptr(), _lib.ptr(kl_out), teacher_stats.data_ptr(), n_actions.data_ptr(),
+                ws.data_ptr(), _lib.stream_ptr()), "dc_ppo_loss_fwd_bwd_teacher")
+        elif old_log_probs is not None:
             _lib.check(lib.dc_ppo_loss_fwd_bwd_kl(
                 lptr, ld_l, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(), old_log_probs.data_ptr(),
                 adv_raw.data_ptr(), ret.data_ptr(), value_ptr, ld_v, _lib.ptr(old_value), _lib.ptr(valid), N,
@@ -797,7 +825,8 @@ def _ppo_dev_call(lib, lptr, ld_l, masks, actions, old_logp, adv_raw, ret, value
 
 
 def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_clip, entropy_coef, vf_coef, hparams=None,
-                     old_value=None, stats=None, valid=None, joint=False, old_log_probs=None, kl_out=None):
+                     old_value=None, stats=None, valid=None, joint=False, old_log_probs=None, kl_out=None,
+                     teacher_log_probs=None, teacher_coef=None, teacher_stats=None):
     """Fused PPO loss + gradients (``optimizer.py:587-589,621-665`` and their backward).
 
     logits/masks/actions: sequences of 5 tensors [..., n_h] in HEAD_KEYS order (any leading dims,
@@ -816,6 +845,10 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     ``old_log_probs`` [..., 65] (needs ``hparams``): the prep-time masked log-prob rows (``selected_logp_rows``); the loss
     then adds the KL penalty ``hparams[HP_KL_COEF] * KL`` (``dc_ppo_loss_fwd_bwd_kl``, either ratio mode), ``stats``
     also holds the exact KL (``_lib.STAT_KL``...), and ``kl_out`` (2 fp32, or None) receives (sum_t KL_t, T_a).
+    ``teacher_log_probs`` [..., 65] (needs ``hparams`` and ``teacher_coef``, 1 fp64 on the device): a teacher policy's
+    masked log-prob rows; the loss then adds ``teacher_coef * KL(teacher || policy)`` (``dc_ppo_loss_fwd_bwd_teacher``,
+    either ratio mode, with or without ``old_log_probs``), and ``teacher_stats`` (``_lib.TEACHER_STATS_SLOTS`` fp32,
+    allocated when None) receives the KL, the KL per head and the term; the result then gains it as a sixth element.
     """
     logits = [_f32c(l.detach()) for l in logits]
     _need_cuda(*logits)
@@ -834,17 +867,21 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     n_actions = torch.empty(5, dtype=torch.int32, device=dev)
     ws = torch.empty(_lib.PPO_WORKSPACE_BYTES, dtype=torch.uint8, device=dev)
     lib = _lib.load()
-    if hparams is not None or valid is not None or joint or old_log_probs is not None:
-        if old_log_probs is not None and hparams is None:
-            raise ValueError("the KL penalty needs the device hyper-parameter block (hparams=)")
+    teacher = teacher_log_probs is not None
+    if hparams is not None or valid is not None or joint or old_log_probs is not None or teacher:
+        if (old_log_probs is not None or teacher) and hparams is None:
+            raise ValueError("the KL penalty and the teacher term need the device hyper-parameter block (hparams=)")
         old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid, joint)
         if old_log_probs is not None:
             old_log_probs = _kl_args(old_log_probs, kl_out, N)
+        if teacher:
+            teacher_log_probs, teacher_stats = _teacher_args(teacher_log_probs, teacher_coef, teacher_stats, N, dev)
         ld = (ctypes.c_int64 * 5)(*HEAD_SIZES)
         _ppo_dev_call(lib, _lib.ptr5(logits), ld, masks, actions, old_logp, adv_raw, ret, value.data_ptr(), 1, old_value,
                       valid, N, hparams, _lib.ptr5(dlogits), ld, dvalue.data_ptr(), 1, out, stats, n_actions, ws, joint,
-                      old_log_probs, kl_out)
-        return out, n_actions, dlogits, dvalue, stats
+                      old_log_probs, kl_out, teacher_log_probs, teacher_coef, teacher_stats)
+        res = (out, n_actions, dlogits, dvalue, stats)
+        return res + (teacher_stats,) if teacher else res
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd(_lib.ptr5(logits), _lib.ptr5(masks), _lib.ptr5(actions),
                                            old_logp.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(), value.data_ptr(),
@@ -1116,14 +1153,16 @@ def value_heads_loss(packed, d_packed, ret, hparams, out, head_stats, old_value=
 
 
 def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e_clip, entropy_coef, vf_coef, hparams=None,
-                    old_value=None, stats=None, valid=None, joint=False, old_log_probs=None, kl_out=None):
+                    old_value=None, stats=None, valid=None, joint=False, old_log_probs=None, kl_out=None,
+                    teacher_log_probs=None, teacher_coef=None, teacher_stats=None):
     """Fused PPO loss where the four small heads and the value head are column ranges of ONE packed ``[N,128]``
     tensor-core GEMM output (``PACK_COLS``) and the target-unit logits are a separate ``[N,40]`` tensor.
 
     Returns (out[16], n_actions[5], d_packed [N,128], d_logits_tu [N,40]): the gradients go straight back into the two
     producers, so no slice/cat kernels run and the five tiny K=131072 weight-gradient GEMMs become one wgmma wgrad.
-    ``hparams`` / ``old_value`` / ``stats`` / ``valid`` / ``joint`` / ``old_log_probs`` / ``kl_out``: as
-    ``ppo_loss_fwd_bwd`` (the fifth element of the result is then ``stats``).
+    ``hparams`` / ``old_value`` / ``stats`` / ``valid`` / ``joint`` / ``old_log_probs`` / ``kl_out`` /
+    ``teacher_log_probs`` / ``teacher_coef`` / ``teacher_stats``: as ``ppo_loss_fwd_bwd`` (the fifth element of the result
+    is then ``stats``, and with a teacher the sixth ``teacher_stats``).
     """
     _need_cuda(packed, logits_tu)
     p2 = _f32c(packed.detach()).reshape(-1, PACK_WIDTH)
@@ -1146,16 +1185,20 @@ def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e
     dptr = _lib._ptr5(col(d_packed, "enum"), col(d_packed, "x"), col(d_packed, "y"), d_tu.data_ptr(), col(d_packed, "ability"))
     ld = (c.c_int64 * 5)(PACK_WIDTH, PACK_WIDTH, PACK_WIDTH, 40, PACK_WIDTH)
     lib = _lib.load()
-    if hparams is not None or valid is not None or joint or old_log_probs is not None:
-        if old_log_probs is not None and hparams is None:
-            raise ValueError("the KL penalty needs the device hyper-parameter block (hparams=)")
+    teacher = teacher_log_probs is not None
+    if hparams is not None or valid is not None or joint or old_log_probs is not None or teacher:
+        if (old_log_probs is not None or teacher) and hparams is None:
+            raise ValueError("the KL penalty and the teacher term need the device hyper-parameter block (hparams=)")
         old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid, joint)
         if old_log_probs is not None:
             old_log_probs = _kl_args(old_log_probs, kl_out, N)
+        if teacher:
+            teacher_log_probs, teacher_stats = _teacher_args(teacher_log_probs, teacher_coef, teacher_stats, N, dev)
         _ppo_dev_call(lib, lptr, ld, masks, actions, old_logp, adv_raw, ret, col(p2, "value"), PACK_WIDTH, old_value, valid,
                       N, hparams, dptr, ld, col(d_packed, "value"), PACK_WIDTH, out, stats, n_actions, ws, joint,
-                      old_log_probs, kl_out)
-        return out, n_actions, d_packed.view_as(packed), d_tu.view_as(logits_tu), stats
+                      old_log_probs, kl_out, teacher_log_probs, teacher_coef, teacher_stats)
+        res = (out, n_actions, d_packed.view_as(packed), d_tu.view_as(logits_tu), stats)
+        return res + (teacher_stats,) if teacher else res
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd_strided(lptr, ld, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(),
                                                    adv_raw.data_ptr(), ret.data_ptr(), col(p2, "value"), PACK_WIDTH, N,

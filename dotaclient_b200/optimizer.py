@@ -170,7 +170,7 @@ class Sequence:
     """
 
     def __init__(self, game_id, weight_version, team_id, observations, actions, masks, values, rewards, hidden,
-                 log_probs_sel=None, old_logp=None, valid=None, old_log_probs=None):
+                 log_probs_sel=None, old_logp=None, valid=None, old_log_probs=None, teacher_log_probs=None):
         self.game_id = game_id
         self.weight_version = weight_version
         self.team_id = team_id
@@ -184,6 +184,7 @@ class Sequence:
         self.old_logp = old_logp
         self.valid = valid          # [S] bool, real steps vs zero padding (set by prep under DotaOptimizer(mask_padding=True))
         self.old_log_probs = old_log_probs  # [S, 65] prep-time masked log-prob rows (set by prep under KL control)
+        self.teacher_log_probs = teacher_log_probs  # [S, 65] the teacher's masked log-prob rows (set by prep with a teacher)
         self.advantages = None
         self.returns = None
 
@@ -227,18 +228,21 @@ class ExperienceBatch:
     ``old_log_probs [S, B, 65]`` (optional) are every head's full masked log-prob rows at experience prep, in head order
     with 0 at illegal entries, which the KL penalty and the KL early stop (``DotaOptimizer(kl_coef=..., kl_stop=...)``)
     compare against; absent from ``tensors()`` when None.
+    ``teacher_log_probs [S, B, 65]`` (optional) are the same rows of a frozen teacher policy, which the kickstarting term
+    (``DotaOptimizer(teacher_model=...)``) compares against; absent from ``tensors()`` when None.
     With ``K > 1`` value heads (``DotaOptimizer(value_heads=...)``) ``returns`` and ``old_values`` are ``[S, B, K]``, one
     column per head; ``advantages`` stay ``[S, B]``, the heads' sum.
     """
     FIELDS = ("advantages", "returns", "old_logp", "h0", "c0", "old_values", "valid", "reset_slot", "reset_h", "reset_c",
-              "old_log_probs")
+              "old_log_probs", "teacher_log_probs")
 
     def __init__(self, observations, masks, actions, old_logp, advantages, returns, h0, c0=None, old_values=None,
-                 valid=None, reset_slot=None, reset_h=None, reset_c=None, old_log_probs=None):
+                 valid=None, reset_slot=None, reset_h=None, reset_c=None, old_log_probs=None, teacher_log_probs=None):
         self.observations, self.masks, self.actions = observations, masks, actions
         self.old_logp, self.advantages, self.returns, self.h0, self.c0 = old_logp, advantages, returns, h0, c0
         self.old_values = old_values
         self.old_log_probs = old_log_probs
+        self.teacher_log_probs = teacher_log_probs
         self.valid = valid
         self.reset_slot, self.reset_h, self.reset_c = reset_slot, reset_h, reset_c
         self._ready = {}        # data_ptr -> event of an upload still to be waited for (``to`` from pinned memory)
@@ -255,11 +259,12 @@ class ExperienceBatch:
 
     def graph_key(self):
         """The shape a captured step graph is specialised to (old_values, valid, the reset tables of a packed batch, the
-        old log-prob rows: more static inputs)."""
+        old and the teacher's log-prob rows: more static inputs)."""
         key = (self.seq_len, self.batch_size, self.old_values is not None)
         key = key if self.valid is None else key + ('valid',)
         key = key if self.reset_slot is None else key + (('reset', self.reset_h.shape[0]),)
-        return key if self.old_log_probs is None else key + ('old_log_probs',)
+        key = key if self.old_log_probs is None else key + ('old_log_probs',)
+        return key if self.teacher_log_probs is None else key + ('teacher_log_probs',)
 
     def reset(self):
         """The ``reset`` operand of ``Policy._recur`` (None for a batch that is not packed)."""
@@ -370,8 +375,12 @@ class ExperienceBatch:
         old_log_probs = None
         if all(getattr(e, 'old_log_probs', None) is not None for e in experiences):
             old_log_probs = stack([torch.as_tensor(e.old_log_probs).float() for e in experiences])
+        teacher_log_probs = None
+        if all(getattr(e, 'teacher_log_probs', None) is not None for e in experiences):
+            teacher_log_probs = stack([torch.as_tensor(e.teacher_log_probs).float() for e in experiences])
         return ExperienceBatch(obs, masks, actions, old, adv, ret, h0.detach(), None if c0 is None else c0.detach(),
-                               old_values=old_values, valid=valid, old_log_probs=old_log_probs)
+                               old_values=old_values, valid=valid, old_log_probs=old_log_probs,
+                               teacher_log_probs=teacher_log_probs)
 
 
 class AdvantageRefresh(typing.NamedTuple):
@@ -462,14 +471,15 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
                        vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False, pack_sequences=False,
                        policy_ratio='per_head', value_norm=False, value_norm_decay=0.99, kl_coef=0.0, kl_target=None,
                        kl_stop=None, recompute_advantages=False, recompute_states=False, value_heads=None,
-                       value_gammas=None):
+                       value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
     vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool,
     pack_sequences a bool that is True only with mask_padding, policy_ratio one of ``POLICY_RATIOS``, value_norm a bool
     and 0 <= value_norm_decay < 1, finite kl_coef >= 0, kl_target None or finite > 0 (and then kl_coef > 0), kl_stop None
     or finite > 0, recompute_advantages and recompute_states bools, value_heads / value_gammas as ``value_head_groups``
-    checks them (value heads refuse V-trace and value_norm).  NaN fails every check."""
+    checks them (value heads refuse V-trace and value_norm), finite teacher_coef >= 0 and teacher_anneal_iterations None
+    or an int >= 1, both left at their defaults without a teacher_model.  NaN fails every check."""
     if not isinstance(recompute_states, bool):
         raise ValueError("recompute_states=%r: must be True or False" % (recompute_states,))
     if not isinstance(recompute_advantages, bool):
@@ -520,6 +530,17 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
                              "doubles or halves it" % (kl_target,))
     if kl_stop is not None and not 0.0 < number('kl_stop', kl_stop) < math.inf:
         raise ValueError("kl_stop=%r: the KL limit must be finite and > 0 (or None: no early stop)" % (kl_stop,))
+    if not 0.0 <= number('teacher_coef', teacher_coef) < math.inf:
+        raise ValueError("teacher_coef=%r: the teacher coefficient must be finite and >= 0" % (teacher_coef,))
+    if teacher_anneal_iterations is not None and (isinstance(teacher_anneal_iterations, bool)
+                                                  or not isinstance(teacher_anneal_iterations, numbers.Integral)
+                                                  or teacher_anneal_iterations < 1):
+        raise ValueError("teacher_anneal_iterations=%r: the anneal length must be an int >= 1 (or None: a fixed "
+                         "teacher_coef)" % (teacher_anneal_iterations,))
+    if teacher_model is None and float(teacher_coef) != 1.0:
+        raise ValueError("teacher_coef=%r needs teacher_model" % (teacher_coef,))
+    if teacher_model is None and teacher_anneal_iterations is not None:
+        raise ValueError("teacher_anneal_iterations=%r needs teacher_model" % (teacher_anneal_iterations,))
     value_head_groups(value_heads, value_gammas, gamma)
     if value_heads is not None and advantage_estimator == 'vtrace':
         raise ValueError("value_heads with advantage_estimator='vtrace': per-head V-trace targets are not defined yet "
@@ -644,6 +665,28 @@ def value_norm_update(state, n, s1, s2, decay):
     m, q, w = state
     d = float(decay)
     return d * m + (1.0 - d) * (s1 / n), d * q + (1.0 - d) * (s2 / n), d * w + (1.0 - d)
+
+
+def load_teacher(path):
+    """The frozen teacher ``Policy`` of ``DotaOptimizer(teacher_model=path)``, on the CPU without gradients: the ``state_dict``
+    file at ``path`` loaded strictly into the architecture it describes (``Policy.from_state_dict``), whose width must be
+    one the kernels run, a multiple of 32.  Raises ``ValueError`` for a missing file or a file that is not a ``Policy``
+    state_dict."""
+    if not os.path.isfile(path):
+        raise ValueError("teacher_model=%r: no such file" % (path,))
+    state = torch.load(path, map_location='cpu')
+    if not isinstance(state, dict):
+        raise ValueError("teacher_model=%r does not hold a state_dict" % (path,))
+    try:
+        teacher = Policy.from_state_dict(state)
+    except ValueError as e:
+        raise ValueError("teacher_model=%r: %s" % (path, e)) from None
+    if teacher.hidden_size % 32:
+        raise ValueError("teacher_model=%r has hidden_size %d; the kernels run multiples of 32"
+                         % (path, teacher.hidden_size))
+    teacher.requires_grad_(False)
+    logger.info('Teacher %s: %s-%d, %d layer(s)', path, teacher.cell, teacher.hidden_size, teacher.num_layers)
+    return teacher
 
 
 def check_minibatch_count(num_minibatches, min_seq_per_epoch):
@@ -991,6 +1034,8 @@ class DotaOptimizer:
     KL_COEF_FILENAME_FMT = "kl_coef_%09d.state"     # the adaptive KL coefficient of the same iteration (kl_target)
     # the K-row value head and its groups of the same iteration (value_heads); the published model holds it folded
     VALUE_HEADS_FILENAME_FMT = "value_heads_%09d.state"
+    # the iterations trained with the teacher, its coefficient and its path, of the same iteration (teacher_model)
+    TEACHER_FILENAME_FMT = "teacher_%09d.state"
     VALUE_NORM_MIN_STD = 1e-2       # floor of the value statistics' sigma: bounds the value head's rescale factor
     BUCKET_NAME = 'dotaservice'
     MODEL_HISTOGRAM_FREQ = 128
@@ -1013,7 +1058,8 @@ class DotaOptimizer:
                  max_grad_norm=0.5, value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0,
                  num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False,
                  value_norm_decay=0.99, kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False,
-                 recompute_states=False, value_heads=None, value_gammas=None):
+                 recompute_states=False, value_heads=None, value_gammas=None, teacher_model=None, teacher_coef=1.0,
+                 teacher_anneal_iterations=None):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
@@ -1023,7 +1069,8 @@ class DotaOptimizer:
                            mask_padding=mask_padding, pack_sequences=pack_sequences, policy_ratio=policy_ratio,
                            value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
                            kl_stop=kl_stop, recompute_advantages=recompute_advantages, recompute_states=recompute_states,
-                           value_heads=value_heads, value_gammas=value_gammas)
+                           value_heads=value_heads, value_gammas=value_gammas, teacher_model=teacher_model,
+                           teacher_coef=teacher_coef, teacher_anneal_iterations=teacher_anneal_iterations)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
         # value heads: one critic column per reward group, each with its own discount.  Prep scans every group
         # (gae_scan_heads), the policy trains on the summed advantage, the value loss is dc_value_heads_loss's and the
@@ -1098,6 +1145,19 @@ class DotaOptimizer:
             torch.manual_seed(7)                    # forked so that constructing an optimizer leaves the caller's RNG alone
             self.policy_base = Policy(hidden_size=hidden_size, cell=cell, num_layers=num_layers,
                                       value_heads=self.n_value_heads)
+        # Kickstarting: the loss adds teacher_coef * KL(pi_teacher || pi) over the legal actions of every sampled head, with
+        # the teacher's rows computed once at prep.  teacher_coef can be scheduled between steps like kl_coef; with
+        # teacher_anneal_iterations, run_iteration sets it to teacher_coef * max(0, 1 - n / N) (n: teacher_iterations) and
+        # retires the teacher at 0.  The teacher is frozen: outside the flat parameters, Adam, the all-reduce and checkpoints
+        self.teacher_model = teacher_model
+        self.teacher_coef = float(teacher_coef)
+        self._teacher_coef0 = self.teacher_coef
+        self.teacher_anneal_iterations = teacher_anneal_iterations
+        self.teacher_iterations = 0
+        self.teacher = None
+        if teacher_model is not None:
+            with torch.random.fork_rng(devices=[]):   # building it draws from the RNG: leave the caller's alone, as above
+                self.teacher = load_teacher(teacher_model).to(self.device)
 
         if self.checkpoint:
             logger.info('Checkpointing to: {}'.format(self.log_dir))
@@ -1126,6 +1186,8 @@ class DotaOptimizer:
                                                       self.VALUE_NORM_FILENAME_FMT % (self.iteration_start - 1)))
                 self._restore_kl_coef(os.path.join(os.path.dirname(pretrained_model),
                                                    self.KL_COEF_FILENAME_FMT % (self.iteration_start - 1)))
+                self._restore_teacher(os.path.join(os.path.dirname(pretrained_model),
+                                                   self.TEACHER_FILENAME_FMT % (self.iteration_start - 1)))
 
         self.policy_base.to(self.device)
         self.flat = FlatParameterSpace(self.policy_base, self.device, kl_tail=self.kl_control)
@@ -1154,20 +1216,30 @@ class DotaOptimizer:
         self._n_metrics = _lib.FINISH_KL_METRICS if self.kl_control else 4
         # value heads: their statistics (dc_value_heads_loss) follow the PPO diagnostics, read back by the same copy
         n_vh = 0 if self.value_heads is None else _lib.VALUE_HEADS_STATS_SLOTS
-        self._result_dev = torch.zeros(self._n_metrics + _lib.PPO_STATS_SLOTS + n_vh, dtype=torch.float32,
+        # the teacher's statistics (KL, per head, the loss term) come last, read back by the same copy
+        n_t = 0 if self.teacher_model is None else _lib.TEACHER_STATS_SLOTS
+        self._result_dev = torch.zeros(self._n_metrics + _lib.PPO_STATS_SLOTS + n_vh + n_t, dtype=torch.float32,
                                        device=self.device)
         self._metrics = self._result_dev[:self._n_metrics]
         self._ppo_stats = self._result_dev[self._n_metrics:self._n_metrics + _lib.PPO_STATS_SLOTS]
-        self._value_head_stats = self._result_dev[self._n_metrics + _lib.PPO_STATS_SLOTS:] if n_vh else None
+        o = self._n_metrics + _lib.PPO_STATS_SLOTS
+        self._value_head_stats = self._result_dev[o:o + n_vh] if n_vh else None
+        self._teacher_stats = self._result_dev[o + n_vh:] if n_t else None
         self._finish_ws = torch.zeros(_lib.FINISH_WORKSPACE_BYTES, dtype=torch.uint8, device=self.device)
         # learning_rate, e_clip, entropy_coef, vf_coef, MAX_GRAD_NORM and value_clip are read by the step's kernels from this
         # device block, rewritten from the pinned host copy before every step: a captured graph of the step holds the
         # block's address, not the values, so assignments between steps reach replayed steps too
         # Value heads: a second block, the first with vf_coef = 0 and no value clip, for the PPO loss, whose value term
         # dc_value_heads_loss replaces; both blocks go up in the one copy
+        # Teacher: its coefficient is one more double after the blocks (not a block slot), uploaded by the same copy
         n_blocks = 1 if self.value_heads is None else 2
-        self._hparams_host_all = torch.zeros((n_blocks, _lib.HPARAM_SLOTS), dtype=torch.float64).pin_memory()
-        self._hparams_dev_all = torch.zeros((n_blocks, _lib.HPARAM_SLOTS), dtype=torch.float64, device=self.device)
+        n_hp = n_blocks * _lib.HPARAM_SLOTS + (0 if self.teacher_model is None else 1)
+        self._hparams_host_flat = torch.zeros(n_hp, dtype=torch.float64).pin_memory()
+        self._hparams_dev_flat = torch.zeros(n_hp, dtype=torch.float64, device=self.device)
+        self._hparams_host_all = self._hparams_host_flat[:n_blocks * _lib.HPARAM_SLOTS].view(n_blocks, _lib.HPARAM_SLOTS)
+        self._hparams_dev_all = self._hparams_dev_flat[:n_blocks * _lib.HPARAM_SLOTS].view(n_blocks, _lib.HPARAM_SLOTS)
+        self._teacher_coef_host = self._hparams_host_flat[n_blocks * _lib.HPARAM_SLOTS:]
+        self._teacher_coef_dev = self._hparams_dev_flat[n_blocks * _lib.HPARAM_SLOTS:]
         self._hparams_host, self._hparams_dev = self._hparams_host_all[0], self._hparams_dev_all[0]
         self._hparams_dev_ppo = self._hparams_dev_all[n_blocks - 1]
         self._hparams_uploaded = None       # the values the device block holds
@@ -1222,6 +1294,35 @@ class DotaOptimizer:
             kc = torch.tensor([self.kl_coef], dtype=torch.float64, device=self.device)
             dist.broadcast(kc, 0)
             self.kl_coef = float(kc.item())
+        if self.teacher_model is not None:  # the iterations trained with the teacher and its coefficient
+            tc = torch.tensor([float(self.teacher_iterations), self.teacher_coef], dtype=torch.float64, device=self.device)
+            dist.broadcast(tc, 0)
+            self.teacher_iterations, self.teacher_coef = int(tc[0].item()), float(tc[1].item())
+
+    def _restore_teacher(self, path):
+        """Resume with a teacher: the iterations already trained with it and its coefficient from ``path`` (written by
+        ``upload_model``).  Without the file both start afresh; without a teacher the file is ignored."""
+        if not os.path.isfile(path):
+            return
+        if self.teacher_model is None:
+            logger.warning('Ignoring %s: this run has no teacher_model', path)
+            return
+        st = torch.load(path, map_location='cpu')
+        logger.info('Restoring the teacher schedule from %s (%d iterations, coefficient %r)', path, st['iterations'],
+                    st['teacher_coef'])
+        self.teacher_iterations, self.teacher_coef = int(st['iterations']), float(st['teacher_coef'])
+        if self.teacher_coef == 0.0 and self.teacher_anneal_iterations is not None:
+            self._retire_teacher()
+
+    def _retire_teacher(self):
+        """The anneal reached 0: prep stops running the teacher, batches carry no teacher rows, the step runs without the
+        term, and the teacher's device memory is released."""
+        if self.teacher is not None:
+            logger.info('The teacher coefficient has annealed to 0: retiring the teacher')
+            self.teacher = None
+            gc.collect()
+            if torch.cuda.is_available():
+                torch.cuda.empty_cache()
 
     def _restore_kl_coef(self, path):
         """Resume with ``kl_target``: the adaptive KL coefficient from ``path`` (written by ``upload_model``).  Without the
@@ -1326,6 +1427,11 @@ class DotaOptimizer:
             if self.kl_target is not None:  # the adaptive KL coefficient the next iteration trains with, for resume
                 torch.save({'kl_coef': self.kl_coef}, os.path.join(self.log_dir, self.KL_COEF_FILENAME_FMT % version))
                 side.append(r'kl_coef_\d{9}\.state')
+            if self.teacher_model is not None:  # the teacher schedule the next iteration continues, for resume
+                torch.save({'iterations': self.teacher_iterations, 'teacher_coef': self.teacher_coef,
+                            'teacher_model': str(self.teacher_model)},
+                           os.path.join(self.log_dir, self.TEACHER_FILENAME_FMT % version))
+                side.append(r'teacher_\d{9}\.state')
             for pattern in side:            # resume only ever needs the newest: bound the disk growth
                 stale = sorted(f for f in os.listdir(self.log_dir) if re.fullmatch(pattern, f))[:-self.ADAM_FILES_KEPT]
                 for f in stale:
@@ -1383,6 +1489,10 @@ class DotaOptimizer:
         V(s_L), the critic's value of its extra observation row: ONE more single-step forward of batch R' (the number of
         such rollouts) from each one's state after its last step, state buffer slot L_i.  The extra row enters neither the
         main pass nor the batch.  Without either key in any rollout none of this runs.
+
+        With a teacher (``teacher_model``) and ``teacher_coef > 0``, one more no-grad forward of the teacher over the same
+        observations, from the teacher's zero state (also for a rollout with ``'initial_hidden'``: the actor's state is the
+        student's), gives the teacher's masked log-prob rows ``teacher_log_probs [Lmax, R, 65]``.
 
         With ``value_norm`` the values and bootstraps read from the normalised head are denormalised first, so the scans,
         ``Sequence.values`` and the batch stay in raw units; at the end the value statistics take this batch's targets and
@@ -1486,6 +1596,14 @@ class DotaOptimizer:
             else:
                 old_logp = ops.selected_logp([logits[k] for k in keys], [masks[k] for k in keys],
                                              [actions[k] for k in keys]).view(Lmax, R, 5)        # :387-390
+            teacher_log_probs = None
+            if self.teacher is not None and self.teacher_coef > 0.0:
+                t = self.teacher
+                ht = torch.zeros((t.num_layers, R, t.hidden_size), dtype=torch.float32, device=dev)
+                t_logits = self._rollout_forward(obs, ht, torch.zeros_like(ht) if t.cell == "lstm" else None, pol=t)[2]
+                teacher_log_probs = ops.selected_logp_rows([t_logits[k] for k in keys], [masks[k] for k in keys],
+                                                           [actions[k] for k in keys])[1].view(Lmax, R, _lib.KL_ROW_FLOATS)
+                del t_logits
             # GAE per rollout over ITS padded length: back-to-back segments, rollout-major
             values_lr = values.reshape((Lmax, R) + self._vh_shape) if vn is None else \
                 ops.value_denorm(values, *vn).view(Lmax, R)
@@ -1533,7 +1651,7 @@ class DotaOptimizer:
                 self._update_value_norm(ret_c, real if self.mask_padding else None)
         return dict(obs=obs, masks=masks, actions=actions, rewards_np=rewards_np, old_logp=old_logp, values_lr=values_lr,
                     adv_c=adv_c, ret_c=ret_c, ybufs=ybufs, cbufs=cbufs, Ls=Ls, Lps=Lps, Lmax=Lmax, same=same, valid=valid,
-                    bootstrap=bootstrap, old_log_probs=old_log_probs,
+                    bootstrap=bootstrap, old_log_probs=old_log_probs, teacher_log_probs=teacher_log_probs,
                     refresh=dict(rewards=rew_c, seg_off=seg, boot=boot, behaviour_logp=blp_c, valid_len=valid_len),
                     state_refresh=dict(h0=h0, c0=c0,
                                        obs_next=obs_next if cut else None,
@@ -1541,14 +1659,15 @@ class DotaOptimizer:
                                        cut_rollout=np.array(cut, dtype=np.int64) if cut else None,
                                        boot_slot=boot_slot if cut else None))
 
-    def _rollout_forward(self, obs, h0, c0):
-        """The no-grad rollout-major forward of experience prep and of the state refresh: the encoder over time-major
+    def _rollout_forward(self, obs, h0, c0, pol=None):
+        """The no-grad rollout-major forward of experience prep and of the state refresh (of ``pol``: the student
+        ``policy_base`` by default, or the teacher): the encoder over time-major
         ``[T, R, ...]`` observations (``Policy.INPUT_KEYS``), every recurrent layer from ``h0`` / ``c0 [L, R, H]`` (c0 None
         for the GRU) keeping its state buffers, and the heads.  Returns ``(ybufs, cbufs, logits, values)``: per layer the
         ``[T + 1, R, H]`` state buffers of ``ops.rnn_stack_forward_states`` (slot t: the state entering step t), the head
         logits and the value columns ``[T, R, K]`` of the packed head output (K = the value heads, 1 without them;
         normalised under ``value_norm``)."""
-        pol = self.policy_base
+        pol = self.policy_base if pol is None else pol
         x, unit_embedding = pol._encode(obs['env'], [obs[k] for k in Policy.INPUT_KEYS[1:]])
         layers = [pol.rnn.layer(k) for k in range(pol.num_layers)]
         ybufs, cbufs = ops.rnn_stack_forward_states(x.contiguous(), layers, h0, c0, pol.cell)
@@ -1562,6 +1681,7 @@ class DotaOptimizer:
         S, pol = self.seq_len, self.policy_base
         p = self._prepare_rollouts(datas)
         obs, masks, actions, ybufs, cbufs, Lps = p['obs'], p['masks'], p['actions'], p['ybufs'], p['cbufs'], p['Lps']
+        t_rows = p.get('teacher_log_probs')
         out = []
         for i, d in enumerate(datas):
             base = int(sum(Lps[:i]))
@@ -1582,7 +1702,8 @@ class DotaOptimizer:
                                hidden=hid,
                                old_logp=p['old_logp'][sl, i],
                                valid=None if p['valid'] is None else p['valid'][:, col + j],
-                               old_log_probs=None if p['old_log_probs'] is None else p['old_log_probs'][sl, i])
+                               old_log_probs=None if p['old_log_probs'] is None else p['old_log_probs'][sl, i],
+                               teacher_log_probs=None if t_rows is None else t_rows[sl, i])
                 seq.advantages = p['adv_c'][base + j * S: base + (j + 1) * S]
                 seq.returns = p['ret_c'][base + j * S: base + (j + 1) * S]
                 sequences.append(seq)
@@ -1642,8 +1763,10 @@ class DotaOptimizer:
         c0 = ops.stack_layers([cb[t_idx, r_idx] for cb in p['cbufs']]) if pol.cell == "lstm" else None
         old_values = chunked(p['values_lr']).contiguous()               # the critic at prep time (value clipping)
         old_log_probs = None if p['old_log_probs'] is None else chunked(p['old_log_probs']).contiguous()
+        t_rows = p.get('teacher_log_probs')
+        teacher_log_probs = None if t_rows is None else chunked(t_rows).contiguous()
         return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values, valid=p['valid'],
-                               old_log_probs=old_log_probs)
+                               old_log_probs=old_log_probs, teacher_log_probs=teacher_log_probs)
 
     def _packed_batch(self, p, lay):
         """The packed ``ExperienceBatch`` of ``pack_layout`` from the prepared ``[L_max, R, ...]`` tensors: every field is
@@ -1673,8 +1796,9 @@ class DotaOptimizer:
             return outs
         keys_o, keys_h = list(p['obs']), list(p['masks'])
         kl_rows = [] if p['old_log_probs'] is None else [p['old_log_probs']]
+        t_rows = [] if p.get('teacher_log_probs') is None else [p['teacher_log_probs']]
         tm = [p['obs'][k] for k in keys_o] + [p['masks'][k] for k in keys_h] + [p['actions'][k] for k in keys_h] + \
-            [p['old_logp'], p['values_lr']] + kl_rows
+            [p['old_logp'], p['values_lr']] + kl_rows + t_rows
         g = gather(tm, idx_tm, Lmax * R)
         obs = dict(zip(keys_o, g[:len(keys_o)]))
         masks = dict(zip(keys_h, g[len(keys_o):len(keys_o) + len(keys_h)]))
@@ -1682,6 +1806,7 @@ class DotaOptimizer:
         n_tm = len(keys_o) + 2 * len(keys_h)
         old_logp, old_values = g[n_tm], g[n_tm + 1]
         old_log_probs = g[n_tm + 2] if kl_rows else None
+        teacher_log_probs = g[n_tm + 2 + len(kl_rows)] if t_rows else None
         # the K returns of a row gathered as one [rows, 1, K] row of K elements
         ret_c = p['ret_c'] if p['ret_c'].dim() == 1 else p['ret_c'].unsqueeze(1)
         adv, ret = gather([p['adv_c'], ret_c], idx_rm, int(sum(Lps)))
@@ -1707,7 +1832,7 @@ class DotaOptimizer:
             return tab
         return ExperienceBatch(obs, masks, actions, old_logp, adv, ret, h0, c0, old_values=old_values, valid=valid,
                                reset_slot=reset_slot, reset_h=table(p['ybufs']), reset_c=table(p['cbufs']) if lstm else None,
-                               old_log_probs=old_log_probs)
+                               old_log_probs=old_log_probs, teacher_log_probs=teacher_log_probs)
 
     @staticmethod
     def list_of_dicts_to_dict_of_lists(x):
@@ -1723,7 +1848,8 @@ class DotaOptimizer:
         backward, all-reduce, finish: ~80 kernel launches -> one graph launch); batches still in flight from the host
         (``prefetch``) run the same kernels launch by launch so that the upload overlaps them.  Either way the step uses
         the current ``learning_rate``, ``e_clip``, ``entropy_coef``, ``vf_coef``, ``MAX_GRAD_NORM`` and ``value_clip``
-        (and under KL control ``kl_coef`` and ``kl_stop``).  A step that ``kl_stop`` skips returns normally, with the
+        (and under KL control ``kl_coef`` and ``kl_stop``, with a teacher ``teacher_coef``).  A step that ``kl_stop`` skips
+        returns normally, with the
         parameters, Adam moments and step counters unchanged; ``last_ppo_stats['kl_skipped']`` is then 1.
         """
         if isinstance(experiences, ExperienceBatch):
@@ -1741,6 +1867,9 @@ class DotaOptimizer:
         if self.kl_control and batch.old_log_probs is None:
             raise ValueError("kl_coef=%r / kl_stop=%r need the log-prob rows of experience prep, and this batch has no "
                              "old_log_probs" % (self.kl_coef, self.kl_stop))
+        if self.teacher_model is not None and self.teacher_coef > 0.0 and batch.teacher_log_probs is None:
+            raise ValueError("teacher_coef=%r needs the teacher's log-prob rows of experience prep, and this batch has no "
+                             "teacher_log_probs" % (self.teacher_coef,))
         if batch.reset_slot is not None and not self.mask_padding:
             raise ValueError("a packed batch (reset_slot) trains only with mask_padding=True: its padding carries no "
                              "advantages or value targets")
@@ -1775,6 +1904,12 @@ class DotaOptimizer:
         if self.kl_control:             # the all-ranks KL of the finish, and whether it skipped the update
             self.last_ppo_stats['kl_all_ranks'] = float(res[_lib.LOSS_SLOTS + 4])
             self.last_ppo_stats['kl_skipped'] = float(res[_lib.LOSS_SLOTS + 5])
+        if self._teacher_step(batch):   # the KL to the teacher (this rank), per head, and the loss term lambda KL_T
+            ts = res[_lib.LOSS_SLOTS + self._result_dev.numel() - _lib.TEACHER_STATS_SLOTS:].tolist()
+            self.last_ppo_stats['teacher/kl'] = ts[0]
+            for h, k in enumerate(keys):
+                self.last_ppo_stats['teacher/kl/' + k] = ts[1 + h]
+            self.last_ppo_stats['loss/teacher'] = ts[6]
         if res[_lib.LOSS_SLOTS + 3] != 0:               # :667-669, :678-679 (parameters were left untouched)
             if math.isnan(float(res[0])):
                 raise ValueError('loss={}, policy_loss={}, entropy_loss={}, value_loss={}'.format(
@@ -1849,9 +1984,10 @@ class DotaOptimizer:
         # value_norm: the statistics of the last prep (mu, sigma), which the loss normalises the raw targets with; off: 0, 0
         mu, sigma = self._value_norm_moments() if self.value_norm else (0.0, 0.0)
         # KL control: the penalty's beta and the early-stop limit (None: 0, no limit)
+        # teacher: its coefficient, the double after the blocks (_teacher_coef_dev)
         vals = (float(self.learning_rate), float(self.e_clip), float(self.entropy_coef), float(self.vf_coef),
                 float(self.MAX_GRAD_NORM), float(self.value_clip or 0.0), mu, sigma, float(self.kl_coef),
-                float(self.kl_stop or 0.0))
+                float(self.kl_stop or 0.0)) + ((float(self.teacher_coef),) if self.teacher_model is not None else ())
         if vals == self._hparams_uploaded:
             return
         h = self._hparams_host.numpy()
@@ -1863,11 +1999,18 @@ class DotaOptimizer:
             self._hparams_host_all[1].copy_(self._hparams_host_all[0])
             hp = self._hparams_host_all[1].numpy()
             hp[_lib.HP_VF_COEF] = hp[_lib.HP_VALUE_CLIP] = 0.0
-        self._hparams_dev_all.copy_(self._hparams_host_all, non_blocking=True)
+        if self.teacher_model is not None:
+            self._teacher_coef_host[0] = float(self.teacher_coef)
+        self._hparams_dev_flat.copy_(self._hparams_host_flat, non_blocking=True)
         # the value head has a gradient only while the value loss is on (optimizer.py:660-662): with vf_coef = 0 the
         # gradient finish skips its tensors (no Adam step, no share of the mean grad norm), like the reference's .grad = None
         self._n_actions[VALUE_SLOT:VALUE_SLOT + 1].fill_(1 if self.vf_coef > 0 else 0)
         self._hparams_uploaded = vals
+
+    def _teacher_step(self, batch):
+        """Whether a step on ``batch`` runs the teacher term: a teacher was given and the batch carries its rows (a batch
+        prepared after the anneal retired it carries none, and runs the step without the term)."""
+        return self.teacher_model is not None and batch.teacher_log_probs is not None
 
     def _enqueue_step(self, batch):
         """Launches one optimizer step (:581-689) on the current stream; returns the device result vectors (loss slots, metrics)."""
@@ -1886,20 +2029,24 @@ class DotaOptimizer:
                                                               active=active)
         valid = batch.valid if self.mask_padding else None
         old_log_probs = batch.old_log_probs if self.kl_control else None
+        teacher_log_probs = batch.teacher_log_probs if self._teacher_step(batch) else None
         batch.wait(batch.old_logp, batch.advantages, batch.returns, batch.old_values, valid, old_log_probs,
-                   *batch.masks.values(), *batch.actions.values(), *batch.observations.values())
+                   teacher_log_probs, *batch.masks.values(), *batch.actions.values(), *batch.observations.values())
         # e_clip / entropy_coef / vf_coef / value_clip are read from the device block (_upload_hparams); padded tokens
         # (valid = False) count for nothing under mask_padding; the policy ratio is fixed per optimizer, so a captured
         # graph of the step keeps it
         heads = self.value_heads is not None
         # value heads: the PPO loss runs with its value term off (_hparams_dev_ppo); the value target it is handed then
         # feeds only an explained variance that dc_value_heads_loss overwrites, so the advantages stand in for it
-        out, n_actions, d_packed, d_tu, _ = ops.ppo_loss_packed(
+        # teacher: the KL term to its rows with the coefficient after the hyper-parameter blocks (_upload_hparams)
+        out, n_actions, d_packed, d_tu = ops.ppo_loss_packed(
             packed, target_unit, [batch.masks[k] for k in keys], [batch.actions[k] for k in keys],
             batch.old_logp, batch.advantages, batch.advantages if heads else batch.returns, self.e_clip,
             self.entropy_coef, self.vf_coef, hparams=self._hparams_dev_ppo, old_value=None if heads else batch.old_values,
             stats=self._ppo_stats, valid=valid, joint=self.policy_ratio == 'joint', old_log_probs=old_log_probs,
-            kl_out=self.flat.kl_tail)
+            kl_out=self.flat.kl_tail, teacher_log_probs=teacher_log_probs,
+            teacher_coef=self._teacher_coef_dev if teacher_log_probs is not None else None,
+            teacher_stats=self._teacher_stats if teacher_log_probs is not None else None)[:4]
         if heads:
             ops.value_heads_loss(packed, d_packed, batch.returns, self._hparams_dev, out, self._value_head_stats,
                                  old_value=batch.old_values, valid=valid, stats=self._ppo_stats)
@@ -2237,8 +2384,19 @@ class DotaOptimizer:
         unpacked = sequence_count(rollout_lens, S)
         return unpacked if unpacked < self.min_seq_per_epoch else sequence_count(rollout_lens, S, pack=True)
 
+    def teacher_anneal(self):
+        """With ``teacher_anneal_iterations`` N: sets ``teacher_coef`` to the constructor's value times max(0, 1 - n / N),
+        n = ``teacher_iterations``, and retires the teacher once that is 0.  ``run_iteration`` calls it first."""
+        if self.teacher_model is None or self.teacher_anneal_iterations is None:
+            return
+        self.teacher_coef = self._teacher_coef0 * max(0.0, 1.0 - self.teacher_iterations / self.teacher_anneal_iterations)
+        if self.teacher_coef == 0.0:
+            self._retire_teacher()
+
     def run_iteration(self, it):
         logger.info('iteration {}/{}'.format(it, self.iterations))
+        self.teacher_anneal()
+        teacher_on = self.teacher is not None
         experiences, subrewards, rollout_lens, weight_ages = [], [], [], []
         start_xp = time.time()
         xp_waits = 0
@@ -2304,7 +2462,8 @@ class DotaOptimizer:
         # measured at the parameters it left unchanged, and its KL is the measurement that stopped the iteration
         for k in ppo_stats[0]:
             if k not in ('kl_all_ranks', 'kl_skipped'):     # value heads: 'loss/value/<name>' next to 'loss/value'
-                metrics[k if k.startswith('loss/') else 'ppo/{}'.format(k)] = float(np.mean([s[k] for s in ppo_stats]))
+                metrics[k if k.startswith(('loss/', 'teacher/')) else 'ppo/{}'.format(k)] = \
+                    float(np.mean([s[k] for s in ppo_stats]))
         if self.kl_control:
             # d: the mean over the steps (a skipped one included) of the all-ranks KL, the same number on every rank, so
             # the adaptive coefficient stays identical across ranks
@@ -2314,6 +2473,10 @@ class DotaOptimizer:
                 metrics['kl/updates_run'], metrics['kl/updates_skipped'] = self.last_kl_updates
             if self.kl_target is not None:                                 # for the next iteration (saved with the model)
                 self.kl_coef = kl_coef_update(self.kl_coef, d, self.kl_target)
+        if self.teacher_model is not None:                                 # the coefficient this iteration trained with
+            metrics['teacher/coef'] = self.teacher_coef
+            if teacher_on:
+                self.teacher_iterations += 1
         if self.mask_padding:                                              # share of the trained tokens that were padding
             metrics['padding_fraction'] = (n_steps - sum(rollout_lens)) / n_steps
         if self.pack_sequences:                                            # share of the sequences packing saved
@@ -2455,7 +2618,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
          mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False, value_norm_decay=0.99,
          kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False, recompute_states=False, value_heads=None,
-         value_gammas=None):
+         value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                        mask_padding=mask_padding, pack_sequences=pack_sequences,
@@ -2463,7 +2626,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
                        value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
                        kl_stop=kl_stop, recompute_advantages=recompute_advantages,
                        recompute_states=recompute_states, value_heads=value_heads,
-                       value_gammas=value_gammas)                                         # before any process-group setup
+                       value_gammas=value_gammas, teacher_model=teacher_model, teacher_coef=teacher_coef,
+                       teacher_anneal_iterations=teacher_anneal_iterations)               # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -2477,7 +2641,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         num_minibatches=num_minibatches, mask_padding=mask_padding, pack_sequences=pack_sequences,
         policy_ratio=policy_ratio, value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef,
         kl_target=kl_target, kl_stop=kl_stop, recompute_advantages=recompute_advantages,
-        recompute_states=recompute_states, value_heads=value_heads, value_gammas=value_gammas)
+        recompute_states=recompute_states, value_heads=value_heads, value_gammas=value_gammas,
+        teacher_model=teacher_model, teacher_coef=teacher_coef, teacher_anneal_iterations=teacher_anneal_iterations)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -2494,7 +2659,8 @@ def build_arg_parser():
     settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm``, ``--value-clip``,
     ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches``, ``--mask-padding``,
     ``--pack-sequences``, ``--policy-ratio``, ``--value-norm``, ``--value-norm-decay``, ``--kl-coef``, ``--kl-target``,
-    ``--kl-stop``, ``--value-heads`` and ``--value-gammas``."""
+    ``--kl-stop``, ``--value-heads``, ``--value-gammas``, ``--teacher-model``, ``--teacher-coef`` and
+    ``--teacher-anneal-iterations``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -2556,6 +2722,14 @@ def build_arg_parser():
                         "(default: one critic of the summed reward)")
     p.add_argument("--value-gammas", type=parse_value_gammas, default=None,
                    help="discounts of some value heads, 'name=0.999;...' (the others take --gamma)")
+    p.add_argument("--teacher-model", type=str, default=None,
+                   help="a Policy state_dict file (any width, cell or depth) whose policy the run is kickstarted from: "
+                        "the loss adds --teacher-coef times the KL from it (default: no teacher)")
+    p.add_argument("--teacher-coef", type=float, default=1.0,
+                   help="coefficient of the KL to the teacher (needs --teacher-model)")
+    p.add_argument("--teacher-anneal-iterations", type=int, default=None,
+                   help="anneal --teacher-coef linearly to 0 over this many iterations, then retire the teacher "
+                        "(needs --teacher-model; default: a fixed coefficient)")
     return p
 
 
@@ -2573,6 +2747,8 @@ if __name__ == '__main__':
              mask_padding=args.mask_padding, pack_sequences=args.pack_sequences, policy_ratio=args.policy_ratio,
              value_norm=args.value_norm, value_norm_decay=args.value_norm_decay, kl_coef=args.kl_coef,
              kl_target=args.kl_target, kl_stop=args.kl_stop, recompute_advantages=args.recompute_advantages,
-             recompute_states=args.recompute_states, value_heads=args.value_heads, value_gammas=args.value_gammas)
+             recompute_states=args.recompute_states, value_heads=args.value_heads, value_gammas=args.value_gammas,
+             teacher_model=args.teacher_model, teacher_coef=args.teacher_coef,
+             teacher_anneal_iterations=args.teacher_anneal_iterations)
     except KeyboardInterrupt:
         pass

@@ -18,6 +18,7 @@ GEMM's ``DC_EUNSUPPORTED`` error.
 CUDA only: calling ``forward`` with CPU tensors raises (there is no CPU fallback).
 """
 import logging
+import re
 
 import numpy as np
 import torch
@@ -106,6 +107,32 @@ class Policy(nn.Module):
         self.affine_unit_attention = nn.Linear(H, 128)
         self.affine_head_ability = nn.Linear(H, 3)
         self.affine_value = nn.Linear(H, self.value_heads)      # created last: value_heads leaves every other init as is
+
+    @classmethod
+    def from_state_dict(cls, state_dict):
+        """The ``Policy`` a ``state_dict`` describes, loaded strictly: ``hidden_size`` from the rows of
+        ``affine_pre_rnn.weight``, ``num_layers`` from the ``rnn.weight_hh_l{k}`` keys, ``cell`` from the rows of
+        ``rnn.weight_hh_l0`` (3H: 'gru', 4H: 'lstm') and ``value_heads`` from the rows of ``affine_value.weight``.  Raises
+        ``ValueError`` for a dict that is not a ``Policy``'s (missing keys, unexpected keys or shapes)."""
+        try:
+            H = int(state_dict['affine_pre_rnn.weight'].shape[0])
+            rows = int(state_dict['rnn.weight_hh_l0'].shape[0])
+            value_heads = int(state_dict['affine_value.weight'].shape[0])
+        except (KeyError, TypeError, AttributeError, IndexError) as e:
+            raise ValueError("not a Policy state_dict: %r" % (e,)) from None
+        num_layers = sum(1 for k in state_dict if re.fullmatch(r'rnn\.weight_hh_l\d+', k))
+        cells = {3 * H: 'gru', 4 * H: 'lstm'}
+        if rows not in cells:
+            raise ValueError("not a Policy state_dict: rnn.weight_hh_l0 has %d rows, neither 3 nor 4 x hidden_size %d"
+                             % (rows, H))
+        if not 1 <= value_heads <= MAX_VALUE_HEADS:
+            raise ValueError("not a Policy state_dict: affine_value.weight has %d rows" % value_heads)
+        pol = cls(hidden_size=H, cell=cells[rows], num_layers=num_layers, value_heads=value_heads)
+        try:
+            pol.load_state_dict(state_dict, strict=True)
+        except RuntimeError as e:
+            raise ValueError("not a Policy state_dict: %s" % e) from None
+        return pol
 
     # ------------------------------------------------------------------ reference API
     def init_hidden(self):

@@ -543,6 +543,37 @@ int dc_ppo_loss_fwd_bwd_kl(const float *const logits[DC_NUM_HEADS], const int64_
                            const int64_t ld_dlogits[DC_NUM_HEADS], float *dvalue, int64_t ld_dvalue, float *out,
                            float *stats, float *kl_out, int32_t *n_actions, void *workspace, dc_stream_t stream);
 
+/* ---- kickstarting: a KL term to a frozen teacher policy (Schmitt et al. 2018) -----------------------------------------
+ * No counterpart in the reference.  With S_t and T_a as for KL control (the counting tokens, their heads with an action
+ * row, and the number of counting tokens with S_t not empty), p_T the teacher's masked softmax and p the current one,
+ * both over the legal entries of the stored mask, in the reference's form:
+ *   KL_T = (1 / T_a) sum_t sum_{h in S_t} sum_{a legal} p_T(a) (log p_T(a) - log p(a))      (0 when T_a = 0)
+ *   loss += lambda KL_T,   dlogits[t, h, a] += (lambda / T_a)(p(a) - p_T(a)) for h in S_t, a legal
+ * with lambda = *teacher_coef.  The same definition as KL control's, with the teacher's rows for the prep-time ones.
+ *
+ * dc_ppo_loss_fwd_bwd_teacher: the arguments of dc_ppo_loss_fwd_bwd_kl, with old_log_probs and kl_out nullable (NULL:
+ *   no KL penalty), plus
+ *   teacher_log_probs [N, DC_KL_ROW_FLOATS]  the teacher's rows, as dc_selected_logp_rows writes them
+ *   teacher_coef       one fp64 device value, lambda >= 0 (kept off the hparams block, read on every launch)
+ *   teacher_stats [DC_TEACHER_STATS_SLOTS] fp32 out: 0 KL_T, 1..5 the per-head KL (sum over the head's action rows of its
+ *                      row's KL to the teacher, over their count; 0 for a head without any), 6 lambda KL_T
+ *   The loss adds lambda KL_T into out[0] (after beta KL when old_log_probs is given).  With lambda = 0 the loss, dlogits,
+ *   dvalue, stats and kl_out are those of _kl (old_log_probs given) or _masked / _joint (NULL) bit for bit; teacher_stats
+ *   still reports the KL.
+ * Algorithmic bytes: those of the entry point it extends + 260 per token (the teacher's rows).  Checked before any CUDA
+ * call: the arguments of _kl and non-null teacher_log_probs, teacher_coef and teacher_stats -> DC_EINVAL.
+ */
+#define DC_TEACHER_STATS_SLOTS 7
+int dc_ppo_loss_fwd_bwd_teacher(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                                const uint8_t *const masks[DC_NUM_HEADS], const uint8_t *const actions[DC_NUM_HEADS],
+                                const float *old_logp, const float *old_log_probs, const float *teacher_log_probs,
+                                const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                                const float *old_value, const uint8_t *valid, int64_t N, const double *hparams,
+                                const double *teacher_coef, int joint, float *const dlogits[DC_NUM_HEADS],
+                                const int64_t ld_dlogits[DC_NUM_HEADS], float *dvalue, int64_t ld_dvalue, float *out,
+                                float *stats, float *kl_out, float *teacher_stats, int32_t *n_actions, void *workspace,
+                                dc_stream_t stream);
+
 /* ---- value normalisation (PopArt, van Hasselt et al. 2016) --------------------------------------------------------
  * No counterpart in the reference, whose critic learns raw returns (optimizer.py:660).
  *   dc_value_norm_stats    out[3] fp64 (device) = count, sum x, sum x^2 over the x[i] [N] with valid[i] != 0 (valid NULL:
