@@ -28,6 +28,9 @@ SIGNATURES = {
     "dc_gae_scan_indexed": (_i32, [_vp, _i32, _vp, _i64, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _vp, _vp, _vp]),
     "dc_vtrace_scan_indexed": (_i32, [_vp, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _f64, _f64, _vp,
                                       _vp, _vp, _vp]),
+    "dc_upgo_scan": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _f64, _vp, _vp, _vp]),
+    "dc_upgo_scan_indexed": (_i32, [_vp, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _f64, _f64, _f64, _vp, _vp,
+                                    _vp]),
     "dc_gae_scan_heads": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _f64, _vp, _vp, _vp]),
     "dc_gae_scan_heads_indexed": (_i32, [_vp, _i32, _vp, _i32, _vp, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _f64, _vp, _vp,
                                          _vp]),
@@ -114,6 +117,7 @@ KL_ROW_FLOATS = 65          # entries of one token's masked log-prob row over th
 TEACHER_STATS_SLOTS = 7
 FINISH_KL_METRICS = 6       # metrics of dc_grad_finish_kl: the four of dc_grad_finish, the all-ranks KL, the skip flag
 VTRACE_STATS_SLOTS = 8      # per-segment fp64 sums written by dc_vtrace_scan (DC_VTRACE_STATS_SLOTS)
+UPGO_STATS_SLOTS = 3        # per-segment fp64 sums written by dc_upgo_scan (DC_UPGO_STATS_SLOTS)
 VALUE_HEADS_MAX = 10        # value heads of dc_gae_scan_heads / dc_value_heads_loss (DC_VALUE_HEADS_MAX)
 VALUE_HEADS_STATS_SLOTS = 20    # dc_value_heads_loss: [k] value loss, [VALUE_HEADS_MAX + k] explained variance of head k
 VALUE_HEADS_WORKSPACE_BYTES = 131072

@@ -12,7 +12,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libdotaclient_b200.so")
 ARCH = "arch=compute_90a,code=sm_90a"       # wgmma and the sm_90a feature set: H100 only
-SOURCES = ["capi.cu", "gae_scan.cu", "vtrace_scan.cu", "gather.cu", "ppo_loss.cu", "grad_finish.cu", "rnn_seq.cu", "gemm_tf32x3.cu", "encoder.cu", "actor.cu",
+SOURCES = ["capi.cu", "gae_scan.cu", "vtrace_scan.cu", "upgo_scan.cu", "gather.cu", "ppo_loss.cu", "grad_finish.cu", "rnn_seq.cu", "gemm_tf32x3.cu", "encoder.cu", "actor.cu",
            "value_norm.cu", "state_refresh.cu", "value_heads.cu", "target_rows.cu"]
 
 

@@ -297,6 +297,70 @@ def vtrace_scan_indexed(rewards, values, logp_target, logp_behaviour, tok, seg_o
     return pg_adv, vs
 
 
+def _upgo_logp(logp_target, logp_behaviour, n_target, n_rows):
+    """The log-prob operands of the UPGO scans: both None (GAE) or both given (V-trace), as fp32 [n, 5]."""
+    if (logp_target is None) != (logp_behaviour is None):
+        raise ValueError("give both logp_target and logp_behaviour (V-trace) or neither (GAE)")
+    if logp_target is None:
+        return None, None
+    logp_target, logp_behaviour = _f32c(logp_target), _f32c(logp_behaviour)
+    if logp_target.numel() != n_target * 5 or logp_behaviour.numel() != n_rows * 5:
+        raise ValueError("logp_target must be [%d, 5] and logp_behaviour [%d, 5]" % (n_target, n_rows))
+    return logp_target, logp_behaviour
+
+
+def upgo_scan(rewards, values, seg_off, adv, gamma, coef, boot_value=None, logp_target=None, logp_behaviour=None,
+              rho_clip=1.0, valid_len=None, stats=False):
+    """Adds ``coef`` times the UPGO advantage A^U into ``adv`` in place (``dc_upgo_scan``; DESIGN.md section 4.2):
+    G_t = r_t + gamma G_{t+1} while the next step's TD error is >= 0, r_t + gamma V_{t+1} after a worse one, and
+    A^U_t = rhob_t (G_t - V_t).  ``rewards``, ``values``, ``seg_off``, ``boot_value`` and ``valid_len`` are as
+    ``vtrace_scan``'s; ``adv`` [n_rows] contiguous fp32, the advantages the base scan wrote.  Without log-probs rhob = 1
+    (GAE); with ``logp_target`` / ``logp_behaviour`` [n_rows, 5] it is V-trace's min(rho_clip, rho).  Returns ``adv``, and
+    with ``stats`` also the per-segment sums ``[n_seg, _lib.UPGO_STATS_SLOTS]`` fp64 (row count, rows that went through
+    to the next step's return, sum of A^U) over the real steps."""
+    _need_cuda(rewards, values, seg_off, adv, boot_value, valid_len, logp_target, logp_behaviour)
+    rewards, values = _f32c(rewards), _f32c(values)
+    n_sub = 1 if rewards.dim() == 1 else rewards.shape[1]
+    n_rows = values.numel()
+    if rewards.numel() != n_rows * n_sub:
+        raise ValueError("rewards have %d elements for %d rows of %d sub-rewards" % (rewards.numel(), n_rows, n_sub))
+    if adv.dtype != torch.float32 or not adv.is_contiguous() or adv.numel() != n_rows:
+        raise ValueError("adv must be a contiguous fp32 tensor of %d elements" % n_rows)
+    logp_target, logp_behaviour = _upgo_logp(logp_target, logp_behaviour, n_rows, n_rows)
+    seg_off = seg_off.to(torch.int64).contiguous()
+    n_seg = seg_off.numel() - 1
+    if boot_value is not None:
+        boot_value = _f32c(boot_value)
+        assert boot_value.numel() == n_seg
+    if valid_len is not None:
+        valid_len = valid_len.to(torch.int64).contiguous()
+        assert valid_len.numel() == n_seg
+    seg_stats = torch.empty((n_seg, _lib.UPGO_STATS_SLOTS), dtype=torch.float64, device=values.device) if stats else None
+    with PROFILE.span("upgo_scan", 1):
+        _lib.check(_lib.load().dc_upgo_scan(rewards.data_ptr(), n_sub, values.data_ptr(), _lib.ptr(logp_target),
+                                            _lib.ptr(logp_behaviour), seg_off.data_ptr(), n_seg, _lib.ptr(valid_len),
+                                            _lib.ptr(boot_value), float(gamma), float(rho_clip), float(coef),
+                                            adv.data_ptr(), _lib.ptr(seg_stats), _lib.stream_ptr()), "dc_upgo_scan")
+    return (adv, seg_stats) if stats else adv
+
+
+def upgo_scan_indexed(rewards, values, tok, seg_off, adv, gamma, coef, boot_value=None, logp_target=None,
+                      logp_behaviour=None, rho_clip=1.0):
+    """``upgo_scan`` with ``vtrace_scan_indexed``'s token layout (``dc_upgo_scan_indexed``): row r reads its value (and
+    target log-probs ``logp_target`` [n_tokens, 5]) at token ``tok[r]`` and adds into ``adv`` there, in place; rows with
+    ``tok[r] < 0`` read 0 and write nothing.  ``logp_behaviour`` [n_rows, 5] stays rollout-major.  The per-segment
+    statistics are not computed."""
+    rewards, n_sub, flat, ld, seg_off, boot_value = _indexed_args(rewards, values, tok, seg_off, adv, adv, boot_value)
+    _need_cuda(logp_target, logp_behaviour)
+    logp_target, logp_behaviour = _upgo_logp(logp_target, logp_behaviour, flat.numel(), tok.numel())
+    with PROFILE.span("upgo_scan_indexed", 1):
+        _lib.check(_lib.load().dc_upgo_scan_indexed(
+            rewards.data_ptr(), n_sub, flat.data_ptr(), ld, _lib.ptr(logp_target), _lib.ptr(logp_behaviour),
+            tok.data_ptr(), seg_off.data_ptr(), seg_off.numel() - 1, None, _lib.ptr(boot_value), float(gamma),
+            float(rho_clip), float(coef), adv.data_ptr(), None, _lib.stream_ptr()), "dc_upgo_scan_indexed")
+    return adv
+
+
 # --------------------------------------------------------------------------------------------- minibatch gather
 _index_staging = {}     # device -> (pinned int64 buffer, event recorded after the last upload from it)
 

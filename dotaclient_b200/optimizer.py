@@ -471,7 +471,8 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
                        vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1, mask_padding=False, pack_sequences=False,
                        policy_ratio='per_head', value_norm=False, value_norm_decay=0.99, kl_coef=0.0, kl_target=None,
                        kl_stop=None, recompute_advantages=False, recompute_states=False, value_heads=None,
-                       value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None):
+                       value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None,
+                       upgo_coef=0.0):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
     vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool,
@@ -479,7 +480,8 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
     and 0 <= value_norm_decay < 1, finite kl_coef >= 0, kl_target None or finite > 0 (and then kl_coef > 0), kl_stop None
     or finite > 0, recompute_advantages and recompute_states bools, value_heads / value_gammas as ``value_head_groups``
     checks them (value heads refuse V-trace and value_norm), finite teacher_coef >= 0 and teacher_anneal_iterations None
-    or an int >= 1, both left at their defaults without a teacher_model.  NaN fails every check."""
+    or an int >= 1, both left at their defaults without a teacher_model, and upgo_coef as ``check_upgo_coef`` checks it.
+    NaN fails every check."""
     if not isinstance(recompute_states, bool):
         raise ValueError("recompute_states=%r: must be True or False" % (recompute_states,))
     if not isinstance(recompute_advantages, bool):
@@ -548,6 +550,17 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
     if value_heads is not None and value_norm:
         raise ValueError("value_heads with value_norm=True: PopArt would need one set of statistics per head and a "
                          "per-row rescale of the value head, which is not implemented")
+    check_upgo_coef(upgo_coef, value_heads)
+
+
+def check_upgo_coef(upgo_coef, value_heads=None):
+    """Raises ``ValueError`` unless ``upgo_coef`` is a finite number >= 0 (not a bool), and 0 with ``value_heads``: the
+    UPGO switch compares one return with one critic value, and heads with different discounts have no single return."""
+    if isinstance(upgo_coef, bool) or not isinstance(upgo_coef, numbers.Real) or not 0.0 <= float(upgo_coef) < math.inf:
+        raise ValueError("upgo_coef=%r: the UPGO coefficient must be a finite number >= 0" % (upgo_coef,))
+    if float(upgo_coef) > 0.0 and value_heads is not None:
+        raise ValueError("upgo_coef=%r with value_heads: UPGO compares one return with one critic value, and value heads "
+                         "with different discounts have no single return" % (upgo_coef,))
 
 
 class ValueHeads(typing.NamedTuple):
@@ -1059,7 +1072,7 @@ class DotaOptimizer:
                  num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False,
                  value_norm_decay=0.99, kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False,
                  recompute_states=False, value_heads=None, value_gammas=None, teacher_model=None, teacher_coef=1.0,
-                 teacher_anneal_iterations=None):
+                 teacher_anneal_iterations=None, upgo_coef=0.0):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
@@ -1070,7 +1083,8 @@ class DotaOptimizer:
                            value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef, kl_target=kl_target,
                            kl_stop=kl_stop, recompute_advantages=recompute_advantages, recompute_states=recompute_states,
                            value_heads=value_heads, value_gammas=value_gammas, teacher_model=teacher_model,
-                           teacher_coef=teacher_coef, teacher_anneal_iterations=teacher_anneal_iterations)
+                           teacher_coef=teacher_coef, teacher_anneal_iterations=teacher_anneal_iterations,
+                           upgo_coef=upgo_coef)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
         # value heads: one critic column per reward group, each with its own discount.  Prep scans every group
         # (gae_scan_heads), the policy trains on the summed advantage, the value loss is dc_value_heads_loss's and the
@@ -1121,6 +1135,11 @@ class DotaOptimizer:
         self.advantage_estimator = advantage_estimator
         self.vtrace_rho_clip, self.vtrace_c_clip = float(vtrace_rho_clip), float(vtrace_c_clip)
         self._vtrace_seg_stats = None       # per-rollout sums of the last V-trace prep (device), see last_vtrace_stats
+        # UPGO (AlphaStar): experience prep adds upgo_coef times the upgoing advantage to the GAE / V-trace advantage
+        # (dc_upgo_scan), and the advantage refresh does the same.  Read at every prep, so it can be scheduled between
+        # iterations; 0 runs nothing.  _upgo_prep: (coefficient, per-segment sums on the device) of the last prep with c > 0
+        self.upgo_coef = float(upgo_coef)
+        self._upgo_prep = None
         self.MAX_GRAD_NORM = float(max_grad_norm)     # shadows the class constant; read before every step, like lr below
         self.value_clip = None if value_clip is None else float(value_clip)
         self.rmq_host, self.rmq_port = rmq_host, rmq_port
@@ -1506,6 +1525,7 @@ class DotaOptimizer:
         if vtrace:
             check_behaviour_logp(datas)                # refused before anything is uploaded
         check_continuation(datas, pol.cell, n_layers, H)
+        upgo = self._upgo_coef_now()                   # so is a coefficient assigned outside its domain
         Ls = [int(d['rewards'].shape[0]) for d in datas]
         Lps = [(L + S - 1) // S * S for L in Ls]
         Lmax = max(Lps)
@@ -1619,15 +1639,15 @@ class DotaOptimizer:
                 rew_c = torch.from_numpy(np.concatenate([rewards_np[i, :Lps[i]] for i in range(R)])).to(dev)
             # [real | padding] per rollout under mask_padding or when cut: the bootstrap follows step L_i
             seg = torch.tensor(seg_np, dtype=torch.int64, device=dev)
-            blp_c = valid_len = None
+            blp_c = lt_c = valid_len = None
             if vtrace:
                 # heads that took no action carry no behaviour log-prob (old_logp is 0 there too); padding rows are 0 already
                 acted = torch.stack([actions[k].any(dim=-1) for k in keys], dim=-1)
                 behaviour_logp = torch.where(acted, behaviour_logp, 0.0)
                 valid_len = torch.from_numpy(seg_valid).pin_memory().to(dev, non_blocking=True)  # padding: no real steps
-                blp_c = rollout_major(behaviour_logp)
+                blp_c, lt_c = rollout_major(behaviour_logp), rollout_major(old_logp)
                 adv_c, ret_c, self._vtrace_seg_stats = ops.vtrace_scan(
-                    rew_c, vals_c, rollout_major(old_logp), blp_c, seg, gamma=self.gamma,
+                    rew_c, vals_c, lt_c, blp_c, seg, gamma=self.gamma,
                     lam=self.gae_lambda, rho_clip=self.vtrace_rho_clip, c_clip=self.vtrace_c_clip, boot_value=boot,
                     valid_len=valid_len, stats=True)
             elif self.value_heads is not None:
@@ -1640,6 +1660,15 @@ class DotaOptimizer:
                 # :417-421; a cut rollout's returns go on past the cut as gamma^(L-t) V(s_L), its advantages from V(s_L)
                 adv_c, ret_c = ops.gae_scan(rew_c, vals_c, seg, gamma=self.gamma, lam=self.gae_lambda, boot_value=boot,
                                             boot_reward=boot)
+            self._upgo_prep = None
+            if upgo > 0.0:
+                # + c A^U over the same segments, values and bootstraps, before the padded rows are zeroed below
+                upgo_valid = valid_len if valid_len is not None else \
+                    torch.from_numpy(seg_valid).pin_memory().to(dev, non_blocking=True)
+                _, upgo_stats = ops.upgo_scan(rew_c, vals_c, seg, adv_c, self.gamma, upgo, boot_value=boot,
+                                              logp_target=lt_c, logp_behaviour=blp_c, rho_clip=self.vtrace_rho_clip,
+                                              valid_len=upgo_valid, stats=True)
+                self._upgo_prep = (upgo, upgo_stats)
             valid = None
             if self.mask_padding:
                 lens = torch.tensor(chunk_valid_lengths(Ls, S), dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
@@ -1931,6 +1960,23 @@ class DotaOptimizer:
         n = max(s[0], 1.0)
         return {'mean_log_rho': s[1] / n, 'mean_clipped_rho': s[2] / n, 'rho_clip_fraction': s[3] / n,
                 'c_clip_fraction': s[4] / n}
+
+    @property
+    def last_upgo_stats(self):
+        """Diagnostics of the last experience prep that ran with ``upgo_coef > 0`` (None before one, or when the last prep
+        ran without), over the rollouts' real steps (padding excluded): ``through_fraction`` (the share of steps whose
+        upgoing return went on through the next step's, because that step's TD error was >= 0) and ``mean_advantage`` (the
+        mean UPGO advantage A^U, before the coefficient).  Read back from the device, which waits for the prep."""
+        if self._upgo_prep is None:
+            return None
+        s = self._upgo_prep[1].sum(dim=0).tolist()
+        n = max(s[0], 1.0)
+        return {'through_fraction': s[1] / n, 'mean_advantage': s[2] / n}
+
+    def _upgo_coef_now(self):
+        """``upgo_coef`` as prep and the advantage refresh read it, checked again: it may be assigned at any time."""
+        check_upgo_coef(self.upgo_coef, self.value_heads)
+        return float(self.upgo_coef)
 
     def _value_norm_moments(self):
         return value_norm_moments(self._value_norm, self.VALUE_NORM_MIN_STD)
@@ -2260,7 +2306,8 @@ class DotaOptimizer:
     def _rescan(self, batch, values, target, boot):
         """Prep's segmented GAE or V-trace scan over prep's rollout-major rewards and segments, reading the raw values
         (and for V-trace the target log-probs ``[S * B, 5]``) at the batch's tokens and writing ``batch.advantages`` /
-        ``batch.returns`` there (``ops.gae_scan_indexed`` / ``vtrace_scan_indexed``), ending the segments on ``boot``."""
+        ``batch.returns`` there (``ops.gae_scan_indexed`` / ``vtrace_scan_indexed``), ending the segments on ``boot``;
+        with ``upgo_coef > 0`` then prep's UPGO term over the same operands (``ops.upgo_scan_indexed``)."""
         r = batch.refresh
         if self.value_heads is not None:
             vh = self.value_heads
@@ -2274,6 +2321,10 @@ class DotaOptimizer:
         else:
             ops.gae_scan_indexed(r.rewards, values, r.tok, r.seg_off, batch.advantages, batch.returns, self.gamma,
                                  self.gae_lambda, boot_value=boot, boot_reward=boot)
+        upgo = self._upgo_coef_now()
+        if upgo > 0.0:                          # + c A^U, as prep adds it
+            ops.upgo_scan_indexed(r.rewards, values, r.tok, r.seg_off, batch.advantages, self.gamma, upgo, boot_value=boot,
+                                  logp_target=target, logp_behaviour=r.behaviour_logp, rho_clip=self.vtrace_rho_clip)
 
     def _refresh_states(self, batch):
         """Recomputes the recurrent states entering the batch's chunks with the current weights (``recompute_states``;
@@ -2487,6 +2538,10 @@ class DotaOptimizer:
         if self.advantage_estimator == 'vtrace':                           # read now: the steps have synced the device
             for k, v in self.last_vtrace_stats.items():
                 metrics['vtrace/{}'.format(k)] = v
+        if self._upgo_prep is not None:                                    # UPGO of this iteration's prep
+            metrics['upgo/coef'] = self._upgo_prep[0]
+            for k, v in self.last_upgo_stats.items():
+                metrics['upgo/{}'.format(k)] = v
         if self.value_norm:                                                # the statistics this iteration trained under
             st = self.value_norm_stats
             metrics['value_norm/mean'], metrics['value_norm/std'] = st['mean'], st['std']
@@ -2618,7 +2673,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
          mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False, value_norm_decay=0.99,
          kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False, recompute_states=False, value_heads=None,
-         value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None):
+         value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None, upgo_coef=0.0):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                        mask_padding=mask_padding, pack_sequences=pack_sequences,
@@ -2627,7 +2682,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
                        kl_stop=kl_stop, recompute_advantages=recompute_advantages,
                        recompute_states=recompute_states, value_heads=value_heads,
                        value_gammas=value_gammas, teacher_model=teacher_model, teacher_coef=teacher_coef,
-                       teacher_anneal_iterations=teacher_anneal_iterations)               # before any process-group setup
+                       teacher_anneal_iterations=teacher_anneal_iterations,
+                       upgo_coef=upgo_coef)                                              # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -2642,7 +2698,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         policy_ratio=policy_ratio, value_norm=value_norm, value_norm_decay=value_norm_decay, kl_coef=kl_coef,
         kl_target=kl_target, kl_stop=kl_stop, recompute_advantages=recompute_advantages,
         recompute_states=recompute_states, value_heads=value_heads, value_gammas=value_gammas,
-        teacher_model=teacher_model, teacher_coef=teacher_coef, teacher_anneal_iterations=teacher_anneal_iterations)
+        teacher_model=teacher_model, teacher_coef=teacher_coef, teacher_anneal_iterations=teacher_anneal_iterations,
+        upgo_coef=upgo_coef)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -2659,8 +2716,8 @@ def build_arg_parser():
     settings ``--gamma``, ``--gae-lambda``, ``--clip-range``, ``--max-grad-norm``, ``--value-clip``,
     ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches``, ``--mask-padding``,
     ``--pack-sequences``, ``--policy-ratio``, ``--value-norm``, ``--value-norm-decay``, ``--kl-coef``, ``--kl-target``,
-    ``--kl-stop``, ``--value-heads``, ``--value-gammas``, ``--teacher-model``, ``--teacher-coef`` and
-    ``--teacher-anneal-iterations``."""
+    ``--kl-stop``, ``--value-heads``, ``--value-gammas``, ``--teacher-model``, ``--teacher-coef``,
+    ``--teacher-anneal-iterations`` and ``--upgo-coef``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -2730,6 +2787,9 @@ def build_arg_parser():
     p.add_argument("--teacher-anneal-iterations", type=int, default=None,
                    help="anneal --teacher-coef linearly to 0 over this many iterations, then retire the teacher "
                         "(needs --teacher-model; default: a fixed coefficient)")
+    p.add_argument("--upgo-coef", type=float, default=0.0,
+                   help="add this times the upgoing (UPGO) advantage, which follows a rollout's return only while the "
+                        "next step does at least as well as the critic expects, to the GAE / V-trace advantage (0: off)")
     return p
 
 
@@ -2749,6 +2809,6 @@ if __name__ == '__main__':
              kl_target=args.kl_target, kl_stop=args.kl_stop, recompute_advantages=args.recompute_advantages,
              recompute_states=args.recompute_states, value_heads=args.value_heads, value_gammas=args.value_gammas,
              teacher_model=args.teacher_model, teacher_coef=args.teacher_coef,
-             teacher_anneal_iterations=args.teacher_anneal_iterations)
+             teacher_anneal_iterations=args.teacher_anneal_iterations, upgo_coef=args.upgo_coef)
     except KeyboardInterrupt:
         pass

@@ -107,6 +107,33 @@ int dc_vtrace_scan_indexed(const float *rewards, int n_sub, const float *values,
                            double gamma, double lam, double rho_clip, double c_clip, float *pg_adv, float *vs,
                            double *seg_stats, dc_stream_t stream);
 
+/* ---- UPGO: the upgoing policy update ----------------------------------------------------------
+ * DotaOptimizer(upgo_coef=c) (Vinyals et al. 2019, AlphaStar): ADDS c * A^U into the advantages `adv` that one of the
+ * scans above wrote, over the same rows and segments.  For the rows lo .. hi-1 of a segment, with V_hi = boot:
+ *   delta_t   = r_t + gamma V_{t+1} - V_t                       float64, three roundings, no FMA
+ *   through_t = (t + 1 < hi) and (delta_{t+1} >= 0)
+ *   G_t       = r_t + gamma * (through_t ? G_{t+1} : V_{t+1})
+ *   A^U_t     = rho-bar_t (G_t - V_t),      adv_t = fp32((double)adv_t + coef * A^U_t)
+ *   rewards, n_sub, values, seg_off, boot_value (NULL = 0), valid_len: as dc_vtrace_scan
+ *   logp_target, logp_behaviour  both NULL (GAE: rho-bar_t = 1) or both given (V-trace: rho-bar_t as dc_vtrace_scan)
+ *   rho_clip > 0                 the truncation rho-bar when the log-probs are given
+ *   seg_stats [n_seg][DC_UPGO_STATS_SLOTS] fp64 or NULL  per-segment sums over the real steps:
+ *       0 token count, 1 #(through_t), 2 sum A^U_t (before coef)
+ * The _indexed form has dc_vtrace_scan_indexed's token layout: row r reads values[tok[r] * ld_values] (ld_values >= 1)
+ * and logp_target[tok[r] * 5 + h] and adds into adv[tok[r]]; tok[r] < 0 reads 0 and writes nothing.
+ * Checked before any CUDA call (DC_EINVAL): n_seg >= 0, 1 <= n_sub < 128, ld_values >= 1, rho_clip > 0 with log-probs,
+ * one log-prob array without the other, and null pointers.  Float64 after the reward reduction; one warp per segment.
+ */
+#define DC_UPGO_STATS_SLOTS 3
+int dc_upgo_scan(const float *rewards, int n_sub, const float *values, const float *logp_target,
+                 const float *logp_behaviour, const int64_t *seg_off, int n_seg, const int64_t *valid_len,
+                 const float *boot_value, double gamma, double rho_clip, double coef, float *adv, double *seg_stats,
+                 dc_stream_t stream);
+int dc_upgo_scan_indexed(const float *rewards, int n_sub, const float *values, int64_t ld_values,
+                         const float *logp_target, const float *logp_behaviour, const int64_t *tok,
+                         const int64_t *seg_off, int n_seg, const int64_t *valid_len, const float *boot_value,
+                         double gamma, double rho_clip, double coef, float *adv, double *seg_stats, dc_stream_t stream);
+
 /* ---- GAE with one value head per reward group ------------------------------------------------
  * DotaOptimizer(value_heads=...): the sub-rewards of a row are split into K groups, each with its own critic column and
  * discount, all sharing lam.  Per segment, as dc_gae_scan, and per group k:
