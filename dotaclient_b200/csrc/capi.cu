@@ -26,7 +26,7 @@ int dc_sm_count() {
 
 extern "C" {
 
-int dc_version(void) { return 114; }
+int dc_version(void) { return 115; }
 
 const char *dc_last_error(void) { return g_err; }
 

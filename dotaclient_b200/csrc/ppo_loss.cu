@@ -69,6 +69,19 @@
 // valid mask (tools/teacher_bench.py, medians of 200 calls): _masked 206 us, _kl 320 us, teacher alone 295 us, teacher and
 // KL 441 us, so the 1-CTA combined instantiation costs 121 us more than _kl, about 1 % of the C2 step.  Algorithmic bytes:
 // + 260 / token read for the teacher's rows (946 B / token with one row set, 1,206 B with both, + valid and old value).
+//
+// Behaviour cloning (`dc_ppo_loss_fwd_bwd_bc`, kBc, per-head path): every rollout is a demonstration and the surrogate is
+// replaced by the negative log-likelihood of its actions,
+//   NLL = (1 / T_a) sum_t sum_{h in S_t} -lp[a],   and (1 / T_a)(p(j) - [j == a]) on the legal entries of every row in S_t,
+// in the loop that already writes the row: no extra row reads and no extra exp (KL(onehot(a) || p) is -log p(a), so this is
+// the kTeacher gradient with the teacher's row replaced by the action).  A row of S_t also stages its -lp[a] and whether the
+// arg-max of its masked logits (the lowest index on ties) is a; the token stages whether every row of S_t is right.  Those
+// 11 staging rows are summed in float64 after the others, in the same fixed order, into bc_stats.  The loss pass reads no
+// old_logp and no advantage (the statistics pass still sums the advantages for out[14] / out[15]) and computes no
+// approximate KL or clip fraction (their slots stay 0); the entropy and value terms and the explained variance are the
+// per-head path's.  ptxas (sm_90a, __launch_bounds__(128, 2)): 255 registers, no spills, 0 bytes stack frame, 53.5 KB dynamic
+// + 12.0 KB static shared memory, 2 CTAs per SM (at 3 CTAs per SM, ptxas's 168 registers spill 32 bytes).  Algorithmic
+// bytes: 686 - 24 = 662 per token for the loss pass (+ 1 valid, + 4 old value).
 #include "dc_common.cuh"
 
 namespace {
@@ -122,6 +135,10 @@ constexpr int kTokJoint = kTokRows, kJointStats = 2;
 constexpr int kKlStats = kHeads;
 // teacher only: the same per head for the KL to the teacher's row (after the KL control rows, if any)
 constexpr int kTeachStats = kHeads;
+// behaviour cloning only: per head the NLL of its action row, the token's all-heads-right flag, per head the arg-max flag
+// (the order of bc_stats)
+constexpr int kBcStats = 2 * kHeads + 1;
+static_assert(DC_BC_STATS_SLOTS == 2 + 2 * kHeads, "bc_stats: the NLL, per head, the token accuracy, per head");
 static_assert(2 * kHeads + 3 < DC_PPO_STATS_SLOTS, "stats output too small");
 static_assert(DC_STAT_KL_PENALTY < DC_PPO_STATS_SLOTS, "stats output too small");
 
@@ -141,6 +158,7 @@ struct Workspace {
     unsigned long long first_rev;    // N - (index of the first token that counts); 0 when no token counts
     double st_kl[kKlStats];          // KL control: per head, the sum over its action rows of the exact KL of the row
     double st_teach[kTeachStats];    // teacher: per head, the sum over its action rows of the KL to the teacher's row
+    double st_bc[kBcStats];          // behaviour cloning: the sums of its staging rows (kBcStats above)
 };
 static_assert(sizeof(Workspace) <= DC_PPO_WORKSPACE_BYTES, "workspace too small");
 
@@ -294,12 +312,17 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
 // the head has an action row here) and, with kl_scale = beta / T_a > 0, its gradient joins the dlogits row.
 // kKl, select (logp_out given): the full masked log-prob row overwrites the logits row in the tile, 0 at illegal entries.
 // kTeach, loss: `trow` is the teacher's log-prob row of head H, used as kKl uses `orow` (t_scale = lambda / T_a).
-template <int H, bool kGrad, bool kKl = false, bool kTeach = false>
+// kBc (behaviour cloning, a loss): no surrogate.  A row with an action a (a row of S_t) writes -lp[a] to *nll_out and its
+// arg-max flag to *acc_out, sets bit H of *bc_in (and of *bc_miss when the arg-max is not a), and adds
+// bc_scale (p - [j == a]) to its legal entries, bc_scale = 1 / T_a.
+template <int H, bool kGrad, bool kKl = false, bool kTeach = false, bool kBc = false>
 __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, const uint8_t *arow, float old_lp,
                                            float adv_n, int n_h, float e_clip, float entropy_coef, float &pol_acc,
                                            float &ent_acc, float *kl_out, float *clip_out, float *logp_out,
                                            const float *orow = nullptr, float kl_scale = 0.f, float *kl_row_out = nullptr,
-                                           const float *trow = nullptr, float t_scale = 0.f, float *t_row_out = nullptr) {
+                                           const float *trow = nullptr, float t_scale = 0.f, float *t_row_out = nullptr,
+                                           float bc_scale = 0.f, float *nll_out = nullptr, float *acc_out = nullptr,
+                                           int *bc_in = nullptr, int *bc_miss = nullptr) {
     constexpr int N = head_n(H);
     float l[N], e[N];
     int mask_any = 0, a_idx = -1;
@@ -349,7 +372,24 @@ __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, con
     }
     ent_acc += ent_row;                   // optimizer.py:644-646 (divided by n_actions at the end)
     float g_lp = 0.f;                     // d loss / d logp[a]
-    if (a_idx >= 0) {
+    if (kBc && a_idx >= 0) {
+        float lpa = lp[0];
+        int best = -1;                    // arg-max of the masked logits, the lowest index on ties
+        float lbest = 0.f;
+#pragma unroll
+        for (int j = 0; j < N; ++j) {
+            lpa = (j == a_idx) ? lp[j] : lpa;
+            if (mrow[j] && (best < 0 || l[j] > lbest)) {
+                best = j;
+                lbest = l[j];
+            }
+        }
+        *nll_out = -lpa;
+        *acc_out = best == a_idx ? 1.f : 0.f;
+        *bc_in |= 1 << H;
+        if (best != a_idx) *bc_miss |= 1 << H;
+    }
+    if (!kBc && a_idx >= 0) {
         float lpa = lp[0];
 #pragma unroll
         for (int j = 1; j < N; ++j) lpa = (j == a_idx) ? lp[j] : lpa;
@@ -387,6 +427,7 @@ __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, con
                 t_row += pt * (lt - lp[j]);
                 if (t_scale > 0.f) g += t_scale * (p[j] - pt);
             }
+            if (kBc && a_idx >= 0 && mrow[j]) g += bc_scale * (j == a_idx ? p[j] - 1.0f : p[j]);   // -log p(a) / T_a
             lrow[j] = g;
         }
         if (kKl && a_idx >= 0) *kl_row_out = kl_row;
@@ -496,10 +537,12 @@ __device__ __forceinline__ void joint_head_bwd(float *lrow, const uint8_t *mrow,
 // kSelectOnly && kKl: the selected log-probs and, written through hp.dlogits (column ranges of the [N, 65] rows), every
 // head's masked log-prob row.  !kSelectOnly && kKl: the loss with the KL penalty (old_rows, kl_out).  kTeacher (a loss):
 // the teacher term (teacher_rows, *teacher_coef, teacher_stats), with or without kKl.
+// kBc (a loss, per-head path, neither kKl nor kTeacher): behaviour cloning, the NLL of the actions in place of the surrogate
+// (bc_stats); old_logp and the advantages are not read.
 // kTeacher asks for 2 CTAs per SM, which lets ptxas use more than the ~168 registers it picks otherwise and spill nothing;
 // the other instantiations keep ptxas's default (minBlocks 0 is "not given"), so their code is unchanged.
-template <bool kSelectOnly, bool kJoint, bool kKl = false, bool kTeacher = false>
-__global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadPtrs hp, const float *__restrict__ old_logp,
+template <bool kSelectOnly, bool kJoint, bool kKl = false, bool kTeacher = false, bool kBc = false>
+__global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_kernel(HeadPtrs hp, const float *__restrict__ old_logp,
                                                           const float *__restrict__ adv_raw,
                                                           const float *__restrict__ ret,
                                                           const float *__restrict__ value, int64_t N, float e_clip,
@@ -513,16 +556,20 @@ __global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadP
                                                           const float *__restrict__ old_rows, float *__restrict__ kl_out,
                                                           const float *__restrict__ teacher_rows,
                                                           const double *__restrict__ teacher_coef,
-                                                          float *__restrict__ teacher_stats) {
+                                                          float *__restrict__ teacher_stats,
+                                                          float *__restrict__ bc_stats) {
     static_assert(!(kSelectOnly && kJoint), "the joint ratio is a loss");
     static_assert(!(kSelectOnly && kTeacher), "the teacher term is a loss");
+    static_assert(!kBc || !(kSelectOnly || kJoint || kKl || kTeacher), "behaviour cloning is a per-head loss of its own");
     constexpr bool kKlLoss = kKl && !kSelectOnly;
     constexpr int kTokKl = kTokRows + (kJoint ? kJointStats : 0);
     constexpr int kTokTeach = kTokKl + (kKlLoss ? kKlStats : 0);
-    constexpr int kRows = kTokTeach + (kTeacher ? kTeachStats : 0);
+    constexpr int kTokBc = kTokTeach + (kTeacher ? kTeachStats : 0);
+    constexpr int kRows = kTokBc + (kBc ? kBcStats : 0);
     constexpr int kSumKl = kStats + (kJoint ? kJointStats : 0);
     constexpr int kSumTeach = kSumKl + (kKlLoss ? kKlStats : 0);
-    constexpr int kSums = kSumTeach + (kTeacher ? kTeachStats : 0);
+    constexpr int kSumBc = kSumTeach + (kTeacher ? kTeachStats : 0);
+    constexpr int kSums = kSumBc + (kBc ? kBcStats : 0);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *s_logits = reinterpret_cast<float *>(smem_raw);
     float *s_old = s_logits + kLogitFloats;
@@ -561,7 +608,7 @@ __global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadP
     stage_rows_f32<9, 9>(s_logits + logit_off(2), hp.logits[2], hp.ld_l[2], t0, count);
     stage_rows_f32<40, 41>(s_logits + logit_off(3), hp.logits[3], hp.ld_l[3], t0, count);
     stage_rows_f32<3, 3>(s_logits + logit_off(4), hp.logits[4], hp.ld_l[4], t0, count);
-    if (!kSelectOnly) stage_rows_f32<5, 5>(s_old, old_logp, 5, t0, count);
+    if (!kSelectOnly && !kBc) stage_rows_f32<5, 5>(s_old, old_logp, 5, t0, count);
 #pragma unroll
     for (int h = 0; h < kHeads; ++h) {
         stage_bytes(s_mask + byte_off(h), hp.masks[h] + t0 * head_n(h), count * head_n(h));
@@ -590,7 +637,7 @@ __global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadP
     if (!kSelectOnly) {
 #pragma unroll
         for (int h = 0; h < kHeads; ++h) cnt[h] = ws->cnt[h];
-        if (use) {
+        if (use && !kBc) {
             // (advantage - mean) / (std + eps), fp32 like optimizer.py:588
             adv_n = __fdiv_rn(__fsub_rn(adv_raw[t0 + t], ws->adv_mean), __fadd_rn(ws->adv_std, 1.1920928955078125e-07f));
         }
@@ -611,6 +658,14 @@ __global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadP
         if (n_a) t_scale = t_coef / (float)n_a;
     }
     float *const s_t_tok = kTeacher ? &s_tok[0][0] + kTokTeach * kTile + t : nullptr;
+    // behaviour cloning: 1 / T_a, and this token's entry in the staging row of head 0's NLL (the rows of kBcStats follow)
+    float bc_scale = 0.f;
+    if (kBc) {
+        const unsigned long long n_a = ws->n_joint;
+        if (n_a) bc_scale = 1.0f / (float)n_a;
+    }
+    float *const s_bc_tok = kBc ? &s_tok[0][0] + kTokBc * kTile + t : nullptr;
+    int bc_in = 0, bc_miss = 0;       // behaviour cloning: the heads of S_t, and those whose arg-max is not the action
     if (live) {
         float lp_sel[kHeads];
         if constexpr (kJoint) {
@@ -651,17 +706,22 @@ __global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadP
 #undef DC_JHEAD
         } else {
 #define DC_HEAD(H)                                                                                              \
-        head_token<H, true, kKl, kTeacher>(s_logits + logit_off(H) + t * head_pitch(H),                          \
+        head_token<H, true, kKl, kTeacher, kBc>(s_logits + logit_off(H) + t * head_pitch(H),                     \
                                  s_mask + byte_off(H) + t * head_n(H),                                               \
-                                 s_act + byte_off(H) + t * head_n(H), kSelectOnly ? 0.f : s_old[t * 5 + H], adv_n,   \
+                                 s_act + byte_off(H) + t * head_n(H),                                                \
+                                 (kSelectOnly || kBc) ? 0.f : s_old[t * 5 + H], adv_n,                               \
                                  use ? cnt[H] : 0, e_clip, entropy_coef, pol[H], ent[H], &s_tok[kStKl + H][t],       \
                                  &s_tok[kStClip + H][t], kSelectOnly ? &lp_sel[H] : nullptr,                         \
                                  s_orows + t * kRowFloats + row_col(H), kl_scale,                                    \
                                  kKlLoss ? s_kl_tok + (H) * kTile : nullptr,                                         \
                                  s_trows + t * kRowFloats + row_col(H), t_scale,                                     \
-                                 kTeacher ? s_t_tok + (H) * kTile : nullptr);
+                                 kTeacher ? s_t_tok + (H) * kTile : nullptr, bc_scale,                               \
+                                 kBc ? s_bc_tok + (H) * kTile : nullptr,                                             \
+                                 kBc ? s_bc_tok + (kHeads + 1 + (H)) * kTile : nullptr, &bc_in, &bc_miss);
         DC_HEAD(0) DC_HEAD(1) DC_HEAD(2) DC_HEAD(3) DC_HEAD(4)
 #undef DC_HEAD
+            // behaviour cloning: the token is right when every head of S_t is (counted over the T_a tokens)
+            if (kBc && bc_in) s_bc_tok[kHeads * kTile] = bc_miss ? 0.f : 1.f;
         }
         if (kSelectOnly) {
 #pragma unroll
@@ -720,10 +780,11 @@ __global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadP
         sums[2 * kHeads] = block_sum(vl, s_red);
         // the diagnostics (s_tok is complete: block_sum synchronised the block): one warp per sum, in float64.  KL control
         // and the teacher need their sums for kl_out / teacher_stats whether or not the diagnostics are asked for.
-        if (stats || kKlLoss || kTeacher) {
+        if (stats || kKlLoss || kTeacher || kBc) {
             const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
             for (int i = warp; i < kSums; i += kTile / 32) {
-                const int row = (kTeacher && i >= kSumTeach) ? kTokTeach + (i - kSumTeach)
+                const int row = (kBc && i >= kSumBc) ? kTokBc + (i - kSumBc)
+                              : (kTeacher && i >= kSumTeach) ? kTokTeach + (i - kSumTeach)
                               : (kKlLoss && i >= kSumKl) ? kTokKl + (i - kSumKl)
                               : (kJoint && i >= kStats) ? kTokJoint + (i - kStats) : (i < kStD ? i : (i < kStR ? kTokD : kTokR));
                 const bool square = i == kStD2 || i == kStR2;
@@ -760,6 +821,10 @@ __global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadP
                 for (int i = 0; i < kTeachStats; ++i)
                     if (s_st[kSumTeach + i] != 0.0) atomicAdd(&ws->st_teach[i], s_st[kSumTeach + i]);
             }
+            if constexpr (kBc) {
+                for (int i = 0; i < kBcStats; ++i)
+                    if (s_st[kSumBc + i] != 0.0) atomicAdd(&ws->st_bc[i], s_st[kSumBc + i]);
+            }
             __threadfence();
             s_last = atomicAdd(&ws->ticket_loss, 1u) == gridDim.x - 1;
         }
@@ -770,7 +835,7 @@ __global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadP
             float policy = 0.f, entropy = 0.f;
             for (int h = 0; h < kHeads; ++h) {
                 const int n = w->cnt[h];
-                const float pl = (!kJoint && n) ? (float)(-w->pol[h] / (double)n) : 0.f;     // optimizer.py:641 / :628
+                const float pl = (!kJoint && !kBc && n) ? (float)(-w->pol[h] / (double)n) : 0.f;   // optimizer.py:641 / :628
                 const float en = n ? (float)(w->ent[h] / (double)n) : 0.f;      // optimizer.py:646 / :629
                 out[9 + h] = pl;
                 out[4 + h] = en;
@@ -780,6 +845,22 @@ __global__ void __launch_bounds__(kTile, kTeacher ? 2 : 0) ppo_loss_kernel(HeadP
             if constexpr (kJoint) {                                             // -(1/T_a) sum_t min(r A, clip(r) A); 0 if T_a = 0
                 const unsigned long long n_a = w->n_joint;
                 policy = n_a ? (float)(-w->pol[0] / (double)n_a) : 0.f;
+            } else if constexpr (kBc) {
+                // NLL = (1 / T_a) sum_t sum_{h in S_t} -log p(a_h) (0 when T_a = 0); out[9 + h] is head h's share of it
+                const unsigned long long n_a = w->n_joint;
+                double nll_sum = 0.0;
+                for (int h = 0; h < kHeads; ++h) {
+                    nll_sum += w->st_bc[h];
+                    out[9 + h] = n_a ? (float)(w->st_bc[h] / (double)n_a) : 0.f;
+                }
+                policy = n_a ? (float)(nll_sum / (double)n_a) : 0.f;
+                bc_stats[0] = policy;
+                bc_stats[1 + kHeads] = n_a ? (float)(w->st_bc[kHeads] / (double)n_a) : 0.f;
+                for (int h = 0; h < kHeads; ++h) {      // over the head's action rows; 0 for a head without any
+                    const int n = w->cnt[h];
+                    bc_stats[1 + h] = n ? (float)(w->st_bc[h] / (double)n) : 0.f;
+                    bc_stats[2 + kHeads + h] = n ? (float)(w->st_bc[kHeads + 1 + h] / (double)n) : 0.f;
+                }
             } else {
                 policy /= (float)kHeads;                                        // optimizer.py:650
             }
@@ -879,9 +960,10 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
                     float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions, void *workspace,
                     dc_stream_t stream, bool joint = false, const float *old_rows = nullptr, float *kl_out = nullptr,
                     const float *teacher_rows = nullptr, const double *teacher_coef = nullptr,
-                    float *teacher_stats = nullptr) {
+                    float *teacher_stats = nullptr, float *bc_stats = nullptr) {
     DC_REQUIRE(N > 0, DC_EINVAL, "dc_ppo_loss_fwd_bwd: N=%lld", (long long)N);
-    DC_REQUIRE(check_heads(logits, masks, actions) && old_logp && adv_raw && ret && value && dvalue && out &&
+    // behaviour cloning (bc_stats given) reads no old_logp
+    DC_REQUIRE(check_heads(logits, masks, actions) && (old_logp || bc_stats) && adv_raw && ret && value && dvalue && out &&
                    n_actions && workspace && ld_logits && ld_dlogits, DC_EINVAL, "dc_ppo_loss_fwd_bwd: null pointer");
     HeadPtrs hp;
     for (int h = 0; h < kHeads; ++h) {
@@ -896,6 +978,17 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
     Workspace *ws = reinterpret_cast<Workspace *>(workspace);
     DC_CUDA(cudaMemsetAsync(ws, 0, sizeof(Workspace), st));
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
+    if (bc_stats) {             // behaviour cloning: the statistics pass counts T_a
+        ppo_stats_kernel<true><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
+        DC_LAUNCH_OK();
+        auto kern = ppo_loss_kernel<false, false, false, false, true>;
+        DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
+        kern<<<blocks, kTile, kSmemBytes, st>>>(hp, nullptr, adv_raw, ret, value, N, e_clip, entropy_coef, vf_coef, old_value,
+                                                valid, hparams, dvalue, out, stats, ws, nullptr, nullptr, nullptr, nullptr,
+                                                nullptr, nullptr, bc_stats);
+        DC_LAUNCH_OK();
+        return DC_OK;
+    }
     if (teacher_rows) {         // the teacher term, with or without KL control, either ratio mode; T_a as below
         ppo_stats_kernel<true><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
         DC_LAUNCH_OK();
@@ -905,7 +998,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
         DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<blocks, kTile, smem, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip, entropy_coef, vf_coef, old_value,
                                           valid, hparams, dvalue, out, stats, ws, nullptr, old_rows, kl_out, teacher_rows,
-                                          teacher_coef, teacher_stats);
+                                          teacher_coef, teacher_stats, nullptr);
         DC_LAUNCH_OK();
         return DC_OK;
     }
@@ -916,7 +1009,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
         DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytesKl));
         kern<<<blocks, kTile, kSmemBytesKl, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip, entropy_coef, vf_coef, old_value,
                                                   valid, hparams, dvalue, out, stats, ws, nullptr, old_rows, kl_out,
-                                                  nullptr, nullptr, nullptr);
+                                                  nullptr, nullptr, nullptr, nullptr);
         DC_LAUNCH_OK();
         return DC_OK;
     }
@@ -928,7 +1021,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
         ppo_loss_kernel<false, true><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
                                                                         entropy_coef, vf_coef, old_value, valid, hparams,
                                                                         dvalue, out, stats, ws, nullptr, nullptr, nullptr, nullptr,
-                                                                        nullptr, nullptr);
+                                                                        nullptr, nullptr, nullptr);
         DC_LAUNCH_OK();
         return DC_OK;
     }
@@ -940,7 +1033,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
     ppo_loss_kernel<false, false><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
                                                                      entropy_coef, vf_coef, old_value, valid, hparams,
                                                                      dvalue, out, stats, ws, nullptr, nullptr, nullptr, nullptr,
-                                                                        nullptr, nullptr);
+                                                                        nullptr, nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -1028,7 +1121,7 @@ extern "C" int dc_selected_logp(const float *const logits[DC_NUM_HEADS], const u
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
     ppo_loss_kernel<true, false><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
         hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-        nullptr, logp_out, nullptr, nullptr, nullptr, nullptr, nullptr);
+        nullptr, logp_out, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -1051,7 +1144,7 @@ extern "C" int dc_selected_logp_rows(const float *const logits[DC_NUM_HEADS], co
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
     ppo_loss_kernel<true, false, true><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
         hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-        nullptr, logp_out, nullptr, nullptr, nullptr, nullptr, nullptr);
+        nullptr, logp_out, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -1088,4 +1181,18 @@ extern "C" int dc_ppo_loss_fwd_bwd_teacher(const float *const logits[DC_NUM_HEAD
                            N, 0.f, 0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions,
                            workspace, stream, joint != 0, old_log_probs, kl_out, teacher_log_probs, teacher_coef,
                            teacher_stats);
+}
+
+extern "C" int dc_ppo_loss_fwd_bwd_bc(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                                      const uint8_t *const masks[DC_NUM_HEADS], const uint8_t *const actions[DC_NUM_HEADS],
+                                      const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                                      const float *old_value, const uint8_t *valid, int64_t N, const double *hparams,
+                                      float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                                      float *dvalue, int64_t ld_dvalue, float *out, float *stats, float *bc_stats,
+                                      int32_t *n_actions, void *workspace, dc_stream_t stream) {
+    DC_REQUIRE(hparams, DC_EINVAL, "dc_ppo_loss_fwd_bwd_bc: null hyper-parameter block");
+    DC_REQUIRE(bc_stats, DC_EINVAL, "dc_ppo_loss_fwd_bwd_bc: null bc_stats");
+    return launch_ppo_loss(logits, ld_logits, masks, actions, nullptr, adv_raw, ret, value, ld_value, old_value, valid, N,
+                           0.f, 0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions, workspace,
+                           stream, false, nullptr, nullptr, nullptr, nullptr, nullptr, bc_stats);
 }

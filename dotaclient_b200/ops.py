@@ -854,13 +854,35 @@ def _teacher_args(teacher_log_probs, teacher_coef, teacher_stats, N, dev):
     return teacher_log_probs, teacher_stats
 
 
+def _bc_args(bc_stats, dev, joint, old_log_probs, teacher_log_probs):
+    """Checks the extra operand of ``dc_ppo_loss_fwd_bwd_bc``: ``bc_stats`` (``_lib.BC_STATS_SLOTS`` fp32, allocated when
+    None), and that nothing that belongs to the policy-gradient objective was asked for with it."""
+    if joint or old_log_probs is not None or teacher_log_probs is not None:
+        raise ValueError("behaviour cloning has no PPO ratio, KL penalty or teacher term (joint / old_log_probs / "
+                         "teacher_log_probs)")
+    _need_cuda(bc_stats)
+    if bc_stats is None:
+        bc_stats = torch.empty(_lib.BC_STATS_SLOTS, dtype=torch.float32, device=dev)
+    assert bc_stats.dtype == torch.float32 and bc_stats.numel() == _lib.BC_STATS_SLOTS and bc_stats.is_contiguous()
+    return bc_stats
+
+
 def _ppo_dev_call(lib, lptr, ld_l, masks, actions, old_logp, adv_raw, ret, value_ptr, ld_v, old_value, valid, N, hparams,
                   dptr, ld_d, dvalue_ptr, ld_dv, out, stats, n_actions, ws, joint=False, old_log_probs=None, kl_out=None,
-                  teacher_log_probs=None, teacher_coef=None, teacher_stats=None):
+                  teacher_log_probs=None, teacher_coef=None, teacher_stats=None, bc_stats=None):
     """``dc_ppo_loss_fwd_bwd_dev``, or ``dc_ppo_loss_fwd_bwd_masked`` when a valid mask is given, or
     ``dc_ppo_loss_fwd_bwd_joint`` (valid or not) when ``joint``; ``dc_ppo_loss_fwd_bwd_kl`` (either ratio mode) when
     ``old_log_probs`` is given; ``dc_ppo_loss_fwd_bwd_teacher`` (either ratio mode, old rows or not) when
-    ``teacher_log_probs`` is given."""
+    ``teacher_log_probs`` is given; ``dc_ppo_loss_fwd_bwd_bc`` (valid or not; ``old_logp`` unused) when ``bc_stats`` is
+    given."""
+    if bc_stats is not None:
+        with PROFILE.span("ppo_loss", 2):
+            _lib.check(lib.dc_ppo_loss_fwd_bwd_bc(
+                lptr, ld_l, _lib.ptr5(masks), _lib.ptr5(actions), adv_raw.data_ptr(), ret.data_ptr(), value_ptr, ld_v,
+                _lib.ptr(old_value), _lib.ptr(valid), N, hparams.data_ptr(), dptr, ld_d, dvalue_ptr, ld_dv, out.data_ptr(),
+                stats.data_ptr(), bc_stats.data_ptr(), n_actions.data_ptr(), ws.data_ptr(), _lib.stream_ptr()),
+                "dc_ppo_loss_fwd_bwd_bc")
+        return
     head = (lptr, ld_l, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(),
             value_ptr, ld_v, _lib.ptr(old_value))
     tail = (N, hparams.data_ptr(), dptr, ld_d, dvalue_ptr, ld_dv, out.data_ptr(), stats.data_ptr(), n_actions.data_ptr(),
@@ -890,7 +912,7 @@ def _ppo_dev_call(lib, lptr, ld_l, masks, actions, old_logp, adv_raw, ret, value
 
 def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_clip, entropy_coef, vf_coef, hparams=None,
                      old_value=None, stats=None, valid=None, joint=False, old_log_probs=None, kl_out=None,
-                     teacher_log_probs=None, teacher_coef=None, teacher_stats=None):
+                     teacher_log_probs=None, teacher_coef=None, teacher_stats=None, bc=False, bc_stats=None):
     """Fused PPO loss + gradients (``optimizer.py:587-589,621-665`` and their backward).
 
     logits/masks/actions: sequences of 5 tensors [..., n_h] in HEAD_KEYS order (any leading dims,
@@ -913,6 +935,10 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     masked log-prob rows; the loss then adds ``teacher_coef * KL(teacher || policy)`` (``dc_ppo_loss_fwd_bwd_teacher``,
     either ratio mode, with or without ``old_log_probs``), and ``teacher_stats`` (``_lib.TEACHER_STATS_SLOTS`` fp32,
     allocated when None) receives the KL, the KL per head and the term; the result then gains it as a sixth element.
+    ``bc`` (needs ``hparams``): behaviour cloning, the negative log-likelihood of the actions in place of the PPO surrogate
+    (``dc_ppo_loss_fwd_bwd_bc``, with or without ``valid``; ``old_logp`` may be None and is not read); ``bc_stats``
+    (``_lib.BC_STATS_SLOTS`` fp32, allocated when None) receives the NLL, per head, the token accuracy and per head, and the
+    result gains it as a sixth element.
     """
     logits = [_f32c(l.detach()) for l in logits]
     _need_cuda(*logits)
@@ -922,8 +948,9 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     for h in range(5):
         assert logits[h].numel() == N * HEAD_SIZES[h] and masks[h].numel() == N * HEAD_SIZES[h] \
             and actions[h].numel() == N * HEAD_SIZES[h], "head %d shape mismatch" % h
-    old_logp, adv_raw, ret, value = _f32c(old_logp), _f32c(adv_raw), _f32c(ret), _f32c(value.detach())
-    assert old_logp.numel() == N * 5 and adv_raw.numel() == N and ret.numel() == N and value.numel() == N
+    old_logp = None if bc else _f32c(old_logp)
+    adv_raw, ret, value = _f32c(adv_raw), _f32c(ret), _f32c(value.detach())
+    assert (bc or old_logp.numel() == N * 5) and adv_raw.numel() == N and ret.numel() == N and value.numel() == N
     dev = logits[0].device
     dlogits = [torch.empty_like(l) for l in logits]
     dvalue = torch.empty_like(value)
@@ -932,10 +959,13 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     ws = torch.empty(_lib.PPO_WORKSPACE_BYTES, dtype=torch.uint8, device=dev)
     lib = _lib.load()
     teacher = teacher_log_probs is not None
-    if hparams is not None or valid is not None or joint or old_log_probs is not None or teacher:
-        if (old_log_probs is not None or teacher) and hparams is None:
-            raise ValueError("the KL penalty and the teacher term need the device hyper-parameter block (hparams=)")
+    if hparams is not None or valid is not None or joint or old_log_probs is not None or teacher or bc:
+        if (old_log_probs is not None or teacher or bc) and hparams is None:
+            raise ValueError("the KL penalty, the teacher term and behaviour cloning need the device hyper-parameter "
+                             "block (hparams=)")
         old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid, joint)
+        if bc:
+            bc_stats = _bc_args(bc_stats, dev, joint, old_log_probs, teacher_log_probs)
         if old_log_probs is not None:
             old_log_probs = _kl_args(old_log_probs, kl_out, N)
         if teacher:
@@ -943,9 +973,9 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
         ld = (ctypes.c_int64 * 5)(*HEAD_SIZES)
         _ppo_dev_call(lib, _lib.ptr5(logits), ld, masks, actions, old_logp, adv_raw, ret, value.data_ptr(), 1, old_value,
                       valid, N, hparams, _lib.ptr5(dlogits), ld, dvalue.data_ptr(), 1, out, stats, n_actions, ws, joint,
-                      old_log_probs, kl_out, teacher_log_probs, teacher_coef, teacher_stats)
+                      old_log_probs, kl_out, teacher_log_probs, teacher_coef, teacher_stats, bc_stats if bc else None)
         res = (out, n_actions, dlogits, dvalue, stats)
-        return res + (teacher_stats,) if teacher else res
+        return res + (teacher_stats,) if teacher else res + (bc_stats,) if bc else res
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd(_lib.ptr5(logits), _lib.ptr5(masks), _lib.ptr5(actions),
                                            old_logp.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(), value.data_ptr(),
@@ -1218,15 +1248,15 @@ def value_heads_loss(packed, d_packed, ret, hparams, out, head_stats, old_value=
 
 def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e_clip, entropy_coef, vf_coef, hparams=None,
                     old_value=None, stats=None, valid=None, joint=False, old_log_probs=None, kl_out=None,
-                    teacher_log_probs=None, teacher_coef=None, teacher_stats=None):
+                    teacher_log_probs=None, teacher_coef=None, teacher_stats=None, bc=False, bc_stats=None):
     """Fused PPO loss where the four small heads and the value head are column ranges of ONE packed ``[N,128]``
     tensor-core GEMM output (``PACK_COLS``) and the target-unit logits are a separate ``[N,40]`` tensor.
 
     Returns (out[16], n_actions[5], d_packed [N,128], d_logits_tu [N,40]): the gradients go straight back into the two
     producers, so no slice/cat kernels run and the five tiny K=131072 weight-gradient GEMMs become one wgmma wgrad.
     ``hparams`` / ``old_value`` / ``stats`` / ``valid`` / ``joint`` / ``old_log_probs`` / ``kl_out`` /
-    ``teacher_log_probs`` / ``teacher_coef`` / ``teacher_stats``: as ``ppo_loss_fwd_bwd`` (the fifth element of the result
-    is then ``stats``, and with a teacher the sixth ``teacher_stats``).
+    ``teacher_log_probs`` / ``teacher_coef`` / ``teacher_stats`` / ``bc`` / ``bc_stats``: as ``ppo_loss_fwd_bwd`` (the fifth
+    element of the result is then ``stats``, and with a teacher the sixth ``teacher_stats``, with ``bc`` ``bc_stats``).
     """
     _need_cuda(packed, logits_tu)
     p2 = _f32c(packed.detach()).reshape(-1, PACK_WIDTH)
@@ -1234,7 +1264,8 @@ def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e
     tu = _f32c(logits_tu.detach()).reshape(N, 40)
     masks = [_u8(m) for m in masks]
     actions = [_u8(a) for a in actions]
-    old_logp, adv_raw, ret = _f32c(old_logp), _f32c(adv_raw), _f32c(ret)
+    old_logp = None if bc else _f32c(old_logp)
+    adv_raw, ret = _f32c(adv_raw), _f32c(ret)
     dev = p2.device
     d_packed = torch.zeros_like(p2)            # the 102 padding columns must carry a zero gradient
     d_tu = torch.empty_like(tu)
@@ -1250,19 +1281,22 @@ def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e
     ld = (c.c_int64 * 5)(PACK_WIDTH, PACK_WIDTH, PACK_WIDTH, 40, PACK_WIDTH)
     lib = _lib.load()
     teacher = teacher_log_probs is not None
-    if hparams is not None or valid is not None or joint or old_log_probs is not None or teacher:
-        if (old_log_probs is not None or teacher) and hparams is None:
-            raise ValueError("the KL penalty and the teacher term need the device hyper-parameter block (hparams=)")
+    if hparams is not None or valid is not None or joint or old_log_probs is not None or teacher or bc:
+        if (old_log_probs is not None or teacher or bc) and hparams is None:
+            raise ValueError("the KL penalty, the teacher term and behaviour cloning need the device hyper-parameter "
+                             "block (hparams=)")
         old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid, joint)
+        if bc:
+            bc_stats = _bc_args(bc_stats, dev, joint, old_log_probs, teacher_log_probs)
         if old_log_probs is not None:
             old_log_probs = _kl_args(old_log_probs, kl_out, N)
         if teacher:
             teacher_log_probs, teacher_stats = _teacher_args(teacher_log_probs, teacher_coef, teacher_stats, N, dev)
         _ppo_dev_call(lib, lptr, ld, masks, actions, old_logp, adv_raw, ret, col(p2, "value"), PACK_WIDTH, old_value, valid,
                       N, hparams, dptr, ld, col(d_packed, "value"), PACK_WIDTH, out, stats, n_actions, ws, joint,
-                      old_log_probs, kl_out, teacher_log_probs, teacher_coef, teacher_stats)
+                      old_log_probs, kl_out, teacher_log_probs, teacher_coef, teacher_stats, bc_stats if bc else None)
         res = (out, n_actions, d_packed.view_as(packed), d_tu.view_as(logits_tu), stats)
-        return res + (teacher_stats,) if teacher else res
+        return res + (teacher_stats,) if teacher else res + (bc_stats,) if bc else res
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd_strided(lptr, ld, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(),
                                                    adv_raw.data_ptr(), ret.data_ptr(), col(p2, "value"), PACK_WIDTH, N,

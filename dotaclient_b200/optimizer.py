@@ -465,6 +465,11 @@ ADVANTAGE_ESTIMATORS = ('gae', 'vtrace')
 # 'per_head': the reference's objective, one clipped ratio per action head; 'joint': one clipped ratio per step, of the
 # whole hierarchical action (the product of the sampled heads' probabilities)
 POLICY_RATIOS = ('per_head', 'joint')
+# 'ppo': the reference's objective, the clipped surrogate on the batch's advantages; 'bc': behaviour cloning, every rollout
+# is a demonstration and the policy term is the negative log-likelihood of its actions (supervised pretraining)
+OBJECTIVES = ('ppo', 'bc')
+# the heads Policy.select_actions samples after each enum value (0 none, 1 move, 2 attack, 3 ability)
+ENUM_FOLLOWS = {0: (), 1: ('x', 'y'), 2: ('target_unit',), 3: ('ability',)}
 
 
 def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=None, *, advantage_estimator='gae',
@@ -472,7 +477,7 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
                        policy_ratio='per_head', value_norm=False, value_norm_decay=0.99, kl_coef=0.0, kl_target=None,
                        kl_stop=None, recompute_advantages=False, recompute_states=False, value_heads=None,
                        value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None,
-                       upgo_coef=0.0):
+                       upgo_coef=0.0, objective='ppo'):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
     vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool,
@@ -480,8 +485,9 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
     and 0 <= value_norm_decay < 1, finite kl_coef >= 0, kl_target None or finite > 0 (and then kl_coef > 0), kl_stop None
     or finite > 0, recompute_advantages and recompute_states bools, value_heads / value_gammas as ``value_head_groups``
     checks them (value heads refuse V-trace and value_norm), finite teacher_coef >= 0 and teacher_anneal_iterations None
-    or an int >= 1, both left at their defaults without a teacher_model, and upgo_coef as ``check_upgo_coef`` checks it.
-    NaN fails every check."""
+    or an int >= 1, both left at their defaults without a teacher_model, upgo_coef as ``check_upgo_coef`` checks it, and
+    objective one of ``OBJECTIVES``; 'bc' refuses what acts only on the policy-gradient term or needs a behaviour policy
+    (V-trace, the joint ratio, KL control, a teacher, UPGO).  NaN fails every check."""
     if not isinstance(recompute_states, bool):
         raise ValueError("recompute_states=%r: must be True or False" % (recompute_states,))
     if not isinstance(recompute_advantages, bool):
@@ -551,6 +557,22 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
         raise ValueError("value_heads with value_norm=True: PopArt would need one set of statistics per head and a "
                          "per-row rescale of the value head, which is not implemented")
     check_upgo_coef(upgo_coef, value_heads)
+    if not isinstance(objective, str) or objective not in OBJECTIVES:
+        raise ValueError("objective=%r: must be one of %s" % (objective, ", ".join(OBJECTIVES)))
+    if objective == 'bc':
+        refused = [("advantage_estimator='vtrace'", advantage_estimator == 'vtrace',
+                    "V-trace corrects for a behaviour policy, and a demonstration has none"),
+                   ("policy_ratio='joint'", policy_ratio == 'joint', "there is no PPO ratio to clip"),
+                   ("kl_coef=%r" % (kl_coef,), float(kl_coef) > 0.0, "there is no prep-time policy to stay close to"),
+                   ("kl_target=%r" % (kl_target,), kl_target is not None, "there is no KL penalty to adapt"),
+                   ("kl_stop=%r" % (kl_stop,), kl_stop is not None, "there is no prep-time policy to stop at"),
+                   ("teacher_model=%r" % (teacher_model,), teacher_model is not None,
+                    "the demonstrations are the teacher; run the teacher term with objective='ppo'"),
+                   ("upgo_coef=%r" % (upgo_coef,), float(upgo_coef) > 0.0, "UPGO changes the advantages, which the "
+                    "behaviour-cloning loss does not read")]
+        for what, bad, why in refused:
+            if bad:
+                raise ValueError("%s with objective='bc': %s" % (what, why))
 
 
 def check_upgo_coef(upgo_coef, value_heads=None):
@@ -996,6 +1018,42 @@ def check_behaviour_logp(datas):
                              % (who, float(blp[t, h]), t, ops.HEAD_KEYS[h]))
 
 
+def check_demonstrations(datas):
+    """Raises ``ValueError``, naming the rollout's ``game_id`` / ``player_id``, the step and the head, when a demonstration's
+    action rows cannot be the log-likelihood's targets: a row with more than one entry set, a set entry that the step's
+    mask makes illegal (its log-probability is -inf), or rows that do not follow the hierarchy ``Policy.select_actions``
+    samples (one enum row; enum 1 -> x and y, 2 -> target_unit, 3 -> ability, 0 -> none; no other head has a row).  The
+    first such step is reported.  Runs on the host before anything is uploaded."""
+    keys = ops.HEAD_KEYS
+    for d in datas:
+        who = "rollout game_id=%r player_id=%r" % (d.get('game_id'), d.get('player_id'))
+        L = int(d['rewards'].shape[0])
+        acts = {k: torch.as_tensor(d['actions'][k]).reshape(L, -1).bool() for k in keys}
+        masks = {k: torch.as_tensor(d['masks'][k]).reshape(L, -1).bool() for k in keys}
+        enum = acts['enum']
+        kind = torch.where(enum.any(dim=1), enum.int().argmax(dim=1), torch.full((L,), -1))
+        found = []                                      # (step, head index, message) of the first failure of each check
+        for h, k in enumerate(keys):
+            checks = [(acts[k].sum(dim=1) > 1, "its action row has more than one entry set"),
+                      ((acts[k] & ~masks[k]).any(dim=1), "its action is illegal under the step's mask")]
+            if k == 'enum':
+                checks.append((kind < 0, "there is no enum row; every step of a demonstration takes an enum action"))
+            else:
+                want = torch.zeros(L, dtype=torch.bool)
+                for e, follow in ENUM_FOLLOWS.items():
+                    if k in follow:
+                        want |= kind == e
+                has = acts[k].any(dim=1)
+                checks.append((has & ~want, "it has an action row, which the step's enum action does not sample"))
+                checks.append((want & ~has, "it has no action row, which the step's enum action samples"))
+            for bad, why in checks:
+                if bool(bad.any()):
+                    t = int(bad.nonzero()[0])
+                    found.append((t, h, "%s: step %d, head %r (enum %d): %s" % (who, t, k, int(kind[t]), why)))
+        if found:
+            raise ValueError("demonstration " + min(found)[2])
+
+
 def check_continuation(datas, cell, num_layers, hidden_size):
     """Raises ``ValueError``, naming the rollout's ``game_id`` / ``player_id``, when one of the optional keys of a rollout
     cut from a longer game is malformed: an ``'initial_hidden'`` that is not the structure ``Policy.init_hidden()`` returns
@@ -1057,6 +1115,7 @@ class DotaOptimizer:
     # steps of about this many tokens
     REFRESH_CHUNK_TOKENS = 32768
     value_heads, n_value_heads, _vh_shape = None, 1, ()     # set by __init__ (value_heads)
+    objective = 'ppo'                                       # set by __init__
     SPEED_KEY = 'steps per s'
     ADAM_BETAS = (0.9, 0.999)       # torch.optim.Adam defaults (:275)
     ADAM_EPS = 1e-8
@@ -1072,7 +1131,7 @@ class DotaOptimizer:
                  num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False,
                  value_norm_decay=0.99, kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False,
                  recompute_states=False, value_heads=None, value_gammas=None, teacher_model=None, teacher_coef=1.0,
-                 teacher_anneal_iterations=None, upgo_coef=0.0):
+                 teacher_anneal_iterations=None, upgo_coef=0.0, objective='ppo'):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
@@ -1084,8 +1143,12 @@ class DotaOptimizer:
                            kl_stop=kl_stop, recompute_advantages=recompute_advantages, recompute_states=recompute_states,
                            value_heads=value_heads, value_gammas=value_gammas, teacher_model=teacher_model,
                            teacher_coef=teacher_coef, teacher_anneal_iterations=teacher_anneal_iterations,
-                           upgo_coef=upgo_coef)
+                           upgo_coef=upgo_coef, objective=objective)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # 'bc': every rollout is a demonstration (check_demonstrations at prep) and the loss is dc_ppo_loss_fwd_bwd_bc's, the
+        # NLL of the demonstrated actions with the entropy and value terms of 'ppo'.  Fixed per optimizer, like policy_ratio
+        self.objective = objective
+        self.last_bc_stats = None           # NLL, accuracy (and per head) of the last 'bc' step
         # value heads: one critic column per reward group, each with its own discount.  Prep scans every group
         # (gae_scan_heads), the policy trains on the summed advantage, the value loss is dc_value_heads_loss's and the
         # published model holds the heads folded into one row.  None: the reference's single critic, and none of this runs
@@ -1237,13 +1300,16 @@ class DotaOptimizer:
         n_vh = 0 if self.value_heads is None else _lib.VALUE_HEADS_STATS_SLOTS
         # the teacher's statistics (KL, per head, the loss term) come last, read back by the same copy
         n_t = 0 if self.teacher_model is None else _lib.TEACHER_STATS_SLOTS
-        self._result_dev = torch.zeros(self._n_metrics + _lib.PPO_STATS_SLOTS + n_vh + n_t, dtype=torch.float32,
+        # behaviour cloning: its statistics (NLL, accuracy, per head) in the same place (a teacher is refused with it)
+        n_bc = _lib.BC_STATS_SLOTS if objective == 'bc' else 0
+        self._result_dev = torch.zeros(self._n_metrics + _lib.PPO_STATS_SLOTS + n_vh + n_t + n_bc, dtype=torch.float32,
                                        device=self.device)
         self._metrics = self._result_dev[:self._n_metrics]
         self._ppo_stats = self._result_dev[self._n_metrics:self._n_metrics + _lib.PPO_STATS_SLOTS]
         o = self._n_metrics + _lib.PPO_STATS_SLOTS
         self._value_head_stats = self._result_dev[o:o + n_vh] if n_vh else None
         self._teacher_stats = self._result_dev[o + n_vh:] if n_t else None
+        self._bc_stats = self._result_dev[o + n_vh:] if n_bc else None
         self._finish_ws = torch.zeros(_lib.FINISH_WORKSPACE_BYTES, dtype=torch.uint8, device=self.device)
         # learning_rate, e_clip, entropy_coef, vf_coef, MAX_GRAD_NORM and value_clip are read by the step's kernels from this
         # device block, rewritten from the pinned host copy before every step: a captured graph of the step holds the
@@ -1524,6 +1590,8 @@ class DotaOptimizer:
         vtrace = self.advantage_estimator == 'vtrace'
         if vtrace:
             check_behaviour_logp(datas)                # refused before anything is uploaded
+        if self.objective == 'bc':
+            check_demonstrations(datas)                # so is a demonstration whose actions have no log-likelihood
         check_continuation(datas, pol.cell, n_layers, H)
         upgo = self._upgo_coef_now()                   # so is a coefficient assigned outside its domain
         Ls = [int(d['rewards'].shape[0]) for d in datas]
@@ -1924,7 +1992,8 @@ class DotaOptimizer:
         res = host.clone()
         keys = ops.HEAD_KEYS
         self.last_ppo_stats = self._ppo_stats_dict(res[_lib.LOSS_SLOTS + self._n_metrics:].tolist(),
-                                                   joint=self.policy_ratio == 'joint', kl=self.kl_control)
+                                                   joint=self.policy_ratio == 'joint', kl=self.kl_control,
+                                                   bc=self.objective == 'bc')
         if self.value_heads is not None:    # per head: its share of the value loss and its explained variance
             hs = res[_lib.LOSS_SLOTS + self._n_metrics + _lib.PPO_STATS_SLOTS:].tolist()
             for k, name in enumerate(self.value_heads.names):
@@ -1939,6 +2008,13 @@ class DotaOptimizer:
             for h, k in enumerate(keys):
                 self.last_ppo_stats['teacher/kl/' + k] = ts[1 + h]
             self.last_ppo_stats['loss/teacher'] = ts[6]
+        if self.objective == 'bc':      # the NLL of the demonstrations (this rank) and the accuracy of the arg-max, per head
+            bs = res[_lib.LOSS_SLOTS + self._result_dev.numel() - _lib.BC_STATS_SLOTS:].tolist()
+            self.last_bc_stats = {'nll': bs[0], 'accuracy': bs[1 + len(keys)]}
+            for h, k in enumerate(keys):
+                self.last_bc_stats['nll/' + k] = bs[1 + h]
+                self.last_bc_stats['accuracy/' + k] = bs[2 + len(keys) + h]
+            self.last_ppo_stats.update({'bc/' + k: v for k, v in self.last_bc_stats.items() if k != 'nll'})
         if res[_lib.LOSS_SLOTS + 3] != 0:               # :667-669, :678-679 (parameters were left untouched)
             if math.isnan(float(res[0])):
                 raise ValueError('loss={}, policy_loss={}, entropy_loss={}, value_loss={}'.format(
@@ -2006,7 +2082,9 @@ class DotaOptimizer:
             ops.value_head_rescale(head.weight.data, head.bias.data, old, new)
 
     @staticmethod
-    def _ppo_stats_dict(st, joint=False, kl=False):
+    def _ppo_stats_dict(st, joint=False, kl=False, bc=False):
+        if bc:                      # no ratio, so no approximate KL or clip fraction
+            return {'explained_variance': st[_lib.STAT_EXPLAINED_VAR]}
         out = {'approx_kl': st[_lib.STAT_APPROX_KL], 'clip_fraction': st[_lib.STAT_CLIP_FRACTION]}
         for h, k in enumerate(ops.HEAD_KEYS):
             out['approx_kl/' + k] = st[_lib.STAT_APPROX_KL + 1 + h]
@@ -2085,6 +2163,8 @@ class DotaOptimizer:
         # value heads: the PPO loss runs with its value term off (_hparams_dev_ppo); the value target it is handed then
         # feeds only an explained variance that dc_value_heads_loss overwrites, so the advantages stand in for it
         # teacher: the KL term to its rows with the coefficient after the hyper-parameter blocks (_upload_hparams)
+        # bc: the NLL of the demonstrated actions in place of the surrogate (old_logp is not read)
+        bc = self.objective == 'bc'
         out, n_actions, d_packed, d_tu = ops.ppo_loss_packed(
             packed, target_unit, [batch.masks[k] for k in keys], [batch.actions[k] for k in keys],
             batch.old_logp, batch.advantages, batch.advantages if heads else batch.returns, self.e_clip,
@@ -2092,7 +2172,8 @@ class DotaOptimizer:
             stats=self._ppo_stats, valid=valid, joint=self.policy_ratio == 'joint', old_log_probs=old_log_probs,
             kl_out=self.flat.kl_tail, teacher_log_probs=teacher_log_probs,
             teacher_coef=self._teacher_coef_dev if teacher_log_probs is not None else None,
-            teacher_stats=self._teacher_stats if teacher_log_probs is not None else None)[:4]
+            teacher_stats=self._teacher_stats if teacher_log_probs is not None else None, bc=bc,
+            bc_stats=self._bc_stats)[:4]
         if heads:
             ops.value_heads_loss(packed, d_packed, batch.returns, self._hparams_dev, out, self._value_head_stats,
                                  old_value=batch.old_values, valid=valid, stats=self._ppo_stats)
@@ -2494,7 +2575,7 @@ class DotaOptimizer:
             self.SPEED_KEY: n_steps / time_it,                             # :501,505 (environment steps per second)
             'reward_per_sec/sum': subrewards_per_sec.sum(axis=1).sum(),
             'loss/sum': losses['loss'].mean(),
-            'loss/policy': losses['policy_loss'].mean(),
+            'loss/bc' if self.objective == 'bc' else 'loss/policy': losses['policy_loss'].mean(),
             'loss/entropy': losses['entropy_loss'].mean(),
             'loss/value': losses['value_loss'].mean(),
             'entropy': torch.stack(list(entropies.values())).sum(dim=0).mean(),
@@ -2513,7 +2594,7 @@ class DotaOptimizer:
         # measured at the parameters it left unchanged, and its KL is the measurement that stopped the iteration
         for k in ppo_stats[0]:
             if k not in ('kl_all_ranks', 'kl_skipped'):     # value heads: 'loss/value/<name>' next to 'loss/value'
-                metrics[k if k.startswith(('loss/', 'teacher/')) else 'ppo/{}'.format(k)] = \
+                metrics[k if k.startswith(('loss/', 'teacher/', 'bc/')) else 'ppo/{}'.format(k)] = \
                     float(np.mean([s[k] for s in ppo_stats]))
         if self.kl_control:
             # d: the mean over the steps (a skipped one included) of the all-ranks KL, the same number on every rank, so
@@ -2673,7 +2754,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          value_clip=None, advantage_estimator='gae', vtrace_rho_clip=1.0, vtrace_c_clip=1.0, num_minibatches=1,
          mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False, value_norm_decay=0.99,
          kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False, recompute_states=False, value_heads=None,
-         value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None, upgo_coef=0.0):
+         value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None, upgo_coef=0.0,
+         objective='ppo'):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                        mask_padding=mask_padding, pack_sequences=pack_sequences,
@@ -2683,7 +2765,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
                        recompute_states=recompute_states, value_heads=value_heads,
                        value_gammas=value_gammas, teacher_model=teacher_model, teacher_coef=teacher_coef,
                        teacher_anneal_iterations=teacher_anneal_iterations,
-                       upgo_coef=upgo_coef)                                              # before any process-group setup
+                       upgo_coef=upgo_coef, objective=objective)                         # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -2699,7 +2781,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         kl_target=kl_target, kl_stop=kl_stop, recompute_advantages=recompute_advantages,
         recompute_states=recompute_states, value_heads=value_heads, value_gammas=value_gammas,
         teacher_model=teacher_model, teacher_coef=teacher_coef, teacher_anneal_iterations=teacher_anneal_iterations,
-        upgo_coef=upgo_coef)
+        upgo_coef=upgo_coef, objective=objective)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -2717,7 +2799,7 @@ def build_arg_parser():
     ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches``, ``--mask-padding``,
     ``--pack-sequences``, ``--policy-ratio``, ``--value-norm``, ``--value-norm-decay``, ``--kl-coef``, ``--kl-target``,
     ``--kl-stop``, ``--value-heads``, ``--value-gammas``, ``--teacher-model``, ``--teacher-coef``,
-    ``--teacher-anneal-iterations`` and ``--upgo-coef``."""
+    ``--teacher-anneal-iterations``, ``--upgo-coef`` and ``--objective``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -2790,6 +2872,9 @@ def build_arg_parser():
     p.add_argument("--upgo-coef", type=float, default=0.0,
                    help="add this times the upgoing (UPGO) advantage, which follows a rollout's return only while the "
                         "next step does at least as well as the critic expects, to the GAE / V-trace advantage (0: off)")
+    p.add_argument("--objective", type=str, choices=OBJECTIVES, default='ppo',
+                   help="'bc' trains the policy on the log-likelihood of the actions of demonstrations (behaviour "
+                        "cloning) instead of the PPO surrogate (reference: ppo)")
     return p
 
 
@@ -2809,6 +2894,7 @@ if __name__ == '__main__':
              kl_target=args.kl_target, kl_stop=args.kl_stop, recompute_advantages=args.recompute_advantages,
              recompute_states=args.recompute_states, value_heads=args.value_heads, value_gammas=args.value_gammas,
              teacher_model=args.teacher_model, teacher_coef=args.teacher_coef,
-             teacher_anneal_iterations=args.teacher_anneal_iterations, upgo_coef=args.upgo_coef)
+             teacher_anneal_iterations=args.teacher_anneal_iterations, upgo_coef=args.upgo_coef,
+             objective=args.objective)
     except KeyboardInterrupt:
         pass

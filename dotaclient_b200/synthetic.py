@@ -59,6 +59,41 @@ def make_rollout(length, seed, game_id=0, team_id=2, weight_version=1, with_canv
     return data
 
 
+def demonstration_rollout(policy, length, seed, game_id=0, team_id=2, weight_version=1):
+    """``make_rollout(length, seed, ...)`` with the actions a demonstrator picked: ``policy`` (a ``Policy`` on a CUDA
+    device) plays every step with ``act_batched``, from its zero state, over the rollout's own observations, open loop (its
+    actions do not change the observations), with uniforms drawn from a generator that ``seed`` fixes.  The legal actions
+    of a step are every enum, x, y and ability entry and a seeded set of at least one target unit (never unit 0).  As an
+    agent stores them, the step's ``masks`` hold the enum row and the legal rows of the heads the enum action sampled, and
+    the other heads' rows are zero."""
+    from dotaclient_b200.ops import HEAD_KEYS
+    data = make_rollout(length, seed, game_id=game_id, team_id=team_id, weight_version=weight_version)
+    L = int(length)
+    g = torch.Generator().manual_seed(int(seed) + 104729)
+    units = torch.rand((L, 40), generator=g) < 0.5
+    units[:, 0] = False
+    units[torch.arange(L), torch.randint(1, 40, (L,), generator=g)] = True
+    u = torch.rand((L, 5), generator=g)
+    legal = {k: torch.ones((L, n), dtype=torch.bool) for k, n in HEAD_SIZES.items()}
+    legal["target_unit"] = units
+    dev = next(policy.parameters()).device
+    hidden = policy.init_hidden()
+    hidden = tuple(x.to(dev) for x in hidden) if isinstance(hidden, tuple) else hidden.to(dev)
+    picks = []
+    for t in range(L):
+        chosen, _, _, _, hidden = policy.act_batched(hidden, {k: v[t:t + 1].to(dev) for k, v in data["observations"].items()},
+                                                     {k: legal[k][t:t + 1].to(dev) for k in HEAD_KEYS}, u[t:t + 1].to(dev))
+        picks.append(torch.stack([chosen[k] for k in HEAD_KEYS], dim=1))
+    picks = torch.cat(picks).long().cpu()                 # [L, 5], -1 where the head was not sampled
+    for h, k in enumerate(HEAD_KEYS):
+        rows = picks[:, h] >= 0
+        data["masks"][k] = torch.where(rows[:, None], legal[k], torch.zeros_like(legal[k]))
+        act = torch.zeros((L, HEAD_SIZES[k]), dtype=torch.bool)
+        act[torch.nonzero(rows).flatten(), picks[rows, h]] = True
+        data["actions"][k] = act
+    return data
+
+
 def split_rollout(data, cuts, initial_hiddens=None):
     """One game's rollout -> the pieces an actor publishing every few steps sends: cut before each step in ``cuts``
     (increasing, each in ``[1, L)``).  Piece p holds steps ``[a, b)``.  Every piece but the last is ``'terminal': False``

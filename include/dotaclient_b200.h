@@ -601,6 +601,35 @@ int dc_ppo_loss_fwd_bwd_teacher(const float *const logits[DC_NUM_HEADS], const i
                                 float *stats, float *kl_out, float *teacher_stats, int32_t *n_actions, void *workspace,
                                 dc_stream_t stream);
 
+/* ---- behaviour cloning: the log-likelihood of a demonstrator's actions (supervised pretraining) ---------------------
+ * No counterpart in the reference.  With S_t and T_a as for KL control (the counting tokens, their heads with an action
+ * row, and the number of counting tokens with S_t not empty), a_{t,h} the action of row (t, h) and p the masked softmax
+ * over the legal entries of the stored mask:
+ *   NLL = (1 / T_a) sum_t sum_{h in S_t} -log p(a_{t,h})                                      (0 when T_a = 0)
+ *   loss = NLL + the entropy term + the value term of dc_ppo_loss_fwd_bwd_masked (clipped or not, value normalisation)
+ *   dlogits[t, h, j] = (1 / T_a)(p(j) - [j == a_{t,h}]) + the entropy gradient, for h in S_t and j legal
+ * There is no surrogate: old_logp is not an argument and the advantages are read only by the statistics pass, for
+ * out[14] / out[15].
+ *
+ * dc_ppo_loss_fwd_bwd_bc: the arguments of dc_ppo_loss_fwd_bwd_masked without old_logp (valid may be NULL), plus
+ *   bc_stats [DC_BC_STATS_SLOTS] fp32 out: 0 NLL, 1..5 the per-head NLL (sum over the head's action rows of -log p(a), over
+ *            their count; 0 for a head without any), 6 the token accuracy (the share of the T_a tokens where every head of
+ *            S_t has its action as the arg-max of its masked logits, the lowest index on ties), 7..11 the per-head
+ *            accuracy (over the head's action rows).
+ *   out: 1 is the NLL and 0 adds it; 9..13 are each head's share of the NLL (sum over its rows / T_a).
+ *   stats: the approximate KL and clip-fraction slots are 0; the explained variance is that of _masked.
+ * Algorithmic bytes: those of dc_ppo_loss_fwd_bwd_masked less the 20 per token of old_logp and the 4 of the advantage in
+ * the loss pass.  Checked before any CUDA call: the arguments of _masked, non-null hparams and bc_stats -> DC_EINVAL.
+ */
+#define DC_BC_STATS_SLOTS 12
+int dc_ppo_loss_fwd_bwd_bc(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                           const uint8_t *const masks[DC_NUM_HEADS], const uint8_t *const actions[DC_NUM_HEADS],
+                           const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                           const float *old_value, const uint8_t *valid, int64_t N, const double *hparams,
+                           float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS], float *dvalue,
+                           int64_t ld_dvalue, float *out, float *stats, float *bc_stats, int32_t *n_actions,
+                           void *workspace, dc_stream_t stream);
+
 /* ---- value normalisation (PopArt, van Hasselt et al. 2016) --------------------------------------------------------
  * No counterpart in the reference, whose critic learns raw returns (optimizer.py:660).
  *   dc_value_norm_stats    out[3] fp64 (device) = count, sum x, sum x^2 over the x[i] [N] with valid[i] != 0 (valid NULL:
