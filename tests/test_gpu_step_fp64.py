@@ -358,10 +358,16 @@ def compare(got, f64, f32, case):
     """-> (largest ratio max|got - f64| / max|f32 - f64| per kind, the largest max|got - f64| / max|f64| of the gradients,
     and the largest share of its bound any output uses; the tensors over their bound)."""
     diag = diagnostic_names(case)
-    names = scalar_names(case)
+    return compare_names(got, f64, f32, [n for n in scalar_names(case) if n not in diag], diag)
+
+
+def compare_names(got, f64, f32, scalars, diag):
+    """``compare`` of the reported values named in ``scalars`` (kind 'scalar') and ``diag`` (kind 'diagnostic') and of
+    every gradient."""
+    names = list(scalars) + list(diag)
     as_t = lambda d: {n: torch.tensor(float(d[n]), dtype=torch.float64) for n in names}      # noqa: E731
-    groups = [("scalar", [n for n in names if n not in diag], as_t(got[0]), as_t(f64[0]), as_t(f32[0])),
-              ("diagnostic", diag, as_t(got[0]), as_t(f64[0]), as_t(f32[0]))]
+    groups = [("scalar", list(scalars), as_t(got[0]), as_t(f64[0]), as_t(f32[0])),
+              ("diagnostic", list(diag), as_t(got[0]), as_t(f64[0]), as_t(f32[0]))]
     for kind in ("weight", "recurrent"):
         groups.append((kind, [n for n in f64[1] if n.startswith("rnn.") == (kind == "recurrent")], got[1], f64[1], f32[1]))
     ratios, over, used = {}, [], 0.0
