@@ -84,6 +84,9 @@ SIGNATURES = {
     "dc_ppo_loss_fwd_bwd_teacher": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp,
                                            _vp, _i64, _vp, _vp, _i32, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp,
                                            _vp, _vp, _vp, _vp]),
+    "dc_ppo_loss_fwd_bwd_dual_clip": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _vp, _vp, _vp, _i64,
+                                             _vp, _vp, _i64, _vp, _vp, _vp, _i32, _ptr5, _c.c_int64 * 5, _vp, _i64, _vp,
+                                             _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dc_ppo_loss_fwd_bwd_bc": (_i32, [_ptr5, _c.c_int64 * 5, _ptr5, _ptr5, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _vp, _ptr5,
                                       _c.c_int64 * 5, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dc_selected_logp_rows": (_i32, [_ptr5, _ptr5, _ptr5, _i64, _vp, _vp, _vp]),
@@ -119,6 +122,9 @@ KL_ROW_FLOATS = 65          # entries of one token's masked log-prob row over th
 TEACHER_STATS_SLOTS = 7
 # dc_ppo_loss_fwd_bwd_bc's bc_stats: 0 the NLL, 1..5 per head, 6 the token accuracy, 7..11 per head (DC_BC_STATS_SLOTS)
 BC_STATS_SLOTS = 12
+# dc_ppo_loss_fwd_bwd_dual_clip's dual_clip_stats: 0 the mean bound fraction over the heads, 1..5 per head, 6 the joint
+# ratio's (DC_DUAL_CLIP_STATS_SLOTS)
+DUAL_CLIP_STATS_SLOTS = 7
 FINISH_KL_METRICS = 6       # metrics of dc_grad_finish_kl: the four of dc_grad_finish, the all-ranks KL, the skip flag
 VTRACE_STATS_SLOTS = 8      # per-segment fp64 sums written by dc_vtrace_scan (DC_VTRACE_STATS_SLOTS)
 UPGO_STATS_SLOTS = 3        # per-segment fp64 sums written by dc_upgo_scan (DC_UPGO_STATS_SLOTS)

@@ -26,7 +26,7 @@ int dc_sm_count() {
 
 extern "C" {
 
-int dc_version(void) { return 115; }
+int dc_version(void) { return 116; }
 
 const char *dc_last_error(void) { return g_err; }
 

@@ -82,6 +82,23 @@
 // per-head path's.  ptxas (sm_90a, __launch_bounds__(128, 2)): 255 registers, no spills, 0 bytes stack frame, 53.5 KB dynamic
 // + 12.0 KB static shared memory, 2 CTAs per SM (at 3 CTAs per SM, ptxas's 168 registers spill 32 bytes).  Algorithmic
 // bytes: 686 - 24 = 662 per token for the loss pass (+ 1 valid, + 4 old value).
+//
+// Dual clip (`dc_ppo_loss_fwd_bwd_dual_clip`, kDual, either ratio mode, with or without kKl and kTeacher; Ye et al. 2020):
+// for a row with a negative normalised advantage A the clipped surrogate s = min(r A, clip(r) A) is floored at c A,
+//   term = max(s, c A) if A < 0, s otherwise,   c = *dual_clip > 1 (a device double next to the hparams block),
+// in head_token for each head's ratio and in the joint-ratio block for the token's.  The gradient is torch.where /
+// torch.maximum's: d term / d s = 1 above the floor, 1/2 on a tie, 0 below it, so a row where the floor binds (s < c A,
+// i.e. r > c) gets no surrogate gradient and keeps its entropy, KL and teacher terms.  With g_s = 1 the arithmetic is the
+// instantiation without kDual's (x * 1 is exact), so a c no ratio reaches gives its results bit for bit.  A bound row stages
+// a 1 in one more row per head (per-head ratios) or one row (joint), summed in float64 after the other staging rows, in the
+// same fixed order, into dual_clip_stats.  No extra bytes.  ptxas (sm_90a, __launch_bounds__(128, 2) for kDual, no spills, no
+// stack frame), registers and static shared memory per head / joint:
+//   alone           207 / 196 registers,  53.5 KB dynamic +  8.9 /  7.8 KB static, 2 CTAs per SM
+//   with kKl        193 / 197 registers,  86.8 KB dynamic + 11.5 / 10.4 KB static, 2 CTAs per SM
+//   with kTeacher   193 / 197 registers,  86.8 KB dynamic + 11.5 / 10.4 KB static, 2 CTAs per SM
+//   with both       195 / 198 registers, 120.1 KB dynamic + 14.1 / 13.0 KB static, 1 CTA per SM
+// The per-head instantiation alone runs at 2 CTAs per SM where _masked runs at 3 (ptxas's default 168 registers, with a
+// 48-byte spill): at 3 CTAs per SM the kDual code would spill too.
 #include "dc_common.cuh"
 
 namespace {
@@ -138,6 +155,9 @@ constexpr int kTeachStats = kHeads;
 // behaviour cloning only: per head the NLL of its action row, the token's all-heads-right flag, per head the arg-max flag
 // (the order of bc_stats)
 constexpr int kBcStats = 2 * kHeads + 1;
+// dual clip only: per head (per-head ratios) or once (the joint ratio) the flag of a row whose cap binds, after the above
+constexpr int kDualStats = kHeads;
+static_assert(DC_DUAL_CLIP_STATS_SLOTS == 2 + kHeads, "dual_clip_stats: the mean, per head, the joint ratio's");
 static_assert(DC_BC_STATS_SLOTS == 2 + 2 * kHeads, "bc_stats: the NLL, per head, the token accuracy, per head");
 static_assert(2 * kHeads + 3 < DC_PPO_STATS_SLOTS, "stats output too small");
 static_assert(DC_STAT_KL_PENALTY < DC_PPO_STATS_SLOTS, "stats output too small");
@@ -159,6 +179,7 @@ struct Workspace {
     double st_kl[kKlStats];          // KL control: per head, the sum over its action rows of the exact KL of the row
     double st_teach[kTeachStats];    // teacher: per head, the sum over its action rows of the KL to the teacher's row
     double st_bc[kBcStats];          // behaviour cloning: the sums of its staging rows (kBcStats above)
+    double st_dual[kDualStats];      // dual clip: per head (joint ratio: [0]) the rows whose cap binds
 };
 static_assert(sizeof(Workspace) <= DC_PPO_WORKSPACE_BYTES, "workspace too small");
 
@@ -308,6 +329,20 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
 }
 
 // ---- pass 2: loss + gradient --------------------------------------------------------------
+// Dual clip of one surrogate s = min(r A, clip(r) A): for A < 0, s <- max(s, c A), with g_s = d max / d s by the autograd
+// of torch.maximum (1 above the cap, 1/2 on a tie, 0 below it; NaN stays NaN as torch.maximum keeps it), and *bound = 1
+// where the cap binds (s < c A).  A >= 0 leaves s and g_s = 1 alone.
+__device__ __forceinline__ void dual_clip_term(float &s, float &g_s, float adv_n, float c, float *bound) {
+    if (adv_n < 0.f) {
+        const float cap = c * adv_n;
+        g_s = s > cap ? 1.f : (s == cap ? 0.5f : 0.f);
+        if (s < cap) {
+            *bound = 1.f;
+            s = cap;
+        }
+    }
+}
+
 // kKl, loss: `orow` is the token's prep-time log-prob row of head H; the exact KL of the row goes to *kl_row_out (when
 // the head has an action row here) and, with kl_scale = beta / T_a > 0, its gradient joins the dlogits row.
 // kKl, select (logp_out given): the full masked log-prob row overwrites the logits row in the tile, 0 at illegal entries.
@@ -315,14 +350,17 @@ __global__ void __launch_bounds__(kTile) ppo_stats_kernel(HeadPtrs hp, const flo
 // kBc (behaviour cloning, a loss): no surrogate.  A row with an action a (a row of S_t) writes -lp[a] to *nll_out and its
 // arg-max flag to *acc_out, sets bit H of *bc_in (and of *bc_miss when the arg-max is not a), and adds
 // bc_scale (p - [j == a]) to its legal entries, bc_scale = 1 / T_a.
-template <int H, bool kGrad, bool kKl = false, bool kTeach = false, bool kBc = false>
+// kDual (dual clip, a loss): for adv_n < 0 the row's term is max(s, dual_c adv_n), s the clipped surrogate; a row where the
+// cap binds (s < dual_c adv_n) writes 1 to *dual_out and gets no surrogate gradient.
+template <int H, bool kGrad, bool kKl = false, bool kTeach = false, bool kBc = false, bool kDual = false>
 __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, const uint8_t *arow, float old_lp,
                                            float adv_n, int n_h, float e_clip, float entropy_coef, float &pol_acc,
                                            float &ent_acc, float *kl_out, float *clip_out, float *logp_out,
                                            const float *orow = nullptr, float kl_scale = 0.f, float *kl_row_out = nullptr,
                                            const float *trow = nullptr, float t_scale = 0.f, float *t_row_out = nullptr,
                                            float bc_scale = 0.f, float *nll_out = nullptr, float *acc_out = nullptr,
-                                           int *bc_in = nullptr, int *bc_miss = nullptr) {
+                                           int *bc_in = nullptr, int *bc_miss = nullptr, float dual_c = 0.f,
+                                           float *dual_out = nullptr) {
     constexpr int N = head_n(H);
     float l[N], e[N];
     int mask_any = 0, a_idx = -1;
@@ -402,12 +440,15 @@ __device__ __forceinline__ void head_token(float *lrow, const uint8_t *mrow, con
         const float lo = 1.0f - e_clip, hi = 1.0f + e_clip;
         const float s1 = ratio * adv_n;                                // :639
         const float s2 = fminf(fmaxf(ratio, lo), hi) * adv_n;          // :640
-        pol_acc += fminf(s1, s2);                                      // :641 (negated, averaged at the end)
+        float surr = fminf(s1, s2), g_s = 1.f;
+        if (kDual) dual_clip_term(surr, g_s, adv_n, dual_c, dual_out);  // max(surr, c A) for A < 0
+        pol_acc += surr;                                               // :641 (negated, averaged at the end)
         // autograd of torch.min(a, b): ties split the gradient in half; clamp passes it inside [lo, hi].
         const float g1 = s1 < s2 ? 1.f : (s1 == s2 ? 0.5f : 0.f);
         const float g2 = s2 < s1 ? 1.f : (s1 == s2 ? 0.5f : 0.f);
         const float in_range = (ratio >= lo && ratio <= hi) ? 1.f : 0.f;
         g_lp = -(1.0f / kHeads) / (float)n_h * adv_n * (g1 + g2 * in_range) * ratio;
+        if (kDual) g_lp *= g_s;
     }
     if (kGrad) {
         const float ce = entropy_coef > 0.f ? entropy_coef / (float)n_h : 0.f;   // optimizer.py:652-656
@@ -539,10 +580,12 @@ __device__ __forceinline__ void joint_head_bwd(float *lrow, const uint8_t *mrow,
 // the teacher term (teacher_rows, *teacher_coef, teacher_stats), with or without kKl.
 // kBc (a loss, per-head path, neither kKl nor kTeacher): behaviour cloning, the NLL of the actions in place of the surrogate
 // (bc_stats); old_logp and the advantages are not read.
-// kTeacher asks for 2 CTAs per SM, which lets ptxas use more than the ~168 registers it picks otherwise and spill nothing;
-// the other instantiations keep ptxas's default (minBlocks 0 is "not given"), so their code is unchanged.
-template <bool kSelectOnly, bool kJoint, bool kKl = false, bool kTeacher = false, bool kBc = false>
-__global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_kernel(HeadPtrs hp, const float *__restrict__ old_logp,
+// kDual (a loss, either ratio mode, with or without kKl and kTeacher): dual clip, the floor under negative-advantage
+// surrogates (*dual_clip, dual_clip_stats).
+// kTeacher, kBc and kDual ask for 2 CTAs per SM, which lets ptxas use more than the ~168 registers it picks otherwise and
+// spill nothing; the other instantiations keep ptxas's default (minBlocks 0 is "not given"), so their code is unchanged.
+template <bool kSelectOnly, bool kJoint, bool kKl = false, bool kTeacher = false, bool kBc = false, bool kDual = false>
+__global__ void __launch_bounds__(kTile, (kTeacher || kBc || kDual) ? 2 : 0) ppo_loss_kernel(HeadPtrs hp, const float *__restrict__ old_logp,
                                                           const float *__restrict__ adv_raw,
                                                           const float *__restrict__ ret,
                                                           const float *__restrict__ value, int64_t N, float e_clip,
@@ -557,19 +600,24 @@ __global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_ker
                                                           const float *__restrict__ teacher_rows,
                                                           const double *__restrict__ teacher_coef,
                                                           float *__restrict__ teacher_stats,
-                                                          float *__restrict__ bc_stats) {
+                                                          float *__restrict__ bc_stats,
+                                                          const double *__restrict__ dual_clip,
+                                                          float *__restrict__ dual_clip_stats) {
     static_assert(!(kSelectOnly && kJoint), "the joint ratio is a loss");
+    static_assert(!kDual || !(kSelectOnly || kBc), "dual clip caps the PPO surrogate");
     static_assert(!(kSelectOnly && kTeacher), "the teacher term is a loss");
     static_assert(!kBc || !(kSelectOnly || kJoint || kKl || kTeacher), "behaviour cloning is a per-head loss of its own");
     constexpr bool kKlLoss = kKl && !kSelectOnly;
     constexpr int kTokKl = kTokRows + (kJoint ? kJointStats : 0);
     constexpr int kTokTeach = kTokKl + (kKlLoss ? kKlStats : 0);
     constexpr int kTokBc = kTokTeach + (kTeacher ? kTeachStats : 0);
-    constexpr int kRows = kTokBc + (kBc ? kBcStats : 0);
+    constexpr int kTokDual = kTokBc + (kBc ? kBcStats : 0);
+    constexpr int kRows = kTokDual + (kDual ? (kJoint ? 1 : kDualStats) : 0);
     constexpr int kSumKl = kStats + (kJoint ? kJointStats : 0);
     constexpr int kSumTeach = kSumKl + (kKlLoss ? kKlStats : 0);
     constexpr int kSumBc = kSumTeach + (kTeacher ? kTeachStats : 0);
-    constexpr int kSums = kSumBc + (kBc ? kBcStats : 0);
+    constexpr int kSumDual = kSumBc + (kBc ? kBcStats : 0);
+    constexpr int kSums = kSumDual + (kDual ? (kJoint ? 1 : kDualStats) : 0);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *s_logits = reinterpret_cast<float *>(smem_raw);
     float *s_old = s_logits + kLogitFloats;
@@ -598,6 +646,7 @@ __global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_ker
         if (kKlLoss) kl_coef = (float)hparams[DC_HP_KL_COEF];
     }
     const float t_coef = kTeacher ? (float)*teacher_coef : 0.f;     // teacher: lambda
+    const float dual_c = kDual ? (float)*dual_clip : 0.f;            // dual clip: c
     const bool vnorm = vn_sigma > 0.0;
     const bool clip_value = old_value != nullptr && value_clip > 0.f;
 
@@ -665,6 +714,8 @@ __global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_ker
         if (n_a) bc_scale = 1.0f / (float)n_a;
     }
     float *const s_bc_tok = kBc ? &s_tok[0][0] + kTokBc * kTile + t : nullptr;
+    // dual clip: this token's entry in the staging row of head 0's bound flag (joint ratio: the token's only one)
+    float *const s_dual_tok = kDual ? &s_tok[0][0] + kTokDual * kTile + t : nullptr;
     int bc_in = 0, bc_miss = 0;       // behaviour cloning: the heads of S_t, and those whose arg-max is not the action
     if (live) {
         float lp_sel[kHeads];
@@ -685,12 +736,15 @@ __global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_ker
                 const float lo = 1.0f - e_clip, hi = 1.0f + e_clip;
                 const float s1 = ratio * adv_n;
                 const float s2 = fminf(fmaxf(ratio, lo), hi) * adv_n;
-                pol[0] += fminf(s1, s2);
+                float surr = fminf(s1, s2), g_s = 1.f;
+                if (kDual) dual_clip_term(surr, g_s, adv_n, dual_c, s_dual_tok);   // as head_token caps each head's
+                pol[0] += surr;
                 // the same autograd rules as head_token: ties of torch.min split, clamp passes inside [lo, hi]
                 const float g1 = s1 < s2 ? 1.f : (s1 == s2 ? 0.5f : 0.f);
                 const float g2 = s2 < s1 ? 1.f : (s1 == s2 ? 0.5f : 0.f);
                 const float in_range = (ratio >= lo && ratio <= hi) ? 1.f : 0.f;
                 g_lp = -1.0f / (float)ws->n_joint * adv_n * (g1 + g2 * in_range) * ratio;
+                if (kDual) g_lp *= g_s;
             }
             // sweep 2 re-reads the tile: without this the compiler keeps every head's sweep-1 values live instead
             asm volatile("" ::: "memory");
@@ -706,7 +760,7 @@ __global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_ker
 #undef DC_JHEAD
         } else {
 #define DC_HEAD(H)                                                                                              \
-        head_token<H, true, kKl, kTeacher, kBc>(s_logits + logit_off(H) + t * head_pitch(H),                     \
+        head_token<H, true, kKl, kTeacher, kBc, kDual>(s_logits + logit_off(H) + t * head_pitch(H),              \
                                  s_mask + byte_off(H) + t * head_n(H),                                               \
                                  s_act + byte_off(H) + t * head_n(H),                                                \
                                  (kSelectOnly || kBc) ? 0.f : s_old[t * 5 + H], adv_n,                               \
@@ -717,7 +771,8 @@ __global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_ker
                                  s_trows + t * kRowFloats + row_col(H), t_scale,                                     \
                                  kTeacher ? s_t_tok + (H) * kTile : nullptr, bc_scale,                               \
                                  kBc ? s_bc_tok + (H) * kTile : nullptr,                                             \
-                                 kBc ? s_bc_tok + (kHeads + 1 + (H)) * kTile : nullptr, &bc_in, &bc_miss);
+                                 kBc ? s_bc_tok + (kHeads + 1 + (H)) * kTile : nullptr, &bc_in, &bc_miss, dual_c,    \
+                                 kDual ? s_dual_tok + (H) * kTile : nullptr);
         DC_HEAD(0) DC_HEAD(1) DC_HEAD(2) DC_HEAD(3) DC_HEAD(4)
 #undef DC_HEAD
             // behaviour cloning: the token is right when every head of S_t is (counted over the T_a tokens)
@@ -780,10 +835,11 @@ __global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_ker
         sums[2 * kHeads] = block_sum(vl, s_red);
         // the diagnostics (s_tok is complete: block_sum synchronised the block): one warp per sum, in float64.  KL control
         // and the teacher need their sums for kl_out / teacher_stats whether or not the diagnostics are asked for.
-        if (stats || kKlLoss || kTeacher || kBc) {
+        if (stats || kKlLoss || kTeacher || kBc || kDual) {
             const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
             for (int i = warp; i < kSums; i += kTile / 32) {
-                const int row = (kBc && i >= kSumBc) ? kTokBc + (i - kSumBc)
+                const int row = (kDual && i >= kSumDual) ? kTokDual + (i - kSumDual)
+                              : (kBc && i >= kSumBc) ? kTokBc + (i - kSumBc)
                               : (kTeacher && i >= kSumTeach) ? kTokTeach + (i - kSumTeach)
                               : (kKlLoss && i >= kSumKl) ? kTokKl + (i - kSumKl)
                               : (kJoint && i >= kStats) ? kTokJoint + (i - kStats) : (i < kStD ? i : (i < kStR ? kTokD : kTokR));
@@ -824,6 +880,10 @@ __global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_ker
             if constexpr (kBc) {
                 for (int i = 0; i < kBcStats; ++i)
                     if (s_st[kSumBc + i] != 0.0) atomicAdd(&ws->st_bc[i], s_st[kSumBc + i]);
+            }
+            if constexpr (kDual) {
+                for (int i = 0; i < kSums - kSumDual; ++i)
+                    if (s_st[kSumDual + i] != 0.0) atomicAdd(&ws->st_dual[i], s_st[kSumDual + i]);
             }
             __threadfence();
             s_last = atomicAdd(&ws->ticket_loss, 1u) == gridDim.x - 1;
@@ -939,6 +999,22 @@ __global__ void __launch_bounds__(kTile, (kTeacher || kBc) ? 2 : 0) ppo_loss_ker
                 }
                 teacher_stats[1 + kHeads] = term;
             }
+            if constexpr (kDual) {
+                // per head: the share of its action rows where the cap binds (0 for a head without any, and under the
+                // joint ratio), their mean over the heads with action rows; the joint ratio: the share of the T_a tokens
+                float sum = 0.f;
+                int used = 0;
+                for (int h = 0; h < kHeads; ++h) {
+                    const int n = w->cnt[h];
+                    const float f = (!kJoint && n) ? (float)(w->st_dual[h] / (double)n) : 0.f;
+                    dual_clip_stats[1 + h] = f;
+                    sum += f;
+                    used += n > 0;
+                }
+                dual_clip_stats[0] = used ? sum / (float)used : 0.f;
+                const unsigned long long n_a = w->n_joint;
+                dual_clip_stats[1 + kHeads] = (kJoint && n_a) ? (float)(w->st_dual[0] / (double)n_a) : 0.f;
+            }
         }
     }
 }
@@ -960,7 +1036,8 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
                     float *dvalue, int64_t ld_dvalue, float *out, float *stats, int32_t *n_actions, void *workspace,
                     dc_stream_t stream, bool joint = false, const float *old_rows = nullptr, float *kl_out = nullptr,
                     const float *teacher_rows = nullptr, const double *teacher_coef = nullptr,
-                    float *teacher_stats = nullptr, float *bc_stats = nullptr) {
+                    float *teacher_stats = nullptr, float *bc_stats = nullptr, const double *dual_clip = nullptr,
+                    float *dual_clip_stats = nullptr) {
     DC_REQUIRE(N > 0, DC_EINVAL, "dc_ppo_loss_fwd_bwd: N=%lld", (long long)N);
     // behaviour cloning (bc_stats given) reads no old_logp
     DC_REQUIRE(check_heads(logits, masks, actions) && (old_logp || bc_stats) && adv_raw && ret && value && dvalue && out &&
@@ -978,6 +1055,33 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
     Workspace *ws = reinterpret_cast<Workspace *>(workspace);
     DC_CUDA(cudaMemsetAsync(ws, 0, sizeof(Workspace), st));
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
+    if (dual_clip_stats) {      // dual clip, either ratio mode, with or without the KL rows and the teacher's
+        // the statistics pass of the entry point without the cap: T_a is counted when a term needs it
+        if (joint || old_rows || teacher_rows)
+            ppo_stats_kernel<true><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
+        else
+            ppo_stats_kernel<false><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
+        DC_LAUNCH_OK();
+        auto kern = ppo_loss_kernel<false, false, false, false, false, true>;
+        if (teacher_rows)
+            kern = old_rows ? (joint ? ppo_loss_kernel<false, true, true, true, false, true>
+                                     : ppo_loss_kernel<false, false, true, true, false, true>)
+                            : (joint ? ppo_loss_kernel<false, true, false, true, false, true>
+                                     : ppo_loss_kernel<false, false, false, true, false, true>);
+        else
+            kern = old_rows ? (joint ? ppo_loss_kernel<false, true, true, false, false, true>
+                                     : ppo_loss_kernel<false, false, true, false, false, true>)
+                            : (joint ? ppo_loss_kernel<false, true, false, false, false, true>
+                                     : ppo_loss_kernel<false, false, false, false, false, true>);
+        const size_t smem = teacher_rows ? (old_rows ? kSmemBytesKlTeacher : kSmemBytesKl)
+                                         : (old_rows ? kSmemBytesKl : kSmemBytes);
+        DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<blocks, kTile, smem, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip, entropy_coef, vf_coef, old_value,
+                                          valid, hparams, dvalue, out, stats, ws, nullptr, old_rows, kl_out, teacher_rows,
+                                          teacher_coef, teacher_stats, nullptr, dual_clip, dual_clip_stats);
+        DC_LAUNCH_OK();
+        return DC_OK;
+    }
     if (bc_stats) {             // behaviour cloning: the statistics pass counts T_a
         ppo_stats_kernel<true><<<blocks, kTile, 0, st>>>(hp, adv_raw, valid, N, ws, n_actions);
         DC_LAUNCH_OK();
@@ -985,7 +1089,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
         DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
         kern<<<blocks, kTile, kSmemBytes, st>>>(hp, nullptr, adv_raw, ret, value, N, e_clip, entropy_coef, vf_coef, old_value,
                                                 valid, hparams, dvalue, out, stats, ws, nullptr, nullptr, nullptr, nullptr,
-                                                nullptr, nullptr, bc_stats);
+                                                nullptr, nullptr, bc_stats, nullptr, nullptr);
         DC_LAUNCH_OK();
         return DC_OK;
     }
@@ -998,7 +1102,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
         DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<blocks, kTile, smem, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip, entropy_coef, vf_coef, old_value,
                                           valid, hparams, dvalue, out, stats, ws, nullptr, old_rows, kl_out, teacher_rows,
-                                          teacher_coef, teacher_stats, nullptr);
+                                          teacher_coef, teacher_stats, nullptr, nullptr, nullptr);
         DC_LAUNCH_OK();
         return DC_OK;
     }
@@ -1009,7 +1113,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
         DC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytesKl));
         kern<<<blocks, kTile, kSmemBytesKl, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip, entropy_coef, vf_coef, old_value,
                                                   valid, hparams, dvalue, out, stats, ws, nullptr, old_rows, kl_out,
-                                                  nullptr, nullptr, nullptr, nullptr);
+                                                  nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
         DC_LAUNCH_OK();
         return DC_OK;
     }
@@ -1021,7 +1125,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
         ppo_loss_kernel<false, true><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
                                                                         entropy_coef, vf_coef, old_value, valid, hparams,
                                                                         dvalue, out, stats, ws, nullptr, nullptr, nullptr, nullptr,
-                                                                        nullptr, nullptr, nullptr);
+                                                                        nullptr, nullptr, nullptr, nullptr, nullptr);
         DC_LAUNCH_OK();
         return DC_OK;
     }
@@ -1033,7 +1137,7 @@ int launch_ppo_loss(const float *const logits[DC_NUM_HEADS], const int64_t ld_lo
     ppo_loss_kernel<false, false><<<blocks, kTile, kSmemBytes, st>>>(hp, old_logp, adv_raw, ret, value, N, e_clip,
                                                                      entropy_coef, vf_coef, old_value, valid, hparams,
                                                                      dvalue, out, stats, ws, nullptr, nullptr, nullptr, nullptr,
-                                                                        nullptr, nullptr, nullptr);
+                                                                        nullptr, nullptr, nullptr, nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -1121,7 +1225,7 @@ extern "C" int dc_selected_logp(const float *const logits[DC_NUM_HEADS], const u
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
     ppo_loss_kernel<true, false><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
         hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-        nullptr, logp_out, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+        nullptr, logp_out, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -1144,7 +1248,7 @@ extern "C" int dc_selected_logp_rows(const float *const logits[DC_NUM_HEADS], co
     const unsigned blocks = (unsigned)((N + kTile - 1) / kTile);
     ppo_loss_kernel<true, false, true><<<blocks, kTile, kSmemBytes, dc_cu_stream(stream)>>>(
         hp, nullptr, nullptr, nullptr, nullptr, N, 0.f, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-        nullptr, logp_out, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+        nullptr, logp_out, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
     DC_LAUNCH_OK();
     return DC_OK;
 }
@@ -1195,4 +1299,29 @@ extern "C" int dc_ppo_loss_fwd_bwd_bc(const float *const logits[DC_NUM_HEADS], c
     return launch_ppo_loss(logits, ld_logits, masks, actions, nullptr, adv_raw, ret, value, ld_value, old_value, valid, N,
                            0.f, 0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions, workspace,
                            stream, false, nullptr, nullptr, nullptr, nullptr, nullptr, bc_stats);
+}
+
+extern "C" int dc_ppo_loss_fwd_bwd_dual_clip(const float *const logits[DC_NUM_HEADS],
+                                             const int64_t ld_logits[DC_NUM_HEADS],
+                                             const uint8_t *const masks[DC_NUM_HEADS],
+                                             const uint8_t *const actions[DC_NUM_HEADS], const float *old_logp,
+                                             const float *old_log_probs, const float *teacher_log_probs,
+                                             const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                                             const float *old_value, const uint8_t *valid, int64_t N,
+                                             const double *hparams, const double *teacher_coef, const double *dual_clip,
+                                             int joint, float *const dlogits[DC_NUM_HEADS],
+                                             const int64_t ld_dlogits[DC_NUM_HEADS], float *dvalue, int64_t ld_dvalue,
+                                             float *out, float *stats, float *kl_out, float *teacher_stats,
+                                             float *dual_clip_stats, int32_t *n_actions, void *workspace,
+                                             dc_stream_t stream) {
+    DC_REQUIRE(hparams, DC_EINVAL, "dc_ppo_loss_fwd_bwd_dual_clip: null hyper-parameter block");
+    DC_REQUIRE(dual_clip && dual_clip_stats, DC_EINVAL, "dc_ppo_loss_fwd_bwd_dual_clip: null dual_clip or dual_clip_stats");
+    // the teacher term: its rows, coefficient and statistics together, or none of them
+    DC_REQUIRE((teacher_log_probs != nullptr) == (teacher_coef != nullptr) &&
+                   (teacher_log_probs != nullptr) == (teacher_stats != nullptr),
+               DC_EINVAL, "dc_ppo_loss_fwd_bwd_dual_clip: teacher_log_probs, teacher_coef and teacher_stats go together");
+    return launch_ppo_loss(logits, ld_logits, masks, actions, old_logp, adv_raw, ret, value, ld_value, old_value, valid,
+                           N, 0.f, 0.f, 0.f, hparams, dlogits, ld_dlogits, dvalue, ld_dvalue, out, stats, n_actions,
+                           workspace, stream, joint != 0, old_log_probs, kl_out, teacher_log_probs, teacher_coef,
+                           teacher_stats, nullptr, dual_clip, dual_clip_stats);
 }

@@ -867,14 +867,28 @@ def _bc_args(bc_stats, dev, joint, old_log_probs, teacher_log_probs):
     return bc_stats
 
 
+def _dual_clip_args(dual_clip, dual_clip_stats, dev):
+    """Checks the extra operands of ``dc_ppo_loss_fwd_bwd_dual_clip``: ``dual_clip`` (1 fp64 on the device, c > 1) and
+    ``dual_clip_stats`` (``_lib.DUAL_CLIP_STATS_SLOTS`` fp32, allocated when None)."""
+    _need_cuda(dual_clip, dual_clip_stats)
+    assert dual_clip.dtype == torch.float64 and dual_clip.numel() == 1
+    if dual_clip_stats is None:
+        dual_clip_stats = torch.empty(_lib.DUAL_CLIP_STATS_SLOTS, dtype=torch.float32, device=dev)
+    assert dual_clip_stats.dtype == torch.float32 and dual_clip_stats.numel() == _lib.DUAL_CLIP_STATS_SLOTS \
+        and dual_clip_stats.is_contiguous()
+    return dual_clip_stats
+
+
 def _ppo_dev_call(lib, lptr, ld_l, masks, actions, old_logp, adv_raw, ret, value_ptr, ld_v, old_value, valid, N, hparams,
                   dptr, ld_d, dvalue_ptr, ld_dv, out, stats, n_actions, ws, joint=False, old_log_probs=None, kl_out=None,
-                  teacher_log_probs=None, teacher_coef=None, teacher_stats=None, bc_stats=None):
+                  teacher_log_probs=None, teacher_coef=None, teacher_stats=None, bc_stats=None, dual_clip=None,
+                  dual_clip_stats=None):
     """``dc_ppo_loss_fwd_bwd_dev``, or ``dc_ppo_loss_fwd_bwd_masked`` when a valid mask is given, or
     ``dc_ppo_loss_fwd_bwd_joint`` (valid or not) when ``joint``; ``dc_ppo_loss_fwd_bwd_kl`` (either ratio mode) when
     ``old_log_probs`` is given; ``dc_ppo_loss_fwd_bwd_teacher`` (either ratio mode, old rows or not) when
     ``teacher_log_probs`` is given; ``dc_ppo_loss_fwd_bwd_bc`` (valid or not; ``old_logp`` unused) when ``bc_stats`` is
-    given."""
+    given; ``dc_ppo_loss_fwd_bwd_dual_clip`` (either ratio mode, with or without the old and the teacher's rows) when
+    ``dual_clip`` is given."""
     if bc_stats is not None:
         with PROFILE.span("ppo_loss", 2):
             _lib.check(lib.dc_ppo_loss_fwd_bwd_bc(
@@ -889,7 +903,15 @@ def _ppo_dev_call(lib, lptr, ld_l, masks, actions, old_logp, adv_raw, ret, value
             ws.data_ptr(), _lib.stream_ptr())
     rows = (old_log_probs is not None) + (teacher_log_probs is not None)
     with PROFILE.span("ppo_loss", 2, _lib.KL_ROW_FLOATS * 4 * N * rows):
-        if teacher_log_probs is not None:
+        if dual_clip is not None:
+            _lib.check(lib.dc_ppo_loss_fwd_bwd_dual_clip(
+                lptr, ld_l, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(), _lib.ptr(old_log_probs),
+                _lib.ptr(teacher_log_probs), adv_raw.data_ptr(), ret.data_ptr(), value_ptr, ld_v, _lib.ptr(old_value),
+                _lib.ptr(valid), N, hparams.data_ptr(), _lib.ptr(teacher_coef), dual_clip.data_ptr(), 1 if joint else 0,
+                dptr, ld_d, dvalue_ptr, ld_dv, out.data_ptr(), stats.data_ptr(), _lib.ptr(kl_out),
+                _lib.ptr(teacher_stats), dual_clip_stats.data_ptr(), n_actions.data_ptr(), ws.data_ptr(),
+                _lib.stream_ptr()), "dc_ppo_loss_fwd_bwd_dual_clip")
+        elif teacher_log_probs is not None:
             _lib.check(lib.dc_ppo_loss_fwd_bwd_teacher(
                 lptr, ld_l, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(), _lib.ptr(old_log_probs),
                 teacher_log_probs.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(), value_ptr, ld_v, _lib.ptr(old_value),
@@ -912,7 +934,8 @@ def _ppo_dev_call(lib, lptr, ld_l, masks, actions, old_logp, adv_raw, ret, value
 
 def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_clip, entropy_coef, vf_coef, hparams=None,
                      old_value=None, stats=None, valid=None, joint=False, old_log_probs=None, kl_out=None,
-                     teacher_log_probs=None, teacher_coef=None, teacher_stats=None, bc=False, bc_stats=None):
+                     teacher_log_probs=None, teacher_coef=None, teacher_stats=None, bc=False, bc_stats=None,
+                     dual_clip=None, dual_clip_stats=None):
     """Fused PPO loss + gradients (``optimizer.py:587-589,621-665`` and their backward).
 
     logits/masks/actions: sequences of 5 tensors [..., n_h] in HEAD_KEYS order (any leading dims,
@@ -939,7 +962,14 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     (``dc_ppo_loss_fwd_bwd_bc``, with or without ``valid``; ``old_logp`` may be None and is not read); ``bc_stats``
     (``_lib.BC_STATS_SLOTS`` fp32, allocated when None) receives the NLL, per head, the token accuracy and per head, and the
     result gains it as a sixth element.
+    ``dual_clip`` (needs ``hparams``; 1 fp64 on the device, c > 1): dual-clip PPO, the surrogate of every row with a
+    negative normalised advantage A is floored at c A (``dc_ppo_loss_fwd_bwd_dual_clip``, either ratio mode, with or
+    without ``valid``, ``old_log_probs`` and ``teacher_log_probs``); ``dual_clip_stats``
+    (``_lib.DUAL_CLIP_STATS_SLOTS`` fp32, allocated when None) receives the shares of the rows where the floor binds, and the
+    result gains it as its last element (after ``teacher_stats`` with a teacher).
     """
+    if bc and dual_clip is not None:
+        raise ValueError("behaviour cloning has no PPO surrogate for dual clip to bound")
     logits = [_f32c(l.detach()) for l in logits]
     _need_cuda(*logits)
     N = logits[0].numel() // HEAD_SIZES[0]
@@ -959,13 +989,16 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
     ws = torch.empty(_lib.PPO_WORKSPACE_BYTES, dtype=torch.uint8, device=dev)
     lib = _lib.load()
     teacher = teacher_log_probs is not None
-    if hparams is not None or valid is not None or joint or old_log_probs is not None or teacher or bc:
-        if (old_log_probs is not None or teacher or bc) and hparams is None:
-            raise ValueError("the KL penalty, the teacher term and behaviour cloning need the device hyper-parameter "
-                             "block (hparams=)")
+    dual = dual_clip is not None
+    if hparams is not None or valid is not None or joint or old_log_probs is not None or teacher or bc or dual:
+        if (old_log_probs is not None or teacher or bc or dual) and hparams is None:
+            raise ValueError("the KL penalty, the teacher term, behaviour cloning and dual clip need the device "
+                             "hyper-parameter block (hparams=)")
         old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid, joint)
         if bc:
             bc_stats = _bc_args(bc_stats, dev, joint, old_log_probs, teacher_log_probs)
+        if dual:
+            dual_clip_stats = _dual_clip_args(dual_clip, dual_clip_stats, dev)
         if old_log_probs is not None:
             old_log_probs = _kl_args(old_log_probs, kl_out, N)
         if teacher:
@@ -973,9 +1006,11 @@ def ppo_loss_fwd_bwd(logits, masks, actions, old_logp, adv_raw, ret, value, e_cl
         ld = (ctypes.c_int64 * 5)(*HEAD_SIZES)
         _ppo_dev_call(lib, _lib.ptr5(logits), ld, masks, actions, old_logp, adv_raw, ret, value.data_ptr(), 1, old_value,
                       valid, N, hparams, _lib.ptr5(dlogits), ld, dvalue.data_ptr(), 1, out, stats, n_actions, ws, joint,
-                      old_log_probs, kl_out, teacher_log_probs, teacher_coef, teacher_stats, bc_stats if bc else None)
+                      old_log_probs, kl_out, teacher_log_probs, teacher_coef, teacher_stats, bc_stats if bc else None,
+                      dual_clip, dual_clip_stats)
         res = (out, n_actions, dlogits, dvalue, stats)
-        return res + (teacher_stats,) if teacher else res + (bc_stats,) if bc else res
+        res = res + (teacher_stats,) if teacher else res + (bc_stats,) if bc else res
+        return res + (dual_clip_stats,) if dual else res
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd(_lib.ptr5(logits), _lib.ptr5(masks), _lib.ptr5(actions),
                                            old_logp.data_ptr(), adv_raw.data_ptr(), ret.data_ptr(), value.data_ptr(),
@@ -1248,16 +1283,20 @@ def value_heads_loss(packed, d_packed, ret, hparams, out, head_stats, old_value=
 
 def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e_clip, entropy_coef, vf_coef, hparams=None,
                     old_value=None, stats=None, valid=None, joint=False, old_log_probs=None, kl_out=None,
-                    teacher_log_probs=None, teacher_coef=None, teacher_stats=None, bc=False, bc_stats=None):
+                    teacher_log_probs=None, teacher_coef=None, teacher_stats=None, bc=False, bc_stats=None,
+                    dual_clip=None, dual_clip_stats=None):
     """Fused PPO loss where the four small heads and the value head are column ranges of ONE packed ``[N,128]``
     tensor-core GEMM output (``PACK_COLS``) and the target-unit logits are a separate ``[N,40]`` tensor.
 
     Returns (out[16], n_actions[5], d_packed [N,128], d_logits_tu [N,40]): the gradients go straight back into the two
     producers, so no slice/cat kernels run and the five tiny K=131072 weight-gradient GEMMs become one wgmma wgrad.
     ``hparams`` / ``old_value`` / ``stats`` / ``valid`` / ``joint`` / ``old_log_probs`` / ``kl_out`` /
-    ``teacher_log_probs`` / ``teacher_coef`` / ``teacher_stats`` / ``bc`` / ``bc_stats``: as ``ppo_loss_fwd_bwd`` (the fifth
-    element of the result is then ``stats``, and with a teacher the sixth ``teacher_stats``, with ``bc`` ``bc_stats``).
+    ``teacher_log_probs`` / ``teacher_coef`` / ``teacher_stats`` / ``bc`` / ``bc_stats`` / ``dual_clip`` /
+    ``dual_clip_stats``: as ``ppo_loss_fwd_bwd`` (the fifth element of the result is then ``stats``, and with a teacher the
+    sixth ``teacher_stats``, with ``bc`` ``bc_stats``; with ``dual_clip`` ``dual_clip_stats`` comes last).
     """
+    if bc and dual_clip is not None:
+        raise ValueError("behaviour cloning has no PPO surrogate for dual clip to bound")
     _need_cuda(packed, logits_tu)
     p2 = _f32c(packed.detach()).reshape(-1, PACK_WIDTH)
     N = p2.shape[0]
@@ -1281,22 +1320,27 @@ def ppo_loss_packed(packed, logits_tu, masks, actions, old_logp, adv_raw, ret, e
     ld = (c.c_int64 * 5)(PACK_WIDTH, PACK_WIDTH, PACK_WIDTH, 40, PACK_WIDTH)
     lib = _lib.load()
     teacher = teacher_log_probs is not None
-    if hparams is not None or valid is not None or joint or old_log_probs is not None or teacher or bc:
-        if (old_log_probs is not None or teacher or bc) and hparams is None:
-            raise ValueError("the KL penalty, the teacher term and behaviour cloning need the device hyper-parameter "
-                             "block (hparams=)")
+    dual = dual_clip is not None
+    if hparams is not None or valid is not None or joint or old_log_probs is not None or teacher or bc or dual:
+        if (old_log_probs is not None or teacher or bc or dual) and hparams is None:
+            raise ValueError("the KL penalty, the teacher term, behaviour cloning and dual clip need the device "
+                             "hyper-parameter block (hparams=)")
         old_value, stats, valid = _ppo_dev_args(hparams, old_value, stats, N, dev, valid, joint)
         if bc:
             bc_stats = _bc_args(bc_stats, dev, joint, old_log_probs, teacher_log_probs)
+        if dual:
+            dual_clip_stats = _dual_clip_args(dual_clip, dual_clip_stats, dev)
         if old_log_probs is not None:
             old_log_probs = _kl_args(old_log_probs, kl_out, N)
         if teacher:
             teacher_log_probs, teacher_stats = _teacher_args(teacher_log_probs, teacher_coef, teacher_stats, N, dev)
         _ppo_dev_call(lib, lptr, ld, masks, actions, old_logp, adv_raw, ret, col(p2, "value"), PACK_WIDTH, old_value, valid,
                       N, hparams, dptr, ld, col(d_packed, "value"), PACK_WIDTH, out, stats, n_actions, ws, joint,
-                      old_log_probs, kl_out, teacher_log_probs, teacher_coef, teacher_stats, bc_stats if bc else None)
+                      old_log_probs, kl_out, teacher_log_probs, teacher_coef, teacher_stats, bc_stats if bc else None,
+                      dual_clip, dual_clip_stats)
         res = (out, n_actions, d_packed.view_as(packed), d_tu.view_as(logits_tu), stats)
-        return res + (teacher_stats,) if teacher else res + (bc_stats,) if bc else res
+        res = res + (teacher_stats,) if teacher else res + (bc_stats,) if bc else res
+        return res + (dual_clip_stats,) if dual else res
     with PROFILE.span("ppo_loss", 2):
         _lib.check(lib.dc_ppo_loss_fwd_bwd_strided(lptr, ld, _lib.ptr5(masks), _lib.ptr5(actions), old_logp.data_ptr(),
                                                    adv_raw.data_ptr(), ret.data_ptr(), col(p2, "value"), PACK_WIDTH, N,

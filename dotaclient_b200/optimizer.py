@@ -477,7 +477,7 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
                        policy_ratio='per_head', value_norm=False, value_norm_decay=0.99, kl_coef=0.0, kl_target=None,
                        kl_stop=None, recompute_advantages=False, recompute_states=False, value_heads=None,
                        value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None,
-                       upgo_coef=0.0, objective='ppo'):
+                       upgo_coef=0.0, objective='ppo', dual_clip=None):
     """Raises ``ValueError`` for PPO settings outside their domain: 0 < gamma <= 1, 0 <= gae_lambda <= 1, clip_range > 0,
     max_grad_norm > 0, value_clip None (off) or >= 0 (0 is off too), advantage_estimator one of ``ADVANTAGE_ESTIMATORS``,
     vtrace_rho_clip > 0, vtrace_c_clip > 0, num_minibatches an int >= 1 (not a bool), mask_padding a bool,
@@ -485,9 +485,10 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
     and 0 <= value_norm_decay < 1, finite kl_coef >= 0, kl_target None or finite > 0 (and then kl_coef > 0), kl_stop None
     or finite > 0, recompute_advantages and recompute_states bools, value_heads / value_gammas as ``value_head_groups``
     checks them (value heads refuse V-trace and value_norm), finite teacher_coef >= 0 and teacher_anneal_iterations None
-    or an int >= 1, both left at their defaults without a teacher_model, upgo_coef as ``check_upgo_coef`` checks it, and
-    objective one of ``OBJECTIVES``; 'bc' refuses what acts only on the policy-gradient term or needs a behaviour policy
-    (V-trace, the joint ratio, KL control, a teacher, UPGO).  NaN fails every check."""
+    or an int >= 1, both left at their defaults without a teacher_model, upgo_coef as ``check_upgo_coef`` checks it,
+    objective one of ``OBJECTIVES`` and dual_clip as ``check_dual_clip`` checks it; 'bc' refuses what acts only on the
+    policy-gradient term or needs a behaviour policy (V-trace, the joint ratio, KL control, a teacher, UPGO, dual clip).
+    NaN fails every check."""
     if not isinstance(recompute_states, bool):
         raise ValueError("recompute_states=%r: must be True or False" % (recompute_states,))
     if not isinstance(recompute_advantages, bool):
@@ -557,6 +558,7 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
         raise ValueError("value_heads with value_norm=True: PopArt would need one set of statistics per head and a "
                          "per-row rescale of the value head, which is not implemented")
     check_upgo_coef(upgo_coef, value_heads)
+    check_dual_clip(dual_clip)
     if not isinstance(objective, str) or objective not in OBJECTIVES:
         raise ValueError("objective=%r: must be one of %s" % (objective, ", ".join(OBJECTIVES)))
     if objective == 'bc':
@@ -569,10 +571,20 @@ def check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip=
                    ("teacher_model=%r" % (teacher_model,), teacher_model is not None,
                     "the demonstrations are the teacher; run the teacher term with objective='ppo'"),
                    ("upgo_coef=%r" % (upgo_coef,), float(upgo_coef) > 0.0, "UPGO changes the advantages, which the "
-                    "behaviour-cloning loss does not read")]
+                    "behaviour-cloning loss does not read"),
+                   ("dual_clip=%r" % (dual_clip,), dual_clip is not None, "there is no PPO surrogate to bound")]
         for what, bad, why in refused:
             if bad:
                 raise ValueError("%s with objective='bc': %s" % (what, why))
+
+
+def check_dual_clip(dual_clip):
+    """Raises ``ValueError`` unless ``dual_clip`` is None (off) or a finite number c > 1 (not a bool): the floor c A under
+    the surrogate of a negative-advantage row must lie below the clipped surrogate's own (1 + clip_range) A at r = 1."""
+    if dual_clip is None:
+        return
+    if isinstance(dual_clip, bool) or not isinstance(dual_clip, numbers.Real) or not 1.0 < float(dual_clip) < math.inf:
+        raise ValueError("dual_clip=%r: the dual-clip constant must be a finite number > 1 (or None: off)" % (dual_clip,))
 
 
 def check_upgo_coef(upgo_coef, value_heads=None):
@@ -1131,7 +1143,7 @@ class DotaOptimizer:
                  num_minibatches=1, mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False,
                  value_norm_decay=0.99, kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False,
                  recompute_states=False, value_heads=None, value_gammas=None, teacher_model=None, teacher_coef=1.0,
-                 teacher_anneal_iterations=None, upgo_coef=0.0, objective='ppo'):
+                 teacher_anneal_iterations=None, upgo_coef=0.0, objective='ppo', dual_clip=None):
         if not 1 <= num_layers <= self.MAX_LAYERS:
             raise ValueError("num_layers=%r: DotaOptimizer trains 1 to %d recurrent layers (the fused gradient-finish kernel "
                              "handles at most %d parameter tensors, 30 + 4 per layer)"
@@ -1143,8 +1155,14 @@ class DotaOptimizer:
                            kl_stop=kl_stop, recompute_advantages=recompute_advantages, recompute_states=recompute_states,
                            value_heads=value_heads, value_gammas=value_gammas, teacher_model=teacher_model,
                            teacher_coef=teacher_coef, teacher_anneal_iterations=teacher_anneal_iterations,
-                           upgo_coef=upgo_coef, objective=objective)
+                           upgo_coef=upgo_coef, objective=objective, dual_clip=dual_clip)
         check_minibatch_count(num_minibatches, min_seq_per_epoch)
+        # dual-clip PPO: the surrogate of every row with a negative normalised advantage A is floored at dual_clip * A
+        # (dc_ppo_loss_fwd_bwd_dual_clip).  On or off is fixed here (the step's graph holds the loss kernel); the value can
+        # be changed between steps, the upload before every step carries it to the device
+        self.dual_clip = None if dual_clip is None else float(dual_clip)
+        self._dual_clip_on = dual_clip is not None
+        self.last_dual_clip_stats = None    # the shares of the rows where the floor binds, of the last step
         # 'bc': every rollout is a demonstration (check_demonstrations at prep) and the loss is dc_ppo_loss_fwd_bwd_bc's, the
         # NLL of the demonstrated actions with the entropy and value terms of 'ppo'.  Fixed per optimizer, like policy_ratio
         self.objective = objective
@@ -1302,14 +1320,18 @@ class DotaOptimizer:
         n_t = 0 if self.teacher_model is None else _lib.TEACHER_STATS_SLOTS
         # behaviour cloning: its statistics (NLL, accuracy, per head) in the same place (a teacher is refused with it)
         n_bc = _lib.BC_STATS_SLOTS if objective == 'bc' else 0
-        self._result_dev = torch.zeros(self._n_metrics + _lib.PPO_STATS_SLOTS + n_vh + n_t + n_bc, dtype=torch.float32,
-                                       device=self.device)
+        # dual clip: the shares of the rows where its floor binds, after all of the above
+        n_dc = _lib.DUAL_CLIP_STATS_SLOTS if self._dual_clip_on else 0
+        self._result_dev = torch.zeros(self._n_metrics + _lib.PPO_STATS_SLOTS + n_vh + n_t + n_bc + n_dc,
+                                       dtype=torch.float32, device=self.device)
         self._metrics = self._result_dev[:self._n_metrics]
         self._ppo_stats = self._result_dev[self._n_metrics:self._n_metrics + _lib.PPO_STATS_SLOTS]
         o = self._n_metrics + _lib.PPO_STATS_SLOTS
         self._value_head_stats = self._result_dev[o:o + n_vh] if n_vh else None
-        self._teacher_stats = self._result_dev[o + n_vh:] if n_t else None
-        self._bc_stats = self._result_dev[o + n_vh:] if n_bc else None
+        self._teacher_stats = self._result_dev[o + n_vh:o + n_vh + n_t] if n_t else None
+        self._bc_stats = self._result_dev[o + n_vh:o + n_vh + n_bc] if n_bc else None
+        self._dual_clip_off = o + n_vh + n_t + n_bc       # offset of the dual-clip statistics in _result_dev
+        self._dual_clip_stats = self._result_dev[self._dual_clip_off:] if n_dc else None
         self._finish_ws = torch.zeros(_lib.FINISH_WORKSPACE_BYTES, dtype=torch.uint8, device=self.device)
         # learning_rate, e_clip, entropy_coef, vf_coef, MAX_GRAD_NORM and value_clip are read by the step's kernels from this
         # device block, rewritten from the pinned host copy before every step: a captured graph of the step holds the
@@ -1317,14 +1339,19 @@ class DotaOptimizer:
         # Value heads: a second block, the first with vf_coef = 0 and no value clip, for the PPO loss, whose value term
         # dc_value_heads_loss replaces; both blocks go up in the one copy
         # Teacher: its coefficient is one more double after the blocks (not a block slot), uploaded by the same copy
+        # Dual clip: its constant c is one more double after those, uploaded by the same copy
         n_blocks = 1 if self.value_heads is None else 2
-        n_hp = n_blocks * _lib.HPARAM_SLOTS + (0 if self.teacher_model is None else 1)
+        n_tc = 0 if self.teacher_model is None else 1
+        n_hp = n_blocks * _lib.HPARAM_SLOTS + n_tc + (1 if self._dual_clip_on else 0)
         self._hparams_host_flat = torch.zeros(n_hp, dtype=torch.float64).pin_memory()
         self._hparams_dev_flat = torch.zeros(n_hp, dtype=torch.float64, device=self.device)
         self._hparams_host_all = self._hparams_host_flat[:n_blocks * _lib.HPARAM_SLOTS].view(n_blocks, _lib.HPARAM_SLOTS)
         self._hparams_dev_all = self._hparams_dev_flat[:n_blocks * _lib.HPARAM_SLOTS].view(n_blocks, _lib.HPARAM_SLOTS)
-        self._teacher_coef_host = self._hparams_host_flat[n_blocks * _lib.HPARAM_SLOTS:]
-        self._teacher_coef_dev = self._hparams_dev_flat[n_blocks * _lib.HPARAM_SLOTS:]
+        o_tc = n_blocks * _lib.HPARAM_SLOTS
+        self._teacher_coef_host = self._hparams_host_flat[o_tc:o_tc + n_tc]
+        self._teacher_coef_dev = self._hparams_dev_flat[o_tc:o_tc + n_tc]
+        self._dual_clip_host = self._hparams_host_flat[o_tc + n_tc:]
+        self._dual_clip_dev = self._hparams_dev_flat[o_tc + n_tc:]
         self._hparams_host, self._hparams_dev = self._hparams_host_all[0], self._hparams_dev_all[0]
         self._hparams_dev_ppo = self._hparams_dev_all[n_blocks - 1]
         self._hparams_uploaded = None       # the values the device block holds
@@ -1945,9 +1972,9 @@ class DotaOptimizer:
         backward, all-reduce, finish: ~80 kernel launches -> one graph launch); batches still in flight from the host
         (``prefetch``) run the same kernels launch by launch so that the upload overlaps them.  Either way the step uses
         the current ``learning_rate``, ``e_clip``, ``entropy_coef``, ``vf_coef``, ``MAX_GRAD_NORM`` and ``value_clip``
-        (and under KL control ``kl_coef`` and ``kl_stop``, with a teacher ``teacher_coef``).  A step that ``kl_stop`` skips
-        returns normally, with the
-        parameters, Adam moments and step counters unchanged; ``last_ppo_stats['kl_skipped']`` is then 1.
+        (and under KL control ``kl_coef`` and ``kl_stop``, with a teacher ``teacher_coef``, with dual clip ``dual_clip``).
+        A step that ``kl_stop`` skips returns normally, with the parameters, Adam moments and step counters unchanged;
+        ``last_ppo_stats['kl_skipped']`` is then 1.
         """
         if isinstance(experiences, ExperienceBatch):
             batch = experiences if experiences.advantages.is_cuda else experiences.to(self.device)
@@ -1970,6 +1997,10 @@ class DotaOptimizer:
         if batch.reset_slot is not None and not self.mask_padding:
             raise ValueError("a packed batch (reset_slot) trains only with mask_padding=True: its padding carries no "
                              "advantages or value targets")
+        if self._dual_clip_on != (self.dual_clip is not None):
+            raise ValueError("dual_clip=%r: dual clip was %s when this optimizer was constructed, and that is fixed (the "
+                             "step's loss kernel depends on it)" % (self.dual_clip, "on" if self._dual_clip_on else "off"))
+        check_dual_clip(self.dual_clip)
         t_enter = time.perf_counter()
         self._upload_hparams()
         slot = batch._slot
@@ -2003,18 +2034,26 @@ class DotaOptimizer:
             self.last_ppo_stats['kl_all_ranks'] = float(res[_lib.LOSS_SLOTS + 4])
             self.last_ppo_stats['kl_skipped'] = float(res[_lib.LOSS_SLOTS + 5])
         if self._teacher_step(batch):   # the KL to the teacher (this rank), per head, and the loss term lambda KL_T
-            ts = res[_lib.LOSS_SLOTS + self._result_dev.numel() - _lib.TEACHER_STATS_SLOTS:].tolist()
+            ts = res[_lib.LOSS_SLOTS + self._dual_clip_off - _lib.TEACHER_STATS_SLOTS:].tolist()
             self.last_ppo_stats['teacher/kl'] = ts[0]
             for h, k in enumerate(keys):
                 self.last_ppo_stats['teacher/kl/' + k] = ts[1 + h]
             self.last_ppo_stats['loss/teacher'] = ts[6]
         if self.objective == 'bc':      # the NLL of the demonstrations (this rank) and the accuracy of the arg-max, per head
-            bs = res[_lib.LOSS_SLOTS + self._result_dev.numel() - _lib.BC_STATS_SLOTS:].tolist()
+            bs = res[_lib.LOSS_SLOTS + self._dual_clip_off - _lib.BC_STATS_SLOTS:].tolist()
             self.last_bc_stats = {'nll': bs[0], 'accuracy': bs[1 + len(keys)]}
             for h, k in enumerate(keys):
                 self.last_bc_stats['nll/' + k] = bs[1 + h]
                 self.last_bc_stats['accuracy/' + k] = bs[2 + len(keys) + h]
             self.last_ppo_stats.update({'bc/' + k: v for k, v in self.last_bc_stats.items() if k != 'nll'})
+        if self._dual_clip_on:          # the shares of the rows where the floor binds (this rank): mean, per head, joint
+            ds = res[_lib.LOSS_SLOTS + self._dual_clip_off:].tolist()
+            self.last_dual_clip_stats = {'fraction': ds[0]}
+            for h, k in enumerate(keys):
+                self.last_dual_clip_stats['fraction/' + k] = ds[1 + h]
+            if self.policy_ratio == 'joint':
+                self.last_dual_clip_stats['fraction/joint'] = ds[1 + len(keys)]
+            self.last_ppo_stats.update({'dual_clip_' + k: v for k, v in self.last_dual_clip_stats.items()})
         if res[_lib.LOSS_SLOTS + 3] != 0:               # :667-669, :678-679 (parameters were left untouched)
             if math.isnan(float(res[0])):
                 raise ValueError('loss={}, policy_loss={}, entropy_loss={}, value_loss={}'.format(
@@ -2108,10 +2147,11 @@ class DotaOptimizer:
         # value_norm: the statistics of the last prep (mu, sigma), which the loss normalises the raw targets with; off: 0, 0
         mu, sigma = self._value_norm_moments() if self.value_norm else (0.0, 0.0)
         # KL control: the penalty's beta and the early-stop limit (None: 0, no limit)
-        # teacher: its coefficient, the double after the blocks (_teacher_coef_dev)
+        # teacher: its coefficient, the double after the blocks (_teacher_coef_dev); dual clip: c, the double after that
         vals = (float(self.learning_rate), float(self.e_clip), float(self.entropy_coef), float(self.vf_coef),
                 float(self.MAX_GRAD_NORM), float(self.value_clip or 0.0), mu, sigma, float(self.kl_coef),
-                float(self.kl_stop or 0.0)) + ((float(self.teacher_coef),) if self.teacher_model is not None else ())
+                float(self.kl_stop or 0.0)) + ((float(self.teacher_coef),) if self.teacher_model is not None else ()) \
+            + ((float(self.dual_clip),) if self._dual_clip_on else ())
         if vals == self._hparams_uploaded:
             return
         h = self._hparams_host.numpy()
@@ -2125,6 +2165,8 @@ class DotaOptimizer:
             hp[_lib.HP_VF_COEF] = hp[_lib.HP_VALUE_CLIP] = 0.0
         if self.teacher_model is not None:
             self._teacher_coef_host[0] = float(self.teacher_coef)
+        if self._dual_clip_on:
+            self._dual_clip_host[0] = float(self.dual_clip)
         self._hparams_dev_flat.copy_(self._hparams_host_flat, non_blocking=True)
         # the value head has a gradient only while the value loss is on (optimizer.py:660-662): with vf_coef = 0 the
         # gradient finish skips its tensors (no Adam step, no share of the mean grad norm), like the reference's .grad = None
@@ -2164,6 +2206,7 @@ class DotaOptimizer:
         # feeds only an explained variance that dc_value_heads_loss overwrites, so the advantages stand in for it
         # teacher: the KL term to its rows with the coefficient after the hyper-parameter blocks (_upload_hparams)
         # bc: the NLL of the demonstrated actions in place of the surrogate (old_logp is not read)
+        # dual clip: the floor c A under negative-advantage surrogates, c after the teacher's coefficient (_upload_hparams)
         bc = self.objective == 'bc'
         out, n_actions, d_packed, d_tu = ops.ppo_loss_packed(
             packed, target_unit, [batch.masks[k] for k in keys], [batch.actions[k] for k in keys],
@@ -2173,7 +2216,8 @@ class DotaOptimizer:
             kl_out=self.flat.kl_tail, teacher_log_probs=teacher_log_probs,
             teacher_coef=self._teacher_coef_dev if teacher_log_probs is not None else None,
             teacher_stats=self._teacher_stats if teacher_log_probs is not None else None, bc=bc,
-            bc_stats=self._bc_stats)[:4]
+            bc_stats=self._bc_stats, dual_clip=self._dual_clip_dev if self._dual_clip_on else None,
+            dual_clip_stats=self._dual_clip_stats)[:4]
         if heads:
             ops.value_heads_loss(packed, d_packed, batch.returns, self._hparams_dev, out, self._value_head_stats,
                                  old_value=batch.old_values, valid=valid, stats=self._ppo_stats)
@@ -2605,6 +2649,8 @@ class DotaOptimizer:
                 metrics['kl/updates_run'], metrics['kl/updates_skipped'] = self.last_kl_updates
             if self.kl_target is not None:                                 # for the next iteration (saved with the model)
                 self.kl_coef = kl_coef_update(self.kl_coef, d, self.kl_target)
+        if self._dual_clip_on:                                             # the constant this iteration trained with
+            metrics['dual_clip/coef'] = self.dual_clip
         if self.teacher_model is not None:                                 # the coefficient this iteration trained with
             metrics['teacher/coef'] = self.teacher_coef
             if teacher_on:
@@ -2755,7 +2801,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
          mask_padding=False, pack_sequences=False, policy_ratio='per_head', value_norm=False, value_norm_decay=0.99,
          kl_coef=0.0, kl_target=None, kl_stop=None, recompute_advantages=False, recompute_states=False, value_heads=None,
          value_gammas=None, teacher_model=None, teacher_coef=1.0, teacher_anneal_iterations=None, upgo_coef=0.0,
-         objective='ppo'):
+         objective='ppo', dual_clip=None):
     check_ppo_settings(gamma, gae_lambda, clip_range, max_grad_norm, value_clip, advantage_estimator=advantage_estimator,
                        vtrace_rho_clip=vtrace_rho_clip, vtrace_c_clip=vtrace_c_clip, num_minibatches=num_minibatches,
                        mask_padding=mask_padding, pack_sequences=pack_sequences,
@@ -2765,7 +2811,8 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
                        recompute_states=recompute_states, value_heads=value_heads,
                        value_gammas=value_gammas, teacher_model=teacher_model, teacher_coef=teacher_coef,
                        teacher_anneal_iterations=teacher_anneal_iterations,
-                       upgo_coef=upgo_coef, objective=objective)                         # before any process-group setup
+                       upgo_coef=upgo_coef, objective=objective,
+                       dual_clip=dual_clip)                                              # before any process-group setup
     check_minibatch_count(num_minibatches, min_seq_per_epoch)
     if dist.is_available() and 'WORLD_SIZE' in os.environ:
         init_distribution()
@@ -2781,7 +2828,7 @@ def main(rmq_host, rmq_port, epochs, min_seq_per_epoch, seq_len, learning_rate,
         kl_target=kl_target, kl_stop=kl_stop, recompute_advantages=recompute_advantages,
         recompute_states=recompute_states, value_heads=value_heads, value_gammas=value_gammas,
         teacher_model=teacher_model, teacher_coef=teacher_coef, teacher_anneal_iterations=teacher_anneal_iterations,
-        upgo_coef=upgo_coef, objective=objective)
+        upgo_coef=upgo_coef, objective=objective, dual_clip=dual_clip)
     if isinstance(dota_optimizer.mq, MessageQueue):
         logger.warning('the built-in MessageQueue is an IN-PROCESS broker (the AMQP transport is out of scope): with no producer '
                        'thread publishing to it in this process run() will wait forever; pass mq=<your pika-backed queue> to '
@@ -2799,7 +2846,7 @@ def build_arg_parser():
     ``--advantage-estimator``, ``--vtrace-rho-clip``, ``--vtrace-c-clip``, ``--num-minibatches``, ``--mask-padding``,
     ``--pack-sequences``, ``--policy-ratio``, ``--value-norm``, ``--value-norm-decay``, ``--kl-coef``, ``--kl-target``,
     ``--kl-stop``, ``--value-heads``, ``--value-gammas``, ``--teacher-model``, ``--teacher-coef``,
-    ``--teacher-anneal-iterations``, ``--upgo-coef`` and ``--objective``."""
+    ``--teacher-anneal-iterations``, ``--upgo-coef``, ``--objective`` and ``--dual-clip``."""
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log-dir", type=str, help="log and job dir name", default=default_log_dir())
     p.add_argument("--ip", type=str, help="mq ip", default='127.0.0.1')
@@ -2875,6 +2922,9 @@ def build_arg_parser():
     p.add_argument("--objective", type=str, choices=OBJECTIVES, default='ppo',
                    help="'bc' trains the policy on the log-likelihood of the actions of demonstrations (behaviour "
                         "cloning) instead of the PPO surrogate (reference: ppo)")
+    p.add_argument("--dual-clip", type=float, default=None, metavar="C",
+                   help="dual-clip PPO: floor the surrogate of every action with a negative advantage A at C * A, C > 1 "
+                        "(Ye et al. 2020 use 3), so that a ratio that has run away stops driving the update (default: off)")
     return p
 
 
@@ -2895,6 +2945,6 @@ if __name__ == '__main__':
              recompute_states=args.recompute_states, value_heads=args.value_heads, value_gammas=args.value_gammas,
              teacher_model=args.teacher_model, teacher_coef=args.teacher_coef,
              teacher_anneal_iterations=args.teacher_anneal_iterations, upgo_coef=args.upgo_coef,
-             objective=args.objective)
+             objective=args.objective, dual_clip=args.dual_clip)
     except KeyboardInterrupt:
         pass

@@ -630,6 +630,41 @@ int dc_ppo_loss_fwd_bwd_bc(const float *const logits[DC_NUM_HEADS], const int64_
                            int64_t ld_dvalue, float *out, float *stats, float *bc_stats, int32_t *n_actions,
                            void *workspace, dc_stream_t stream);
 
+/* ---- dual-clip PPO: a floor under the surrogate of negative-advantage rows (Ye et al. 2020) -------------------------
+ * No counterpart in the reference.  With A_t the token's normalised advantage (as every loss entry point normalises it),
+ * r the ratio (per head, or the joint ratio of the token) and s = min(r A_t, clip(r, 1 - eps, 1 + eps) A_t) the clipped
+ * surrogate, each row's term becomes
+ *   term = s                  if A_t >= 0
+ *   term = max(s, c A_t)      if A_t <  0,        c = *dual_clip > 1
+ * so the term of a row with A_t < 0 stays bounded as r grows.  The gradient is the autograd of
+ * torch.where(A < 0, torch.maximum(s, c A), s): a row where the cap binds (s < c A, that is r > c) gets no surrogate
+ * gradient, a tie splits it in half.  Per-head and joint means, the entropy and value terms, the KL penalty and the teacher
+ * term are those of dc_ppo_loss_fwd_bwd_teacher.
+ *
+ * dc_ppo_loss_fwd_bwd_dual_clip: the arguments of dc_ppo_loss_fwd_bwd_teacher, with old_log_probs and kl_out nullable (NULL:
+ *   no KL penalty) and teacher_log_probs, teacher_coef and teacher_stats nullable together (NULL: no teacher term), plus
+ *   dual_clip          one fp64 device value, c > 1 (kept off the hparams block, read on every launch)
+ *   dual_clip_stats [DC_DUAL_CLIP_STATS_SLOTS] fp32 out: 1..5 per head the share of its action rows where the cap binds
+ *                      (0 for a head without any, and under the joint ratio), 0 their mean over the heads with action
+ *                      rows, 6 the share of the T_a tokens where the joint ratio's cap binds (0 with per-head ratios).
+ *   With a c no ratio reaches, the loss, dlogits, dvalue, stats, kl_out and teacher_stats are those of the entry point the
+ *   call would otherwise be (_masked / _dev, _joint, _kl or _teacher) bit for bit.
+ * Algorithmic bytes: those of the entry point it extends; the cap adds no traffic.  Checked before any CUDA call: the
+ * arguments of _masked, non-null hparams, dual_clip and dual_clip_stats, and the teacher's three pointers all given or all
+ * NULL -> DC_EINVAL.
+ */
+#define DC_DUAL_CLIP_STATS_SLOTS 7
+int dc_ppo_loss_fwd_bwd_dual_clip(const float *const logits[DC_NUM_HEADS], const int64_t ld_logits[DC_NUM_HEADS],
+                                  const uint8_t *const masks[DC_NUM_HEADS], const uint8_t *const actions[DC_NUM_HEADS],
+                                  const float *old_logp, const float *old_log_probs, const float *teacher_log_probs,
+                                  const float *adv_raw, const float *ret, const float *value, int64_t ld_value,
+                                  const float *old_value, const uint8_t *valid, int64_t N, const double *hparams,
+                                  const double *teacher_coef, const double *dual_clip, int joint,
+                                  float *const dlogits[DC_NUM_HEADS], const int64_t ld_dlogits[DC_NUM_HEADS],
+                                  float *dvalue, int64_t ld_dvalue, float *out, float *stats, float *kl_out,
+                                  float *teacher_stats, float *dual_clip_stats, int32_t *n_actions, void *workspace,
+                                  dc_stream_t stream);
+
 /* ---- value normalisation (PopArt, van Hasselt et al. 2016) --------------------------------------------------------
  * No counterpart in the reference, whose critic learns raw returns (optimizer.py:660).
  *   dc_value_norm_stats    out[3] fp64 (device) = count, sum x, sum x^2 over the x[i] [N] with valid[i] != 0 (valid NULL:
